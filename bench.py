@@ -4,6 +4,7 @@ bench.py -- megapixels/second through pipe_color2d_slic_features_model_graphcut 
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on host cores
+    python bench.py ... --dump-outputs DIR                     # also write what the last timed step computed as DIR/*.npy
 
 Workload (BASELINE.json configs[1], SURVEY.md section 8d "config 2"): one synthetic 2048x2048 RGB float64 image per
 GPU per step -- Voronoi regions with 3 class means + gaussian noise, sp_size 29 (4 987 seeds), colour-mean descriptors,
@@ -49,7 +50,7 @@ def headline_config(n_gpus):
     return {'workload': WORKLOAD, 'images_per_step_per_gpu': 1, 'sp_size': SP_SIZE, 'sp_regul': SP_REGUL,
             'nb_classes': NB_CLASSES, 'gc_regul': GC_REGUL, 'features': 'color mean', 'class_model': 'StandardScaler + full-covariance GMM (n_init 9, max_iter 99)',
             'parallelism': 'independent images sharded over %d GPU(s) / host processes' % n_gpus,
-            'l2': 'no explicit flush: per-step working set (f64 image 100 MB + Lab 100 MB + soft output 100 MB) exceeds the 126 MB L2'}
+            'l2': 'no explicit flush: per-step working set (f64 image 100 MB + Lab 100 MB + soft output 100 MB) exceeds the 50 MB L2'}
 
 
 def probe_reference_libs():
@@ -126,7 +127,7 @@ def load_peaks():
         with open(path) as f:
             p = json.load(f)
         return float(p['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet 3.35 TB/s, not measured)'
 
 
 def load_tensor_peak():
@@ -137,20 +138,7 @@ def load_tensor_peak():
             p = json.load(f)
         if 'bf16_tflops' in p:
             return float(p['bf16_tflops']), 'measured (MEASURED_PEAKS.json bf16_tflops, burst)'
-    return 1590.0, 'fallback (B200_PROFILING.md 1.59 PFLOP/s)'
-
-
-TRAFFIC_SOURCE = 'profiles/r02c_assign_traffic.json'
-
-
-def load_traffic():
-    """DRAM bytes per k_assign launch from the committed `ncu --set full` capture (profiles/), or None"""
-    path = os.path.join(ROOT, TRAFFIC_SOURCE)
-    try:
-        with open(path) as f:
-            return int(json.load(f)['traffic_bytes_per_launch'])
-    except (OSError, KeyError, ValueError):
-        return None
+    return 989.0, 'fallback (H100 SXM data sheet, dense bf16 989 TFLOP/s at 700 W, not measured)'
 
 
 class ClockSampler(object):
@@ -179,6 +167,7 @@ class ClockSampler(object):
             return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['nvidia-smi unavailable']}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         sm = [float(r[0]) for r in self.rows if r and r[0].replace('.', '').isdigit()]
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace('.', '').isdigit()]
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
@@ -275,9 +264,8 @@ def run_reference(args):
     if rank != 0:
         return
     cores = os.cpu_count() or 1
-    # the reference's own rule is NB_WORKERS = 0.6 * cpu_count (pipelines.py:43); on the 128-CPU host of the B200 box the path
-    # stops scaling at ~16 processes (measured r01: 1 -> 0.86, 8 -> 7.9, 16 -> 12.0, 32 -> 10.1, 64 -> 6.8 MPix/s; memory bound),
-    # so 16 workers is the reference's best case and keeps a step at a few seconds
+    # the reference's own rule is NB_WORKERS = 0.6 * cpu_count (pipelines.py:43); the path is memory bound and on a large host
+    # stops scaling at ~16 processes, so 16 workers is the reference's best case and keeps a step at a few seconds
     workers = args.ref_workers or min(16, max(1, int(0.6 * cores)))
     n_img = workers  # one bounded sample per step: `workers` images through the process pool
     pool = ReferencePool(n_img, workers)
@@ -375,8 +363,11 @@ def run_ours(args):
         sampler.start()
     # timed region 1 (the `value`): the device part replayed as one CUDA graph per image (pipelines._run_resident_graph)
     n0 = lib.isb_launch_count()
-    ms_res, _ = timed(step_resident, args.steps)
+    ms_res, (d_segm, d_soft) = timed(step_resident, args.steps)
     launches = lib.isb_launch_count() - n0
+    # the engine reuses its result buffers: copy the last timed step's outputs before anything else runs
+    dumped = host_outputs(d_segm, d_soft) if args.dump_outputs else None
+    del d_segm, d_soft
     # timed region 2 (same steps, eager launches): per-stage CUDA events on the launching stream -> `stages` and the roofline
     pipelines.USE_CUDA_GRAPHS = False
     step_resident()
@@ -400,7 +391,7 @@ def run_ours(args):
         return None
 
     batch_once()
-    ms_batch, _ = timed(batch_once, 2)
+    ms_batch, _ = timed(batch_once, args.steps)
     clocks = sampler.stop() if rank == 0 else None
 
     stages = {lib.isb_profile_stage_name(i).decode(): {'ms_per_step': ms_arr[i] / args.steps, 'launches_per_step': cnt_arr[i] / args.steps}
@@ -425,6 +416,8 @@ def run_ours(args):
         if world > 1:
             dist.destroy_process_group()
         return
+    if dumped is not None:
+        write_outputs(args.dump_outputs, dumped)
     line = {
         'metric': METRIC, 'value': value, 'unit': 'MPix/s', 'n_gpus': world, 'steps': args.steps, 'warmup': max(args.warmup, 3),
         'ms_per_step': ms_res / args.steps, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f64',
@@ -434,11 +427,11 @@ def run_ours(args):
                 'd2h_bytes_per_step': int(segm.nbytes + soft.nbytes), 'source': 'pinned host ndarray'},
         'e2e_pageable': {'value': world * args.steps * mpix / (ms_page / 1e3), 'unit': 'MPix/s', 'ms_per_step': ms_page / args.steps,
                          'source': 'ordinary (pageable) numpy array, as a caller of the reference API would pass it'},
-        'e2e_batch': {'value': world * 2 * nbatch * mpix / (ms_batch / 1e3), 'unit': 'MPix/s', 'images_per_call': nbatch,
+        'e2e_batch': {'value': world * args.steps * nbatch * mpix / (ms_batch / 1e3), 'unit': 'MPix/s', 'images_per_call': nbatch,
                       'note': 'segment_images_batch: same host-in/host-out path, copies of consecutive images overlapped on 3 streams'},
         'gpu_launches': int(launches),
         'roofline': {'kernel': 'k_assign (slic_assign)', 'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
-                     'frac': achieved / peak, 'traffic': load_traffic(), 'traffic_source': TRAFFIC_SOURCE, 'peak_source': peak_src,
+                     'frac': achieved / peak, 'peak_source': peak_src,
                      'algorithmic_bytes_per_launch': ASSIGN_BYTES_PER_PX * H * W, 'launch_ms': t_assign * 1e3,
                      'bytes_per_px': '16 = SURVEY.md section 8(d) (f32 image 12 + label 4)',
                      'f64_layout': {'bytes_per_px': ASSIGN_LAYOUT_BYTES_PER_PX, 'achieved': achieved_layout, 'frac': achieved_layout / peak,
@@ -470,6 +463,26 @@ def run_ours(args):
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+#: pixels of segm_soft in the dump: a fixed, seeded sample (the whole float64 array of a 2048x2048 image is 96 MiB)
+DUMP_SOFT_PIXELS = 1 << 20
+
+
+def host_outputs(d_segm, d_soft):
+    """the arrays a caller of the timed path receives, on the host: segm whole, segm_soft at a seeded sample of pixels"""
+    segm = d_segm.cpu().numpy()
+    soft = d_soft.reshape(-1, d_soft.shape[-1])
+    idx = np.sort(np.random.RandomState(0).choice(soft.shape[0], min(DUMP_SOFT_PIXELS, soft.shape[0]), replace=False))
+    import torch
+    soft = soft[torch.from_numpy(idx).to(soft.device)].cpu().numpy()
+    return {'segm': segm.astype(np.float32), 'segm_soft_sample': soft.astype(np.float64), 'segm_soft_sample_pixels': idx.astype(np.float64)}
+
+
+def write_outputs(directory, arrays):
+    os.makedirs(directory, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(directory, name + '.npy'), arr)
 
 
 def run_tiled(args):
@@ -642,18 +655,18 @@ def run_texture(args):
 
 def lm_roofline(lm_ms, H, W):
     """tensor-bound roofline of the Leung-Malik stage: algorithmic flops = one multiply-add per tap (3 channels x 76 kernels x 33^2 x 2
-    per pixel, SURVEY 8d); executed = what the tcgen05 contraction issues (76 -> 80 filters, 33 -> 40 taps per kernel row, three TF32
+    per pixel, SURVEY 8d); executed = what the wgmma contraction issues (76 -> 80 filters, 33 -> 40 taps per kernel row, three TF32
     products per multiply)"""
     if not lm_ms:
         return None
     peak, peak_source = load_tensor_peak()
     algo = 3 * 76 * 33 * 33 * 2 * H * W / (lm_ms / 1e3) / 1e12
     executed = 3 * 80 * 33 * 40 * 2 * 3 * H * W / (lm_ms / 1e3) / 1e12
-    return {'kernel': 'k_lm_conv_ts (lm_texture stage: FP64 background blur + tcgen05 contraction + fused statistics)', 'bound': 'tensor',
+    return {'kernel': 'k_lm_conv_wg (lm_texture stage: FP64 background blur + wgmma contraction + fused statistics)', 'bound': 'tensor',
             'unit': 'TFLOP/s', 'achieved': algo, 'peak': peak, 'frac': algo / peak, 'peak_source': peak_source,
             'executed_tf32': executed, 'executed_frac_of_tf32_peak': executed / (peak / 2),
             'note': 'achieved = algorithmic flops over the WHOLE lm_texture stage time (CUDA events); peak = measured dense bf16 (TF32 runs '
-                    'at half of it); the contraction kernel alone and its ncu capture: profiles/r02_lm_tcgen05.md'}
+                    'at half of it)'}
 
 
 def run_rg2sp(args):
@@ -728,7 +741,12 @@ def main():
     ap.add_argument('--workload', default='config2', choices=['config2', 'config3', 'config4', 'config5'],
                     help='config2 = the headline line (default); config5 = one 8192x8192 image banded over the GPUs (extra)')
     ap.add_argument('--tiled-side', type=int, default=8192)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the timed path computed in its last step as DIR/<name>.npy (segm whole as float32, segm_soft '
+                         'at %d seeded pixels as float64, with those pixels\' flat indices); headline workload only' % DUMP_SOFT_PIXELS)
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != 'ours' or args.workload != 'config2'):
+        ap.error('--dump-outputs writes the outputs of the headline workload (config2) of this repo\'s path')
     if args.impl == 'reference':
         run_reference(args)
     elif args.workload == 'config5':

@@ -1,6 +1,6 @@
 """
 Drop-in alias: ``import imsegm.pipelines`` (``superpixels``, ``descriptors``, ``graph_cuts``) resolves to the
-B200-native implementation in ``pyimsegm_b200`` for the SLIC -> features -> GraphCut hot path of Borda/pyImSegm and for the
+H100-native implementation in ``pyimsegm_b200`` for the SLIC -> features -> GraphCut hot path of Borda/pyImSegm and for the
 region growing (RG2SP) built on it.  Modules of the reference outside that path (classification, annotation, ...) are not provided.
 """
 import sys

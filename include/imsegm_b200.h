@@ -1,5 +1,5 @@
 /*
- * imsegm_b200.h -- C-ABI of the B200-native SLIC -> descriptors -> GraphCut hot path of Borda/pyImSegm.
+ * imsegm_b200.h -- C-ABI of the H100-native (sm_90a) SLIC -> descriptors -> GraphCut hot path of Borda/pyImSegm.
  *
  * Every entry point takes plain DEVICE pointers (unless a parameter says "host"), sizes and a CUDA stream
  * (cudaStream_t passed as void*), returns 0 on success or a negative isb_status, never allocates what it
@@ -270,8 +270,8 @@ int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, const int32_t*
                         double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream);
 
 /* compute_texture_desc_lm_img2d_clr (imsegm/descriptors.py:1041-1106): sigma-150 background subtraction (reflect, all three
- * axes), Leung-Malik filter bank (33x33 kernels) as an implicit GEMM on the tensor cores (tcgen05.mma kind::tf32 with the 3xTF32
- * split, FP32 accumulators in tensor memory, operands staged by TMA), max over the orientations of a battery, clip at 1e6,
+ * axes), Leung-Malik filter bank (33x33 kernels) as an implicit GEMM on the tensor cores (wgmma.mma_async with TF32 inputs and the 3xTF32
+ * split, FP32 accumulators in registers, operands staged by TMA), max over the orientations of a battery, clip at 1e6,
  * log-norm scaling, per-superpixel mean / std / energy -- the responses never leave the SM.
  *   bg_weights : device, 2*bg_radius+1 doubles (scipy's gaussian kernel, sigma 150 -> radius 600); bg_radius 0 = no background
  *   chmix_host : HOST, 3x3 doubles: the same kernel folded onto the reflected length-3 channel axis
@@ -298,14 +298,11 @@ int isb_lm_texture_accumulate(const void* img, int dtype, const int32_t* seg, in
 int isb_lm_texture_finish(int nb, int n_batt, int flags, const double* acc, const int32_t* counts, double* feat, int ld, int col0,
                           isb_stream_t stream);
 
-/* known-answer test of the tensor-core plumbing (tests/test_gpu_umma.py): D[128, N] = A[128, K] * B[N, K]^T with tcgen05.mma
- * kind::tf32 in one CTA; A, B row-major f32 holding tf32-representable values, N % 16 == 0 (<= 256), K % 8 == 0 (<= 64).
- * variant 0 = the descriptor convention the library uses; 1 = leading/stride byte offsets swapped (diagnostic only);
- * 2 = A written into tensor memory with tcgen05.st and read from there by the instruction (the form the contraction uses). */
-int isb_umma_selftest(const float* A, const float* B, int N, int K, int variant, float* D, isb_stream_t stream);
-/* profiling aid: clocks that `reps` back-to-back tcgen05.mma kind::tf32 instructions (M 128, K 8, the given N) take on each of `ctas`
- * CTAs; mode bit 0 = rotate over several accumulators, bit 1 = A operand from tensor memory.  cycles: device, [ctas] int64 */
-int isb_umma_rate(int N, int reps, int mode, int ctas, long long* cycles, isb_stream_t stream);
+/* known-answer test of the tensor-core plumbing (tests/test_gpu_umma.py): D[128, N] = A[128, K] * B[N, K]^T with wgmma.mma_async
+ * (TF32 inputs, FP32 accumulators) in one CTA of two warpgroups; A, B row-major f32 holding tf32-representable values,
+ * N in {16, 48, 80, 240, 256}, K % 8 == 0 (<= 64).  variant 0 = A and B from K-major unswizzled shared memory, 1 = the same with the
+ * descriptor's LBO / SBO fields swapped (diagnostic), 2 = A from registers (the form the contraction uses). */
+int isb_wgmma_selftest(const float* A, const float* B, int N, int K, int variant, float* D, isb_stream_t stream);
 /* profiling aid: clocks per dependent FP64 add / multiply / fma (one warp, chains of n operations); out: device, 4 doubles */
 int isb_fp64_latency(int n, double* out, isb_stream_t stream);
 

@@ -24,7 +24,7 @@ _LIB = None
 
 
 def build(force=False):
-    """compile oracle/liboracle.so (and oracle/_ref when /root/reference exists) with the committed Makefile"""
+    """compile oracle/liboracle.so (and oracle/_ref when $IMSEGM_REFERENCE names a checkout of the reference) with the committed Makefile"""
     so = os.path.join(_HERE, 'liboracle.so')
     srcs = [os.path.join(_HERE, f) for f in ('slic_oracle.c', 'slic3d_oracle.c', 'stats_oracle.c', 'gc_oracle.cpp')]
     stale = (not os.path.isfile(so)) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
@@ -32,8 +32,9 @@ def build(force=False):
         subprocess.check_call(['make', '-C', _HERE, 'liboracle.so'], stdout=subprocess.DEVNULL)
     ref_dir = os.path.join(_HERE, '_ref')
     has_ref = os.path.isdir(ref_dir) and any(f.startswith('features_cython') for f in os.listdir(ref_dir))
-    if os.path.isdir('/root/reference') and (force or not has_ref):
-        subprocess.call(['make', '-C', _HERE, 'ref'], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+    ref_tree = os.environ.get('IMSEGM_REFERENCE')
+    if ref_tree and os.path.isdir(ref_tree) and (force or not has_ref):
+        subprocess.call(['make', '-C', _HERE, 'ref', 'REF=' + os.path.abspath(ref_tree)], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
 
 
 def lib():

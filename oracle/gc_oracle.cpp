@@ -5,7 +5,7 @@
  *     imsegm/graph_cuts.py:735-744   gco.cut_general_graph(edges, edge_weights, unary_cost, pairwise_cost,
  *                                                          algorithm='expansion', n_iter=-1)
  *     imsegm/region_growing.py:148,1698,1715   (same call with n_iter=999)
- * The arithmetic lives in a third-party dependency that is NOT vendored in /root/reference and not installed
+ * The arithmetic lives in a third-party dependency that is NOT vendored in the reference and not installed
  * here: gco-wrapper >= 3.0.8 (requirements.txt:14; Borda/pyGCO wrapping GCO v3.0, Veksler & Delong).
  * Restated from its published behaviour:
  *   - (Python side, restated in oracle/energies.py) float energies are integerised: unary and edge weights are

@@ -3,7 +3,7 @@
  *
  * CPU restatement of skimage.segmentation.slic for a single-channel VOLUME, as imsegm/superpixels.py:104-106 calls it
  *     slic(np.array(im), n_segments, compactness, multichannel=False, spacing=space, sigma=1)
- * (scikit-image 0.14-0.18, absent from /root/reference -- requirements.txt:9 -- PARITY UNPINNED, like the 2-D restatement in
+ * (scikit-image 0.14-0.18, absent from the reference -- requirements.txt:9 -- PARITY UNPINNED, like the 2-D restatement in
  * slic_oracle.c whose arithmetic this file repeats with a depth axis):
  *   1. gaussian pre-blur, sigma / spacing per axis, scipy semantics (symmetric 1-D correlate, mode reflect), axes z, y, x
  *   2. k-means of _slic_cython: window +-2*step per axis about each centre, distance

@@ -5,7 +5,7 @@
  * SLIC superpixel algorithm the reference calls at
  *     imsegm/superpixels.py:61-63   ski_segm.slic(img, n_segments, compactness, sigma=1,
  *                                                 enforce_connectivity=True, slic_zero=slico)
- * The arithmetic lives in a third-party dependency that is NOT vendored in /root/reference and not
+ * The arithmetic lives in a third-party dependency that is NOT vendored in the reference and not
  * installed in this image: scikit-image (requirements.txt:9 "scikit-image >= 0.14.0"; effective < 0.19
  * because superpixels.py:105 passes `multichannel=`).  This file restates the published algorithm of
  * skimage.segmentation.slic / _slic_cython / _enforce_label_connectivity_cython for 2-D multichannel

@@ -77,8 +77,7 @@ SIGNATURES = {
     'isb_lm_texture_accumulate': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _i, C.POINTER(_d), _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     'isb_lm_texture_finish': (_i, [_i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     'isb_lm_texture': (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _i, C.POINTER(_d), _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _sz, _vp]),
-    'isb_umma_selftest': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
-    'isb_umma_rate': (_i, [_i, _i, _i, _i, _vp, _vp]),
+    'isb_wgmma_selftest': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     'isb_fp64_latency': (_i, [_i, _vp, _vp]),
     'isb_fill_i32': (_i, [_vp, _ll, _i, _vp]),
     'isb_combine': (_i, [_vp, _vp, _ll, _i, _vp]),
@@ -131,7 +130,7 @@ def check(status):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise NativeLibraryError('pyimsegm_b200 needs a CUDA device (B200 / sm_100a); there is no CPU fallback')
+        raise NativeLibraryError('pyimsegm_b200 needs a CUDA device (H100 / sm_90a); there is no CPU fallback')
     return torch
 
 

@@ -1,5 +1,5 @@
 """
-Build the CUDA extension ``libimsegm_b200.so`` in-tree with nvcc for sm_100a.
+Build the CUDA extension ``libimsegm_b200.so`` in-tree with nvcc for sm_90a (H100).
 
 The library exports the C-ABI of ``include/imsegm_b200.h``; Python binds it with ctypes (``_lib.py``).
 ``python -m pyimsegm_b200.build`` or ``__graft_entry__.build()``.
@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libimsegm_b200.so')
 
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 # -fmad=false: the SLIC sources must reproduce the oracle's IEEE double arithmetic bit for bit
 FLAGS = ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC', '-fmad=false']
 

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the imsegm_b200 CUDA sources (sm_100a only).
+// common.cuh -- shared helpers for the imsegm_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1243,7 +1243,7 @@ extern "C" int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, con
         ISB_LAUNCH_CHECK();
     }
     int blocks = (N + 255) / 256;
-    if (blocks > 148) blocks = 148;
+    if (blocks > 132) blocks = 132;
     k_gmm_predict<<<blocks, 256, 0, st>>>(N, n_dev, D, K, n_init, w, proba, params_out);
     ISB_LAUNCH_CHECK();
     return ISB_OK;

@@ -10,16 +10,16 @@
 //     (a thread owns a column and 16 consecutive output rows, the 1201 weights slide through registers), the other axis
 //     reuses it on a transposed copy; the channel axis (length 3, reflected 1201-tap kernel) folds into a 3x3 mix.
 // (2) contraction: implicit GEMM  response[pixel, filter] = sum_taps patch[pixel, tap] * K[tap, filter]  on the TENSOR
-//     cores: tcgen05.mma kind::tf32 with the 3xTF32 split (a_hi b_hi + a_hi b_lo + a_lo b_hi, FP32 accumulate in tensor memory),
-//     which keeps the result at f32 accuracy -- the reference rounds every response to f32 before its statistics
-//     (descriptors.py:233).  Source rows and the pre-split weights arrive by TMA; the patch matrices live in tensor memory.
+//     cores: wgmma.mma_async with TF32 inputs and the 3xTF32 split (a_hi b_hi + a_hi b_lo + a_lo b_hi, FP32 accumulate in
+//     registers), which keeps the result at f32 accuracy -- the reference rounds every response to f32 before its statistics
+//     (descriptors.py:233).  Source rows and the pre-split weights arrive by TMA; the patch matrices are gathered into registers.
 //     FLOPs: 3 channels x 76 kernels x 33^2 x 2 = 496 584 per pixel (x3 for the split).
 // (3) epilogue, fused: max over the orientations of a battery (quad shuffles), clip, then sum r and sum r^2 per
 //     (superpixel, battery, channel) and globally per battery -- the responses are never written to memory.  The
 //     log-norm scale is applied to the sums afterwards (mean and std scale with a, energy with a^2).
 // Tolerance against the float64 oracle: 2e-4 relative on the features (stated in tests/test_gpu_texture.py).
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -156,22 +156,23 @@ __global__ void __launch_bounds__(256) k_lm_mix_sub(const double* __restrict__ i
 
 // ---------------------------------------------------------------- (2)+(3) contraction + statistics ---------------------------------
 //
-// Implicit GEMM on the 5th-generation tensor cores: tcgen05.mma kind::tf32, accumulators AND the A operand in tensor memory.
-//   M = 128 consecutive pixels of one image row, N = the padded filter count (80 full bank / 48 short bank),
+// Implicit GEMM on the Hopper tensor cores: wgmma.mma_async kind tf32, FP32 accumulators in registers.
+//   M = 128 consecutive pixels of one image row (two warpgroups of 64), N = the padded filter count (80 full bank / 48 short bank),
 //   K = the 33 taps of one kernel row padded to 40 (5 instructions of K = 8), one such product per (output row, kernel row).
 // A CTA (persistent, one per SM) owns tiles of TR = 3 output rows x 128 pixels of one channel.  For every SOURCE row s of the
-// tile (3 + 32 of them) the patch matrix A_s[m][k] = row_s[x0 + m + k] is formed ONCE and used for every output row r with kernel
-// row dy = s - r:  acc[r] += A_s * B_dy^T.
+// tile (3 + 32 of them) the patch matrix A_s[m][k] = row_s[x0 + m + k] is used for every output row r with kernel row
+// dy = s - r:  acc[r] += A_s * B_dy^T.  A_s is a Toeplitz matrix, so it is never formed: every thread gathers its register
+// fragments of A_s straight from the staged source row (four consecutive-ish floats per instruction, no bank conflicts).
 // 3xTF32: image and weights are pre-split into a tf32 value and a tf32 remainder; acc += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi
 // (FP32 accumulate) keeps f32 accuracy -- the reference rounds every response to f32 before its statistics (descriptors.py:233).
-// Warp roles (448 threads):
-//   warp 0     TMA: the split weights of kernel row dy (cp.async.bulk, one piece per lane) into the weight ring, the source rows
-//              (2-D tensor-map loads of the reflect-padded hi / lo planes) into a 4-slot ring
-//   warp 1     allocates tensor memory; one lane issues every tcgen05.mma and the commits that free the rings
-//   warps 2-9  patch-matrix producers: raw row -> A_s (hi, lo) in tensor memory (tcgen05.st), a lane quarter per warp
-//   warps 10-13 epilogue: tcgen05.ld the 3 x N accumulators of a pixel, max over the orientations of a battery, clip, then
-//              run-length sums of r and r^2 along the row per (battery, output row) -> atomics on the per-superpixel sums.
-// The responses are never written to memory.
+// Warp roles (288 threads):
+//   warps 0-7  two consumer warpgroups: A fragments from the staged row, 3 x 5 x 3 wgmma per source row, then the epilogue:
+//              max over the orientations of a battery (quad shuffles), clip, run-length sums of r and r^2 along the row per
+//              (battery, output row) -> atomics on the per-superpixel sums.  The responses are never written to memory.
+//   warp 8     TMA producer: the split weights of kernel row dy (one cp.async.bulk per slice) into a ring of NBT slices, the
+//              source rows (2-D tensor-map loads of the reflect-padded hi / lo planes) into a ring of NRAW slots
+// A weight slice is loaded once per tile and serves the three output rows; the accumulators of a tile (3 x NPAD / 2 floats per
+// thread) stay in registers until its epilogue.
 
 constexpr int KW = 33;                    // kernel edge
 constexpr int KRAD = 16;
@@ -183,8 +184,8 @@ constexpr int SROWS = TR + KW - 1;        // source rows per tile
 constexpr int RAWW = TM + KPAD;           // floats of one staged source row
 constexpr int RAW_PITCH = 768;            // bytes between the hi and the lo row of a raw slot (TMA destinations 128-byte aligned)
 constexpr int NRAW = 4;                   // ring depth of the staged source rows
-constexpr int LM_PROD = 256;                // patch-matrix producer threads: two per pixel of the M tile (value / remainder)
-constexpr int LM_THREADS = 64 + LM_PROD + 128;
+constexpr int LM_CONS = 256;              // consumer threads: two warpgroups
+constexpr int LM_THREADS = LM_CONS + 32;     // + the producer warp
 
 struct LmTcArgs {
     const float* w_tc;   // [KW][hi|lo][KC][NPAD/8][8][4]: the weights of every kernel row in operand layout
@@ -209,273 +210,217 @@ template <int NPAD> __host__ __device__ constexpr int lm_batt_of_col(int col)
     return (col - Bk::GS * Bk::NG) < Bk::NS ? 5 * ((col - Bk::GS * Bk::NG) / 3) + 2 + (col - Bk::GS * Bk::NG) % 3 : -1;
 }
 
-// How the instruction stream is cut, and why.  Measured on B200 (scripts/dev_umma_rate.py, profiles/r02_lm_tcgen05.md): a tcgen05.mma
-// kind::tf32 of M 128 x K 8 costs  max(~104, N/2 + 43) clocks with A in shared memory,  max(~104, N/2 + 10) with A in tensor memory:
-// a floor of ~104 clocks per instruction whatever N is, and 4 KB of A per instruction is more than shared memory can feed beside B.
-// The first tcgen05 version of this kernel (one N = 80 instruction per output row, both operands in shared memory, 1485 instructions
-// per tile) ran 12.4 ms per 2048 x 2048 image with the tensor pipe 57 % busy.  This one
-//   * keeps the patch matrices A_s (value and remainder, 2 x 40 columns, lane = pixel) in TENSOR MEMORY: the producers write them
-//     with tcgen05.st, the instruction reads only the weights from shared memory;
-//   * runs the three output rows of a tile as ONE instruction of N = 3 x NPAD: A_s is the same for them, their accumulators are
-//     adjacent tensor-memory columns, and the three weight slices (kernel rows s-2, s-1, s) are adjacent in shared memory because the
-//     weight ring is laid out per 16-byte k-chunk ([half][k-chunk][slot][NPAD/8 groups][8 x 16 B]; the first two slots are mirrored
-//     behind the last so that a window of three never wraps).  525 instructions per tile instead of 1485, 130 clocks each at N = 240.
-// Tensor-memory budget (512 columns): the accumulators of one tile (3 x 80 = 240; the short bank has room for two tiles) + a ring of
-// patch-matrix stages of 80 columns.
+// Shared memory: a ring of NBT weight slices, each [hi|lo][KC k-chunks][NPAD/8 filter groups][8 x 16 B] exactly as w_tc holds a kernel
+// row (descriptor LBO = one k-chunk, SBO = 128 B), the source-row ring, the battery maxima of a tile and its labels.
 template <int NPAD> struct LmTs {
     using Bk = LmBank<NPAD>;
-    static constexpr int NACC = (2 * TR * NPAD + 2 * 2 * KPAD <= 512) ? 2 : 1;       // accumulator buffers
-    static constexpr int A_COL0 = (NACC * TR * NPAD + 31) / 32 * 32;                 // first patch-matrix column
-    static constexpr int NAT = (512 - A_COL0) / (2 * KPAD) > 3 ? 3 : (512 - A_COL0) / (2 * KPAD);   // patch-matrix stages
-    static constexpr int NBT = NPAD == 80 ? 5 : 8;                                   // weight slices in flight (logical ring)
-    static constexpr int PHYS = NBT + TR - 1;                                        // physical slots: the first TR-1 are mirrored at the end
-    static constexpr int SLOTC = (NPAD / 8) * 128;                                   // bytes of one (slice, half, k-chunk): NPAD filters x 4 taps
-    static constexpr int B_LBO = PHYS * SLOTC;                                       // bytes between the two k-chunks of an instruction
-    static constexpr int B_HALF = KC * B_LBO;                                        // bytes of the value (or remainder) ring
+    static constexpr int NBT = NPAD == 80 ? 5 : 8;                                   // weight slices in flight
+    static constexpr int SLOTC = (NPAD / 8) * 128;                                   // bytes of one (half, k-chunk): NPAD filters x 4 taps
     static constexpr int B_SLICE = 2 * KC * SLOTC;                                   // bytes of one weight slice (value + remainder)
     static constexpr int TS = Bk::NBATT + 1;
     static constexpr int OFF_B = 0;
-    static constexpr int OFF_RAW = OFF_B + 2 * B_HALF;
+    static constexpr int OFF_RAW = OFF_B + NBT * B_SLICE;
     static constexpr int OFF_T = OFF_RAW + NRAW * 2 * RAW_PITCH;
     static constexpr int OFF_LAB = OFF_T + TR * TM * TS * 4;
     static constexpr int OFF_BAR = OFF_LAB + TR * TM * 4;
-    static constexpr int N_BAR = 2 * NRAW + 2 * NAT + 2 * NBT + NACC + NACC * TR;
-    static constexpr int OFF_TMEM = OFF_BAR + N_BAR * 8;
-    static constexpr int BYTES = OFF_TMEM + 16;
-    static_assert(NAT >= 2, "tensor memory budget: at least two patch-matrix stages");
-    static_assert(A_COL0 + NAT * 2 * KPAD <= 512, "tensor memory budget");
-    static_assert(NBT >= TR + 1, "the weight ring must hold a window of TR slices and one in flight");
-    static_assert(TR * NPAD <= 256, "one instruction spans the accumulators of all output rows");
+    static constexpr int N_BAR = 2 * NRAW + 2 * NBT;
+    static constexpr int BYTES = OFF_BAR + N_BAR * 8;
+    static_assert(NBT >= TR + 1, "the weight ring must hold the TR slices in use and one in flight");
+    static_assert(OFF_RAW % 128 == 0, "TMA destinations are 128-byte aligned");
+    static_assert((Bk::GS * Bk::NG) % 8 == 0 && 8 % Bk::GS == 0, "an 8-column accumulator group holds whole oriented batteries");
     static_assert(BYTES <= 227 * 1024, "shared memory budget");
 };
 
-template <int NPAD>
-__global__ void __launch_bounds__(LM_THREADS, 1) k_lm_conv_ts(const __grid_constant__ CUtensorMap tmap, LmTcArgs a)
+// acc[r] += A_s * B_{s-r}^T for the output rows r = R_LO..R_HI, 3xTF32 (small terms first); slice dy of the tile is ring slot
+// (jb_base + dy) % NBT, j0 = jb_base + s
+template <int NPAD, int R_LO, int R_HI>
+__device__ __forceinline__ void lm_issue(float (&acc)[TR][NPAD / 2], const uint32_t (&ah)[KPAD / 8][4], const uint32_t (&al)[KPAD / 8][4],
+                                         uint32_t b_ring, uint32_t j0)
 {
-    using namespace umma;
+    using namespace wgmma;
+    using Sm = LmTs<NPAD>;
+    wg_fence();
+#pragma unroll
+    for (int r = R_LO; r <= R_HI; ++r) {
+        const uint32_t b_hi = b_ring + ((j0 - r) % Sm::NBT) * Sm::B_SLICE, b_lo = b_hi + KC * Sm::SLOTC;
+#pragma unroll
+        for (int kk = 0; kk < KPAD / 8; ++kk) {
+            const uint64_t bh = smem_desc(b_hi + kk * 2 * Sm::SLOTC, Sm::SLOTC, 128);
+            const uint64_t bl = smem_desc(b_lo + kk * 2 * Sm::SLOTC, Sm::SLOTC, 128);
+            mma_tf32_rs(acc[r], al[kk], bh, 1);
+            mma_tf32_rs(acc[r], ah[kk], bl, 1);
+            mma_tf32_rs(acc[r], ah[kk], bh, 1);
+        }
+    }
+    wg_commit();
+    wg_wait<0>();
+}
+
+template <int NPAD>
+__global__ void __launch_bounds__(LM_THREADS, 1) k_lm_conv_wg(const __grid_constant__ CUtensorMap tmap, LmTcArgs a)
+{
+    using namespace wgmma;
     using Sm = LmTs<NPAD>;
     using Bk = LmBank<NPAD>;
-    constexpr int NAT = Sm::NAT, NBT = Sm::NBT, NACC = Sm::NACC;
+    constexpr int NBT = Sm::NBT;
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
     const uint32_t bar0 = sbase + Sm::OFF_BAR;
     auto raw_full = [&](uint32_t i) { return bar0 + 8u * i; };
     auto raw_empty = [&](uint32_t i) { return bar0 + 8u * (NRAW + i); };
-    auto a_full = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + i); };
-    auto a_empty = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + NAT + i); };
-    auto b_full = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + 2 * NAT + i); };
-    auto b_empty = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + 2 * NAT + NBT + i); };
-    auto acc_full = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + 2 * NAT + 2 * NBT + i); };
-    auto acc_empty = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + 2 * NAT + 2 * NBT + NACC + i); };   // one per (buffer, output row)
-    uint32_t* tmem_slot = (uint32_t*)(smem + Sm::OFF_TMEM);
+    auto b_full = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + i); };
+    auto b_empty = [&](uint32_t i) { return bar0 + 8u * (2 * NRAW + NBT + i); };
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NRAW; ++i) { mbar_init(raw_full(i), 1); mbar_init(raw_empty(i), LM_PROD / 32); }
-        for (int i = 0; i < NAT; ++i) { mbar_init(a_full(i), LM_PROD / 32); mbar_init(a_empty(i), 1); }
-        for (int i = 0; i < NBT; ++i) { mbar_init(b_full(i), 1); mbar_init(b_empty(i), 1); }
-        for (int i = 0; i < NACC; ++i) mbar_init(acc_full(i), 1);
-        for (int i = 0; i < NACC * TR; ++i) mbar_init(acc_empty(i), TM);
+        for (int i = 0; i < NRAW; ++i) { mbar_init(raw_full(i), 1); mbar_init(raw_empty(i), LM_CONS / 32); }
+        for (int i = 0; i < NBT; ++i) { mbar_init(b_full(i), 1); mbar_init(b_empty(i), LM_CONS / 32); }
         fence_mbar_init();
         prefetch_tmap(&tmap);
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tbase = *tmem_slot;
 
     const int tiles_per_ch = a.tiles_x * a.tiles_y;
     const int n_tiles = 3 * tiles_per_ch;
 
-    if (warp == 0) {
+    if (warp == LM_CONS / 32) {
         // ------------------------------------------------------------ TMA producer ------------------------------------------------
-        // the whole warp: lane c < 2 KC copies piece c of a weight slice (every lane issues its own cp.async.bulk in one warp
-        // instruction -- one thread issuing all twenty was the busiest thread of the CTA), two more lanes load the source row
-        uint32_t jr = 0, jb = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-            const int ch = t / tiles_per_ch, rem = t - ch * tiles_per_ch;
-            const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
-            const int x0 = tx * TM, y0 = a.y_first + ty * TR;
-            for (int s = 0; s < SROWS; ++s) {
-                if (s < KW) {
-                    // kernel row s: 2 x KC pieces of NPAD filters x 4 taps, each to its k-chunk's ring (and to the mirror slot)
-                    const uint32_t slot = jb % NBT, ph = (jb / NBT) & 1;
-                    const bool mirror = slot < TR - 1;
-                    mbar_wait(b_empty(slot), ph ^ 1);
-                    if (lane == 0) mbar_arrive_expect_tx(b_full(slot), (mirror ? 2 : 1) * Sm::B_SLICE);
-                    __syncwarp();
-                    if (lane < 2 * KC) {
-                        const float* src = a.w_tc + (size_t)s * (Sm::B_SLICE / 4) + (size_t)lane * (Sm::SLOTC / 4);
-                        const uint32_t dst = sbase + Sm::OFF_B + (uint32_t)lane * Sm::B_LBO + slot * Sm::SLOTC;
-                        bulk_g2s(dst, src, Sm::SLOTC, b_full(slot));
-                        if (mirror) bulk_g2s(dst + NBT * Sm::SLOTC, src, Sm::SLOTC, b_full(slot));
-                    }
-                    ++jb;
-                }
-                const uint32_t slot = jr % NRAW, ph = (jr / NRAW) & 1;
-                mbar_wait(raw_empty(slot), ph ^ 1);
-                if (lane == 0) mbar_arrive_expect_tx(raw_full(slot), 2 * RAWW * 4);
-                __syncwarp();
-                if (lane < 2) {
-                    const uint32_t dst = sbase + Sm::OFF_RAW + slot * 2 * RAW_PITCH + lane * RAW_PITCH;
-                    tma_load_2d(dst, &tmap, x0, (3 * lane + ch) * a.Hp + y0 + s, raw_full(slot));
-                }
-                ++jr;
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer --------------------------------------------------
         if (lane == 0) {
-            uint32_t jr = 0, jb_base = 0, it = 0;
-            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-                const uint32_t buf = it % NACC;
-                const uint32_t acc0 = tbase + buf * (TR * NPAD);
+            uint32_t jr = 0, jb = 0;
+            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+                const int ch = t / tiles_per_ch, rem = t - ch * tiles_per_ch;
+                const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
+                const int x0 = tx * TM, y0 = a.y_first + ty * TR;
                 for (int s = 0; s < SROWS; ++s) {
-                    const uint32_t st = jr % NAT;
-                    if (s < KW) { const uint32_t jb = jb_base + s; mbar_wait(b_full(jb % NBT), (jb / NBT) & 1); }
-                    mbar_wait(a_full(st), (jr / NAT) & 1);
-                    // source row s < TR is the first to touch the accumulator of output row s: the epilogue hands the rows of the
-                    // previous tile back one by one, so the first instructions of this tile overlap its reading of the later rows
-                    if (s < TR) mbar_wait(acc_empty(buf * TR + s), ((it / NACC) & 1) ^ 1);
-                    tc_fence_after();
-                    const uint32_t a_hi = tbase + Sm::A_COL0 + st * (2 * KPAD), a_lo = a_hi + KPAD;
-                    // output rows r_lo..r_hi take this source row with kernel rows dy = s - r; ascending dy = ascending slot = descending r,
-                    // and the accumulator of row r sits at column (TR-1-r) NPAD, so one instruction of N = nr NPAD covers them all
-                    const int r_hi = s < TR ? s : TR - 1, r_lo = s >= KW ? s - (KW - 1) : 0;
-                    const int nr = r_hi - r_lo + 1;
-                    const uint32_t b0 = sbase + Sm::OFF_B + ((jb_base + s - r_hi) % NBT) * Sm::SLOTC;    // slice dy = s - r_hi, value ring
-                    const uint32_t d0 = acc0 + (TR - 1 - r_hi) * NPAD;
-                    const uint32_t idesc = instr_desc(FMT_TF32, TM, nr * NPAD);
-                    // row r_hi = s < TR meets its accumulator for the first time (dy = 0): its very first instruction overwrites, alone
-                    const bool fresh = s < TR;
-#pragma unroll
-                    for (int kk = 0; kk < KPAD / 8; ++kk) {
-                        const uint64_t bh = smem_desc(b0 + kk * 2 * Sm::B_LBO, Sm::B_LBO, 128);
-                        const uint64_t bl = smem_desc(b0 + Sm::B_HALF + kk * 2 * Sm::B_LBO, Sm::B_LBO, 128);
-                        if (kk == 0 && fresh) {
-                            mma_tf32_ts(d0, a_lo, bh, instr_desc(FMT_TF32, TM, NPAD), 0u);
-                            if (nr > 1)
-                                mma_tf32_ts(d0 + NPAD, a_lo, smem_desc(b0 + Sm::SLOTC, Sm::B_LBO, 128), instr_desc(FMT_TF32, TM, (nr - 1) * NPAD), 1u);
-                        } else {
-                            mma_tf32_ts(d0, a_lo + kk * 8, bh, idesc, 1u);                    // small terms first
-                        }
-                        mma_tf32_ts(d0, a_hi + kk * 8, bl, idesc, 1u);
-                        mma_tf32_ts(d0, a_hi + kk * 8, bh, idesc, 1u);
+                    if (s < KW) {
+                        // kernel row s: value and remainder in one piece
+                        const uint32_t slot = jb % NBT;
+                        mbar_wait(b_empty(slot), ((jb / NBT) & 1) ^ 1);
+                        mbar_arrive_expect_tx(b_full(slot), Sm::B_SLICE);
+                        bulk_g2s(sbase + Sm::OFF_B + slot * Sm::B_SLICE, a.w_tc + (size_t)s * (Sm::B_SLICE / 4), Sm::B_SLICE, b_full(slot));
+                        ++jb;
                     }
-                    tc_commit(a_empty(st));                                              // the patch matrices of row s are free again
-                    if (s >= TR - 1) tc_commit(b_empty((jb_base + s - (TR - 1)) % NBT)); // kernel row s - (TR-1) had its last use
+                    const uint32_t slot = jr % NRAW;
+                    mbar_wait(raw_empty(slot), ((jr / NRAW) & 1) ^ 1);
+                    mbar_arrive_expect_tx(raw_full(slot), 2 * RAWW * 4);
+                    const uint32_t dst = sbase + Sm::OFF_RAW + slot * 2 * RAW_PITCH;
+                    tma_load_2d(dst, &tmap, x0, ch * a.Hp + y0 + s, raw_full(slot));
+                    tma_load_2d(dst + RAW_PITCH, &tmap, x0, (3 + ch) * a.Hp + y0 + s, raw_full(slot));
                     ++jr;
                 }
-                tc_commit(acc_full(buf));
-                jb_base += KW;
             }
         }
-    } else if (warp < 2 + LM_PROD / 32) {
-        // ------------------------------------------------------------ patch-matrix producers ---------------------------------------
-        // a warp may touch the tensor-memory lanes 32 (warp % 4) .. +31: pixel m = that lane; of the two warps that share a lane quarter
-        // one writes the tf32 values, the other the remainders
-        const int q = warp & 3, m = 32 * q + lane, part = (warp - 2) >> 2;
-        uint32_t jr = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-            for (int s = 0; s < SROWS; ++s, ++jr) {
-                const uint32_t rs = jr % NRAW, st = jr % NAT;
-                mbar_wait(raw_full(rs), (jr / NRAW) & 1);
-                mbar_wait(a_empty(st), ((jr / NAT) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t* src = (const uint32_t*)(smem + Sm::OFF_RAW + rs * 2 * RAW_PITCH + part * RAW_PITCH) + m;
-                const uint32_t dst = tbase + ((uint32_t)(32 * q) << 16) + Sm::A_COL0 + st * (2 * KPAD) + part * KPAD;
-#pragma unroll
-                for (int kk = 0; kk < KPAD / 8; ++kk) {
-                    uint32_t r[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) r[j] = src[8 * kk + j];
-                    tmem_st8(dst + 8 * kk, r);
-                }
-                tmem_wait_st();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) { mbar_arrive(a_full(st)); mbar_arrive(raw_empty(rs)); }
-            }
-        }
-    } else {
-        // ------------------------------------------------------------ epilogue ------------------------------------------------------
-        const int e = threadIdx.x - (64 + LM_PROD);   // 0..127
-        const int q = warp & 3;                   // tensor-memory lane quarter this warp may read
-        const int m = 32 * q + lane;
-        float* T = (float*)(smem + Sm::OFF_T);
-        int* s_lab = (int*)(smem + Sm::OFF_LAB);
-        const bool walker = e < 2 * TR * Bk::NBATT;
-        const int p = e >> 1, half = e & 1;
-        const int wr = p / Bk::NBATT, wb = p - wr * Bk::NBATT;
-        double g2 = 0.0;
-        uint32_t it = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-            const int ch = t / tiles_per_ch, rem = t - ch * tiles_per_ch;
-            const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
-            const int x0 = tx * TM, y0 = a.y_first + ty * TR;
-            const uint32_t buf = it % NACC;
-#pragma unroll
-            for (int r = 0; r < TR; ++r) {
-                const int y = y0 + r, x = x0 + m;
-                s_lab[r * TM + m] = (y < a.y_end && x < a.W) ? a.seg[(size_t)y * a.W + x] : -1;
-            }
-            mbar_wait(acc_full(buf), (it / NACC) & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int r = 0; r < TR; ++r) {
-                float bat[Bk::NBATT];
-#pragma unroll
-                for (int b = 0; b < Bk::NBATT; ++b) bat[b] = -INFINITY;
-#pragma unroll
-                for (int c = 0; c < NPAD / 16; ++c) {
-                    if (16 * c >= Bk::GS * Bk::NG + Bk::NS) continue;       // padding columns only
-                    float v[16];
-                    tmem_ld16(tbase + ((uint32_t)(32 * q) << 16) + buf * (TR * NPAD) + (TR - 1 - r) * NPAD + 16 * c, v);
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int b = lm_batt_of_col<NPAD>(16 * c + j);
-                        if (b >= 0) bat[b] = fmaxf(bat[b], v[j]);
-                    }
-                }
-#pragma unroll
-                for (int b = 0; b < Bk::NBATT; ++b) T[(r * TM + m) * Sm::TS + b] = fminf(bat[b], 1.e6f);   // MAX_SIGNAL_RESPONSE
-                tc_fence_before();
-                mbar_arrive(acc_empty(buf * TR + r));                       // this row's accumulator is in shared memory: the next tile may use it
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (walker) {
-                // one (output row, battery) pair and half a row per thread: run-length sums along x, flushed when the label changes
-                const size_t fstride = (size_t)a.n_batt * 3;
-                double s1 = 0.0, s2 = 0.0;
-                int cur = -1;
-                const int* lab = s_lab + wr * TM + half * (TM / 2);
-                const float* tv = T + (size_t)(wr * TM + half * (TM / 2)) * Sm::TS + wb;
-                for (int i = 0; i < TM / 2; ++i) {
-                    const int lb = lab[i];
-                    if (lb != cur) {
-                        if (cur >= 0) {
-                            atomicAdd(&a.S1[(size_t)cur * fstride + wb * 3 + ch], s1);
-                            atomicAdd(&a.S2[(size_t)cur * fstride + wb * 3 + ch], s2);
-                            g2 += s2;
-                        }
-                        cur = lb; s1 = 0.0; s2 = 0.0;
-                    }
-                    if (lb >= 0) { const double v = (double)tv[(size_t)i * Sm::TS]; s1 += v; s2 += v * v; }
-                }
-                if (cur >= 0) {
-                    atomicAdd(&a.S1[(size_t)cur * fstride + wb * 3 + ch], s1);
-                    atomicAdd(&a.S2[(size_t)cur * fstride + wb * 3 + ch], s2);
-                    g2 += s2;
-                }
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-        if (walker && g2 != 0.0) atomicAdd(&a.G2[wb], g2);
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tbase, 512);
+
+    // ---------------------------------------------------------------- consumers --------------------------------------------------
+    const int e = threadIdx.x;                         // 0..255
+    const int tq = lane & 3;
+    const int m0 = 16 * warp + (lane >> 2);            // pixel of accumulator rows i % 4 < 2; m0 + 8 for the others (warp 4.. = rows 64..)
+    float* T = (float*)(smem + Sm::OFF_T);
+    int* s_lab = (int*)(smem + Sm::OFF_LAB);
+    const bool walker = e < 2 * TR * Bk::NBATT;
+    const int p = e >> 1, half = e & 1;
+    const int wr = p / Bk::NBATT, wb = p - wr * Bk::NBATT;
+    double g2 = 0.0;
+    uint32_t jr = 0, jb_base = 0;
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, jb_base += KW) {
+        const int ch = t / tiles_per_ch, rem = t - ch * tiles_per_ch;
+        const int ty = rem / a.tiles_x, tx = rem - ty * a.tiles_x;
+        const int x0 = tx * TM, y0 = a.y_first + ty * TR;
+        float acc[TR][NPAD / 2];
+#pragma unroll
+        for (int r = 0; r < TR; ++r)
+#pragma unroll
+            for (int i = 0; i < NPAD / 2; ++i) acc[r][i] = 0.f;
+        for (int s = 0; s < SROWS; ++s, ++jr) {
+            if (s < KW) { const uint32_t jb = jb_base + s; mbar_wait(b_full(jb % NBT), (jb / NBT) & 1); }
+            const uint32_t rs = jr % NRAW;
+            mbar_wait(raw_full(rs), (jr / NRAW) & 1);
+            // A fragments: rows m0 / m0 + 8, taps tq / tq + 4 of every K = 8 step -> row_s[m + k]
+            const float* hi = (const float*)(smem + Sm::OFF_RAW + rs * 2 * RAW_PITCH) + m0 + tq;
+            const float* lo = hi + RAW_PITCH / 4;
+            uint32_t ah[KPAD / 8][4], al[KPAD / 8][4];
+#pragma unroll
+            for (int kk = 0; kk < KPAD / 8; ++kk) {
+                ah[kk][0] = __float_as_uint(hi[8 * kk]); ah[kk][1] = __float_as_uint(hi[8 * kk + 8]);
+                ah[kk][2] = __float_as_uint(hi[8 * kk + 4]); ah[kk][3] = __float_as_uint(hi[8 * kk + 12]);
+                al[kk][0] = __float_as_uint(lo[8 * kk]); al[kk][1] = __float_as_uint(lo[8 * kk + 8]);
+                al[kk][2] = __float_as_uint(lo[8 * kk + 4]); al[kk][3] = __float_as_uint(lo[8 * kk + 12]);
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(raw_empty(rs));
+            // output rows R_LO..R_HI take this source row with kernel row dy = s - r; the range is a compile-time property of the
+            // call so that every wgmma of the warpgroup sits on one straight path
+            const uint32_t b0 = sbase + Sm::OFF_B;
+            const uint32_t j0 = jb_base + s;
+            if (s == 0) lm_issue<NPAD, 0, 0>(acc, ah, al, b0, j0);
+            else if (s < TR - 1) lm_issue<NPAD, 0, TR - 2>(acc, ah, al, b0, j0);
+            else if (s < KW) lm_issue<NPAD, 0, TR - 1>(acc, ah, al, b0, j0);
+            else if (s < SROWS - 1) lm_issue<NPAD, 1, TR - 1>(acc, ah, al, b0, j0);
+            else lm_issue<NPAD, TR - 1, TR - 1>(acc, ah, al, b0, j0);
+            if (s >= TR - 1) {                                 // kernel row s - (TR-1) had its last use
+                __syncwarp();
+                if (lane == 0) mbar_arrive(b_empty((jb_base + s - (TR - 1)) % NBT));
+            }
+        }
+        // ------------------------------------------------------------ epilogue ------------------------------------------------------
+        for (int i = e; i < TR * TM; i += LM_CONS) {
+            const int y = y0 + i / TM, x = x0 + i % TM;
+            s_lab[i] = (y < a.y_end && x < a.W) ? a.seg[(size_t)y * a.W + x] : -1;
+        }
+#pragma unroll
+        for (int r = 0; r < TR; ++r) {
+#pragma unroll
+            for (int j = 0; j < NPAD / 8; ++j) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float* row = T + (size_t)(r * TM + m0 + 8 * h) * Sm::TS;
+                    const float v0 = acc[r][4 * j + 2 * h], v1 = acc[r][4 * j + 2 * h + 1];
+                    const int c0 = 8 * j + 2 * tq;
+                    if (8 * j < Bk::GS * Bk::NG) {
+                        // an oriented battery spans GS adjacent columns = GS / 2 threads of the quad
+                        float v = fmaxf(v0, v1);
+                        v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+                        if (Bk::GS == 8) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+                        if (tq % (Bk::GS / 2) == 0) row[lm_batt_of_col<NPAD>(c0)] = fminf(v, 1.e6f);   // MAX_SIGNAL_RESPONSE
+                    } else {
+                        const int b0 = lm_batt_of_col<NPAD>(c0), b1 = lm_batt_of_col<NPAD>(c0 + 1);
+                        if (b0 >= 0) row[b0] = fminf(v0, 1.e6f);
+                        if (b1 >= 0) row[b1] = fminf(v1, 1.e6f);
+                    }
+                }
+            }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(LM_CONS) : "memory");
+        if (walker) {
+            // one (output row, battery) pair and half a row per thread: run-length sums along x, flushed when the label changes
+            const size_t fstride = (size_t)a.n_batt * 3;
+            double s1 = 0.0, s2 = 0.0;
+            int cur = -1;
+            const int* lab = s_lab + wr * TM + half * (TM / 2);
+            const float* tv = T + (size_t)(wr * TM + half * (TM / 2)) * Sm::TS + wb;
+            for (int i = 0; i < TM / 2; ++i) {
+                const int lb = lab[i];
+                if (lb != cur) {
+                    if (cur >= 0) {
+                        atomicAdd(&a.S1[(size_t)cur * fstride + wb * 3 + ch], s1);
+                        atomicAdd(&a.S2[(size_t)cur * fstride + wb * 3 + ch], s2);
+                        g2 += s2;
+                    }
+                    cur = lb; s1 = 0.0; s2 = 0.0;
+                }
+                if (lb >= 0) { const double v = (double)tv[(size_t)i * Sm::TS]; s1 += v; s2 += v * v; }
+            }
+            if (cur >= 0) {
+                atomicAdd(&a.S1[(size_t)cur * fstride + wb * 3 + ch], s1);
+                atomicAdd(&a.S2[(size_t)cur * fstride + wb * 3 + ch], s2);
+                g2 += s2;
+            }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(LM_CONS) : "memory");
+    }
+    if (walker && g2 != 0.0) atomicAdd(&a.G2[wb], g2);
 }
 
 // reflect-padded, tf32-split planes for the tensor-map loads: P[c][yp][xp] = split(img[c][reflect(yp - 16)][reflect(xp - 16)]);
@@ -574,8 +519,8 @@ static int launch_lm_conv(const CUtensorMap& tmap, const LmTcArgs& a, int n_tile
     ISB_CUDA_CHECK(cudaGetDevice(&dev));
     ISB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int grid = n_tiles < sms ? n_tiles : sms;   // persistent: one CTA per SM, tiles round-robin
-    ISB_CUDA_CHECK(cudaFuncSetAttribute(k_lm_conv_ts<NPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, LmTs<NPAD>::BYTES));
-    k_lm_conv_ts<NPAD><<<grid, LM_THREADS, LmTs<NPAD>::BYTES, st>>>(tmap, a);
+    ISB_CUDA_CHECK(cudaFuncSetAttribute(k_lm_conv_wg<NPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, LmTs<NPAD>::BYTES));
+    k_lm_conv_wg<NPAD><<<grid, LM_THREADS, LmTs<NPAD>::BYTES, st>>>(tmap, a);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }
@@ -607,7 +552,7 @@ static int lm_accumulate(const void* img, int dtype, const int32_t* seg, int H, 
     const LmDims d = lm_dims(H, W);
     k_lm_pad_split<<<dim3((d.Wp + 255) / 256, d.Hp, 3), 256, 0, st>>>(w.imgf, H, W, d.Hp, d.Wp, w.planes);
     ISB_LAUNCH_CHECK();
-    umma::EncodeTiledFn encode = umma::encode_tiled_fn();
+    wgmma::EncodeTiledFn encode = wgmma::encode_tiled_fn();
     if (!encode) { isb_set_error("cuTensorMapEncodeTiled is not available from this driver"); return ISB_ERR_UNSUPPORTED; }
     CUtensorMap tmap;
     {

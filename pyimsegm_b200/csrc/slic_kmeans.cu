@@ -18,7 +18,7 @@
 // Per sweep HBM traffic (algorithmic): read Lab 24 B/px + write label 4 B/px (assign); the update re-reads
 // labels and member colours through L2.
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include <float.h>
 #include <string.h>
 
@@ -191,10 +191,10 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
         // the three Lab planes of the tile arrive as ONE 3-D tensor-map load (32 x 32 x 3 doubles, out-of-image elements read as 0)
         // while every warp gathers the candidate clusters; the distance loop waits on the mbarrier
         if (threadIdx.x == 0) {
-            umma::mbar_init(umma::smem_u32(&s_bar), 1);
-            umma::fence_mbar_init();
-            umma::mbar_arrive_expect_tx(umma::smem_u32(&s_bar), 3 * TILE * TILE * 8);
-            umma::tma_load_3d(umma::smem_u32(&s_px[0][0][0]), &lab_map, tx0, ty0, 0, umma::smem_u32(&s_bar));
+            wgmma::mbar_init(wgmma::smem_u32(&s_bar), 1);
+            wgmma::fence_mbar_init();
+            wgmma::mbar_arrive_expect_tx(wgmma::smem_u32(&s_bar), 3 * TILE * TILE * 8);
+            wgmma::tma_load_3d(wgmma::smem_u32(&s_px[0][0][0]), &lab_map, tx0, ty0, 0, wgmma::smem_u32(&s_bar));
         }
     } else {
         double v[3][AROWS];
@@ -299,7 +299,7 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
             s_lb[rank] = r > 0.f ? (double)(r * r * 0.999f) * s.sw * 0.999 : 0.0;
         }
         __syncthreads();
-        if (use_tma) umma::mbar_wait(umma::smem_u32(&s_bar), 0);   // phase 0 completes once; later rounds pass immediately
+        if (use_tma) wgmma::mbar_wait(wgmma::smem_u32(&s_bar), 0);   // phase 0 completes once; later rounds pass immediately
         if (xin) {
             const double xd = (double)x;
             // this thread's pixels: column x, AROWS consecutive rows: the float form of the column and the centre of the run
@@ -406,9 +406,10 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
 // counted in xchg[6n]); the result goes to the exchange record xchg[6k..6k+5] = bits(cy, cx, c0, c1, c2), state (1 alive,
 // 2 died) and every other band leaves zeros there, so that an integer sum over the bands is an exact merge.
 // A warp's time is the length of its cluster's dependent chain, so the launch should be ONE wave: UWARPS warps per CTA and UBLOCKS CTAs
-// per SM give 148 x UWARPS x UBLOCKS resident warps -- with 2 x 17 that is 5 032, enough for the ~5 000 clusters of a 2048 x 2048 image at
-// sp_size 29 (8 x 4 = 4 736 left 5 % of the clusters for a second wave that cost as much as the first).
-constexpr int UWARPS = 2, UBLOCKS = 17;
+// per SM give 132 x UWARPS x UBLOCKS resident warps on an H100 -- with 2 x 19 that is 5 016, enough for the ~5 000 clusters of a
+// 2048 x 2048 image at sp_size 29 (a second wave for the last few percent costs as much as the first).  The 48 registers this allows
+// spill a few words.
+constexpr int UWARPS = 2, UBLOCKS = 19;
 template <bool BAND>
 __global__ void __launch_bounds__(32 * UWARPS, UBLOCKS) k_update(KmState s, const double* __restrict__ lab, const int* __restrict__ labels,
                                                                  long long* __restrict__ xchg)
@@ -631,7 +632,7 @@ static int rebin(KmState& s, const double* seeds_yx, cudaStream_t st)
 // plane pitches (W and plane stride even) and a 16-byte aligned base; otherwise the kernel stages the tile with ordinary loads.
 static bool make_lab_map(CUtensorMap& map, const double* lab, int rows, int W, size_t plane_stride)
 {
-    umma::EncodeTiledFn encode = umma::encode_tiled_fn();
+    wgmma::EncodeTiledFn encode = wgmma::encode_tiled_fn();
     if (!encode || (W & 1) || (plane_stride & 1) || ((uintptr_t)lab & 15)) return false;
     const cuuint64_t gdim[3] = { (cuuint64_t)W, (cuuint64_t)rows, 3 };
     const cuuint64_t gstride[2] = { (cuuint64_t)W * sizeof(double), (cuuint64_t)plane_stride * sizeof(double) };

@@ -217,7 +217,7 @@ static int minmax_launch(const void* img, int dtype, size_t n, double* minmax_ou
     ISB_CUDA_CHECK(cudaMemsetAsync(mm, 0xFF, sizeof(unsigned long long), st));
     ISB_CUDA_CHECK(cudaMemsetAsync(mm + 1, 0x00, sizeof(unsigned long long), st));
     int blocks = (int)((n + 256 * 8 - 1) / (256 * 8));
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     k_minmax<<<blocks, 256, 0, st>>>(img, dtype, n, mm);
     ISB_LAUNCH_CHECK();

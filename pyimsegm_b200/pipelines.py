@@ -440,7 +440,7 @@ def train_classif_color2d_slic_features(list_images, list_annots, dict_features,
     """ the supervised training wrapper of the reference (pipelines.py:293-379).  Its data step is available here
     (:func:`wrapper_compute_color2d_slic_features_labels`); the classifier zoo, hyper-parameter search and dataset balancing it
     hands the data to (``imsegm/classification.py``) are outside the accelerated hot path (SURVEY.md section 2, row 8) """
-    raise NotImplementedError('supervised classifier training (imsegm.classification) is outside the B200 hot path; '
+    raise NotImplementedError('supervised classifier training (imsegm.classification) is outside the GPU hot path; '
                               'use wrapper_compute_color2d_slic_features_labels for the features and labels')
 
 

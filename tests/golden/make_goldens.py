@@ -1,9 +1,9 @@
 """
 Generate tests/golden/reference_vectors.npz by RUNNING THE REFERENCE ITSELF where that is possible in this container.
 
-    python tests/golden/make_goldens.py          (needs /root/reference and oracle/_ref/features_cython, i.e. `make -C oracle ref`)
+    IMSEGM_REFERENCE=<reference checkout> python tests/golden/make_goldens.py   (needs oracle/_ref/features_cython, i.e. `make -C oracle ref`)
 
-What runs: the reference's own modules imported from /root/reference -- imsegm.descriptors, imsegm.graph_cuts, imsegm.labeling,
+What runs: the reference's own modules imported from $IMSEGM_REFERENCE -- imsegm.descriptors, imsegm.graph_cuts, imsegm.labeling,
 imsegm.superpixels -- with its only native module (features_cython.pyx) compiled unchanged into oracle/_ref.  Packages that are
 not installable here (scikit-image, gco, matplotlib, nibabel, ...) are replaced by inert stubs, so only functions that never touch
 them can be called: the colour / gray statistics and their drivers, the Leung-Malik bank and the whole texture descriptor (scipy +
@@ -20,7 +20,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get('IMSEGM_REFERENCE', '/root/reference')
+REF = os.environ['IMSEGM_REFERENCE']
 
 
 def import_reference():

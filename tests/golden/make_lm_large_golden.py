@@ -1,6 +1,6 @@
 """
 Generate tests/golden/lm_large.npz: the reference's OWN Leung-Malik texture descriptor (imsegm/descriptors.py:1041-1106, run from
-/root/reference with its Cython module compiled unchanged, see make_goldens.py) on an image LARGER than the sigma-150 background
+$IMSEGM_REFERENCE with its Cython module compiled unchanged, see make_goldens.py) on an image LARGER than the sigma-150 background
 kernel (1201 taps) on both axes -- 1280 x 1280, textured, full bank (20 batteries, 76 kernels), mean / std / energy.
 
     python tests/golden/make_lm_large_golden.py         (~10-15 min of CPU: 228 float64 33x33 convolutions of 1280^2 + the blur)

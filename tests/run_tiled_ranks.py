@@ -1,5 +1,5 @@
 """
-torchrun entry of tests/test_gpu_tiled.py::test_two_ranks_nccl (and of `gpurun --gpus N`): one process per GPU, one band (or two)
+torchrun entry of tests/test_gpu_tiled.py::test_two_ranks_nccl (and of a run over N GPUs): one process per GPU, one band (or two)
 per process, NCCL between them.  Every rank checks its own rows against the oracle; rank 0 prints TILED-RANKS-OK.
 """
 import os

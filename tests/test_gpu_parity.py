@@ -1,4 +1,6 @@
 """GPU parity tests proper: the CUDA path (through the C-ABI) against the CPU oracle on the same seeded inputs."""
+import os
+
 import numpy as np
 import pytest
 
@@ -47,6 +49,11 @@ def test_slic_label_map_bit_exact(oracle, case):
     assert set(np.unique(got)) == set(range(got.max() + 1))
 
 
+def _reference_module_outputs():
+    """outputs of the reference's features_cython.pyx compiled unchanged, on the inputs of the tests below"""
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_cython_module.npz'))
+
+
 def test_color_stats_match_oracle_and_reference_module(oracle):
     from pyimsegm_b200 import descriptors as ds
     img, _ = synth_regions(300, 400, seed=3)
@@ -55,10 +62,9 @@ def test_color_stats_match_oracle_and_reference_module(oracle):
         for name, fn_o in (('mean', oracle.color2d_mean), ('energy', oracle.color2d_energy), ('std', oracle.color2d_std)):
             got = getattr(ds, 'cython_img2d_color_%s' % name)(im, seg)
             np.testing.assert_allclose(got, fn_o(im, seg), rtol=1e-6, atol=1e-9)
-    fc = oracle.ref_features_cython()
-    if fc is not None:
-        ref = np.array(fc.computeColorImage2dEnergy(img.astype(np.float32), seg.astype(np.int32)))
-        np.testing.assert_allclose(ds.cython_img2d_color_energy(img, seg), ref, rtol=1e-6, atol=1e-9)
+    # the reference module's computeColorImage2dEnergy(img as float32, seg) on this image, stored
+    ref = _reference_module_outputs()['slic_regions_energy']
+    np.testing.assert_allclose(ds.cython_img2d_color_energy(img, seg), ref, rtol=1e-6, atol=1e-9)
     fts, names = ds.compute_image2d_color_statistic(img, seg, ('mean', 'std', 'energy', 'meanGrad'))
     want = oracle.image2d_color_statistic(img, seg, ('mean', 'std', 'energy', 'meanGrad'))
     assert fts.shape == (seg.max() + 1, 12) and len(names) == 12
@@ -351,16 +357,15 @@ def test_remaining_native_functions(oracle):
     assert ds.cython_ray_features_seg2d(seg, (60, 40), 30).astype(int).tolist() == [74, 55, 28, 10, 5, 4, 4, 5, 9, 30, 57, 75]
     assert ds.cython_ray_features_seg2d(seg, (40, 60), 20).astype(int).tolist() == \
         [54, 57, 58, 55, 50, 43, 38, 31, 26, 24, 22, 22, 23, 26, 29, 34, 41, 48]
-    fc = oracle.ref_features_cython()
+    gold = _reference_module_outputs()      # the reference module's computeRayFeaturesBinary2d at these positions, stored
     noise = rng.rand(40, 60) < 0.08
     pos = np.stack([rng.randint(0, 40, 25), rng.randint(0, 60, 25)], 1)
+    assert np.array_equal(pos, gold['ray_noise_pos'])
     for edge, e in (('up', 1), ('down', -1)):
         got = ds.cython_ray_features_seg2d(noise, pos, 7.5, edge)
-        for p, g in zip(pos, got):
+        for p, g, ref in zip(pos, got, gold['ray_noise_' + edge]):
             assert np.array_equal(g, oracle.ray_features2d(noise, p, 7.5, e))
-            if fc is not None:
-                ref = np.array(fc.computeRayFeaturesBinary2d(noise.astype(np.int8), np.array(p, dtype=np.int32), 7.5, e))
-                np.testing.assert_allclose(g, ref, rtol=1e-5)
+            np.testing.assert_allclose(g, ref, rtol=1e-5)
 
 
 @pytest.mark.parametrize('sp_size,regul,shape', [(4, 0.3, (96, 128)), (5, 0.15, (77, 101)), (60, 0.2, (200, 260)), (9, 0.5, (33, 47))])

@@ -146,7 +146,7 @@ def test_two_ranks_nccl():
     """the same checks with two processes, one GPU each, merged by NCCL all_reduce / broadcast"""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip('needs two GPUs (run `gpurun --gpus 2 -- python -m pytest tests -m gpu -k two_ranks`)')
+        pytest.skip('needs two GPUs (on a host with two: python -m pytest tests -m gpu -k two_ranks)')
     cmd = [sys.executable, '-m', 'torch.distributed.run', '--nnodes=1', '--nproc-per-node=2', '--master-addr', '127.0.0.1',
            '--master-port', '29571', os.path.join(ROOT, 'tests', 'run_tiled_ranks.py')]
     out = subprocess.run(cmd, cwd=ROOT, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=600)

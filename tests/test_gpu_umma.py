@@ -1,8 +1,9 @@
-"""Known-answer test of the tcgen05 plumbing (csrc/umma.cuh): one CTA computes D[128, N] = A[128, K] . B[N, K]^T with tcgen05.mma
-kind::tf32 from K-major, unswizzled shared-memory operands and reads the FP32 accumulator back from tensor memory.  The Leung-Malik
-contraction (csrc/lm_texture.cu) uses exactly these operand layouts and descriptor encodings."""
-import ctypes as C
+"""Known-answer test of the tensor-core plumbing (csrc/wgmma.cuh): one CTA of two warpgroups computes D[128, N] = A[128, K] . B[N, K]^T
+with wgmma.mma_async (TF32 inputs, FP32 accumulators in registers) from K-major, unswizzled shared-memory operands.  The Leung-Malik
+contraction (csrc/lm_texture.cu) uses exactly these operand layouts and descriptor encodings.
 
+The module and test names come from the earlier tcgen05 version of the contraction; they are kept so that the same test ids check
+the same shapes and tolerances, now through wgmma."""
 import numpy as np
 import pytest
 
@@ -19,7 +20,7 @@ def _run(lib, torch, A, B, variant):
     N, K = B.shape
     dA, dB = torch.from_numpy(A).cuda(), torch.from_numpy(B).cuda()
     dD = torch.zeros((128, N), dtype=torch.float32, device='cuda')
-    _lib.check(lib.isb_umma_selftest(_lib.ptr(dA), _lib.ptr(dB), N, K, variant, _lib.ptr(dD), _lib.stream_ptr()))
+    _lib.check(lib.isb_wgmma_selftest(_lib.ptr(dA), _lib.ptr(dB), N, K, variant, _lib.ptr(dD), _lib.stream_ptr()))
     torch.cuda.synchronize()
     return dD.cpu().numpy()
 
@@ -37,12 +38,13 @@ def test_tcgen05_tf32_gemm_known_answer(N, K):
     err = np.abs(got - want).max()
     if err > 1e-4:
         alt = np.abs(_run(lib, torch, A, B, 1) - want).max()
-        raise AssertionError('tcgen05 GEMM wrong: max err %g (with LBO/SBO swapped: %g)' % (err, alt))
+        raise AssertionError('wgmma GEMM wrong: max err %g (with LBO/SBO swapped: %g)' % (err, alt))
 
 
 @pytest.mark.parametrize('N,K', [(80, 40), (48, 40), (240, 64)])
 def test_tcgen05_tf32_gemm_a_operand_in_tensor_memory(N, K):
-    """the TS form: A written into tensor memory with tcgen05.st (lane = row, one column per tf32 element), B from shared memory"""
+    """the A operand in the form the contraction feeds it: per-thread register fragments (there is no tensor memory on sm_90),
+    B from shared memory"""
     from pyimsegm_b200 import _lib
     torch = _lib.require_cuda()
     lib = _lib.lib()

@@ -1,5 +1,7 @@
 """CPU tests: the oracle against every golden vector the reference's own doctests hold for the hot path
 (SURVEY.md section 4), against the reference's Cython module compiled unchanged (oracle/_ref), and against SciPy."""
+import os
+
 import numpy as np
 import pytest
 from scipy import ndimage
@@ -87,17 +89,16 @@ def test_color_statistics_goldens(oracle):
 
 
 def test_restatement_equals_reference_cython_module(oracle):
-    fc = oracle.ref_features_cython()
-    if fc is None:
-        pytest.skip('oracle/_ref not built (no /root/reference on this box)')
+    """against the outputs of the reference's features_cython.pyx compiled unchanged, stored in tests/golden/reference_cython_module.npz
+    (computeColorImage2dMean / Energy / Variance on this seeded input; the variance was given the module's own mean as float32)"""
+    ref = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_cython_module.npz'))
     rng = np.random.RandomState(3)
     img = rng.random_sample((60, 70, 3)).astype(np.float32)
     seg = (np.arange(60)[:, None] // 8 * 9 + np.arange(70)[None, :] // 8).astype(np.int32)
-    mean_ref = np.array(fc.computeColorImage2dMean(img, seg))
+    mean_ref = ref['mean']
     np.testing.assert_allclose(oracle.color2d_mean(img, seg), mean_ref, rtol=1e-12)
-    np.testing.assert_allclose(oracle.color2d_energy(img, seg), np.array(fc.computeColorImage2dEnergy(img, seg)), rtol=1e-7)
-    var_ref = np.array(fc.computeColorImage2dVariance(img, seg, mean_ref.astype(np.float32)))
-    np.testing.assert_allclose(oracle.color2d_std(img, seg, mean_ref) ** 2, var_ref, rtol=1e-6)
+    np.testing.assert_allclose(oracle.color2d_energy(img, seg), ref['energy'], rtol=1e-7)
+    np.testing.assert_allclose(oracle.color2d_std(img, seg, mean_ref) ** 2, ref['variance'], rtol=1e-6)
 
 
 def test_graph_goldens(oracle):
