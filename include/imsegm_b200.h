@@ -269,6 +269,36 @@ int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, const int32_t*
                         double reg_covar, int use_scaler, unsigned long long seed, const int32_t* init_labels, double* proba,
                         double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream);
 
+/* predict_proba of a caller-fitted class model -- replaces the host round trip of segment_color2d_slic_features_model_graphcut
+ * (imsegm/pipelines.py:160-241) with a model from estim_model_classes_group (:113-157) or a trained classifier
+ * (imsegm/classification.py:101).  The tables come from pyimsegm_b200/class_models.py; every call is timed under the 'gmm' stage.
+ * Rows are [N, ...] with the real row count read from the optional device int32 n_dev (<= N); nothing syncs or allocates.
+ *
+ * isb_class_transform: the model's feature transform.  out[n] = PCA(scaler(x[n])) with NaN -> 0 first;
+ *   feat [N, ld] f64 (first D_in columns); sc_mean / sc_scale: optional [D_in] ((x - mean) / scale, either may be NULL);
+ *   pca_comp: optional [D_out, D_in] components_, then pca_mean [D_out] = mean_ components_^T and pca_scale: optional [D_out]
+ *   (whitening, sqrt(explained_variance_) clipped at eps); without PCA D_out == D_in.  ws: isb_class_transform_workspace_bytes. */
+size_t isb_class_transform_workspace_bytes(int N, int D_in, int has_pca);
+int isb_class_transform(const double* feat, int N, int ld, const int32_t* n_dev, int D_in, const double* sc_mean, const double* sc_scale,
+                        const double* pca_comp, const double* pca_mean, const double* pca_scale, int D_out, double* out, void* ws,
+                        size_t ws_bytes, isb_stream_t stream);
+/* Gaussian mixture (GaussianMixture / BayesianGaussianMixture, any covariance type expanded to the full form):
+ *   proba[n, k] = softmax_k(log_const[k] - (D log 2 pi + |x[n] U_k - bvec[k]|^2) / 2)
+ *   x [N, D] f64; prec_chol [K, D, D] (U_k); bvec [K, D] = means_k U_k; log_const [K] (log-det of U_k + log weight + the BGM terms).
+ *   D <= 232, K <= 8 (else ISB_ERR_UNSUPPORTED); D > 16 runs the fit's batched FP64 GEMM in ws (isb_mixture_predict_workspace_bytes). */
+size_t isb_mixture_predict_workspace_bytes(int N, int D, int K);
+int isb_mixture_predict_proba(const double* x, int N, const int32_t* n_dev, int D, int K, const double* prec_chol, const double* bvec,
+                              const double* log_const, double* proba, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* decision tree / random forest / extra trees (single output): n_trees trees in structure-of-arrays node tables of n_nodes entries
+ * (children as global node indices, -1 at a leaf), tree e starting at roots[e]; value [n_nodes, K] the leaf class fractions.
+ * A sample goes left iff (double)(float)x[feature] <= threshold (sklearn's float32 input).  proba = the leaf values added in tree
+ * order, divided by n_trees when average != 0: bit-identical to ForestClassifier.predict_proba with n_jobs=None.  K <= 64.
+ *   ws: isb_forest_predict_workspace_bytes(N, n_trees) (the leaf of every (sample, tree)) */
+size_t isb_forest_predict_workspace_bytes(int N, int n_trees);
+int isb_forest_predict_proba(const double* x, int N, const int32_t* n_dev, int D, int n_trees, const int32_t* roots, const int32_t* feature,
+                             const double* threshold, const int32_t* left, const int32_t* right, int n_nodes, const double* value, int K,
+                             int average, double* proba, void* ws, size_t ws_bytes, isb_stream_t stream);
+
 /* compute_texture_desc_lm_img2d_clr (imsegm/descriptors.py:1041-1106): sigma-150 background subtraction (reflect, all three
  * axes), Leung-Malik filter bank (33x33 kernels) as an implicit GEMM on the tensor cores (wgmma.mma_async with TF32 inputs and the 3xTF32
  * split, FP32 accumulators in registers, operands staged by TMA), max over the orientations of a battery, clip at 1e6,

@@ -1168,6 +1168,36 @@ __global__ void __launch_bounds__(256) k_gmm_predict(int N_in, const int* n_dev,
     }
 }
 
+// predict_proba of a caller-fitted mixture, small D: one thread per sample, sklearn's order y = x U - (mu U), q = |y|^2,
+// log p_k = c_k - (D log 2 pi + q) / 2, then log-sum-exp and exp (c_k folds everything that does not depend on the sample)
+__global__ void __launch_bounds__(256) k_mix_proba(const double* __restrict__ x, int N_in, const int* n_dev, int D, int K,
+                                                   const double* __restrict__ pc, const double* __restrict__ bvec,
+                                                   const double* __restrict__ cst, double* __restrict__ proba)
+{
+    const int N = n_dev ? min(*n_dev, N_in) : N_in;
+    for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x) {
+        const double* xr = x + (size_t)n * D;
+        double lw[KMAX];
+        double mx = -DBL_MAX;
+        for (int k = 0; k < K; ++k) {
+            const double* U = pc + (size_t)k * D * D;
+            double q = 0;
+            for (int j = 0; j < D; ++j) {
+                double y = 0;
+                for (int i = 0; i < D; ++i) y = fma(xr[i], U[i * D + j], y);
+                const double t = y - bvec[k * D + j];
+                q = fma(t, t, q);
+            }
+            lw[k] = -0.5 * (D * 1.8378770664093453 + q) + cst[k];
+            mx = fmax(mx, lw[k]);
+        }
+        double s = 0;
+        for (int k = 0; k < K; ++k) s += exp(lw[k] - mx);
+        const double lse = mx + log(s);
+        for (int k = 0; k < K; ++k) proba[(size_t)n * K + k] = exp(lw[k] - lse);
+    }
+}
+
 static size_t carve_gmm(GmmWs& w, void* ws, size_t bytes, int N, int D, int K, int n_init)
 {
     WsCarver c(ws, bytes);
@@ -1245,6 +1275,44 @@ extern "C" int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, con
     int blocks = (N + 255) / 256;
     if (blocks > 132) blocks = 132;
     k_gmm_predict<<<blocks, 256, 0, st>>>(N, n_dev, D, K, n_init, w, proba, params_out);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" size_t isb_mixture_predict_workspace_bytes(int N, int D, int K)
+{
+    if (N <= 0 || D <= DMAX || K <= 0) return 0;
+    return isb_align(sizeof(double) * (size_t)K * N * D);
+}
+
+extern "C" int isb_mixture_predict_proba(const double* x, int N, const int32_t* n_dev, int D, int K, const double* prec_chol, const double* bvec,
+                                         const double* log_const, double* proba, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    ISB_REQUIRE(x && prec_chol && bvec && log_const && proba, "null pointer");
+    ISB_REQUIRE(N > 0 && D > 0 && K > 0, "bad sizes");
+    if (D > DBIG || K > KMAX) { isb_set_error("device mixture handles D <= %d and K <= %d (got D=%d K=%d)", DBIG, KMAX, D, K); return ISB_ERR_UNSUPPORTED; }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (D <= DMAX) {
+        ProfScope prof(ISB_PROF_GMM, st);
+        int blocks = (N + 255) / 256;
+        if (blocks > 132 * 8) blocks = 132 * 8;
+        k_mix_proba<<<blocks, 256, 0, st>>>(x, N, n_dev, D, K, prec_chol, bvec, log_const, proba);
+        ISB_LAUNCH_CHECK();
+        return ISB_OK;
+    }
+    // large D: Y[k] = X U[k] by the batched GEMM of the fit, then the fit's predict epilogue with (b, c) in place of (mu U, log-det + log w)
+    ISB_REQUIRE(ws && ws_bytes >= isb_mixture_predict_workspace_bytes(N, D, K), "workspace too small");
+    ProfScope prof(ISB_PROF_GMM, st);
+    GmmWs w = {};
+    w.big = (double*)ws;
+    w.bvec = const_cast<double*>(bvec);
+    w.ldw = const_cast<double*>(log_const);
+    const size_t sND = (size_t)N * D, sDD = (size_t)D * D;
+    const BatchStride bs = { 0, 0, 0, sDD, 0, sND, 0 };
+    k_dgemm_batched<false, false><<<dim3((D + TN - 1) / TN, (N + TM - 1) / TM, K), 256, 0, st>>>(
+        x, D, prec_chol, D, w.big, D, bs, N, D, D, n_dev, 1, nullptr, K, 0, 1, 0, FuseW());
+    ISB_LAUNCH_CHECK();
+    k_big_proba<<<(N + 7) / 8, 256, 0, st>>>(N, n_dev, D, K, 0, w, proba, nullptr);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }

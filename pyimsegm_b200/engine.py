@@ -149,13 +149,14 @@ class Engine(object):
             if c + len(slots) < nchunks:
                 futs[c + len(slots)] = submit(c + len(slots))
 
-    def const_device(self, arr, name):
+    def const_device(self, arr, name, digest=None):
         """small host array that rarely changes between calls (seed grid, pairwise table, filter taps): every distinct content gets
         its OWN device tensor, uploaded once and never overwritten -- no copy in steady state, and a captured CUDA graph that read
-        one of them keeps reading the right values whatever other configurations run in between"""
+        one of them keeps reading the right values whatever other configurations run in between.  ``digest``: a content digest the
+        caller already holds (it must change whenever ``arr`` does), which saves hashing a large table on every call"""
         import hashlib
         arr = np.ascontiguousarray(arr)
-        key = (name, arr.shape, arr.dtype.str, hashlib.blake2b(arr.tobytes(), digest_size=16).digest())
+        key = (name, arr.shape, arr.dtype.str, digest if digest is not None else hashlib.blake2b(arr.tobytes(), digest_size=16).digest())
         cache = self.__dict__.setdefault('_consts', {})
         hit = cache.get(key)
         if hit is not None:
@@ -372,6 +373,35 @@ class Engine(object):
                                          C.c_double(reg_covar), int(bool(use_scaler)), C.c_ulonglong(int(seed)), _lib.ptr(d_init),
                                          _lib.ptr(proba), _lib.ptr(params), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
         return proba, params
+
+    def class_model_predict(self, d_feat, cm, d_n=None):
+        """predict_proba of a compiled caller-fitted model (class_models.CompiledModel) on features [N, >= n_features_in] (device):
+        returns proba [N, K] device, asynchronous; the model's tables are device constants keyed on its digest"""
+        torch, lib = self.torch, self.lib
+        N, ld = int(d_feat.shape[0]), int(d_feat.stride(0))
+        t = {name: self.const_device(arr, 'cm_' + name, digest=cm.digest) for name, arr in cm.tables.items()}
+        st = _lib.stream_ptr()
+        x = self.buf('cm_x', (N, cm.n_dims), torch.float64)
+        wsb = lib.isb_class_transform_workspace_bytes(N, cm.n_features_in, int('pca_comp' in t))
+        ws = self.buf('ws_cm', (max(wsb, 1),), torch.uint8)
+        self._ck(lib.isb_class_transform(_lib.ptr(d_feat), N, ld, _lib.ptr(d_n), cm.n_features_in, _lib.ptr(t.get('sc_mean')),
+                                         _lib.ptr(t.get('sc_scale')), _lib.ptr(t.get('pca_comp')), _lib.ptr(t.get('pca_mean')),
+                                         _lib.ptr(t.get('pca_scale')), cm.n_dims, _lib.ptr(x), _lib.ptr(ws), C.c_size_t(wsb), st))
+        K = cm.n_classes
+        proba = self.buf('proba', (N, K), torch.float64)
+        if cm.kind == 'mixture':
+            wsb = lib.isb_mixture_predict_workspace_bytes(N, cm.n_dims, K)
+            ws = self.buf('ws_cm_predict', (max(wsb, 1),), torch.uint8)
+            self._ck(lib.isb_mixture_predict_proba(_lib.ptr(x), N, _lib.ptr(d_n), cm.n_dims, K, _lib.ptr(t['prec_chol']), _lib.ptr(t['bvec']),
+                                                   _lib.ptr(t['log_const']), _lib.ptr(proba), _lib.ptr(ws), C.c_size_t(wsb), st))
+        else:
+            n_trees, n_nodes = len(cm.tables['roots']), len(cm.tables['left'])
+            wsb = lib.isb_forest_predict_workspace_bytes(N, n_trees)
+            ws = self.buf('ws_cm_predict', (max(wsb, 1),), torch.uint8)
+            self._ck(lib.isb_forest_predict_proba(_lib.ptr(x), N, _lib.ptr(d_n), cm.n_dims, n_trees, _lib.ptr(t['roots']), _lib.ptr(t['feature']),
+                                                  _lib.ptr(t['threshold']), _lib.ptr(t['left']), _lib.ptr(t['right']), n_nodes,
+                                                  _lib.ptr(t['value']), K, int(cm.average), _lib.ptr(proba), _lib.ptr(ws), C.c_size_t(wsb), st))
+        return proba
 
     def gather(self, d_seg, lut_i=None, lut_p=None):
         torch, lib = self.torch, self.lib

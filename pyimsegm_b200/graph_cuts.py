@@ -29,6 +29,9 @@ MIN_MAX_EDGE_WEIGHT = 1e3
 #: the default 'GMM' class model is fitted on the GPU (isb_gmm_fit_predict) when it fits the device kernel
 #: (<= 16 features, <= 8 classes, no PCA); set False to force scikit-learn on the host
 USE_DEVICE_GMM = True
+#: a caller-fitted model (segment_color2d_slic_features_model_graphcut, segment_images_batch(model_pipeline=...), segment_resident)
+#: that class_models.compile_model supports runs its predict_proba on the device; set False to force the host round trip
+USE_DEVICE_PREDICT = True
 #: seed of the device k-means++ initialisation (the reference leaves its model unseeded)
 RANDOM_SEED = 0
 #: D <= 16 runs as one kernel (a CTA per restart), 16 < D <= 256 (colour + Leung-Malik = 189) as batched FP64 GEMMs

@@ -10,13 +10,15 @@ and return values):
 * :func:`compute_color2d_superpixels_features`          (reference pipelines.py:244-270)
 
 The image goes to the device once; label map, features, class model, graph, energies and the cut never leave it and the
-host synchronises ONCE, when the results are downloaded.  (A user-supplied model, or one the device GMM does not cover, costs
-one round trip: features [N, D] down, probabilities [N, K] up.)
+host synchronises ONCE, when the results are downloaded.  A caller-fitted mixture or tree model is compiled to device tables
+(:mod:`.class_models`) and evaluated there too; any other model, or a self-fitted one the device GMM does not cover, costs one
+round trip: features [N, D] down, probabilities [N, K] up.
 """
 import logging
 
 import numpy as np
 
+from .class_models import CompiledModel, compile_model
 from .descriptors import FEATURES_SET_COLOR, compute_selected_features_img2d, flags_are_native, native_feature_layout
 from .engine import get_engine
 from .graph_cuts import (_edge_mode, compute_pairwise_cost, device_gmm_applicable, estim_class_model,
@@ -161,32 +163,53 @@ def _features_key(dict_features):
     return tuple(sorted((k, tuple(v)) for k, v in dict_features.items()))
 
 
+def _compiled_model(model, dict_features):
+    """the device form of a caller-fitted model for the native path (its feature count has to match the native feature layout), or
+    None: then its predict_proba runs on the host"""
+    from . import graph_cuts
+    if not graph_cuts.USE_DEVICE_PREDICT or not flags_are_native(dict_features):
+        return None
+    cm = compile_model(model)
+    if cm is None or cm.n_features_in != native_feature_layout(dict_features)[1]:
+        return None
+    return cm
+
+
 def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, soft_sink=None):
     """the whole hot path on the device.  ``model`` is either ('fit', nb_classes, use_scaler, max_iter) -> the default
-    GMM is fitted on the GPU and NOTHING syncs with the host until the results are ready; or a callable
+    GMM is fitted on the GPU and NOTHING syncs with the host until the results are ready; or a
+    :class:`~.class_models.CompiledModel` -> a caller-fitted model evaluated on the device, again without a sync; or a callable
     proba_fn(features) -> one round trip (features down, probabilities up) as in the reference.
     ``soft_sink(d_seg, d_proba)``: the caller takes ``segm_soft = proba[slic]`` itself as soon as the probabilities exist
     (it does not depend on the graph cut) -- then ``d_soft`` is returned as None.
-    With a device-fitted model and colour features the two halves -- image -> class probabilities, probabilities -> cut and LUT
-    gathers -- are CUDA-graph replays (:func:`_graph_call`); the image then has to sit in one of the engine's cached buffers.
+    With a device-fitted or compiled model and colour features the two halves -- image -> class probabilities, probabilities -> cut
+    and LUT gathers -- are CUDA-graph replays (:func:`_graph_call`); the image then has to sit in one of the engine's cached buffers.
     Returns (d_segm, d_soft, check): ``check`` is None or (d_n_edges, edge_cap) still to be verified by the caller."""
     no_cut = (not isinstance(gc_regul, (list, np.ndarray))) and gc_regul <= 0
-    if isinstance(model, tuple):
-        _, nb_classes, use_scaler, max_iter = model
+    if isinstance(model, (tuple, CompiledModel)):
         from . import graph_cuts
-        n_init = max(1, int(np.sqrt(max_iter)))
         if not hasattr(image, 'is_cuda'):
             image = eng.to_device(_supported_dtype(_as_rgb_like(np.asarray(image))), 'image')
-        graphable = (USE_CUDA_GRAPHS and not no_cut and all(k == 'color' for k in dict_features) and flags_are_native(dict_features)
-                     and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES)
+        graphable = (USE_CUDA_GRAPHS and not no_cut and all(k == 'color' for k in dict_features) and flags_are_native(dict_features))
+        if isinstance(model, CompiledModel):
+            nb_classes, model_key = model.n_classes, ('compiled', model.digest)
 
-        def first_half():
-            res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
-            d_proba, _ = eng.gmm_fit_predict(res.d_feat, nb_classes, n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED,
-                                             d_n=res.d_n_labels)
-            return res, d_proba
+            def first_half():
+                res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
+                return res, eng.class_model_predict(res.d_feat, model, d_n=res.d_n_labels)
+        else:
+            _, nb_classes, use_scaler, max_iter = model
+            model_key = model
+            n_init = max(1, int(np.sqrt(max_iter)))
+            graphable = graphable and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES
 
-        key1 = ('probabilities', id(eng), image.data_ptr(), tuple(image.shape), str(image.dtype), model, _features_key(dict_features),
+            def first_half():
+                res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
+                d_proba, _ = eng.gmm_fit_predict(res.d_feat, nb_classes, n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED,
+                                                 d_n=res.d_n_labels)
+                return res, d_proba
+
+        key1 = ('probabilities', id(eng), image.data_ptr(), tuple(image.shape), str(image.dtype), model_key, _features_key(dict_features),
                 sp_size, sp_regul)
         res, d_proba = _graph_call(eng, key1, first_half) if graphable else first_half()
         if no_cut:
@@ -239,7 +262,12 @@ def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_t
     native = image.ndim == 3 and flags_are_native(dict_features) and gc_edge_type not in ('color', 'features')
     if not native or debug_visual is not None:
         # general path: every stage still runs on the device, but through the numpy-facing stage functions
-        proba_fn = model if callable(model) else (lambda f: estim_class_model(f, model[1], 'GMM', None, model[2], model[3]).predict_proba(f))
+        if isinstance(model, CompiledModel):
+            proba_fn = model.predict_proba
+        elif callable(model):
+            proba_fn = model
+        else:
+            proba_fn = lambda f: estim_class_model(f, model[1], 'GMM', None, model[2], model[3]).predict_proba(f)  # noqa: E731
         slic, features = compute_color2d_superpixels_features(image, dict_features, sp_size=sp_size, sp_regul=sp_regul)
         if debug_visual is not None:
             img3 = image if image.ndim == 3 else np.stack([image] * 3, axis=-1)
@@ -328,7 +356,10 @@ def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIM
     if not native:
         return [segment_color2d_slic_features_model_graphcut(im, model_pipeline, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)
                 for im in list_images]
-    model = ('fit', nb_classes, use_scaler, 99) if model_pipeline is None else model_pipeline.predict_proba
+    if model_pipeline is None:
+        model = ('fit', nb_classes, use_scaler, 99)
+    else:
+        model = _compiled_model(model_pipeline, dict_features) or model_pipeline.predict_proba
     classes = getattr(model_pipeline, 'classes_', None)
     engines = _batch_engines(nb_streams)
     torch = engines[0][0].torch
@@ -469,7 +500,12 @@ def pipe_gray3d_slic_features_model_graphcut(image, nb_classes, dict_features, s
 def segment_resident(d_image, model, dict_features, sp_size=30, sp_regul=0.2, gc_regul=1., gc_edge_type='model'):
     """ the same hot path with the image ALREADY on the device (a cuda tensor [H, W, 3]) and the results left
     there: returns (segm int32 [H, W], segm_soft float64 [H, W, K]) device tensors.  ``model`` is a callable
-    proba_fn(features) or ('fit', nb_classes, use_scaler, max_iter) for the GPU-fitted default GMM. """
+    proba_fn(features), a fitted model (or its bound ``predict_proba``) -- evaluated on the device when
+    :func:`~.class_models.compile_model` supports it -- or ('fit', nb_classes, use_scaler, max_iter) for the GPU-fitted default GMM.
+    The indices in ``segm`` are not mapped through the model's ``classes_``. """
+    if not isinstance(model, (tuple, CompiledModel)):
+        fitted = model.__self__ if getattr(model, '__name__', None) == 'predict_proba' and hasattr(model, '__self__') else model
+        model = _compiled_model(fitted, dict_features) or (model if callable(model) else model.predict_proba)
     return _run_resident(get_engine(), d_image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)[:2]
 
 
@@ -515,5 +551,7 @@ def segment_color2d_slic_features_model_graphcut(image, model_pipeline, dict_fea
     """
     logging.info('PIPELINE Superpixels-Features-Model-GraphCut')
     classes = getattr(model_pipeline, 'classes_', None)
-    return _segment(image, model_pipeline.predict_proba, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, debug_visual,
-                    classes=classes)
+    model = model_pipeline.predict_proba
+    if debug_visual is None and np.ndim(image) == 3 and gc_edge_type not in ('color', 'features'):
+        model = _compiled_model(model_pipeline, dict_features) or model
+    return _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, debug_visual, classes=classes)
