@@ -140,6 +140,11 @@ def require_cuda():
     return torch
 
 
+def dtype_code(dtype):
+    """DTYPE_CODES entry of a numpy or torch dtype"""
+    return DTYPE_CODES[str(dtype).replace('torch.', '')]
+
+
 def ptr(t):
     """device pointer of a torch tensor (or None)"""
     return None if t is None else C.c_void_p(t.data_ptr())

@@ -156,7 +156,7 @@ def _device_median(img, seg, channels):
     out = eng.buf('median_out', (nb, channels), eng.torch.float64)
     wsb = eng.lib.isb_segment_median_workspace_bytes(C.c_longlong(n_px), nb)
     ws = eng.buf('ws_median', (wsb,), eng.torch.uint8)
-    code = _lib.DTYPE_CODES[str(img.dtype)]
+    code = _lib.dtype_code(img.dtype)
     _lib.check(eng.lib.isb_segment_median(_lib.ptr(d_img), code, _lib.ptr(d_seg), C.c_longlong(n_px), channels, nb, _lib.ptr(out), _lib.ptr(ws),
                                           C.c_size_t(wsb), _lib.stream_ptr()))
     return eng.to_host(out).copy()
@@ -183,7 +183,7 @@ def _device_gray_stats(img, seg, flags):
     feat = eng.buf('feat_gray', (nb, len(flags)), eng.torch.float64)
     wsb = eng.lib.isb_gray_stats_workspace_bytes(nb)
     ws = eng.buf('ws_gray', (wsb,), eng.torch.uint8)
-    _lib.check(eng.lib.isb_gray_stats(_lib.ptr(d_img), _lib.DTYPE_CODES[str(img.dtype)], _lib.ptr(d_seg), C.c_longlong(img.size), nb, bits,
+    _lib.check(eng.lib.isb_gray_stats(_lib.ptr(d_img), _lib.dtype_code(img.dtype), _lib.ptr(d_seg), C.c_longlong(img.size), nb, bits,
                                       _lib.ptr(feat), len(flags), 0, _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
     return eng.to_host(feat).copy()
 

@@ -17,9 +17,39 @@ FLAG_BITS = {'mean': 1, 'std': 2, 'energy': 4}
 #: (reference graph_cuts.py:646)
 EDGE_MODES = {'': (0, 0), 'model': (1, 1), 'model_lT': (1, 0), 'model_l1': (2, 0), 'model_l2': (3, 0), 'spatial': (0, 1)}
 
+#: initial capacity of a device edge table, in edges per node (per upper bound of the label count) of a 2-D label map, twice
+#: that for a volume; grown x4 whenever a table overflows.  The device then reports cap + 1 edges and writes no row past cap.
+EDGE_CAP_PER_NODE = 8
+
+
+def edge_capacity(nb, ndim=2):
+    """rows of a new device edge table for ``nb`` nodes of a ``ndim``-D label map"""
+    return max(64, int(EDGE_CAP_PER_NODE * (ndim - 1) * int(nb)))
+
+
+def edges_fit(n_edges, cap):
+    """whether a table of ``cap`` rows held all ``n_edges`` the device counted; if not, the capacity grows x4 and the caller redoes
+    the work that filled it"""
+    global EDGE_CAP_PER_NODE
+    if int(n_edges) <= cap:
+        return True
+    EDGE_CAP_PER_NODE *= 4
+    return False
+
+
+def flag_bits(flags):
+    """statistic names -> (bit mask of the C-ABI, columns per 3-channel source: three per statistic)"""
+    bits = 0
+    for f in flags:
+        bits |= FLAG_BITS[f]
+    return bits, 3 * bin(bits).count('1')
+
 
 def gaussian_half_kernel(sigma, truncate=4.0):
-    """half of scipy.ndimage's normalised 1-D Gaussian: [w0, w1 .. wr], radius r = int(truncate * sigma + 0.5)"""
+    """half of scipy.ndimage's normalised 1-D Gaussian: [w0, w1 .. wr], radius r = int(truncate * sigma + 0.5); ``sigma <= 0``
+    gives the identity [1] of radius 0 (no blur, as scipy skips such an axis)"""
+    if sigma <= 0:
+        return np.ones(1), 0
     radius = int(truncate * float(sigma) + 0.5)
     x = np.arange(-radius, radius + 1)
     phi = np.exp(-0.5 / (sigma * sigma) * x ** 2)
@@ -73,6 +103,12 @@ class Engine(object):
         self.lib = _lib.lib()
         self.device = self.torch.device('cuda', self.torch.cuda.current_device() if device is None else device)
         self._bufs = {}
+        self._consts = {}
+        self._stage = None
+        self._side = None
+        #: CUDA graphs captured on this engine's buffers: once there is one, an outgrown buffer is retired instead of freed
+        self.graphs_captured = 0
+        self._retired = []
 
     # -- memory helpers ------------------------------------------------------------------------------------------
     def buf(self, name, shape, dtype):
@@ -85,9 +121,9 @@ class Engine(object):
         n = int(np.prod(shape)) if shape else 1
         cur = self._bufs.get(name)
         if cur is None or cur.dtype != dtype or cur.numel() < n:
-            if cur is not None and getattr(self, 'graphs_captured', 0):
+            if cur is not None and self.graphs_captured:
                 # a captured CUDA graph may hold the address of the old block: keep it alive instead of returning it to the allocator
-                self.__dict__.setdefault('_retired', []).append(cur)
+                self._retired.append(cur)
             cur = torch.empty(max(n, 1), dtype=dtype, device=self.device)
             self._bufs[name] = cur
         return cur[:n].view(shape)
@@ -118,7 +154,7 @@ class Engine(object):
         buffers (numpy releases the GIL while copying) and every chunk is sent by an asynchronous DMA as soon as it is complete, so
         the host copies overlap the transfers."""
         torch = self.torch
-        if getattr(self, '_stage', None) is None:
+        if self._stage is None:
             from concurrent.futures import ThreadPoolExecutor
             slots = [torch.empty(self.STAGE_CHUNK, dtype=torch.uint8, pin_memory=True) for _ in range(self.STAGE_SLOTS)]
             self._stage = (slots, [t.numpy() for t in slots], [torch.cuda.Event() for _ in slots], [False] * len(slots),
@@ -157,32 +193,63 @@ class Engine(object):
         import hashlib
         arr = np.ascontiguousarray(arr)
         key = (name, arr.shape, arr.dtype.str, digest if digest is not None else hashlib.blake2b(arr.tobytes(), digest_size=16).digest())
-        cache = self.__dict__.setdefault('_consts', {})
-        hit = cache.get(key)
+        hit = self._consts.get(key)
         if hit is not None:
             return hit
         if self.torch.cuda.is_current_stream_capturing():
             raise RuntimeError('constant %r is new while a CUDA graph is being captured' % name)
         dst = self.torch.from_numpy(arr).to(self.device)
-        cache[key] = dst
+        self._consts[key] = dst
         return dst
 
     def pinned_empty(self, shape, dtype):
         """pinned host tensor (torch's caching host allocator recycles the blocks once the result is dropped)"""
         return self.torch.empty(tuple(shape), dtype=dtype, pin_memory=True)
 
-    def to_host(self, t, sync=True):
-        out = self.pinned_empty(t.shape, t.dtype)
-        out.copy_(t, non_blocking=True)
-        if sync:
-            self.torch.cuda.current_stream().synchronize()
+    def download(self, tensors):
+        """enqueue D2H copies of device tensors into pinned host tensors on the current stream and record one event after them:
+        returns (host tensors, event); the host tensors hold the data once the event has completed"""
+        hosts = []
+        for t in tensors:
+            h = self.pinned_empty(t.shape, t.dtype)
+            h.copy_(t, non_blocking=True)
+            hosts.append(h)
+        done = self.torch.cuda.Event()
+        done.record()
+        return hosts, done
+
+    def to_host(self, t):
+        (out, ), done = self.download((t, ))
+        done.synchronize()
         return out.numpy()
 
     def side_stream(self):
         """a second CUDA stream of this engine (copies that may overlap the kernels of the main stream)"""
-        if getattr(self, '_side', None) is None:
+        if self._side is None:
             self._side = self.torch.cuda.Stream(device=self.device)
         return self._side
+
+    def early_soft(self, d_seg, d_proba):
+        """segm_soft = proba[seg] needs only the class probabilities: gather it and start its (large) download on the side stream,
+        so that both overlap what the current stream does next (building and cutting the graph).  Returns (pinned host tensor,
+        event); nothing may overwrite ``d_seg`` or ``d_proba`` before the event has completed"""
+        torch = self.torch
+        side = self.side_stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            _, d_soft = self.gather(d_seg, None, d_proba)
+            (host, ), done = self.download((d_soft, ))
+        return host, done
+
+    def edge_table(self, build, nb, ndim=2):
+        """``build(cap) -> (edges, n_edges device int32[1], ...)`` with a table of :func:`edge_capacity` rows, redone larger until
+        the table holds every edge (one synchronisation per attempt): returns (E, what ``build`` returned)"""
+        while True:
+            cap = edge_capacity(nb, ndim)
+            out = build(cap)
+            E = int(self.to_host(out[1])[0])
+            if edges_fit(E, cap):
+                return E, out
 
     def _ck(self, rc):
         _lib.check(rc)
@@ -194,14 +261,11 @@ class Engine(object):
         torch, lib = self.torch, self.lib
         H, W = int(d_img.shape[0]), int(d_img.shape[1])
         Cn = 1 if d_img.dim() == 2 else int(d_img.shape[2])
-        code = _lib.DTYPE_CODES[str(d_img.dtype).replace('torch.', '')]
+        code = _lib.dtype_code(d_img.dtype)
         st = _lib.stream_ptr()
         lab = self.buf('lab', (3, H, W), torch.float64)
         mm = self.buf('minmax', (4,), torch.float64)
-        if sigma > 0:
-            w_half, radius = gaussian_half_kernel(sigma)
-        else:
-            w_half, radius = np.ones(1), 0
+        w_half, radius = gaussian_half_kernel(sigma)
         self._ck(lib.isb_slic_prepare(_lib.ptr(d_img), code, H, W, Cn, w_half.ctypes.data_as(C.POINTER(C.c_double)), radius,
                                       C.c_double(1.0 / compactness), int(bool(rescale)), _lib.ptr(lab), _lib.ptr(mm), st))
         seeds, ty, tx = slic_seed_grid(H, W, n_segments)
@@ -215,14 +279,20 @@ class Engine(object):
                                      int(bool(slic_zero)), _lib.ptr(km), None, _lib.ptr(ws), C.c_size_t(wsb), st))
         if not enforce_connectivity:
             return km, None
+        return self.enforce_connectivity(km, n_segments, min_size_factor, max_size_factor)
+
+    def enforce_connectivity(self, d_km, n_segments, min_size_factor=0.5, max_size_factor=3):
+        """connectivity pass over a k-means label map [H,W] (device): returns (labels int32 [H,W] device, n_labels device int32[1])"""
+        torch, lib = self.torch, self.lib
+        H, W = int(d_km.shape[0]), int(d_km.shape[1])
         segment_size = 1 * H * W / n_segments
         min_size, max_size = int(min_size_factor * segment_size), int(max_size_factor * segment_size)
         cwsb = lib.isb_connectivity_workspace_bytes(H, W)
         cws = self.buf('ws_conn', (cwsb,), torch.uint8)
         out = self.buf('labels', (H, W), torch.int32)
         n_labels = self.buf('n_labels', (1,), torch.int32)
-        self._ck(lib.isb_enforce_connectivity(_lib.ptr(km), H, W, min_size, max_size, _lib.ptr(out), _lib.ptr(n_labels),
-                                              _lib.ptr(cws), C.c_size_t(cwsb), st))
+        self._ck(lib.isb_enforce_connectivity(_lib.ptr(d_km), H, W, min_size, max_size, _lib.ptr(out), _lib.ptr(n_labels),
+                                              _lib.ptr(cws), C.c_size_t(cwsb), _lib.stream_ptr()))
         return out, n_labels
 
     def slic3d(self, d_vol, n_segments, compactness, spacing=(1, 1, 1), sigma=1.0, max_iter=10, enforce_connectivity=True,
@@ -230,12 +300,12 @@ class Engine(object):
         """device SLIC of a single-channel volume [D, H, W] (csrc/slic3d.cu); returns (labels int32 [D,H,W], n_labels or None)"""
         torch, lib = self.torch, self.lib
         D, H, W = (int(v) for v in d_vol.shape)
-        code = _lib.DTYPE_CODES[str(d_vol.dtype).replace('torch.', '')]
+        code = _lib.dtype_code(d_vol.dtype)
         st = _lib.stream_ptr()
         spacing = np.ascontiguousarray(spacing, dtype=np.float64)
         halves = []
         for axis, sig in enumerate(np.array([sigma, sigma, sigma], dtype=np.float64) / spacing):
-            w_half, radius = gaussian_half_kernel(sig) if sigma > 0 else (np.ones(1), 0)
+            w_half, radius = gaussian_half_kernel(sig)
             halves.append((self.to_device(w_half, 'slic3d_w%d' % axis), radius))
         tmp = self.buf('slic3d_tmp', (D, H, W), torch.float64)
         scaled = self.buf('slic3d_vol', (D, H, W), torch.float64)
@@ -263,12 +333,10 @@ class Engine(object):
                                                 C.c_size_t(cwsb), st))
         return out, n_labels
 
-    def graph3d(self, d_seg, nb, cap=None):
+    def graph3d(self, d_seg, nb, cap):
         """6-connected label pairs and centres (z, y, x) of a device label volume: (edges [cap,2], n_edges dev, cap, centres [nb,3])"""
         torch, lib = self.torch, self.lib
         D, H, W = (int(v) for v in d_seg.shape)
-        if cap is None:
-            cap = max(64, 16 * int(nb))
         wsb = lib.isb_adjacency_workspace_bytes(int(nb), int(cap))
         ws = self.buf('ws_adj', (wsb,), torch.uint8)
         edges = self.buf('edges', (cap, 2), torch.int32)
@@ -291,11 +359,8 @@ class Engine(object):
         """colour statistics (+centroids) of a [H,W,3] device image over labels [H,W] int32 in [0, nb)"""
         torch, lib = self.torch, self.lib
         H, W = int(d_seg.shape[0]), int(d_seg.shape[1])
-        code = 0 if d_img is None else _lib.DTYPE_CODES[str(d_img.dtype).replace('torch.', '')]
-        bits = 0
-        for f in flags:
-            bits |= FLAG_BITS[f]
-        ncol = 3 * bin(bits).count('1')
+        code = 0 if d_img is None else _lib.dtype_code(d_img.dtype)
+        bits, ncol = flag_bits(flags)
         if feat is None and ncol:
             feat = self.buf('feat', (nb, ncol), torch.float64)
         ld = int(feat.shape[1]) if feat is not None else 0
@@ -308,12 +373,10 @@ class Engine(object):
         return feat, centres, counts
 
     # -- (iii) graph, energies, alpha-expansion ---------------------------------------------------------------------
-    def adjacency(self, d_seg, nb, cap=None):
+    def adjacency(self, d_seg, nb, cap):
         """unique 4-connected label pairs; returns (edges int32 [cap,2] device, n_edges device int32[1], cap)"""
         torch, lib = self.torch, self.lib
         H, W = int(d_seg.shape[0]), int(d_seg.shape[1])
-        if cap is None:
-            cap = max(64, 8 * int(nb))
         wsb = lib.isb_adjacency_workspace_bytes(int(nb), int(cap))
         ws = self.buf('ws_adj', (wsb,), torch.uint8)
         edges = self.buf('edges', (cap, 2), torch.int32)
@@ -403,10 +466,13 @@ class Engine(object):
                                                   _lib.ptr(t['value']), K, int(cm.average), _lib.ptr(proba), _lib.ptr(ws), C.c_size_t(wsb), st))
         return proba
 
-    def gather(self, d_seg, lut_i=None, lut_p=None):
+    def gather(self, d_seg, lut_i=None, lut_p=None, out_i=None):
+        """``lut_i[d_seg]`` (into ``out_i`` when given, a contiguous [H,W] int32 tensor) and ``lut_p[d_seg]`` of a contiguous label map
+        [H,W] (device, one launch): returns (segm or None, segm_soft or None)"""
         torch, lib = self.torch, self.lib
         H, W = int(d_seg.shape[0]), int(d_seg.shape[1])
-        out_i = self.buf('segm', (H, W), torch.int32) if lut_i is not None else None
+        if lut_i is not None and out_i is None:
+            out_i = self.buf('segm', (H, W), torch.int32)
         K = int(lut_p.shape[1]) if lut_p is not None else 0
         out_p = self.buf('segm_soft', (H, W, K), torch.float64) if lut_p is not None else None
         self._ck(lib.isb_gather(_lib.ptr(d_seg), C.c_longlong(H * W), _lib.ptr(lut_i), _lib.ptr(lut_p), K, _lib.ptr(out_i),

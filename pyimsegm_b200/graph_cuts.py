@@ -327,13 +327,33 @@ def _edge_mode(edge_type):
     return EDGE_MODES.get(edge_type, EDGE_MODES[''])
 
 
-def _device_graph(eng, segments):
-    """label map -> (device labels, nb, device edges, E, device centres)"""
-    segments = np.asarray(segments)
+def _device_energies(eng, segments, proba, edge_type, edge_cost, pairwise):
+    """label map [H, W] + class probabilities [>= nb, K] -> (device edges, E, what :meth:`~.engine.Engine.gc_energies` returns)"""
     nb = int(segments.max()) + 1
+    if len(proba) < nb:
+        raise ValueError('max vertex %i exceed size of proba %r' % (nb - 1, proba.shape))
+    mode = _edge_mode(edge_type)
     d_seg = eng.to_device(segments.astype(np.int32, copy=False), 'seg_in')
     d_edges, E = device_adjacency(eng, d_seg, nb)
-    return d_seg, nb, d_edges, E
+    d_proba = eng.to_device(proba, 'proba')
+    centres = None
+    if mode[1]:
+        _, centres, _ = eng.segment_stats(None, d_seg, nb, (), want_centres=True)
+    return d_edges, E, eng.gc_energies(d_proba, d_edges, E, None, centres, mode, float(edge_cost), pairwise)
+
+
+def device_graphcut(eng, res, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, edge_cap):
+    """graph-cut tail of the device pipelines over the label map ``res.d_seg`` and its centroids ``res.d_centres``: adjacency,
+    energies, alpha-expansion (all asynchronous).  ``nb`` may be an upper bound of the label count when ``d_n_nodes`` (device
+    scalar) carries the real one.  Returns (class per label [nb] device, n_edges device int32[1]); the result only holds when the
+    table of ``edge_cap`` rows took every edge, see :func:`~.engine.edges_fit`"""
+    K = int(d_proba.shape[1])
+    pairwise = compute_pairwise_cost(gc_regul, (nb, K))
+    d_edges, d_n_edges, _ = eng.adjacency(res.d_seg, nb, edge_cap)
+    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, edge_cap, d_n_edges, res.d_centres, _edge_mode(gc_edge_type), 1.0,
+                                                       pairwise, d_n_nodes=d_n_nodes)
+    d_labels, _, _ = eng.alpha_expansion(nb, K, edge_cap, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, -1, d_n_nodes=d_n_nodes)
+    return d_labels, d_n_edges
 
 
 def compute_edge_weights(segments, image=None, features=None, proba=None, edge_type=''):
@@ -374,17 +394,9 @@ def compute_edge_weights(segments, image=None, features=None, proba=None, edge_t
         return edges, weights
     if segments.ndim == 3:
         return _edge_weights_volume(eng, segments, proba, edge_type)
-    mode = _edge_mode(edge_type)
-    d_seg, nb, d_edges, E = _device_graph(eng, segments)
     K = 1 if proba is None else int(np.asarray(proba).shape[1])
-    p = np.ones((nb, K)) if proba is None else np.ascontiguousarray(proba, dtype=np.float64)
-    if len(p) < nb:
-        raise ValueError('max vertex %i exceed size of proba %r' % (nb - 1, p.shape))
-    d_proba = eng.to_device(p, 'proba')
-    centres = None
-    if mode[1]:
-        _, centres, _ = eng.segment_stats(None, d_seg, nb, (), want_centres=True)
-    _, edge_w, _, _, _ = eng.gc_energies(d_proba, d_edges, E, None, centres, mode, 1.0, np.zeros((K, K)))
+    p = np.ones((int(segments.max()) + 1, K)) if proba is None else np.ascontiguousarray(proba, dtype=np.float64)
+    d_edges, E, (_, edge_w, _, _, _) = _device_energies(eng, segments, p, edge_type, 1.0, np.zeros((K, K)))
     edges = eng.to_host(d_edges[:E]).copy() if E else np.zeros((0, 2), dtype=np.int32)
     weights = eng.to_host(edge_w[:E]).copy() if E else np.zeros(0)
     return edges, weights
@@ -396,13 +408,7 @@ def _edge_weights_volume(eng, segments, proba, edge_type):
     _edge_mode(edge_type)     # validates the name
     nb = int(segments.max()) + 1
     d_seg = eng.to_device(segments.astype(np.int32, copy=False), 'seg_in3d')
-    cap = None
-    while True:
-        d_edges, d_n, cap, d_centres = eng.graph3d(d_seg, nb, cap)
-        E = int(eng.to_host(d_n)[0])
-        if E <= cap:
-            break
-        cap = 2 * E
+    E, (d_edges, _, _, d_centres) = eng.edge_table(lambda cap: eng.graph3d(d_seg, nb, cap), nb, ndim=3)
     edges = eng.to_host(d_edges[:E]).copy() if E else np.zeros((0, 2), dtype=np.int32)
     if not E:
         return edges, np.zeros(0)
@@ -446,16 +452,8 @@ def segment_graph_cut_general(segments, proba, image=None, features=None, gc_reg
         unary_cost = compute_unary_cost(proba)
         graph_labels = cut_general_graph(edges, edge_weights, unary_cost, pairwise_cost, n_iter=-1)
     else:
-        mode = _edge_mode(edge_type)
-        d_seg, nb, d_edges, E = _device_graph(eng, segments)
-        if len(proba) < nb:
-            raise ValueError('max vertex %i exceed size of proba %r' % (nb - 1, proba.shape))
-        d_proba = eng.to_device(proba, 'proba')
-        centres = None
-        if mode[1]:
-            _, centres, _ = eng.segment_stats(None, d_seg, nb, (), want_centres=True)
-        unary, edge_w, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, E, None, centres, mode, float(edge_cost),
-                                                                    pairwise_cost)
+        d_edges, E, (unary, edge_w, unary_i, edge_wi, smooth_i) = _device_energies(eng, segments, proba, edge_type, edge_cost,
+                                                                                    pairwise_cost)
         labels, _, _ = eng.alpha_expansion(len(proba), proba.shape[1], E, None, d_edges, edge_wi, unary_i, smooth_i, -1)
         graph_labels = eng.to_host(labels).copy()
         if debug_visual is not None:

@@ -20,9 +20,8 @@ import numpy as np
 
 from .class_models import CompiledModel, compile_model
 from .descriptors import FEATURES_SET_COLOR, compute_selected_features_img2d, flags_are_native, native_feature_layout
-from .engine import get_engine
-from .graph_cuts import (_edge_mode, compute_pairwise_cost, device_gmm_applicable, estim_class_model,
-                         segment_graph_cut_general)
+from .engine import edge_capacity, edges_fit, get_engine
+from .graph_cuts import device_gmm_applicable, estim_class_model, segment_graph_cut_general
 from .superpixels import _as_rgb_like, _supported_dtype, slic_params
 
 #: basic features extracted from superpixels (reference pipelines.py:35)
@@ -90,8 +89,6 @@ def compute_color2d_superpixels_features(image, dict_features, sp_size=30, sp_re
         slic = eng.to_host(res.d_seg).astype(np.int64)
         features = eng.to_host(res.d_feat[:nb]).copy()
     else:
-        if sp_regul <= 0.:
-            raise ValueError('slic. regularisation must be positive')
         from .superpixels import segment_slic_img2d
         slic = segment_slic_img2d(image, sp_size=sp_size, relative_compact=sp_regul)
         features, _ = compute_selected_features_img2d(image, slic, dict_features)
@@ -99,30 +96,9 @@ def compute_color2d_superpixels_features(image, dict_features, sp_size=30, sp_re
     return slic, features
 
 
-def _device_graphcut(eng, res, nb, d_proba, K, gc_regul, gc_edge_type, d_n_nodes=None, want_soft=True, edge_cap=None):
-    """device tail of the pipeline: adjacency, energies, alpha-expansion, LUT gathers (all asynchronous).
-    ``nb`` may be an upper bound of the label count when ``d_n_nodes`` (device scalar) carries the real one.
-    Returns (d_labels, d_segm, d_soft, d_n_edges, edge_cap)."""
-    pairwise = compute_pairwise_cost(gc_regul, (nb, K))
-    d_edges, d_n_edges, edge_cap = eng.adjacency(res.d_seg, nb, edge_cap)
-    mode = _edge_mode(gc_edge_type)
-    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, edge_cap, d_n_edges, res.d_centres, mode, 1.0, pairwise,
-                                                       d_n_nodes=d_n_nodes)
-    d_labels, _, _ = eng.alpha_expansion(nb, K, edge_cap, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, -1, d_n_nodes=d_n_nodes)
-    d_segm, d_soft = eng.gather(res.d_seg, d_labels, d_proba if want_soft else None)
-    return d_labels, d_segm, d_soft, d_n_edges, edge_cap
-
-
 def _argmin_labels_device(eng, proba):
     graph_labels = np.argmin(np.abs(-np.log(np.clip(proba, 0.01, 0.99))), axis=-1).astype(np.int32)
     return eng.to_device(graph_labels, 'gc_labels_in')
-
-
-#: start the download of segm_soft (it only needs the class probabilities) on a side stream while the graph is cut
-EARLY_SOFT_DOWNLOAD = True
-
-#: initial capacity of the device edge table, in edges per (upper bound of) superpixel; grown x4 on overflow
-EDGE_CAP_PER_NODE = [8]
 
 
 #: replay the device part of the path as CUDA graphs once a configuration has been seen twice (the ~70 kernel launches of an image
@@ -151,7 +127,7 @@ def _graph_call(eng, key, fn):
         with torch.cuda.graph(graph, stream=side):
             out = fn()
         cur.wait_stream(side)
-        eng.graphs_captured = getattr(eng, 'graphs_captured', 0) + 1      # from now on the engine never frees a buffer it outgrows
+        eng.graphs_captured += 1      # from now on the engine never frees a buffer it outgrows
         entry = _GRAPHS[key] = (graph, out, int(eng.lib.isb_launch_count() - n0))
     graph, out, n_kernels = entry
     graph.replay()
@@ -175,85 +151,70 @@ def _compiled_model(model, dict_features):
     return cm
 
 
-def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, soft_sink=None):
+def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, early_soft=False):
     """the whole hot path on the device.  ``model`` is either ('fit', nb_classes, use_scaler, max_iter) -> the default
     GMM is fitted on the GPU and NOTHING syncs with the host until the results are ready; or a
     :class:`~.class_models.CompiledModel` -> a caller-fitted model evaluated on the device, again without a sync; or a callable
     proba_fn(features) -> one round trip (features down, probabilities up) as in the reference.
-    ``soft_sink(d_seg, d_proba)``: the caller takes ``segm_soft = proba[slic]`` itself as soon as the probabilities exist
-    (it does not depend on the graph cut) -- then ``d_soft`` is returned as None.
     With a device-fitted or compiled model and colour features the two halves -- image -> class probabilities, probabilities -> cut
     and LUT gathers -- are CUDA-graph replays (:func:`_graph_call`); the image then has to sit in one of the engine's cached buffers.
-    Returns (d_segm, d_soft, check): ``check`` is None or (d_n_edges, edge_cap) still to be verified by the caller."""
+    Returns (d_segm, soft, check): ``soft`` is the device segm_soft, or with ``early_soft`` and a graph cut the (pinned host tensor,
+    event) of :meth:`~.engine.Engine.early_soft`; ``check`` is None or (d_n_edges, edge_cap) still to be verified by the caller
+    (:func:`~.engine.edges_fit`)."""
+    from . import graph_cuts
     no_cut = (not isinstance(gc_regul, (list, np.ndarray))) and gc_regul <= 0
-    if isinstance(model, (tuple, CompiledModel)):
-        from . import graph_cuts
-        if not hasattr(image, 'is_cuda'):
-            image = eng.to_device(_supported_dtype(_as_rgb_like(np.asarray(image))), 'image')
-        graphable = (USE_CUDA_GRAPHS and not no_cut and all(k == 'color' for k in dict_features) and flags_are_native(dict_features))
-        if isinstance(model, CompiledModel):
-            nb_classes, model_key = model.n_classes, ('compiled', model.digest)
+    if not hasattr(image, 'is_cuda'):
+        image = eng.to_device(_supported_dtype(_as_rgb_like(np.asarray(image))), 'image')
+    on_device = isinstance(model, (tuple, CompiledModel))
+    graphable = (on_device and USE_CUDA_GRAPHS and not no_cut and all(k == 'color' for k in dict_features)
+                 and flags_are_native(dict_features))
+    if isinstance(model, CompiledModel):
+        model_key = ('compiled', model.digest)
 
-            def first_half():
-                res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
-                return res, eng.class_model_predict(res.d_feat, model, d_n=res.d_n_labels)
-        else:
-            _, nb_classes, use_scaler, max_iter = model
-            model_key = model
-            n_init = max(1, int(np.sqrt(max_iter)))
-            graphable = graphable and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES
+        def predict(res):
+            return eng.class_model_predict(res.d_feat, model, d_n=res.d_n_labels)
+    elif on_device:
+        _, nb_classes, use_scaler, max_iter = model
+        model_key = model
+        n_init = max(1, int(np.sqrt(max_iter)))
+        graphable = graphable and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES
 
-            def first_half():
-                res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
-                d_proba, _ = eng.gmm_fit_predict(res.d_feat, nb_classes, n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED,
-                                                 d_n=res.d_n_labels)
-                return res, d_proba
+        def predict(res):
+            return eng.gmm_fit_predict(res.d_feat, nb_classes, n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED, d_n=res.d_n_labels)[0]
+
+    proba = None
+    if on_device:
+        def first_half():
+            res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
+            return res, predict(res)
 
         key1 = ('probabilities', id(eng), image.data_ptr(), tuple(image.shape), str(image.dtype), model_key, _features_key(dict_features),
                 sp_size, sp_regul)
         res, d_proba = _graph_call(eng, key1, first_half) if graphable else first_half()
-        if no_cut:
-            nb = int(eng.to_host(res.d_n_labels)[0])
-            d_labels = _argmin_labels_device(eng, eng.to_host(d_proba[:nb]))
-            return eng.gather(res.d_seg, d_labels, d_proba) + (None, )
-        cap = max(64, EDGE_CAP_PER_NODE[0] * res.nb_bound)
-        if soft_sink is not None:
-            soft_sink(res.d_seg, d_proba)
-
-        def second_half():
-            return _device_graphcut(eng, res, res.nb_bound, d_proba, nb_classes, gc_regul, gc_edge_type, d_n_nodes=res.d_n_labels,
-                                    want_soft=soft_sink is None, edge_cap=cap)
-
-        key2 = ('cut', id(eng), res.d_seg.data_ptr(), d_proba.data_ptr(), res.d_centres.data_ptr(), res.shape, res.nb_bound, nb_classes,
-                float(gc_regul) if graphable else None, gc_edge_type, cap, soft_sink is None)
-        _, d_segm, d_soft, d_n_edges, cap = _graph_call(eng, key2, second_half) if graphable else second_half()
-        return d_segm, d_soft, (d_n_edges, cap)
-    res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
-    nb = int(eng.to_host(res.d_n_labels)[0])
-    features = eng.to_host(res.d_feat[:nb]).copy()
-    features[np.isnan(features)] = 0
-    proba = np.ascontiguousarray(model(features), dtype=np.float64)
-    logging.debug('list of probabilities: %r', proba.shape)
-    d_proba = eng.to_device(proba, 'proba')
+        nb, d_n_nodes = res.nb_bound, res.d_n_labels
+    else:
+        res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
+        nb, d_n_nodes = int(eng.to_host(res.d_n_labels)[0]), None
+        features = eng.to_host(res.d_feat[:nb]).copy()
+        features[np.isnan(features)] = 0
+        proba = np.ascontiguousarray(model(features), dtype=np.float64)
+        logging.debug('list of probabilities: %r', proba.shape)
+        d_proba = eng.to_device(proba, 'proba')
     if no_cut:
+        if proba is None:
+            proba = eng.to_host(d_proba[:int(eng.to_host(d_n_nodes)[0])])
         return eng.gather(res.d_seg, _argmin_labels_device(eng, proba), d_proba) + (None, )
-    cap = max(64, EDGE_CAP_PER_NODE[0] * nb)
-    if soft_sink is not None:
-        soft_sink(res.d_seg, d_proba)
-    _, d_segm, d_soft, d_n_edges, cap = _device_graphcut(eng, res, nb, d_proba, proba.shape[1], gc_regul, gc_edge_type,
-                                                         want_soft=soft_sink is None, edge_cap=cap)
-    return d_segm, d_soft, (d_n_edges, cap)
+    cap = edge_capacity(nb)
+    soft = eng.early_soft(res.d_seg, d_proba) if early_soft else None
 
+    def second_half():
+        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, cap)
+        return eng.gather(res.d_seg, d_labels, None if early_soft else d_proba) + (d_n_edges, )
 
-def _download_results(eng, tensors):
-    """D2H into pinned buffers with ONE synchronisation; returns numpy views"""
-    outs = []
-    for t in tensors:
-        h = eng.pinned_empty(t.shape, t.dtype)
-        h.copy_(t, non_blocking=True)
-        outs.append(h)
-    eng.torch.cuda.current_stream().synchronize()
-    return [h.numpy() for h in outs]
+    key2 = ('cut', id(eng), res.d_seg.data_ptr(), d_proba.data_ptr(), res.d_centres.data_ptr(), res.shape, res.nb_bound,
+            int(d_proba.shape[1]), float(gc_regul) if graphable else None, gc_edge_type, cap, not early_soft)
+    d_segm, d_soft, d_n_edges = _graph_call(eng, key2, second_half) if graphable else second_half()
+    return d_segm, (soft if early_soft else d_soft), (d_n_edges, cap)
 
 
 def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, debug_visual, classes=None):
@@ -281,42 +242,20 @@ def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_t
         if classes is not None:
             graph_labels = classes[graph_labels]
         return graph_labels[slic], segm_soft
-    torch = eng.torch
-    early = {}
-
-    def soft_sink(d_seg, d_proba):
-        # segm_soft = proba[slic] needs only the class probabilities: its gather and its (large) download run on a side stream
-        # while the main stream builds and cuts the graph
-        side = eng.side_stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            _, d_soft = eng.gather(d_seg, None, d_proba)
-            host = eng.pinned_empty(d_soft.shape, d_soft.dtype)
-            host.copy_(d_soft, non_blocking=True)
-            event = torch.cuda.Event()
-            event.record(side)
-        early['host'], early['event'] = host, event
-
     while True:
-        early.clear()
-        d_segm, d_soft, check = _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type,
-                                              soft_sink=soft_sink if EARLY_SOFT_DOWNLOAD else None)
-        if check is None or not early:   # no graph cut / overlap switched off: both gathers were done at the end of the main stream
-            if check is not None:
-                segm, soft, n_edges = _download_results(eng, (d_segm, d_soft, check[0]))
-                if int(n_edges[0]) <= check[1]:
-                    break
-                EDGE_CAP_PER_NODE[0] *= 4
-                continue
-            segm, soft = _download_results(eng, (d_segm, d_soft))
+        d_segm, soft, check = _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, early_soft=True)
+        if check is None:   # no graph cut: both gathers were done at the end of the main stream
+            (segm, soft), done = eng.download((d_segm, soft))
+            done.synchronize()
             break
-        segm, n_edges = _download_results(eng, (d_segm, check[0]))
-        early['event'].synchronize()
-        soft = early['host'].numpy()
+        (segm, n_edges), done = eng.download((d_segm, check[0]))
+        done.synchronize()
+        soft, soft_done = soft
+        soft_done.synchronize()
         # the next call reuses the buffers the side stream has just read: nothing of this call is left in flight
-        if int(n_edges[0]) <= check[1]:
+        if edges_fit(n_edges[0], check[1]):
             break
-        EDGE_CAP_PER_NODE[0] *= 4  # the device edge table overflowed (> 8 edges per superpixel on average): redo larger
+    segm, soft = segm.numpy(), soft.numpy()
     if classes is not None:
         segm = np.asarray(classes)[segm]
     return segm, soft
@@ -334,6 +273,31 @@ def _batch_engines(nb_streams):
     while len(pool) < nb_streams:
         pool.append((Engine(dev), torch.cuda.Stream(device=dev)))
     return pool[:nb_streams]
+
+
+def _over_streams(list_images, nb_streams, max_in_flight, launch, finish):
+    """``launch(eng, image) -> (pinned host tensors, event, extra)`` for consecutive images alternating over ``nb_streams`` CUDA
+    streams with their own engines, at most ``max_in_flight`` images ahead of ``finish(index, host tensors, extra)``, which runs in
+    input order once the event has completed: returns what ``finish`` returned, per image"""
+    engines = _batch_engines(nb_streams)
+    torch = engines[0][0].torch
+    results, pending = [None] * len(list_images), []
+
+    def flush(limit):
+        while len(pending) > limit:
+            idx, (hosts, done, extra) = pending.pop(0)
+            done.synchronize()
+            results[idx] = finish(idx, hosts, extra)
+
+    caller_stream = torch.cuda.current_stream()
+    for i, image in enumerate(list_images):
+        eng, stream = engines[i % nb_streams]
+        stream.wait_stream(caller_stream)
+        with torch.cuda.stream(stream):
+            pending.append((i, launch(eng, np.asarray(image))))
+        flush(max_in_flight)
+    flush(0)
+    return results
 
 
 def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIMPLE, sp_size=30, sp_regul=0.2, use_scaler=True,
@@ -361,42 +325,19 @@ def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIM
     else:
         model = _compiled_model(model_pipeline, dict_features) or model_pipeline.predict_proba
     classes = getattr(model_pipeline, 'classes_', None)
-    engines = _batch_engines(nb_streams)
-    torch = engines[0][0].torch
-    results = [None] * len(list_images)
-    pending = []   # (index, pinned tensors, event, check)
 
-    def _finish(item):
-        idx, hosts, event, check = item
-        event.synchronize()
-        segm, soft = hosts[0].numpy(), hosts[1].numpy()
-        if check is not None and int(hosts[2].numpy()[0]) > check[1]:
-            EDGE_CAP_PER_NODE[0] *= 4  # edge table overflow (not seen in practice): redo this image through the single-image path
-            segm, soft = _segment(list_images[idx], model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, None, classes=classes)
-        elif classes is not None:
-            segm = np.asarray(classes)[segm]
-        results[idx] = (segm, soft)
+    def launch(eng, image):
+        d_segm, d_soft, check = _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)
+        return eng.download((d_segm, d_soft) + ((check[0], ) if check is not None else ())) + (check, )
 
-    caller_stream = torch.cuda.current_stream()
-    for i, image in enumerate(list_images):
-        eng, stream = engines[i % nb_streams]
-        stream.wait_stream(caller_stream)
-        with torch.cuda.stream(stream):
-            d_segm, d_soft, check = _run_resident(eng, np.asarray(image), model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)
-            tensors = (d_segm, d_soft) + ((check[0], ) if check is not None else ())
-            hosts = []
-            for t in tensors:
-                h = eng.pinned_empty(t.shape, t.dtype)
-                h.copy_(t, non_blocking=True)
-                hosts.append(h)
-            event = torch.cuda.Event()
-            event.record(stream)
-        pending.append((i, hosts, event, check))
-        while len(pending) > max_in_flight:
-            _finish(pending.pop(0))
-    while pending:
-        _finish(pending.pop(0))
-    return results
+    def finish(idx, hosts, check):
+        if check is not None and not edges_fit(hosts[2][0], check[1]):
+            # the edge table overflowed: redo this image through the single-image path
+            return _segment(list_images[idx], model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, None, classes=classes)
+        segm = hosts[0].numpy()
+        return (segm if classes is None else np.asarray(classes)[segm]), hosts[1].numpy()
+
+    return _over_streams(list_images, nb_streams, max_in_flight, launch, finish)
 
 
 def compute_features_batch(list_images, dict_features, sp_size=30, sp_regul=0.2, nb_streams=3, max_in_flight=6):
@@ -408,34 +349,16 @@ def compute_features_batch(list_images, dict_features, sp_size=30, sp_regul=0.2,
     """
     if not flags_are_native(dict_features) or any(np.ndim(im) != 3 for im in list_images):
         return [compute_color2d_superpixels_features(im, dict_features, sp_size=sp_size, sp_regul=sp_regul)[1] for im in list_images]
-    engines = _batch_engines(nb_streams)
-    torch = engines[0][0].torch
-    results, pending = [None] * len(list_images), []
+    def launch(eng, image):
+        res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
+        return eng.download((res.d_feat, res.d_n_labels)) + (None, )
 
-    def _finish(item):
-        idx, h_feat, h_n, event = item
-        event.synchronize()
-        features = h_feat.numpy()[:int(h_n.numpy()[0])].copy()
+    def finish(idx, hosts, _):
+        features = hosts[0].numpy()[:int(hosts[1][0])].copy()
         features[np.isnan(features)] = 0
-        results[idx] = features
+        return features
 
-    caller_stream = torch.cuda.current_stream()
-    for i, image in enumerate(list_images):
-        eng, stream = engines[i % nb_streams]
-        stream.wait_stream(caller_stream)
-        with torch.cuda.stream(stream):
-            res = _device_slic_features(eng, np.asarray(image), dict_features, sp_size, sp_regul)
-            h_feat, h_n = eng.pinned_empty(res.d_feat.shape, res.d_feat.dtype), eng.pinned_empty((1, ), torch.int32)
-            h_feat.copy_(res.d_feat, non_blocking=True)
-            h_n.copy_(res.d_n_labels, non_blocking=True)
-            event = torch.cuda.Event()
-            event.record(stream)
-        pending.append((i, h_feat, h_n, event))
-        while len(pending) > max_in_flight:
-            _finish(pending.pop(0))
-    while pending:
-        _finish(pending.pop(0))
-    return results
+    return _over_streams(list_images, nb_streams, max_in_flight, launch, finish)
 
 
 def wrapper_compute_color2d_slic_features_labels(img_annot, sp_size, sp_regul, dict_features, label_purity):
@@ -502,7 +425,10 @@ def segment_resident(d_image, model, dict_features, sp_size=30, sp_regul=0.2, gc
     there: returns (segm int32 [H, W], segm_soft float64 [H, W, K]) device tensors.  ``model`` is a callable
     proba_fn(features), a fitted model (or its bound ``predict_proba``) -- evaluated on the device when
     :func:`~.class_models.compile_model` supports it -- or ('fit', nb_classes, use_scaler, max_iter) for the GPU-fitted default GMM.
-    The indices in ``segm`` are not mapped through the model's ``classes_``. """
+    The indices in ``segm`` are not mapped through the model's ``classes_``.
+    Nothing here waits for the device, so the edge count of the graph cut is not checked against its table as the host-facing
+    pipelines do: after the connectivity pass every superpixel is connected, the region graph of a 2-D map is planar with at most
+    3N - 6 edges, and the table holds 8 per node of an upper bound of N. """
     if not isinstance(model, (tuple, CompiledModel)):
         fitted = model.__self__ if getattr(model, '__name__', None) == 'predict_proba' and hasattr(model, '__self__') else model
         model = _compiled_model(fitted, dict_features) or (model if callable(model) else model.predict_proba)

@@ -128,13 +128,8 @@ def get_segment_diffs_3d_conn6(grid):
 
 def device_adjacency(eng, d_seg, nb):
     """(edges [E,2] int32 host array) of a device label map with labels in [0, nb); grows the table on overflow"""
-    cap = None
-    while True:
-        edges, n_edges, cap = eng.adjacency(d_seg, nb, cap)
-        E = int(eng.to_host(n_edges)[0])
-        if E <= cap:
-            return edges, E
-        cap *= 4
+    E, (edges, _, _) = eng.edge_table(lambda cap: eng.adjacency(d_seg, nb, cap), nb)
+    return edges, E
 
 
 def make_graph_segm_connect_grid2d_conn4(grid):

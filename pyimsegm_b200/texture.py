@@ -12,7 +12,7 @@ import itertools
 import numpy as np
 
 from . import _lib
-from .engine import FLAG_BITS, get_engine
+from .engine import flag_bits, get_engine
 
 #: sigma of the background that is subtracted before filtering (descriptors.py:1078)
 BACKGROUND_SIGMA = 150
@@ -135,10 +135,8 @@ def device_lm_features(eng, d_img, d_seg, nb, flags, bank_type='normal', feat=No
     """run isb_lm_texture on device buffers; returns (feat tensor [nb, ld], names, n_cols)"""
     torch, lib = eng.torch, eng.lib
     names, d_w, NP, orient, n_batt = _device_bank(bank_type)
-    bits = 0
-    for f in flags:
-        bits |= FLAG_BITS[f]
-    ncol = n_batt * 3 * bin(bits).count('1')
+    bits, cols = flag_bits(flags)
+    ncol = n_batt * cols
     if feat is None:
         feat = eng.buf('feat_lm', (nb, ncol), torch.float64)
     H, W = int(d_seg.shape[0]), int(d_seg.shape[1])
@@ -146,7 +144,7 @@ def device_lm_features(eng, d_img, d_seg, nb, flags, bank_type='normal', feat=No
     d_wbg = eng.const_device(w_bg, 'lm_bg_w')
     wsb = lib.isb_lm_workspace_bytes(H, W, int(nb), n_batt)
     ws = eng.buf('ws_lm', (wsb,), torch.uint8)
-    code = _lib.DTYPE_CODES[str(d_img.dtype).replace('torch.', '')]
+    code = _lib.dtype_code(d_img.dtype)
     _lib.check(lib.isb_lm_texture(_lib.ptr(d_img), code, _lib.ptr(d_seg), H, W, int(nb), _lib.ptr(d_wbg), radius,
                                   mix.ctypes.data_as(C.POINTER(C.c_double)), _lib.ptr(d_w), NP, orient, n_batt, bits,
                                   _lib.ptr(feat), int(feat.shape[1]), int(col0), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))

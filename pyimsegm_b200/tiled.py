@@ -26,7 +26,7 @@ import logging
 import numpy as np
 
 from . import _lib
-from .engine import FLAG_BITS, gaussian_half_kernel, get_engine, slic_seed_grid
+from .engine import edge_capacity, edges_fit, flag_bits, gaussian_half_kernel, get_engine, slic_seed_grid
 
 OP_SUM_I64, OP_MAX_I64, OP_MIN_F64, OP_MAX_F64, OP_SUM_F64 = 0, 1, 2, 3, 4
 
@@ -126,13 +126,10 @@ def slic_tiled(image, n_segments, compactness, sigma=1.0, max_iter=10, slic_zero
     if image.ndim == 2:
         image = image[:, :, None]
     H, W, Cn = int(image.shape[0]), int(image.shape[1]), int(image.shape[2])
-    code = _lib.DTYPE_CODES[str(image.dtype)]
+    code = _lib.dtype_code(image.dtype)
     itemsize = image.dtype.itemsize
     st = _lib.stream_ptr()
-    if sigma > 0:
-        w_half, radius = gaussian_half_kernel(sigma)
-    else:
-        w_half, radius = np.ones(1), 0
+    w_half, radius = gaussian_half_kernel(sigma)
     seeds, ty, tx = slic_seed_grid(H, W, n_segments)
     n_seeds = len(seeds)
     step = float(max(1, ty, tx))
@@ -230,15 +227,7 @@ def slic_tiled(image, n_segments, compactness, sigma=1.0, max_iter=10, slic_zero
     if not enforce_connectivity:
         res.d_seg = full
         return res
-    segment_size = 1 * H * W / n_segments
-    min_size, max_size = int(min_size_factor * segment_size), int(max_size_factor * segment_size)
-    cwsb = lib.isb_connectivity_workspace_bytes(H, W)
-    cws = eng.buf('ws_conn', (cwsb,), torch.uint8)
-    out = eng.buf('labels', (H, W), torch.int32)
-    n_labels = eng.buf('n_labels', (1,), torch.int32)
-    _lib.check(lib.isb_enforce_connectivity(_lib.ptr(full), H, W, min_size, max_size, _lib.ptr(out), _lib.ptr(n_labels), _lib.ptr(cws),
-                                            C.c_size_t(cwsb), st))
-    res.d_seg, res.d_n_labels = out, n_labels
+    res.d_seg, res.d_n_labels = eng.enforce_connectivity(full, n_segments, min_size_factor, max_size_factor)
     res.nb_bound = eng.slic_label_bound(H, W, n_segments, min_size_factor)
     return res
 
@@ -252,13 +241,11 @@ def color_stats_tiled(res, image_dtype, channels, flags, comm=None, eng=None, fe
     H, W = res.shape
     if channels != 3:
         raise ValueError('the colour statistics need a 3-channel image')
-    code = _lib.DTYPE_CODES[str(np.dtype(image_dtype))]
+    code = _lib.dtype_code(np.dtype(image_dtype))
     itemsize = np.dtype(image_dtype).itemsize
     nb = int(res.nb_bound)
     st = _lib.stream_ptr()
-    bits = 0
-    for f in flags:
-        bits |= FLAG_BITS[f]
+    bits, ncol = flag_bits(flags)
     acc = eng.buf('tb_acc', (nb, 6), torch.float64)
     iacc = eng.buf('tb_iacc', (nb, 3), torch.int64)
     acc.zero_()
@@ -286,7 +273,6 @@ def color_stats_tiled(res, image_dtype, channels, flags, comm=None, eng=None, fe
             _lib.check(lib.isb_segment_stats_deviation(img_ptr, code, seg_ptr, bd.own_hi - bd.own_lo, W, nb, _lib.ptr(acc), _lib.ptr(iacc),
                                                        _lib.ptr(meanf), _lib.ptr(var), st))
         comm.all_reduce(var, 'sum')
-    ncol = 3 * bin(bits).count('1')
     if feat is None:
         feat = eng.buf('feat', (nb, max(ncol, 1)), torch.float64)
     centres = eng.buf('centres', (nb, 2), torch.float64)
@@ -310,13 +296,11 @@ def texture_stats_tiled(res, image_dtype, flags, bank_type='normal', comm=None, 
     torch, lib = eng.torch, eng.lib
     comm = comm or default_comm()
     H, W = res.shape
-    code = _lib.DTYPE_CODES[str(np.dtype(image_dtype))]
+    code = _lib.dtype_code(np.dtype(image_dtype))
     itemsize = np.dtype(image_dtype).itemsize
     nb = int(res.nb_bound)
     st = _lib.stream_ptr()
-    bits = 0
-    for f in flags:
-        bits |= FLAG_BITS[f]
+    bits, cols = flag_bits(flags)
     _, d_w, NP, orient, n_batt = _device_bank(bank_type)
     w_bg, radius, mix = background_kernel()
     d_wbg = eng.const_device(w_bg, 'lm_bg_w')
@@ -339,7 +323,7 @@ def texture_stats_tiled(res, image_dtype, flags, bank_type='normal', comm=None, 
                                                  _lib.ptr(acc), _lib.ptr(counts), _lib.ptr(ws), C.c_size_t(wsb), st))
     comm.all_reduce(acc, 'sum')
     comm.all_reduce(counts, 'sum')
-    ncol = n_batt * 3 * bin(bits).count('1')
+    ncol = n_batt * cols
     if feat is None:
         feat = eng.buf('feat_lm', (nb, ncol), torch.float64)
     _lib.check(lib.isb_lm_texture_finish(nb, n_batt, bits, _lib.ptr(acc), _lib.ptr(counts), _lib.ptr(feat), int(feat.shape[1]), int(col0), st))
@@ -375,8 +359,6 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
     """
     from . import graph_cuts
     from .descriptors import flags_are_native, native_feature_layout
-    from .graph_cuts import compute_pairwise_cost
-    from .pipelines import EDGE_CAP_PER_NODE, _edge_mode
     from .superpixels import _as_rgb_like, _supported_dtype, slic_params
     if sp_regul <= 0.:
         raise ValueError('slic. regularisation must be positive')
@@ -387,15 +369,13 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
                                   % dict_features)
     margin = LM_ROW_MARGIN if any(k.startswith('tLM') for k, _, _, _ in layout) else 0
     eng = get_engine()
-    torch, lib = eng.torch, eng.lib
+    torch = eng.torch
     comm = comm or default_comm()
     image = _supported_dtype(_as_rgb_like(np.asarray(image)))
     H, W = int(image.shape[0]), int(image.shape[1])
     n_seg, compact = slic_params((H, W), sp_size, sp_regul)
     if n_seg < 1:
         raise ValueError('superpixel size %r is larger than the image %r' % (sp_size, tuple(image.shape)))
-    st = _lib.stream_ptr()
-    K = int(nb_classes)
     n_init = max(1, int(np.sqrt(max_iter)))
     force_whole, redo_front = False, True
     while True:
@@ -403,60 +383,30 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
             res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
                              force_whole=force_whole, raw_margin=margin)
             features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
-            nb = int(res.nb_bound)
-            d_proba, _ = eng.gmm_fit_predict(res.d_feat, K, n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED, d_n=res.d_n_labels)
+            d_proba, _ = eng.gmm_fit_predict(res.d_feat, int(nb_classes), n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED,
+                                             d_n=res.d_n_labels)
             redo_front = False
         lo, hi = res.bands[res.local[0]].own_lo, res.bands[res.local[-1]].own_hi
-        rows = hi - lo
-        seg_ptr = C.c_void_p(res.d_seg.data_ptr() + lo * W * 4)
-        # segm_soft = proba[slic] of the owned rows needs only the class probabilities: its gather and its (large) download run on
-        # a side stream while the main stream builds and cuts the graph
-        h_soft = soft_done = None
-        if want_soft:
-            side = eng.side_stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                d_soft = eng.buf('segm_soft', (rows, W, K), torch.float64)
-                _lib.check(lib.isb_gather(seg_ptr, C.c_longlong(rows * W), None, _lib.ptr(d_proba), K, None, _lib.ptr(d_soft),
-                                          _lib.stream_ptr()))
-                h_soft = eng.pinned_empty(d_soft.shape, d_soft.dtype)
-                h_soft.copy_(d_soft, non_blocking=True)
-                soft_done = torch.cuda.Event()
-                soft_done.record(side)
-        cap = max(64, EDGE_CAP_PER_NODE[0] * nb)
-        pairwise = compute_pairwise_cost(gc_regul, (nb, K))
-        d_edges, d_n_edges, cap = eng.adjacency(res.d_seg, nb, cap)
-        _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, cap, d_n_edges, res.d_centres, _edge_mode(gc_edge_type), 1.0,
-                                                           pairwise, d_n_nodes=res.d_n_labels)
-        d_labels, _, _ = eng.alpha_expansion(nb, K, cap, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, -1, d_n_nodes=res.d_n_labels)
+        soft = eng.early_soft(res.d_seg[lo:hi], d_proba) if want_soft else None
+        cap = edge_capacity(res.nb_bound)
+        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res, res.nb_bound, d_proba, gc_regul, gc_edge_type, res.d_n_labels, cap)
         # 5) LUT gather of the owned rows
-        if gather_segm:
-            d_full = eng.buf('segm', (H, W), torch.int32)
-            d_segm = d_full[lo:hi]
-        else:
-            d_segm = eng.buf('segm', (rows, W), torch.int32)
-        _lib.check(lib.isb_gather(seg_ptr, C.c_longlong(rows * W), _lib.ptr(d_labels), None, K, _lib.ptr(d_segm), None, st))
+        d_full = eng.buf('segm', (H, W), torch.int32) if gather_segm else None
+        d_segm, _ = eng.gather(res.d_seg[lo:hi], d_labels, out_i=d_full[lo:hi] if gather_segm else None)
         if gather_segm and comm.world > 1:
             for r in range(comm.world):
                 blo = res.bands[r * bands_per_rank].own_lo
                 bhi = res.bands[(r + 1) * bands_per_rank - 1].own_hi
                 comm.broadcast(d_full[blo:bhi], r)
-        outs = [d_full if gather_segm else d_segm, d_n_edges, res.d_err]
-        host = []
-        for t in outs:
-            h = eng.pinned_empty(t.shape, t.dtype)
-            h.copy_(t, non_blocking=True)
-            host.append(h)
-        torch.cuda.current_stream().synchronize()
-        if soft_done is not None:
-            soft_done.synchronize()
-        host.append(h_soft)
-        if int(host[2][0]) != 0 and not force_whole:
+        (h_segm, n_edges, err), done = eng.download((d_full if gather_segm else d_segm, d_n_edges, res.d_err))
+        done.synchronize()
+        if soft is not None:
+            soft[1].synchronize()
+        if int(err[0]) != 0 and not force_whole:
             # orphan pixels beyond the halo (see slic_tiled): same answer on every rank, so every rank takes this branch
             logging.warning('banded SLIC met orphan pixels beyond the halo, redoing the sweeps on the whole image on every GPU')
             force_whole = redo_front = True
             continue
-        if int(host[1][0]) <= cap:
+        if edges_fit(n_edges[0], cap):
             break
-        EDGE_CAP_PER_NODE[0] *= 4
-    return host[0].numpy(), (host[3].numpy() if want_soft else None), (lo, hi)
+    return h_segm.numpy(), (soft[0].numpy() if want_soft else None), (lo, hi)

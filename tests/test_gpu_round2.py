@@ -157,7 +157,7 @@ def test_config3_shaped_pipeline_with_a_shared_model(oracle):
 
 
 def test_cuda_graph_replay_equals_eager_launches():
-    """pipelines._run_resident_graph: the device part of the path captured once and replayed per image (batch API and
+    """pipelines._graph_call: the device part of the path captured once and replayed per image (batch API and
     segment_resident) must give exactly what the eager launches give, for every image of the batch"""
     from pyimsegm_b200 import pipelines as pl
     imgs = [synth_regions(200, 264, seed=s)[0] for s in (31, 32, 33, 34, 35)]
@@ -189,3 +189,40 @@ def test_graph_replay_survives_other_configurations_in_between():
     for segm, soft in runs[1:] + [again]:
         assert np.array_equal(segm, runs[0][0])
         np.testing.assert_allclose(soft, runs[0][1], rtol=1e-6, atol=1e-9)
+
+
+def test_edge_table_overflow_is_redone_with_a_larger_table():
+    """a device edge table too small for the region graph: the device counts cap + 1 edges and writes no row past cap, the host
+    grows the table and redoes the work.  With a first table of a quarter edge per node every path overflows at least once and
+    must give what it gives at the default capacity"""
+    from pyimsegm_b200 import engine, graph_cuts
+    from pyimsegm_b200 import pipelines as pl
+    from pyimsegm_b200.tiled import pipe_color2d_slic_features_model_graphcut_tiled
+    imgs = [synth_regions(320, 384, seed=s)[0] for s in (51, 52, 53)]
+    feats, kw = {'color': ['mean']}, dict(sp_size=12, sp_regul=0.2)
+    slic, _ = pl.compute_color2d_superpixels_features(imgs[0], feats, **kw)
+    assert slic.max() + 1 > 500         # well above the 64-row floor of the table
+    proba = np.random.RandomState(0).dirichlet(np.ones(3), slic.max() + 1)
+    calls = {
+        'single': lambda: [pl.pipe_color2d_slic_features_model_graphcut(imgs[0], 3, feats, **kw)],
+        'batch': lambda: pl.segment_images_batch(imgs, 3, feats, **kw),
+        'banded': lambda: [pipe_color2d_slic_features_model_graphcut_tiled(imgs[0], 3, feats, bands_per_rank=2, **kw)[:2]],
+        'edge_weights': lambda: [graph_cuts.compute_edge_weights(slic, proba=proba, edge_type='model')],
+    }
+    default = engine.EDGE_CAP_PER_NODE
+    try:
+        for name, call in calls.items():
+            engine.EDGE_CAP_PER_NODE = default
+            want = call()
+            engine.EDGE_CAP_PER_NODE = 0.25
+            got = call()
+            assert engine.EDGE_CAP_PER_NODE > 0.25, '%s: the table was never grown' % name
+            assert len(got) == len(want)
+            for (g0, g1), (w0, w1) in zip(got, want):
+                assert np.array_equal(g0, w0), name
+                if name == 'edge_weights':
+                    assert np.array_equal(g1, w1)
+                else:
+                    np.testing.assert_allclose(g1, w1, rtol=1e-6, atol=1e-9)   # the redo recomputes the colour statistics (atomics)
+    finally:
+        engine.EDGE_CAP_PER_NODE = default
