@@ -11,9 +11,9 @@
 //
 // The centroid update of the original is a raster-order SEQUENTIAL double sum per cluster; a tree/atomic
 // reduction changes the last ulp and flips exact ties (flat image regions tie all the time).  It is
-// reproduced exactly: one warp per cluster walks the cluster's window in raster order, ballots the member
-// pixels of each 32-wide chunk, compacts their colours into shared memory in lane (= raster) order, and three
-// lanes add them one at a time.  Coordinate sums are integers (exact in any order).
+// reproduced exactly: one CTA per cluster walks the cluster's member box in raster order, its gather warps ballot
+// the member pixels of each 32-wide chunk and compact their colours into shared memory in raster order, and three
+// lanes of an adder warp add them one at a time.  Coordinate sums are integers (exact in any order).
 //
 // Per sweep HBM traffic (algorithmic): read Lab 24 B/px + write label 4 B/px (assign); the update re-reads
 // labels and member colours through L2.
@@ -400,147 +400,203 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
     }
 }
 
-// centroid sums: one warp per cluster, raster-order sequential double adds (see header).
+// centroid sums: one CTA per cluster, raster-order sequential double adds (see header).
 // BAND: this GPU holds a row band of the image.  A cluster is summed by the band that owns the row of its centre (every
 // member lies within 2*step rows of the centre the assignment used, i.e. inside that band's slab -- checked, violations are
 // counted in xchg[6n]); the result goes to the exchange record xchg[6k..6k+5] = bits(cy, cx, c0, c1, c2), state (1 alive,
 // 2 died) and every other band leaves zeros there, so that an integer sum over the bands is an exact merge.
-// A warp's time is the length of its cluster's dependent chain, so the launch should be ONE wave: UWARPS warps per CTA and UBLOCKS CTAs
-// per SM give 132 x UWARPS x UBLOCKS resident warps on an H100 -- with 2 x 19 that is 5 016, enough for the ~5 000 clusters of a
-// 2048 x 2048 image at sp_size 29 (a second wave for the last few percent costs as much as the first).  The 48 registers this allows
-// spill a few words.
-constexpr int UWARPS = 2, UBLOCKS = 19;
-template <bool BAND>
-__global__ void __launch_bounds__(32 * UWARPS, UBLOCKS) k_update(KmState s, const double* __restrict__ lab, const int* __restrict__ labels,
-                                                                 long long* __restrict__ xchg)
+//
+// The member box is cut into strips of USTRIP chunks (a chunk = 32 pixels of one box row) in raster chunk order.  The UGATHER gather
+// warps share a strip, UCPW consecutive chunks each: they load the labels and ballot the members, the per-chunk member counts are
+// scanned across the gather warps, and only the member lanes load their colours and store them at their raster position in the
+// strip buffer.  The last warp is the adder: three of its lanes (one per channel) run the sequential chain over one buffer while
+// the gather warps fill the other.  Named barriers hand the buffers over (FULL: the strip is stored, EMPTY: its adds are done), so
+// neither side waits for a whole-CTA barrier.  A strip is a fixed number of chunks: a large box just takes more strips.
+// A CTA's time is mostly its adder's chain plus a few memory latencies (box, labels, colours of the first strip), so the kernel
+// wants many clusters in flight per SM: 3 gather warps, 12-chunk strips (19 KB of shared memory) and 9 CTAs per SM, which leave 56
+// registers -- the kernel fits them without spilling (at 10 CTAs it spills, and it was slower with 4 or 2 gather warps on H100).
+// CTAs take the clusters from the last to the first: k_assign has just streamed the image top to bottom, so the bottom rows are
+// still in L2 when the first CTAs need them, and the next k_assign finds the top rows there.
+constexpr int UGATHER = 3, UCPW = 4, USTRIP = UGATHER * UCPW;
+constexpr int UTHREADS = 32 * (UGATHER + 1), UBLOCKS = 9;
+// one channel row of a strip buffer: the members, the zero padding and one look-ahead group of the adds; the extra 4 words put
+// the three rows the adder lanes read at once on different banks
+constexpr int USTRIDE = 32 * USTRIP + 12;
+constexpr int UBAR_FULL = 1, UBAR_EMPTY = 3, UBAR_SCAN = 5;   // FULL and EMPTY: one barrier per buffer; 0 is __syncthreads
+
+// named barriers with immediate operands (ptxas then reserves only the ids in use); ID + b selects the barrier of buffer b
+template <int ID, int N> __device__ __forceinline__ void bar_sync(int b = 0)
 {
-    __shared__ double buf[UWARPS][3][72];   // two 32-pixel chunks + the zero padding + one look-ahead group
+    if (b) asm volatile("bar.sync %0, %1;" ::"n"(ID + 1), "n"(N) : "memory");
+    else asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+template <int ID, int N> __device__ __forceinline__ void bar_arrive(int b)
+{
+    if (b) asm volatile("bar.arrive %0, %1;" ::"n"(ID + 1), "n"(N) : "memory");
+    else asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+
+template <bool BAND>
+__global__ void __launch_bounds__(UTHREADS, UBLOCKS) k_update(KmState s, const double* __restrict__ lab, const int* __restrict__ labels,
+                                                              long long* __restrict__ xchg)
+{
+    __shared__ __align__(16) double buf[2][3][USTRIDE];
+    __shared__ int s_cnt[2][USTRIP];   // members per chunk of the strip in the buffer
+    __shared__ int s_tot[2];           // members of the strip in the buffer
+    __shared__ long long s_int[UGATHER][3];
+    __shared__ double s_acc[3];
+    __shared__ int4 s_box;
+    __shared__ int s_skip;
     const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
-    const int k = blockIdx.x * UWARPS + wl;
-    if (k >= s.n) return;
-    // the box of this cluster's members, gathered by k_assign (empty when the cluster has no pixel)
-    const int4 o = s.obb[k];
-    if (BAND) {
-        __syncwarp(); // every lane has its copy of the box before lane 0 resets it
-        const bool alive = s.bin_of[k] >= 0;
-        const int cr = alive ? (int)s.cy[k] : 0;   // row of the centre the assignment used
-        if (lane == 0) {
+    const int k = s.n - 1 - blockIdx.x;   // last cluster first (see above)
+    if (threadIdx.x == 0) {
+        // the box of this cluster's members, gathered by k_assign (empty when the cluster has no pixel)
+        const int4 o = s.obb[k];
+        int skip = 0;
+        if (BAND) {
+            const bool alive = s.bin_of[k] >= 0;
+            const int cr = alive ? (int)s.cy[k] : 0;   // row of the centre the assignment used
             if (o.y >= o.x && (!alive || o.x + s.y_off < cr - s.halo || o.y + s.y_off > cr + s.halo))
                 atomicAdd((unsigned long long*)&xchg[6 * (size_t)s.n], 1ull);
             s.obb[k] = make_int4(INT_MAX, -1, INT_MAX, -1);
+            skip = !alive || cr < s.own_lo || cr >= s.own_hi;
         }
-        if (!alive || cr < s.own_lo || cr >= s.own_hi) return;
+        s_box = o; s_skip = skip;
     }
+    __syncthreads();
+    if (s_skip) return;
+    const int4 o = s_box;
     const int y0 = o.x, y1 = o.y + 1, x0 = o.z, x1 = o.w + 1;
-    const size_t HW = s.pstride;
-    double acc = 0.0;
-    long long cnt = 0, sy = 0, sx = 0;
-    // the box is walked in raster order, 32 pixels at a time.  The loads are the latency that bounds this kernel, so label AND
-    // colours of the chunks two ahead are requested (unconditionally: the box is ~2x the members, the extra reads hit L2)
-    // before the current chunk is compacted and added.
     const int nchunk = (x1 > x0) ? (x1 - x0 + 31) / 32 : 0;
     const int total = (y1 > y0) ? (y1 - y0) * nchunk : 0;
-    int ly = y0, lxb = x0;   // load cursor
-    int cy_ = y0, cxb = x0;  // consume cursor
-    int Lq[2];
-    double Vq[2][3];
-    auto issue = [&](int sl, bool valid) {
-        const int x = lxb + lane;
-        Lq[sl] = -1;
-        if (valid && x < x1) {
-            const size_t p = (size_t)ly * s.W + x;
-            Lq[sl] = labels[p];
-            Vq[sl][0] = lab[p]; Vq[sl][1] = lab[HW + p]; Vq[sl][2] = lab[2 * HW + p];
-        }
-        lxb += 32;
-        if (lxb >= x1) { lxb = x0; ++ly; }
-    };
-    issue(0, total > 0);
-    issue(1, total > 1);
-    for (int it = 0; it < total; it += 2) {
-        // two consecutive chunks per round: one compaction, one pair of warp barriers, one run of adds
-        const bool two = it + 1 < total;
-        const int l0 = Lq[0], l1 = two ? Lq[1] : -1;
-        const double a0_ = Vq[0][0], a1_ = Vq[0][1], a2_ = Vq[0][2];
-        const double b0_ = Vq[1][0], b1_ = Vq[1][1], b2_ = Vq[1][2];
-        const int ya = cy_, xa = cxb + lane;
-        cxb += 32;
-        if (cxb >= x1) { cxb = x0; ++cy_; }
-        const int yb = cy_, xb_ = cxb + lane;
-        cxb += 32;
-        if (cxb >= x1) { cxb = x0; ++cy_; }
-        issue(0, it + 2 < total);
-        issue(1, it + 3 < total);
-        const bool m0 = l0 == k, m1 = l1 == k;
-        const unsigned mask0 = __ballot_sync(0xffffffffu, m0), mask1 = __ballot_sync(0xffffffffu, m1);
-        if (!(mask0 | mask1)) continue;
-        const int nm0 = __popc(mask0), nm1 = __popc(mask1), nm = nm0 + nm1;
+    const int nstrip = (total + USTRIP - 1) / USTRIP;
+    if (wl < UGATHER) {
+        const size_t HW = s.pstride;
         const unsigned below = (1u << lane) - 1u;
-        if (m0) {
-            const int pos = __popc(mask0 & below);
-            buf[wl][0][pos] = a0_; buf[wl][1][pos] = a1_; buf[wl][2][pos] = a2_;
-            sx += xa;
-        }
-        if (m1) {
-            const int pos = nm0 + __popc(mask1 & below);
-            buf[wl][0][pos] = b0_; buf[wl][1][pos] = b1_; buf[wl][2][pos] = b2_;
-            sx += xb_;
-        }
-        cnt += nm;
-        sy += (long long)(ya + s.y_off) * nm0 + (long long)(yb + s.y_off) * nm1;
-        // pad the run to a multiple of four with +0.0: x + (+0.0) == x for every x the sum can take (it starts at +0.0 and can
-        // therefore never be -0.0), so the padded adds change nothing and the add loop has no remainder
-        if (lane < 4) { buf[wl][0][nm + lane] = 0.0; buf[wl][1][nm + lane] = 0.0; buf[wl][2][nm + lane] = 0.0; }
-        __syncwarp();
-        if (lane < 3) {
-            // sequential adds in raster order; the next four operands are loaded while the current four are added (the loads do not
-            // depend on the running sum, only the adds form the chain)
-            const double* bsrc = buf[wl][lane];
-            const int ng = (nm + 3) >> 2;
-            double c0 = bsrc[0], c1 = bsrc[1], c2 = bsrc[2], c3 = bsrc[3];
-            for (int g = 1; g <= ng; ++g) {
-                const double n0 = bsrc[4 * g], n1 = bsrc[4 * g + 1], n2 = bsrc[4 * g + 2], n3 = bsrc[4 * g + 3];   // (one group past the end: inside the buffer)
-                acc = __dadd_rn(__dadd_rn(__dadd_rn(__dadd_rn(acc, c0), c1), c2), c3);
-                c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-            }
-        }
-        __syncwarp();
-    }
+        long long cnt = 0, sy = 0, sx = 0;
+        // chunk j of this warp in strip i: its row and this lane's column (out of the box: no pixel)
+        auto chunk_at = [&](int i, int j, int& y, int& x) {
+            const int c = i * USTRIP + wl * UCPW + j;
+            const int r = c / nchunk;
+            y = y0 + r; x = x0 + 32 * (c - r * nchunk) + lane;
+            return c < total && x < x1;
+        };
+        // the labels of the next strip are requested while the current one is compacted
+        int lbl[UCPW];
+        auto load_labels = [&](int i) {
 #pragma unroll
-    for (int d = 16; d > 0; d >>= 1) sx += __shfl_xor_sync(0xffffffffu, sx, d);
+            for (int j = 0; j < UCPW; ++j) {
+                int y, x;
+                lbl[j] = (i < nstrip && chunk_at(i, j, y, x)) ? labels[(size_t)y * s.W + x] : -1;
+            }
+        };
+        load_labels(0);
+        for (int i = 0; i < nstrip; ++i) {
+            const int b = i & 1;
+            unsigned mask[UCPW];
+            double v[UCPW][3];
+#pragma unroll
+            for (int j = 0; j < UCPW; ++j) {
+                int y, x;
+                chunk_at(i, j, y, x);
+                const bool m = lbl[j] == k;
+                mask[j] = __ballot_sync(0xffffffffu, m);
+                if (m) {
+                    const size_t p = (size_t)y * s.W + x;
+                    v[j][0] = lab[p]; v[j][1] = lab[HW + p]; v[j][2] = lab[2 * HW + p];
+                    ++cnt; sy += y + s.y_off; sx += x;
+                }
+            }
+            load_labels(i + 1);
+            if (lane == 0) {
+#pragma unroll
+                for (int j = 0; j < UCPW; ++j) s_cnt[b][wl * UCPW + j] = __popc(mask[j]);
+            }
+            bar_sync<UBAR_SCAN, 32 * UGATHER>();
+            // exclusive scan of the chunk counts: where each chunk's members start in the strip
+            const int cl = lane < USTRIP ? s_cnt[b][lane] : 0;
+            int incl = cl;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
+            const int excl = incl - cl, nm = __shfl_sync(0xffffffffu, incl, 31);
+            if (i >= 2) bar_sync<UBAR_EMPTY, UTHREADS>(b);   // the adds of strip i - 2 are done with this buffer
+#pragma unroll
+            for (int j = 0; j < UCPW; ++j) {
+                const int start = __shfl_sync(0xffffffffu, excl, wl * UCPW + j);
+                if ((mask[j] >> lane) & 1u) {
+                    const int pos = start + __popc(mask[j] & below);
+                    buf[b][0][pos] = v[j][0]; buf[b][1][pos] = v[j][1]; buf[b][2][pos] = v[j][2];
+                }
+            }
+            // pad the strip to a multiple of four with +0.0: x + (+0.0) == x for every x the sum can take (it starts at +0.0 and can
+            // therefore never be -0.0), so the padded adds change nothing and the add loop has no remainder
+            if (wl == 0 && lane < 4) {
+                buf[b][0][nm + lane] = 0.0; buf[b][1][nm + lane] = 0.0; buf[b][2][nm + lane] = 0.0;
+                if (lane == 0) s_tot[b] = nm;
+            }
+            bar_arrive<UBAR_FULL, UTHREADS>(b);
+        }
+#pragma unroll
+        for (int d = 16; d > 0; d >>= 1) {
+            cnt += __shfl_xor_sync(0xffffffffu, cnt, d); sy += __shfl_xor_sync(0xffffffffu, sy, d); sx += __shfl_xor_sync(0xffffffffu, sx, d);
+        }
+        if (lane == 0) { s_int[wl][0] = cnt; s_int[wl][1] = sy; s_int[wl][2] = sx; }
+    } else {
+        double acc = 0.0;
+        for (int i = 0; i < nstrip; ++i) {
+            const int b = i & 1;
+            bar_sync<UBAR_FULL, UTHREADS>(b);
+            if (lane < 3) {
+                // sequential adds in raster order; the next four operands are loaded while the current four are added (the loads do not
+                // depend on the running sum, only the adds form the chain)
+                const double2* bsrc = reinterpret_cast<const double2*>(buf[b][lane]);
+                const int ng = (s_tot[b] + 3) >> 2;
+                double2 c01 = bsrc[0], c23 = bsrc[1];
+                for (int g = 1; g <= ng; ++g) {
+                    const double2 n01 = bsrc[2 * g], n23 = bsrc[2 * g + 1];   // (one group past the end: inside the buffer)
+                    acc = __dadd_rn(__dadd_rn(__dadd_rn(__dadd_rn(acc, c01.x), c01.y), c23.x), c23.y);
+                    c01 = n01; c23 = n23;
+                }
+            }
+            __syncwarp();
+            if (i + 2 < nstrip) bar_arrive<UBAR_EMPTY, UTHREADS>(b);   // the gather warps wait for this only if they refill the buffer
+        }
+        if (lane < 3) s_acc[lane] = acc;
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    long long cnt = 0, sy = 0, sx = 0;
+#pragma unroll
+    for (int w = 0; w < UGATHER; ++w) { cnt += s_int[w][0]; sy += s_int[w][1]; sx += s_int[w][2]; }
     // centroid = sums / count with IEEE divisions (the original divides every feature by the element count), new window,
     // bin of the new centre; a cluster without pixels is dead for good
-    const double a0 = __shfl_sync(0xffffffffu, acc, 0), a1 = __shfl_sync(0xffffffffu, acc, 1), a2 = __shfl_sync(0xffffffffu, acc, 2);
+    const double a0 = s_acc[0], a1 = s_acc[1], a2 = s_acc[2];
     if (BAND) {
-        if (lane == 0) {
-            long long* r = xchg + 6 * (size_t)k;
-            if (cnt > 0) {
-                const double dn = (double)cnt;
-                r[0] = __double_as_longlong(__ddiv_rn((double)sy, dn)); r[1] = __double_as_longlong(__ddiv_rn((double)sx, dn));
-                r[2] = __double_as_longlong(__ddiv_rn(a0, dn)); r[3] = __double_as_longlong(__ddiv_rn(a1, dn));
-                r[4] = __double_as_longlong(__ddiv_rn(a2, dn));
-                r[5] = 1;
-            } else r[5] = 2;
-        }
-        return;
-    }
-    if (lane == 0) {
-        int4 w = make_int4(0, 0, 0, 0);
-        int bin = -1;
+        long long* r = xchg + 6 * (size_t)k;
         if (cnt > 0) {
             const double dn = (double)cnt;
-            const double cy = __ddiv_rn((double)sy, dn), cx = __ddiv_rn((double)sx, dn);
-            s.cy[k] = cy; s.cx[k] = cx;
-            s.c0[k] = __ddiv_rn(a0, dn); s.c1[k] = __ddiv_rn(a1, dn); s.c2[k] = __ddiv_rn(a2, dn);
-            w = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
-            const int by = min(max((int)cy / s.B, 0), s.nby - 1), bx = min(max((int)cx / s.B, 0), s.nbx - 1);
-            bin = by * s.nbx + bx;
-            atomicAdd(&s.bin_fill[bin], 1);
-        }
-        s.win[k] = w;
-        s.bin_of[k] = bin;
-        s.obb[k] = make_int4(INT_MAX, -1, INT_MAX, -1);
+            r[0] = __double_as_longlong(__ddiv_rn((double)sy, dn)); r[1] = __double_as_longlong(__ddiv_rn((double)sx, dn));
+            r[2] = __double_as_longlong(__ddiv_rn(a0, dn)); r[3] = __double_as_longlong(__ddiv_rn(a1, dn));
+            r[4] = __double_as_longlong(__ddiv_rn(a2, dn));
+            r[5] = 1;
+        } else r[5] = 2;
+        return;
     }
+    int4 w = make_int4(0, 0, 0, 0);
+    int bin = -1;
+    if (cnt > 0) {
+        const double dn = (double)cnt;
+        const double cy = __ddiv_rn((double)sy, dn), cx = __ddiv_rn((double)sx, dn);
+        s.cy[k] = cy; s.cx[k] = cx;
+        s.c0[k] = __ddiv_rn(a0, dn); s.c1[k] = __ddiv_rn(a1, dn); s.c2[k] = __ddiv_rn(a2, dn);
+        w = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
+        const int by = min(max((int)cy / s.B, 0), s.nby - 1), bx = min(max((int)cx / s.B, 0), s.nbx - 1);
+        bin = by * s.nbx + bx;
+        atomicAdd(&s.bin_fill[bin], 1);
+    }
+    s.win[k] = w;
+    s.bin_of[k] = bin;
+    s.obb[k] = make_int4(INT_MAX, -1, INT_MAX, -1);
 }
 
 // band mode: take the merged exchange records (see k_update<true>) into the replicated cluster state
@@ -680,7 +736,7 @@ extern "C" int isb_slic_kmeans(const double* lab_planar, int H, int W, const dou
             launch_assign(s, lab_map, use_tma, lab_planar, labels, st);
         }
         ISB_LAUNCH_CHECK();
-        { ProfScope p(ISB_PROF_UPDATE, st); k_update<false><<<(n_seeds + UWARPS - 1) / UWARPS, 32 * UWARPS, 0, st>>>(s, lab_planar, labels, nullptr); }
+        { ProfScope p(ISB_PROF_UPDATE, st); k_update<false><<<n_seeds, UTHREADS, 0, st>>>(s, lab_planar, labels, nullptr); }
         ISB_LAUNCH_CHECK();
         if (slic_zero) {
             const size_t npx = (size_t)H * W;
@@ -756,7 +812,7 @@ extern "C" int isb_slic_band_update(const isb_slic_band_t* b, int64_t* xchg, isb
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope p(ISB_PROF_UPDATE, st);
     ISB_CUDA_CHECK(cudaMemsetAsync(xchg, 0, sizeof(int64_t) * (6 * (size_t)s.n + 1), st));
-    k_update<true><<<(s.n + UWARPS - 1) / UWARPS, 32 * UWARPS, 0, st>>>(s, b->lab_slab, b->labels_slab, (long long*)xchg);
+    k_update<true><<<s.n, UTHREADS, 0, st>>>(s, b->lab_slab, b->labels_slab, (long long*)xchg);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }
