@@ -250,7 +250,8 @@ size_t isb_alpha_expansion_workspace_bytes(int N, int K, int E);
 int isb_alpha_expansion(int N, const int32_t* n_nodes_dev /* optional device N */, int K, int E, const int32_t* n_edges_dev,
                         const int32_t* edges, const int32_t* edge_wi,
                         const int32_t* unary_i, const int32_t* smooth_i, int n_iter, int32_t* labels, int64_t* energy_out,
-                        int32_t* stats_out /* optional [8]: moves, flows, sweeps, global relabels, BFS levels, smem flag, 0, 0 */, void* ws, size_t ws_bytes,
+                        int32_t* stats_out /* optional [8]: moves, flows, sweeps, global relabels, BFS levels, smem flag,
+                                              a move refused for a terminal capacity >= 2^29, one refused for a pair capacity >= 2^30 */, void* ws, size_t ws_bytes,
                         isb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------

@@ -351,13 +351,14 @@ def integerise(edge_w, unary, pairwise):
     return w, u, v
 
 
-def alpha_expansion_int(edges, w, unary, pairwise, n_iter=-1, return_energy=False):
-    edges = np.ascontiguousarray(edges, dtype=np.int32)
+def alpha_expansion_int(edges, w, unary, pairwise, n_iter=-1, return_energy=False, init=None):
+    """``init``: starting labeling [N] (pyGCO's init_labels); all zeros when None"""
+    edges = np.ascontiguousarray(edges, dtype=np.int32).reshape(-1, 2)
     w = np.ascontiguousarray(w, dtype=np.int32)
     unary = np.ascontiguousarray(unary, dtype=np.int32)
     pairwise = np.ascontiguousarray(pairwise, dtype=np.int32)
     N, K = unary.shape
-    labels = np.zeros(N, dtype=np.int32)
+    labels = np.zeros(N, dtype=np.int32) if init is None else np.array(init, dtype=np.int32).reshape(N)
     energy = C.c_int64(0)
     moves = C.c_int(0)
     lib().oracle_alpha_expansion(N, K, len(edges), _p(edges, C.c_int32), _p(w, C.c_int32), _p(unary, C.c_int32),

@@ -26,7 +26,7 @@
 // unique minimiser with the most sites switched -- so labels equal the oracle's whatever the flow algorithm.
 // An expansion on a label that already failed on the SAME labeling is skipped (same input, same answer).
 //
-// When 20 N/8 + 16 max_arcs_per_CTA bytes exceed the dynamic shared memory the same code runs with the state in
+// When 24 N/8 + 16 max_arcs_per_CTA bytes exceed the dynamic shared memory the same code runs with the state in
 // the global workspace (L2 resident) -- the per-rank base pointers then simply point into global arrays.
 // This stage is latency/SMEM bound, not HBM bound: report time, not a roofline fraction (SURVEY.md section 8d).
 #include "common.cuh"
@@ -57,7 +57,8 @@ struct GcArgs {
     long long* red;   // [8] cluster-wide reduction scratch
     int* newlab;
     // state in global memory (used when it does not fit in the cluster's shared memory)
-    int* g_node;      // [5][N]  excess | tcap | h0 | h1 | hmin
+    long long* g_excess; // [N]  excess
+    int* g_node;      // [4][N]  tcap | h0 | h1 | hmin
     int* g_arc;       // [4][A]  res | dstp | revp | srcl
     int dyn_bytes;
 };
@@ -108,7 +109,7 @@ __global__ void __launch_bounds__(NT) k_gc_build_csr(GcArgs a)
 
 // per-rank base pointers of the distributed state (DSMEM addresses, or slices of the global arrays)
 struct Peers {
-    int* excess[CS]; int* tcap[CS]; int* h[2][CS]; int* res[CS];
+    long long* excess[CS]; int* tcap[CS]; int* h[2][CS]; int* res[CS];
 };
 
 struct Ctx {
@@ -116,13 +117,19 @@ struct Ctx {
     int rank, npc, n_lo, n_cnt, a_lo, a_cnt; // this CTA's node range [n_lo, n_lo+n_cnt) and arc range [a_lo, a_lo+a_cnt)
     const int* edges; const int* w; const int* D; const int* V;
     // local slices
-    int* excess; int* tcap; int* h[2]; int* hmin; int* res; int* dstp; int* revp; int* srcl;
+    long long* excess; int* tcap; int* h[2]; int* hmin; int* res; int* dstp; int* revp; int* srcl;
     Peers* peers;
     int* s_V; long long* s_red; int* flags0; // flags0 = rank 0's flag words (DSMEM)
     long long* red;
 };
 
 __device__ __forceinline__ int smooth(const Ctx& c, int la, int lb) { return c.K <= KMAX_S ? c.s_V[la * c.K + lb] : c.V[la * c.K + lb]; }
+
+// 64-bit atomic add on a node's excess (local, DSMEM or global); subtraction adds the negated amount.  Returns the old value.
+__device__ __forceinline__ long long add_excess(long long* p, long long v)
+{
+    return (long long)atomicAdd((unsigned long long*)p, (unsigned long long)v);
+}
 
 __device__ long long block_sum_ll(long long v, long long* s_red)
 {
@@ -214,13 +221,13 @@ __device__ bool sweep(cg::cluster_group& cl, const Ctx& c, int cur, int& turn)
     // node pass: the sink arc first; foreign CTAs may already push into excess[u], so it is only touched atomically
     for (int u = threadIdx.x; u < c.n_cnt; u += NT) {
         c.hmin[u] = HINF;
-        const int ex = *(volatile int*)&c.excess[u];
+        const long long ex = *(volatile long long*)&c.excess[u];
         if (ex <= 0 || h[u] == HINF) continue;
         const int tc = c.tcap[u];
         if (tc > 0) {
-            const int d = ex < tc ? ex : tc;
+            const int d = ex < tc ? (int)ex : tc;
             c.tcap[u] = tc - d;
-            atomicSub(&c.excess[u], d);
+            add_excess(&c.excess[u], -(long long)d);
         }
     }
     __syncthreads();
@@ -229,24 +236,24 @@ __device__ bool sweep(cg::cluster_group& cl, const Ctx& c, int cur, int& turn)
         const int r = *(volatile int*)&c.res[i];
         if (r <= 0) continue;
         const int u = c.srcl[i];
-        const int ex = *(volatile int*)&c.excess[u];
+        const long long ex = *(volatile long long*)&c.excess[u];
         if (ex <= 0) continue;
         const int hu = h[u];
         if (hu == HINF) continue;
         const int p = c.dstp[i];
         if (HGT(cur, p) != hu - 1) continue;
-        int d = ex < r ? ex : r;
-        const int old = atomicSub(&c.excess[u], d);
+        int d = ex < r ? (int)ex : r;
+        const long long old = add_excess(&c.excess[u], -(long long)d);
         if (old < d) { // over-claimed: give back what was not there
-            const int have = old > 0 ? old : 0;
-            atomicAdd(&c.excess[u], d - have);
+            const int have = old > 0 ? (int)old : 0;
+            add_excess(&c.excess[u], d - have);
             d = have;
         }
         if (d > 0) {
             atomicSub(&c.res[i], d);
             const int q = c.revp[i];
             atomicAdd(&c.peers->res[q >> LBITS][q & LMASK], d);
-            atomicAdd(&c.peers->excess[p >> LBITS][p & LMASK], d);
+            add_excess(&c.peers->excess[p >> LBITS][p & LMASK], d);
         }
     }
     cl.sync();
@@ -310,12 +317,14 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) k_alpha_expa
     c.a_cnt = s_alo[c.rank + 1] - c.a_lo;
     int apc = 0;
     for (int r = 0; r < CS; ++r) apc = max(apc, s_alo[r + 1] - s_alo[r]);
-    const size_t smem_need = sizeof(int) * (5 * (size_t)c.npc + 4 * (size_t)apc);
+    const size_t smem_need = sizeof(long long) * (size_t)c.npc + sizeof(int) * (4 * (size_t)c.npc + 4 * (size_t)apc);
     const bool in_smem = smem_need <= (size_t)a.dyn_bytes;
     if (in_smem) {
-        int* q = (int*)dyn; // identical layout in every CTA: excess | tcap | h0 | h1 | hmin | res | dstp | revp | srcl
-        c.excess = q; c.tcap = q + c.npc; c.h[0] = q + 2 * c.npc; c.h[1] = q + 3 * c.npc; c.hmin = q + 4 * c.npc;
-        int* s = q + 5 * c.npc;
+        // identical layout in every CTA: excess (64-bit) | tcap | h0 | h1 | hmin | res | dstp | revp | srcl
+        c.excess = (long long*)dyn;
+        int* q = (int*)(c.excess + c.npc);
+        c.tcap = q; c.h[0] = q + c.npc; c.h[1] = q + 2 * c.npc; c.hmin = q + 3 * c.npc;
+        int* s = q + 4 * c.npc;
         c.res = s; c.dstp = s + apc; c.revp = s + 2 * apc; c.srcl = s + 3 * apc;
         if (threadIdx.x < CS) {
             const int r = threadIdx.x;
@@ -328,14 +337,14 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) k_alpha_expa
     } else {
         int* gn = a.g_node; int* ga = a.g_arc;
         const size_t Nn = (size_t)a.N, Aa = 2 * (size_t)(a.E_cap > 0 ? a.E_cap : 1);
-        c.excess = gn + c.n_lo; c.tcap = gn + Nn + c.n_lo; c.h[0] = gn + 2 * Nn + c.n_lo; c.h[1] = gn + 3 * Nn + c.n_lo;
-        c.hmin = gn + 4 * Nn + c.n_lo;
+        c.excess = a.g_excess + c.n_lo; c.tcap = gn + c.n_lo; c.h[0] = gn + Nn + c.n_lo; c.h[1] = gn + 2 * Nn + c.n_lo;
+        c.hmin = gn + 3 * Nn + c.n_lo;
         c.res = ga + c.a_lo; c.dstp = ga + Aa + c.a_lo; c.revp = ga + 2 * Aa + c.a_lo; c.srcl = ga + 3 * Aa + c.a_lo;
         if (threadIdx.x < CS) {
             const int r = threadIdx.x;
             const int nlo = min(r * c.npc, N);
-            s_peers.excess[r] = gn + nlo; s_peers.tcap[r] = gn + Nn + nlo;
-            s_peers.h[0][r] = gn + 2 * Nn + nlo; s_peers.h[1][r] = gn + 3 * Nn + nlo;
+            s_peers.excess[r] = a.g_excess + nlo; s_peers.tcap[r] = gn + nlo;
+            s_peers.h[0][r] = gn + Nn + nlo; s_peers.h[1][r] = gn + 2 * Nn + nlo;
             s_peers.res[r] = ga + s_alo[r];
         }
     }
@@ -374,7 +383,7 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) k_alpha_expa
         }
         cl.sync();
         const int Vaa = smooth(c, alpha, alpha);
-        int bad = 0;
+        int nonsub = 0, wide = 0;
         for (int i = threadIdx.x; i < c.a_cnt; i += NT) {
             const int g = c.a_lo + i;
             const int ed = a.a_eid[g];
@@ -390,7 +399,8 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) k_alpha_expa
                 // capacity P1 on a->b, P2 on b->a (P1 + P2 = P).  Same energy function, hence the same minimisers, but residual
                 // paths exist in both directions from the start (short BFS distances, far fewer sweeps).
                 const long long Pl = B + C - A - Dd;
-                if (Pl < 0 || Pl > 0x3fffffff) bad = 1;
+                if (Pl < 0) nonsub = 1;
+                else if (Pl > 0x3fffffff) wide = 1;
                 const long long p2 = Pl >> 1, p1 = Pl - p2;
                 atomicAdd((unsigned long long*)&a.u0[va], (unsigned long long)A);
                 atomicAdd((unsigned long long*)&a.u1[va], (unsigned long long)(C - p2));
@@ -407,7 +417,11 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) k_alpha_expa
             const int q = c.revp[i];
             c.peers->res[q >> LBITS][q & LMASK] = P2;
         }
-        if (cluster_or(cl, c, bad, turn)) return false; // non-submodular (GCO refuses it) or capacities beyond 2^30
+        if (cluster_or(cl, c, nonsub | wide, turn)) {
+            // a non-submodular pair fails the move silently (GCO refuses it too); a pair capacity of 2^30 or more is reported in stats[7]
+            if (cluster_or(cl, c, wide, turn) && threadIdx.x == 0) s_stats[7] = 1;
+            return false;
+        }
         int big = 0;
         for (int v = threadIdx.x; v < c.n_cnt; v += NT) {
             const int g = c.n_lo + v;
@@ -416,11 +430,11 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) k_alpha_expa
             const bool act = lab[g] != alpha;
             const long long ex = act ? x1 - m : 0, tc = act ? x0 - m : 0;
             if (ex > 0x1fffffff || tc > 0x1fffffff) big = 1;
-            c.excess[v] = (int)ex;
+            c.excess[v] = ex;
             c.tcap[v] = (int)tc;
         }
-        // 32-bit excess is safe while terminal capacities stay below 2^29 and the incoming arc capacities below 2^30 in sum
-        // (degree < ~5000 at pyGCO's scales); refuse the move loudly otherwise
+        // sink capacities are 32-bit: a terminal capacity of 2^29 or more refuses the move and is reported in stats[6].  The excess
+        // is 64-bit: it never exceeds the node's terminal capacity plus its incoming pair capacities (each below 2^30), whatever the degree
         if (cluster_or(cl, c, big, turn)) { if (threadIdx.x == 0) s_stats[6] = 1; return false; }
         // ---- max-flow (phase 1) ----
         if (threadIdx.x == 0) ++s_stats[1];
@@ -517,7 +531,7 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) k_alpha_expa
 
 struct GcWs {
     int* off; int* fill; int* a_src; int* a_dst; int* a_rev; int* a_eid; long long* u0; long long* u1; long long* red; int* newlab;
-    int* g_node; int* g_arc;
+    long long* g_excess; int* g_node; int* g_arc;
 };
 
 static size_t carve_gc(GcWs& w, void* ws, size_t bytes, int N, int E)
@@ -528,7 +542,8 @@ static size_t carve_gc(GcWs& w, void* ws, size_t bytes, int N, int E)
     w.a_src = c.take<int>(2 * e); w.a_dst = c.take<int>(2 * e); w.a_rev = c.take<int>(2 * e); w.a_eid = c.take<int>(2 * e);
     w.u0 = c.take<long long>(N); w.u1 = c.take<long long>(N); w.red = c.take<long long>(8);
     w.newlab = c.take<int>(N);
-    w.g_node = c.take<int>(5 * (size_t)N);
+    w.g_excess = c.take<long long>(N);
+    w.g_node = c.take<int>(4 * (size_t)N);
     w.g_arc = c.take<int>(4 * 2 * e);
     return isb_align(c.off);
 }
@@ -558,7 +573,7 @@ extern "C" int isb_alpha_expansion(int N, const int32_t* n_nodes_dev, int K, int
     a.labels = labels; a.energy_out = (long long*)energy_out; a.stats = stats_out;
     a.off = w.off; a.fill = w.fill; a.a_src = w.a_src; a.a_dst = w.a_dst; a.a_rev = w.a_rev; a.a_eid = w.a_eid;
     a.u0 = w.u0; a.u1 = w.u1; a.red = w.red; a.newlab = w.newlab;
-    a.g_node = w.g_node; a.g_arc = w.g_arc;
+    a.g_excess = w.g_excess; a.g_node = w.g_node; a.g_arc = w.g_arc;
     // always launch with the full dynamic smem: the kernel decides from the REAL node/edge counts (device scalars)
     // whether the flow state fits in the cluster's shared memory or stays in the global workspace
     const size_t smem_max = 227 * 1024 - 8 * 1024; // leave room for the static arrays

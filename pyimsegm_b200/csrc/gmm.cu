@@ -369,6 +369,8 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
                 }
                 if (lab[n] != bk) { lab[n] = bk; changed = 1; }
             }
+            // the pass below reads labels that other threads of this CTA have just written: all of them must be in place first
+            changed = __syncthreads_or(changed);
             // new centres: count and coordinate sums of every cluster in ONE quantity-parallel pass over sample slices
             // (quantity q = (k, j): j == 0 the count, j >= 1 the sum of coordinate j-1); quantity Q carries the "changed" flag
             const int Q = K * (1 + D);                 // <= 8 * 17 = 136 < GT
@@ -383,7 +385,7 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
                 }
                 s_part[threadIdx.x] = a;
             }
-            changed = __syncthreads_or(changed);
+            __syncthreads();
             double t = 0;
             if ((int)threadIdx.x < Q) { for (int s2 = 0; s2 < S; ++s2) t += s_part[s2 * (Q + 1) + threadIdx.x]; }
             else if ((int)threadIdx.x == Q) t = changed ? 1.0 : 0.0;

@@ -520,8 +520,22 @@ def cut_general_graph(edges, edge_weights, unary_cost, pairwise_cost, n_iter=-1,
     init = None
     if init_labels is not None:
         init = eng.to_device(np.ascontiguousarray(init_labels, dtype=np.int32), 'init_labels')
-    labels, _, _ = eng.alpha_expansion(N, K, E, None, d_edges, d_w, d_un, d_pw, int(n_iter), init)
-    return eng.to_host(labels).copy()
+    labels, _, stats = eng.alpha_expansion(N, K, E, None, d_edges, d_w, d_un, d_pw, int(n_iter), init)
+    (labels, stats), done = eng.download((labels, stats))
+    done.synchronize()
+    _raise_on_refused_move(stats.numpy())
+    return labels.numpy().copy()
+
+
+def _raise_on_refused_move(stats):
+    """the device refuses an expansion move whose capacities do not fit its 32-bit flow arrays (``stats`` of isb_alpha_expansion);
+    GCO would solve that move, so the labels would differ from pyGCO's: raise instead of returning them"""
+    if stats[6]:
+        raise RuntimeError('alpha-expansion: a terminal capacity of a move reached 2^29 (unary costs plus the edge terms they absorb '
+                           'must stay below 2^29)')
+    if stats[7]:
+        raise RuntimeError('alpha-expansion: a pair capacity of a move reached 2^30 (w_ij * (V[a, alpha] + V[alpha, b] - V[a, b] - '
+                           'V[alpha, alpha]) must stay below 2^30)')
 
 
 def cut_grid_graph(unary_cost, pairwise_cost, cost_v, cost_h, n_iter=-1, algorithm='expansion'):
