@@ -269,6 +269,26 @@ int isb_gmm_params_len(int D, int K);
 int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, const int32_t* n_dev, int K, int n_init, int max_iter, double tol,
                         double reg_covar, int use_scaler, unsigned long long seed, const int32_t* init_labels, double* proba,
                         double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* the same fit for either mixture of the reference's estim_model variants: kind 0 = GaussianMixture (exactly isb_gmm_fit_predict),
+ * kind 1 = BayesianGaussianMixture (full covariance, dirichlet_process, default priors: weight concentration 1/K, mean precision 1,
+ * mean = mean of the scaled features, degrees of freedom D, covariance = their np.cov).  For kind 1 the params_out layout is the GMM
+ * one with nk (responsibility sums + 10 eps) in place of the weights, the posterior means and (normalised) covariances, the ELBO as
+ * lower_bound, followed by mean_prior[D] | covariance_prior[D,D].  Same limits and errors as isb_gmm_fit_predict. */
+size_t isb_mixture_fit_workspace_bytes(int kind, int N, int D, int K, int n_init);
+int isb_mixture_fit_params_len(int kind, int D, int K);
+int isb_mixture_fit_predict(int kind, const double* feat, int N, int D, int ld, const int32_t* n_dev, int K, int n_init, int max_iter,
+                            double tol, double reg_covar, int use_scaler, unsigned long long seed, const int32_t* init_labels, double* proba,
+                            double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* PCA fit of the reference's pca_coef (sklearn PCA, covariance_eigh solver) on StandardScaler'd features (use_scaler 0: as given):
+ *   n_components > 0 keeps that many components (<= D); else coef in (0, 1) picks them from the explained variance ratio.
+ *   params_out (isb_pca_params_len(D) doubles): scaler mean[D] | scaler scale[D] | mean_[D] | components_[D,D] (all of them,
+ *   descending, sign-flipped) | explained_variance_[D] | explained_variance_ratio_[D] | singular_values_[D] | mean_ components_^T [D] |
+ *   n_components | noise_variance | n_samples | ok;  n_components_out: optional device int32.  The transform is isb_class_transform
+ *   with these tables.  D <= 232 (else ISB_ERR_UNSUPPORTED), N >= 2. */
+size_t isb_pca_workspace_bytes(int N, int D);
+int isb_pca_params_len(int D);
+int isb_pca_fit(const double* feat, int N, int D, int ld, const int32_t* n_dev, int use_scaler, double coef, int n_components,
+                double* params_out, int32_t* n_components_out, void* ws, size_t ws_bytes, isb_stream_t stream);
 
 /* predict_proba of a caller-fitted class model -- replaces the host round trip of segment_color2d_slic_features_model_graphcut
  * (imsegm/pipelines.py:160-241) with a model from estim_model_classes_group (:113-157) or a trained classifier

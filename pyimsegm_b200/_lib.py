@@ -72,6 +72,12 @@ SIGNATURES = {
     'isb_gmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'isb_gmm_params_len': (_i, [_i, _i]),
     'isb_gmm_fit_predict': (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _d, _d, _i, C.c_ulonglong, _vp, _vp, _vp, _vp, _sz, _vp]),
+    'isb_mixture_fit_workspace_bytes': (_sz, [_i, _i, _i, _i, _i]),
+    'isb_mixture_fit_params_len': (_i, [_i, _i, _i]),
+    'isb_mixture_fit_predict': (_i, [_i, _vp, _i, _i, _i, _vp, _i, _i, _i, _d, _d, _i, C.c_ulonglong, _vp, _vp, _vp, _vp, _sz, _vp]),
+    'isb_pca_workspace_bytes': (_sz, [_i, _i]),
+    'isb_pca_params_len': (_i, [_i]),
+    'isb_pca_fit': (_i, [_vp, _i, _i, _i, _vp, _i, _d, _i, _vp, _vp, _vp, _sz, _vp]),
     'isb_class_transform_workspace_bytes': (_sz, [_i, _i, _i]),
     'isb_class_transform': (_i, [_vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _sz, _vp]),
     'isb_mixture_predict_workspace_bytes': (_sz, [_i, _i, _i]),

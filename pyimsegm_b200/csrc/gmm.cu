@@ -11,6 +11,12 @@
 // k-means++ / Lloyd with a counter-based RNG (the reference leaves the model unseeded, so only the algorithm,
 // not a label-for-label result, can be matched; tests compare against sklearn from a shared initialisation).
 // N is tiny (superpixels, not pixels): this stage is latency bound, it exists to remove the host sync.
+//
+// The same kernels also fit sklearn.mixture.BayesianGaussianMixture (full covariance, dirichlet_process, default priors), the
+// model of estim_model='BGM': template parameter KIND = MIX_BGM swaps the parameter update (Normal-Wishart posterior from the same
+// sufficient statistics), the per-component constant of the E-step (digamma terms) and the lower bound (the ELBO).  KIND = MIX_GMM
+// is the GaussianMixture code unchanged.  isb_pca_fit (end of file) is the PCA(covariance_eigh) that the reference puts between the
+// scaler and the mixture when pca_coef is given.
 #include "common.cuh"
 #include <float.h>
 #include <cooperative_groups.h>
@@ -25,6 +31,7 @@ constexpr int KS = 8;        // split-K factor of the M-step Gram matrices
 constexpr int DBIG = 232;    // feature dimensions of the large-D path (batched GEMMs, e.g. colour + Leung-Malik = 189); the packed
                              // lower triangle of one covariance (D (D + 1) / 2 doubles) has to fit the shared memory of a CTA
 constexpr int KMAX = 8;      // mixture components handled on the device
+constexpr int MIX_GMM = 0, MIX_BGM = 1;   // KIND of the fit kernels
 
 struct GmmWs {
     double* xs;       // [N, D] standardised features
@@ -45,6 +52,9 @@ struct GmmWs {
     double* tot;      // [n_init, K, 1 + D] k-means counts / coordinate sums
     double* state;    // [n_init, 4]        lower bound of the previous E-step, done, -, failed
     int* flag;        // [1]                restarts still running
+    // BayesianGaussianMixture only
+    double* prior;    // [D + D D]          mean_prior_ | covariance_prior_ (np.cov of the scaled features, ddof 1)
+    double* bld;      // [n_init, K]        log|prec_chol| of the large-D path (the lower bound needs it without the other terms)
 };
 
 __host__ __device__ inline int pstride(int K, int D) { return K + K * D + 2 * K * D * D + 4; }
@@ -122,6 +132,63 @@ __device__ __forceinline__ double log_prob_all(const double* x, int D, int K, co
     return mx + log(s);
 }
 
+// ---- BayesianGaussianMixture terms (sklearn/mixture/_bayesian_mixture.py, weight_concentration_prior = 1 / K,
+// mean_precision_prior = 1, degrees_of_freedom_prior = D).  nk[k] is the responsibility sum + 10 eps, exactly sklearn's nk.
+
+// digamma for x > 0: the recurrence psi(x) = psi(x + 1) - 1 / x up to x >= 10, then the asymptotic series to x^-14 (the first
+// omitted term is below 1e-16 there).  Every argument of the fit is >= 1 / 16 (the concentration prior is >= 1 / KMAX).
+__device__ double digamma_d(double x)
+{
+    double r = 0.0;
+    while (x < 10.0) { r -= 1.0 / x; x += 1.0; }
+    const double f = 1.0 / (x * x);
+    const double t = f * (-1.0 / 12 + f * (1.0 / 120 + f * (-1.0 / 252 + f * (1.0 / 240 + f * (-1.0 / 132 + f * (691.0 / 32760 + f * (-1.0 / 12)))))));
+    return r + log(x) - 0.5 / x + t;
+}
+
+// E[log pi_k] of the stick-breaking weights (_estimate_log_weights): a_j = 1 + nk_j, b_j = 1 / K + sum_{i > j} nk_i
+__device__ double bgm_log_weight(int k, int K, const double* nk)
+{
+    double acc = 0.0, lw = 0.0;
+    for (int j = 0; j <= k; ++j) {
+        double t = 0.0;
+        for (int i = K - 1; i > j; --i) t += nk[i];   // np.cumsum(nk[::-1])[-2::-1]
+        const double a = 1.0 + nk[j], b = 1.0 / K + t, ds = digamma_d(a + b);
+        if (j < k) acc += digamma_d(b) - ds;
+        else lw = digamma_d(a) - ds;
+    }
+    return lw + acc;
+}
+
+// the per-component constant of the E-step (_estimate_log_prob + _estimate_log_weights) given log|prec_chol_k| = ld:
+//   ld - D/2 log nu + (D log 2 + sum_i psi((nu - i) / 2) - D / beta) / 2 + E[log pi_k],   nu = D + nk, beta = 1 + nk
+__device__ double bgm_log_const(int k, int K, int D, const double* nk, double ld)
+{
+    const double nu = D + nk[k], beta = 1.0 + nk[k];
+    double psi = 0.0;
+    for (int i = 0; i < D; ++i) psi += digamma_d(0.5 * (nu - i));
+    const double log_lambda = D * 0.6931471805599453 + psi;
+    return ld - 0.5 * D * log(nu) + 0.5 * (log_lambda - D / beta) + bgm_log_weight(k, K, nk);
+}
+
+// the parameter part of the lower bound (_compute_lower_bound without the -sum r log r term); ld[k] = log|prec_chol_k|
+__device__ double bgm_lower_params(int K, int D, const double* nk, const double* ld)
+{
+    double wish = 0.0, lnw = 0.0, lbeta = 0.0;
+    for (int k = 0; k < K; ++k) {
+        const double nu = D + nk[k];
+        double lg = 0.0;
+        for (int i = 0; i < D; ++i) lg += lgamma(0.5 * (nu - i));
+        wish += -(nu * (ld[k] - 0.5 * D * log(nu)) + nu * D * 0.5 * 0.6931471805599453 + lg);
+        double t = 0.0;
+        for (int i = K - 1; i > k; --i) t += nk[i];
+        const double a = 1.0 + nk[k], b = 1.0 / K + t;
+        lnw += lgamma(a) + lgamma(b) - lgamma(a + b);   // betaln
+        lbeta += log(1.0 + nk[k]);
+    }
+    return -wish + lnw - 0.5 * D * lbeta;
+}
+
 // ---- the single-kernel path (D <= DMAX): one thread-block CLUSTER of CL CTAs per restart ------------------------------------------
 // The samples of a restart are cut into CL contiguous ranges, one per CTA of the cluster.  Every CTA keeps a bit-identical replica of
 // the model parameters in its shared memory; what crosses the CTAs are the partial sums of the reductions (log-likelihood, component
@@ -165,9 +232,11 @@ __device__ double cluster_vec_sum(double part, int nq, const ClusterCtx& c)
 
 // parameters from responsibilities (sklearn _estimate_gaussian_parameters + _compute_precision_cholesky) over the samples
 // [n_lo, n_hi) of this CTA, merged over the cluster; `par` is this CTA's shared-memory replica.
-// returns false when a covariance is not positive definite (the same answer in every CTA)
+// returns false when a covariance is not positive definite (the same answer in every CTA).
+// MIX_BGM: the weights slot keeps nk, the means and covariances become the posterior's (_estimate_means, _estimate_wishart_full)
+template <int KIND>
 __device__ bool m_step(const double* __restrict__ xs, const double* __restrict__ resp, int n_lo, int n_hi, int N, int D, int K, double reg,
-                       double* par, double* s_part, const ClusterCtx& c)
+                       double* par, double* s_part, const ClusterCtx& c, const double* __restrict__ prior)
 {
     double* wts = par; double* mu = par + K; double* cov = mu + K * D; double* pc = cov + (size_t)K * D * D;
     // pass 1: nk and means, quantity-parallel over sample slices
@@ -227,6 +296,22 @@ __device__ bool m_step(const double* __restrict__ xs, const double* __restrict__
         }
         __syncthreads();
     }
+    if (KIND == MIX_BGM) {
+        // covariance_prior + nk sk + nk beta0 / beta_k (xk - m0)(xk - m0)^T, over nu_k; then means = (beta0 m0 + nk xk) / beta_k
+        const double* m0 = prior; const double* C0 = prior + D;
+        for (int i = threadIdx.x; i < K * D * D; i += GT) {
+            const int k = i / (D * D), a = (i / D) % D, b = i % D;
+            const double nk = wts[k];
+            const double da = mu[k * D + a] - m0[a], db = mu[k * D + b] - m0[b];
+            cov[i] = (C0[a * D + b] + nk * cov[i] + nk * 1.0 / (1.0 + nk) * (da * db)) / (D + nk);
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < K * D; i += GT) {
+            const double nk = wts[i / D];
+            mu[i] = (1.0 * m0[i % D] + nk * mu[i]) / (1.0 + nk);
+        }
+        __syncthreads();
+    }
     // Cholesky cov = L L^T, prec_chol = (L^-1)^T, one thread per component
     __shared__ int s_bad;
     if (threadIdx.x == 0) s_bad = 0;
@@ -257,12 +342,15 @@ __device__ bool m_step(const double* __restrict__ xs, const double* __restrict__
         }
     }
     __syncthreads();
-    for (int k = threadIdx.x; k < K; k += GT) wts[k] = wts[k] / N;
-    __syncthreads();
+    if (KIND == MIX_GMM) {
+        for (int k = threadIdx.x; k < K; k += GT) wts[k] = wts[k] / N;
+        __syncthreads();
+    }
     return s_bad == 0;
 }
 
 // one cluster of CL CTAs per restart (gridDim.x = n_init * CL, cluster dimension CL set at launch)
+template <int KIND>
 __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int D, int K, int max_iter, double tol, double reg,
                                                unsigned long long seed, const int* __restrict__ init_labels, int CL, GmmWs w)
 {
@@ -271,6 +359,7 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
     __shared__ double s_x[GT];
     __shared__ double s_red[GT / 32];
     __shared__ double s_logdet[KMAX];
+    __shared__ double s_lower;
     __shared__ double s_cent[KMAX * DMAX];
     __shared__ double s_tot[KMAX * (1 + DMAX)];
     __shared__ int s_pick;
@@ -414,7 +503,7 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
     __syncthreads();
 
     // ---- EM ----
-    bool ok = m_step(xs, resp, n_lo, n_hi, N, D, K, reg, par, s_part, c);
+    bool ok = m_step<KIND>(xs, resp, n_lo, n_hi, N, D, K, reg, par, s_part, c, w.prior);
     double lower = -DBL_MAX;
     int it = 0, conv = 0;
     if (ok) {
@@ -423,7 +512,7 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
             if (threadIdx.x < K) {
                 double ld = 0;
                 for (int j = 0; j < D; ++j) ld += log(pc[(size_t)threadIdx.x * D * D + j * D + j]);
-                s_logdet[threadIdx.x] = ld + log(wts[threadIdx.x]);
+                s_logdet[threadIdx.x] = KIND == MIX_BGM ? bgm_log_const(threadIdx.x, K, D, wts, ld) : ld + log(wts[threadIdx.x]);
             }
             __syncthreads();
             double acc = 0;
@@ -431,11 +520,31 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
                 double lw[KMAX];
                 double lse = log_prob_all(xs + (size_t)n * D, D, K, wts, mu, pc, s_logdet, lw);
                 for (int k = 0; k < K; ++k) resp[(size_t)n * K + k] = exp(lw[k] - lse);
-                acc += lse;
+                if (KIND == MIX_BGM) {
+                    for (int k = 0; k < K; ++k) acc += exp(lw[k] - lse) * (lw[k] - lse);   // sum r log r
+                } else {
+                    acc += lse;
+                }
             }
-            lower = cluster_sum(acc, c) / N;
-            ok = m_step(xs, resp, n_lo, n_hi, N, D, K, reg, par, s_part, c);
+            if (KIND == MIX_GMM) lower = cluster_sum(acc, c) / N;
+            const double ent = KIND == MIX_BGM ? cluster_sum(acc, c) : 0.0;
+            ok = m_step<KIND>(xs, resp, n_lo, n_hi, N, D, K, reg, par, s_part, c, w.prior);
             if (!ok) break;
+            if (KIND == MIX_BGM) {
+                // the ELBO with the parameters of this M-step and the responsibilities of the E-step before it
+                if (threadIdx.x == 0) {
+                    double ldk[KMAX];
+                    for (int k = 0; k < K; ++k) {
+                        double ld = 0;
+                        for (int j = 0; j < D; ++j) ld += log(pc[(size_t)k * D * D + j * D + j]);
+                        ldk[k] = ld;
+                    }
+                    s_lower = -ent + bgm_lower_params(K, D, wts, ldk);
+                }
+                __syncthreads();
+                lower = s_lower;
+                __syncthreads();
+            }
             if (it > 1 && fabs(lower - prev) < tol) { conv = 1; break; }
         }
         if (it > max_iter) it = max_iter;
@@ -771,6 +880,9 @@ __global__ void __launch_bounds__(1024) k_big_means(int N_in, const int* n_dev, 
 
 // per (restart, component): covariance from the split-K Gram partials, Cholesky factor (to global memory for k_big_inv), log-determinant
 // + log weight.  One CTA of 1024 threads; L lives in shared memory as a packed lower triangle (row i at i (i + 1) / 2).
+// MIX_BGM: the covariance is the Wishart posterior's, an affine function of the same Gram matrix; the means become the posterior's
+// once the covariance has read xk; the weights slot keeps nk; ldw gets the BGM constant and bld the bare log-determinant
+template <int KIND>
 __global__ void __launch_bounds__(1024) k_big_chol(int N_in, const int* n_dev, int D, int K, double reg, GmmWs w)
 {
     extern __shared__ double Ls[];
@@ -794,11 +906,20 @@ __global__ void __launch_bounds__(1024) k_big_chol(int N_in, const int* n_dev, i
         const int src = a <= b ? a * D + b : b * D + a;
         double g = 0;
         for (int sp = 0; sp < KS; ++sp) g += G[(size_t)sp * D * D + src];
-        const double c = g / nk + (a == b ? reg : 0.0);
+        double c = g / nk + (a == b ? reg : 0.0);
+        if (KIND == MIX_BGM) {
+            const double* mu = par + K + (size_t)k * D;
+            const double da = mu[a] - w.prior[a], db = mu[b] - w.prior[b];
+            c = (w.prior[D + a * D + b] + nk * c + nk * 1.0 / (1.0 + nk) * (da * db)) / (D + nk);
+        }
         Cm[i] = c;
         if (b <= a) Ls[a * (a + 1) / 2 + b] = c;
     }
     __syncthreads();
+    if (KIND == MIX_BGM) {
+        double* mu = par + K + (size_t)k * D;
+        for (int d = tid; d < D; d += T) mu[d] = (1.0 * w.prior[d] + nk * mu[d]) / (1.0 + nk);
+    }
     // blocked right-looking Cholesky on the packed lower triangle, panels of PB columns, three block-wide barriers per PANEL:
     //   (a) the PB x PB diagonal block, unblocked, by one warp (lane = row of the block, warp barriers only)
     //   (b) the panel below it: every row solves its own small triangular system against the finished diagonal block
@@ -875,11 +996,18 @@ __global__ void __launch_bounds__(1024) k_big_chol(int N_in, const int* n_dev, i
         if (lane == 0) {
             double t = 0;
             for (int i = 0; i < 32; ++i) t += s_ld[i];
-            w.ldw[init * K + k] = t + log(nk / N);
+            if (KIND == MIX_BGM) {
+                w.bld[init * K + k] = t;
+                w.ldw[init * K + k] = bgm_log_const(k, K, D, wts, t);   // reads nk of every component: nothing overwrites them
+            } else {
+                w.ldw[init * K + k] = t + log(nk / N);
+            }
         }
     }
-    __syncthreads();   // every thread has read nk = wts[k]
-    if (tid == 0) wts[k] = nk / N;
+    if (KIND == MIX_GMM) {
+        __syncthreads();   // every thread has read nk = wts[k]
+        if (tid == 0) wts[k] = nk / N;
+    }
 }
 
 // prec_chol = (L^-1)^T of one (restart, component) pair, the columns of Z = L^-1 dealt round-robin to CHOL_SPLIT CTAs x 32 warps:
@@ -953,6 +1081,8 @@ __global__ void __launch_bounds__(1024) k_big_bvec(int D, int K, GmmWs w)
 }
 
 // E-step after the GEMM: warp per sample; log N_k from |Y[r,k][n] - b[r,k]|^2, responsibilities, per-block log-likelihood sums
+// (MIX_BGM: per-block sums of sum_k r log r, the data term of the ELBO)
+template <int KIND>
 __global__ void __launch_bounds__(256) k_big_estep(int N_in, const int* n_dev, int D, int K, GmmWs w)
 {
     const int init = blockIdx.y;
@@ -984,6 +1114,11 @@ __global__ void __launch_bounds__(256) k_big_estep(int N_in, const int* n_dev, i
                 w.resp[((size_t)init * N_in + n) * K + k] = r;
                 w.sresp[((size_t)init * N_in + n) * K + k] = sqrt(r);
             }
+        if (KIND == MIX_BGM) {
+            double e = 0;
+            for (int k = 0; k < K; ++k) e += exp(lw[k] - lse) * (lw[k] - lse);
+            lse = e;
+        }
     }
     if (lane == 0) s_lse[wl] = lse;
     __syncthreads();
@@ -995,6 +1130,7 @@ __global__ void __launch_bounds__(256) k_big_estep(int N_in, const int* n_dev, i
 }
 
 // after E + M: the lower bound of this iteration, convergence, bookkeeping (sklearn: the M-step runs before the test)
+template <int KIND>
 __global__ void k_big_converge(int N_in, const int* n_dev, int D, int K, int n_init, int it, int max_iter, double tol, GmmWs w)
 {
     const int N = n_dev ? min(*n_dev, N_in) : N_in;
@@ -1009,7 +1145,8 @@ __global__ void k_big_converge(int N_in, const int* n_dev, int D, int K, int n_i
         if (st[1] == 0.0) {
             double t = 0;
             for (int i = 0; i < nblk; ++i) t += w.lowpart[(size_t)init * stride + i];
-            const double lower = t / N;
+            const double lower = KIND == MIX_BGM ? -t + bgm_lower_params(K, D, w.par + (size_t)init * pstride(K, D), w.bld + init * K)
+                                                 : t / N;
             const bool conv = it > 1 && fabs(lower - st[0]) < tol;
             st[0] = lower;
             tail[0] = lower; tail[1] = (double)it; tail[2] = conv ? 1.0 : 0.0; tail[3] = 1.0;
@@ -1069,6 +1206,7 @@ __global__ void __launch_bounds__(256) k_big_proba(int N_in, const int* n_dev, i
     }
 }
 
+template <int KIND>
 static int fit_big(int N, const int* n_dev, int D, int K, int n_init, int max_iter, double tol, double reg, unsigned long long seed,
                    const int* init_labels, GmmWs& w, cudaStream_t st, int* best_out)
 {
@@ -1077,7 +1215,7 @@ static int fit_big(int N, const int* n_dev, int D, int K, int n_init, int max_it
     const size_t sND = (size_t)N * D, sDD = (size_t)D * D;
     const int ps = pstride(K, D);
     const size_t chol_smem = sizeof(double) * (size_t)D * (D + 1) / 2;
-    ISB_CUDA_CHECK(cudaFuncSetAttribute(k_big_chol, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chol_smem));
+    ISB_CUDA_CHECK(cudaFuncSetAttribute(k_big_chol<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chol_smem));
     ISB_CUDA_CHECK(cudaFuncSetAttribute(k_big_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chol_smem));
     auto m_step = [&]() -> int {
         k_big_means<<<dim3(K, n_init, (D + 31) / 32), 1024, 0, st>>>(N, n_dev, D, K, w);
@@ -1090,7 +1228,7 @@ static int fit_big(int N, const int* n_dev, int D, int K, int n_init, int max_it
                 w.xs, D, w.xs, D, w.gram, D, bs, D, D, N, n_dev, 0, w.state, K, 1, KS, 0, fw);
             ISB_LAUNCH_CHECK();
         }
-        k_big_chol<<<dim3(K, n_init), 1024, chol_smem, st>>>(N, n_dev, D, K, reg, w);
+        k_big_chol<KIND><<<dim3(K, n_init), 1024, chol_smem, st>>>(N, n_dev, D, K, reg, w);
         ISB_LAUNCH_CHECK();
         k_big_inv<<<dim3(K, n_init, CHOL_SPLIT), 1024, chol_smem, st>>>(D, K, w);
         ISB_LAUNCH_CHECK();
@@ -1108,10 +1246,10 @@ static int fit_big(int N, const int* n_dev, int D, int K, int n_init, int max_it
                 w.xs, D, w.par + K + K * D + (size_t)K * sDD, D, w.big, D, bs, N, D, D, n_dev, 1, w.state, K, 0, 1, 1, FuseW());
             ISB_LAUNCH_CHECK();
         }
-        k_big_estep<<<dim3((N + 7) / 8, n_init), 256, 0, st>>>(N, n_dev, D, K, w);
+        k_big_estep<KIND><<<dim3((N + 7) / 8, n_init), 256, 0, st>>>(N, n_dev, D, K, w);
         ISB_LAUNCH_CHECK();
         if (int rc = m_step()) return rc;
-        k_big_converge<<<1, 1024, 0, st>>>(N, n_dev, D, K, n_init, it, max_iter, tol, w);
+        k_big_converge<KIND><<<1, 1024, 0, st>>>(N, n_dev, D, K, n_init, it, max_iter, tol, w);
         ISB_LAUNCH_CHECK();
         int running = 0;
         ISB_CUDA_CHECK(cudaMemcpyAsync(&running, w.flag, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1133,6 +1271,7 @@ static int fit_big(int N, const int* n_dev, int D, int K, int n_init, int max_it
 }
 
 // select the best restart, evaluate predict_proba for every sample, export the parameters
+template <int KIND>
 __global__ void __launch_bounds__(256) k_gmm_predict(int N_in, const int* n_dev, int D, int K, int n_init, GmmWs w, double* proba,
                                                     double* params_out)
 {
@@ -1155,7 +1294,7 @@ __global__ void __launch_bounds__(256) k_gmm_predict(int N_in, const int* n_dev,
     if (threadIdx.x < K) {
         double ld = 0;
         for (int j = 0; j < D; ++j) ld += log(pc[(size_t)threadIdx.x * D * D + j * D + j]);
-        s_logdet[threadIdx.x] = ld + log(wts[threadIdx.x]);
+        s_logdet[threadIdx.x] = KIND == MIX_BGM ? bgm_log_const(threadIdx.x, K, D, wts, ld) : ld + log(wts[threadIdx.x]);
     }
     __syncthreads();
     for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x) {
@@ -1200,7 +1339,31 @@ __global__ void __launch_bounds__(256) k_mix_proba(const double* __restrict__ x,
     }
 }
 
-static size_t carve_gmm(GmmWs& w, void* ws, size_t bytes, int N, int D, int K, int n_init)
+// BayesianGaussianMixture priors from the scaled features: mean_prior_ = X.mean(0), covariance_prior_ = np.cov(X.T) (ddof 1).
+// One CTA per feature pair (a <= b): both column means, then the centred cross product.
+__global__ void __launch_bounds__(GT) k_bgm_prior(int N_in, const int* n_dev, int D, GmmWs w)
+{
+    __shared__ double s_red[GT / 32];
+    const int N = n_dev ? min(*n_dev, N_in) : N_in;
+    int t = blockIdx.x, a = 0;
+    while (t >= D - a) { t -= D - a; ++a; }
+    const int b = a + t;
+    const double* xs = w.xs;
+    double sa = 0, sb = 0;
+    for (int n = threadIdx.x; n < N; n += GT) { sa += xs[(size_t)n * D + a]; sb += xs[(size_t)n * D + b]; }
+    const double ma = block_sum_d(sa, s_red) / N;
+    const double mb = block_sum_d(sb, s_red) / N;
+    double v = 0;
+    for (int n = threadIdx.x; n < N; n += GT) v += (xs[(size_t)n * D + a] - ma) * (xs[(size_t)n * D + b] - mb);
+    const double c = block_sum_d(v, s_red) / (N - 1);
+    if (threadIdx.x == 0) {
+        w.prior[D + a * D + b] = c;
+        w.prior[D + b * D + a] = c;
+        if (a == b) w.prior[a] = ma;
+    }
+}
+
+static size_t carve_gmm(GmmWs& w, void* ws, size_t bytes, int N, int D, int K, int n_init, int kind = MIX_GMM)
 {
     WsCarver c(ws, bytes);
     w.xs = c.take<double>((size_t)N * D);
@@ -1222,6 +1385,324 @@ static size_t carve_gmm(GmmWs& w, void* ws, size_t bytes, int N, int D, int K, i
         w.state = c.take<double>((size_t)n_init * 4);
         w.flag = c.take<int>(1);
     }
+    w.prior = w.bld = nullptr;
+    if (kind == MIX_BGM) {
+        w.prior = c.take<double>((size_t)D + (size_t)D * D);
+        w.bld = c.take<double>((size_t)n_init * K);
+    }
+    return isb_align(c.off);
+}
+
+template <int KIND>
+static int mixture_fit_predict(const double* feat, int N, int D, int ld, const int32_t* n_dev, int K, int n_init, int max_iter, double tol,
+                               double reg_covar, int use_scaler, unsigned long long seed, const int32_t* init_labels, double* proba,
+                               double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    ISB_REQUIRE(feat && proba && ws, "null pointer");
+    ISB_REQUIRE(N > 0 && D > 0 && ld >= D && K > 0 && n_init > 0 && max_iter > 0, "bad sizes");
+    if (D > DBIG || K > KMAX) {
+        isb_set_error("device %s handles D <= %d and K <= %d (got D=%d K=%d)", KIND == MIX_BGM ? "mixture" : "GMM", DBIG, KMAX, D, K);
+        return ISB_ERR_UNSUPPORTED;
+    }
+    GmmWs w;
+    size_t need = carve_gmm(w, ws, ws_bytes, N, D, K, n_init, KIND);
+    ISB_REQUIRE(need <= ws_bytes, "workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfScope prof(ISB_PROF_GMM, st);
+    if (D > DMAX) {
+        int best = -1;
+        k_big_scale<<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
+        ISB_LAUNCH_CHECK();
+        if (KIND == MIX_BGM) {
+            k_bgm_prior<<<D * (D + 1) / 2, GT, 0, st>>>(N, n_dev, D, w);
+            ISB_LAUNCH_CHECK();
+            if (params_out)   // the priors follow the GMM layout of params_out
+                ISB_CUDA_CHECK(cudaMemcpyAsync(params_out + 2 * D + pstride(K, D) + 1, w.prior, sizeof(double) * ((size_t)D + (size_t)D * D),
+                                               cudaMemcpyDeviceToDevice, st));
+        }
+        if (int rc = fit_big<KIND>(N, n_dev, D, K, n_init, max_iter, tol, reg_covar, seed, init_labels, w, st, &best)) return rc;
+        if (best >= 0) {
+            k_big_proba<<<(N + 7) / 8, 256, 0, st>>>(N, n_dev, D, K, best, w, proba, params_out);
+            ISB_LAUNCH_CHECK();
+            return ISB_OK;
+        }
+        // every restart failed: fall through to k_gmm_predict, which reports it (NaN probabilities, ok = 0)
+    } else {
+        k_gmm_scale<<<D, GT, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
+        ISB_LAUNCH_CHECK();
+        if (KIND == MIX_BGM) {
+            k_bgm_prior<<<D * (D + 1) / 2, GT, 0, st>>>(N, n_dev, D, w);
+            ISB_LAUNCH_CHECK();
+            if (params_out)   // the priors follow the GMM layout of params_out
+                ISB_CUDA_CHECK(cudaMemcpyAsync(params_out + 2 * D + pstride(K, D) + 1, w.prior, sizeof(double) * ((size_t)D + (size_t)D * D),
+                                               cudaMemcpyDeviceToDevice, st));
+        }
+        // one thread-block cluster per restart; the cluster size follows the (upper bound of the) sample count
+        const int CL = N <= 1024 ? 1 : (N <= 4096 ? 2 : (N <= 16384 ? 4 : 8));
+        const size_t par_bytes = sizeof(double) * (size_t)pstride(K, D);
+        ISB_CUDA_CHECK(cudaFuncSetAttribute(k_gmm_fit<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)par_bytes));
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(n_init * CL); cfg.blockDim = dim3(GT); cfg.dynamicSmemBytes = par_bytes; cfg.stream = st;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+        ISB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_gmm_fit<KIND>, N, n_dev, D, K, max_iter, tol, reg_covar, seed, init_labels, CL, w));
+        ISB_LAUNCH_CHECK();
+    }
+    int blocks = (N + 255) / 256;
+    if (blocks > 132) blocks = 132;
+    k_gmm_predict<KIND><<<blocks, 256, 0, st>>>(N, n_dev, D, K, n_init, w, proba, params_out);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// PCA fit: sklearn.decomposition.PCA with the covariance_eigh solver (the one it picks for N >= 10 D, D <= 1000 -- every superpixel
+// feature table), restated on the device:  C = (X^T X - n mu mu^T) / (n - 1) on the scaled features, symmetric eigensolver, descending
+// order, negative eigenvalues clipped to 0, svd_flip(u_based_decision=False) on the rows of components_, explained variance ratio,
+// component count from the ratio (float pca_coef) or as given, noise variance.
+// X^T X is the split-K Gram GEMM of the mixture M-step; the eigensolver is Householder tridiagonalisation + implicit QL (the rotations
+// of one QL sweep are found by one thread, then every thread applies them to its row of the eigenvector matrix), one CTA of 1024
+// threads, the matrices in global memory (L2 resident, <= 430 KB each).
+// ---------------------------------------------------------------------------------------------------------------------
+
+struct PcaWs {
+    double* xs;       // [N, D] scaled features
+    double* scale;    // [2 D] scaler mean, scale
+    double* gram;     // [KS, D, D] split-K partials of X^T X (tiles on or above the diagonal)
+    double* A;        // [D, D] covariance, reduced in place
+    double* Zt;       // [D, D] eigenvector matrix, transposed: Zt[c * D + r] = Z[r][c] (row c = eigenvector c)
+    double* Hv;       // [D, D] Householder vectors (row k: vector of step k at its absolute indices k + 1 ..)
+    double* hs;       // [D]    their h = |v|^2 / 2 (0: step skipped)
+};
+
+constexpr int PT = 1024;   // threads of the eigensolver CTA
+
+__device__ double block_sum_pt(double v, double* s_red)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double t = 0;
+    for (int i = 0; i < PT / 32; ++i) t += s_red[i];
+    return t;
+}
+
+// params_out (isb_pca_params_len(D) doubles): scaler mean[D] | scaler scale[D] | mean_[D] | components_[D, D] | explained_variance_[D] |
+// explained_variance_ratio_[D] | singular_values_[D] | mean_ components_^T [D] | n_components | noise_variance | n_samples | ok
+__global__ void __launch_bounds__(PT) k_pca_eig(int N_in, const int* n_dev, int D, double coef, int n_req, PcaWs p, double* out,
+                                              int* n_comp_out)
+{
+    __shared__ double s_red[PT / 32];
+    __shared__ double s_mean[DBIG], s_v[DBIG], s_p[DBIG], s_d[DBIG], s_e[DBIG], s_rs[DBIG], s_rc[DBIG];
+    __shared__ int s_rank[DBIG];
+    __shared__ int s_nrot, s_i0, s_done, s_fail;
+    const int N = n_dev ? min(*n_dev, N_in) : N_in;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = PT / 32;
+    const int n = D;
+    double* A = p.A; double* Zt = p.Zt;
+    // mean_ of the scaled features: warps over the samples, lanes over 32 features at a time, warp partials in warp order
+    for (int d0 = 0; d0 < D; d0 += 32) {
+        const int d = d0 + lane;
+        double a = 0;
+        if (d < D) for (int i = wid; i < N; i += nw) a += p.xs[(size_t)i * D + d];
+        __shared__ double s_acc[PT / 32][33];
+        s_acc[wid][lane] = a;
+        __syncthreads();
+        if (wid == 0 && d < D) { double t = 0; for (int i = 0; i < nw; ++i) t += s_acc[i][lane]; s_mean[d] = t / N; }
+        __syncthreads();
+    }
+    // C = (X^T X - n mu mu^T) / (n - 1); the Gram partials added in split order, (a, b) below the diagonal read from (b, a)
+    for (int i = tid; i < n * n; i += PT) {
+        const int a = i / n, b = i % n, src = a <= b ? a * n + b : b * n + a;
+        double g = 0;
+        for (int sp = 0; sp < KS; ++sp) g += p.gram[(size_t)sp * n * n + src];
+        A[i] = (g - (double)N * s_mean[a] * s_mean[b]) / (double)(N - 1);
+        Zt[i] = a == b ? 1.0 : 0.0;
+    }
+    __syncthreads();
+    // Householder tridiagonalisation: step k maps A[k+1.., k] to (alpha, 0, ..) with H = I - v v^T / h
+    for (int k = 0; k + 2 < n; ++k) {
+        const int m = n - k - 1, o = k + 1;
+        double sq = 0;
+        for (int i = 1 + tid; i < m; i += PT) { const double x = A[(size_t)(o + i) * n + k]; sq += x * x; }
+        const double tail = block_sum_pt(sq, s_red);
+        const double x0 = A[(size_t)o * n + k];
+        if (tail == 0.0) {   // already tridiagonal in this column
+            if (tid == 0) { s_e[k] = x0; s_d[k] = A[(size_t)k * n + k]; p.hs[k] = 0.0; }
+            __syncthreads();
+            continue;
+        }
+        const double sigma = x0 * x0 + tail;
+        const double alpha = -copysign(sqrt(sigma), x0), h = sigma - x0 * alpha;
+        for (int i = tid; i < m; i += PT) {
+            const double v = i == 0 ? x0 - alpha : A[(size_t)(o + i) * n + k];
+            s_v[i] = v;
+            p.Hv[(size_t)k * n + o + i] = v;
+        }
+        if (tid == 0) { s_e[k] = alpha; s_d[k] = A[(size_t)k * n + k]; p.hs[k] = h; }
+        __syncthreads();
+        // p = A_sub v / h, a warp per row
+        for (int i = wid; i < m; i += nw) {
+            double a = 0;
+            for (int j = lane; j < m; j += 32) a += A[(size_t)(o + i) * n + o + j] * s_v[j];
+#pragma unroll
+            for (int q = 16; q > 0; q >>= 1) a += __shfl_xor_sync(0xffffffffu, a, q);
+            if (lane == 0) s_p[i] = a / h;
+        }
+        __syncthreads();
+        double vp = 0;
+        for (int i = tid; i < m; i += PT) vp += s_v[i] * s_p[i];
+        const double kc = block_sum_pt(vp, s_red) / (2.0 * h);
+        for (int i = tid; i < m; i += PT) s_p[i] = s_p[i] - kc * s_v[i];   // q
+        __syncthreads();
+        for (int i = tid; i < m * m; i += PT) {
+            const int r = i / m, c = i % m;
+            A[(size_t)(o + r) * n + o + c] -= s_v[r] * s_p[c] + s_p[r] * s_v[c];
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        if (n >= 2) { s_d[n - 2] = A[(size_t)(n - 2) * n + n - 2]; s_e[n - 2] = A[(size_t)(n - 1) * n + n - 2]; }
+        s_d[n - 1] = A[(size_t)(n - 1) * n + n - 1];
+        s_e[n - 1] = 0.0;
+    }
+    __syncthreads();
+    // Q = H_0 H_1 .. H_{n-3}, built from the last reflector: Q_sub -= v (v^T Q_sub) / h, columns >= k + 1
+    for (int k = n - 3; k >= 0; --k) {
+        const double h = p.hs[k];
+        if (h == 0.0) continue;
+        const int o = k + 1, m = n - o;
+        const double* v = p.Hv + (size_t)k * n + o;
+        for (int c = wid; c < m; c += nw) {
+            double a = 0;
+            for (int r = lane; r < m; r += 32) a += v[r] * Zt[(size_t)(o + c) * n + o + r];
+#pragma unroll
+            for (int q = 16; q > 0; q >>= 1) a += __shfl_xor_sync(0xffffffffu, a, q);
+            if (lane == 0) s_p[c] = a / h;
+        }
+        __syncthreads();
+        for (int i = tid; i < m * m; i += PT) {
+            const int c = i / m, r = i % m;
+            Zt[(size_t)(o + c) * n + o + r] -= v[r] * s_p[c];
+        }
+        __syncthreads();
+    }
+    // implicit QL with shifts on (d, e): thread 0 finds the rotations of a sweep, every thread applies them to its row of Z
+    {
+        int l = 0, iter = 0;
+        if (tid == 0) { s_fail = 0; }
+        while (true) {
+            if (tid == 0) {
+                s_nrot = 0; s_done = 0;
+                while (l < n) {
+                    int mm = l;
+                    for (; mm < n - 1; ++mm) { const double dd = fabs(s_d[mm]) + fabs(s_d[mm + 1]); if (fabs(s_e[mm]) + dd == dd) break; }
+                    if (mm == l) { ++l; iter = 0; continue; }
+                    if (iter++ == 60) { s_fail = 1; ++l; iter = 0; continue; }
+                    double g = (s_d[l + 1] - s_d[l]) / (2.0 * s_e[l]);
+                    double r = hypot(g, 1.0);
+                    g = s_d[mm] - s_d[l] + s_e[l] / (g + copysign(r, g));
+                    double sn = 1.0, c = 1.0, pp = 0.0;
+                    int i = mm - 1;
+                    bool under = false;
+                    for (; i >= l; --i) {
+                        double f = sn * s_e[i], b = c * s_e[i];
+                        s_e[i + 1] = (r = hypot(f, g));
+                        if (r == 0.0) { s_d[i + 1] -= pp; s_e[mm] = 0.0; under = true; break; }
+                        sn = f / r; c = g / r; g = s_d[i + 1] - pp; r = (s_d[i] - g) * sn + 2.0 * c * b; s_d[i + 1] = g + (pp = sn * r); g = c * r - b;
+                        s_rs[s_nrot] = sn; s_rc[s_nrot] = c; ++s_nrot;
+                    }
+                    s_i0 = mm - 1;
+                    if (!under) { s_d[l] -= pp; s_e[l] = g; s_e[mm] = 0.0; }
+                    break;   // apply this sweep's rotations
+                }
+                if (l >= n) s_done = 1;
+            }
+            __syncthreads();
+            const int nrot = s_nrot, i0 = s_i0;
+            if (nrot > 0 && tid < n) {
+                // rotation t acts on columns i = i0 - t and i + 1 of Z
+                for (int t = 0; t < nrot; ++t) {
+                    const int i = i0 - t;
+                    const double sn = s_rs[t], c = s_rc[t];
+                    const double f = Zt[(size_t)(i + 1) * n + tid], zi = Zt[(size_t)i * n + tid];
+                    Zt[(size_t)(i + 1) * n + tid] = sn * zi + c * f;
+                    Zt[(size_t)i * n + tid] = c * zi - sn * f;
+                }
+            }
+            const int done = s_done;
+            __syncthreads();
+            if (done) break;
+        }
+    }
+    // descending order (eigh is ascending, sklearn flips it), clip at 0, svd_flip on the rows, ratios, component count
+    for (int i = tid; i < n; i += PT) {
+        const double di = s_d[i];
+        int rk = 0;
+        for (int j = 0; j < n; ++j) rk += (s_d[j] > di || (s_d[j] == di && j > i)) ? 1 : 0;
+        s_rank[i] = rk;
+    }
+    __syncthreads();
+    double* o_mean = out + 2 * D; double* o_comp = out + 3 * D; double* o_ev = o_comp + (size_t)D * D;
+    double* o_ratio = o_ev + D; double* o_sv = o_ratio + D; double* o_mproj = o_sv + D; double* o_tail = o_mproj + D;
+    for (int i = tid; i < 2 * D; i += PT) out[i] = p.scale[i];
+    for (int i = tid; i < D; i += PT) o_mean[i] = s_mean[i];
+    for (int i = wid; i < n; i += nw) {   // a warp per eigenvector: the first entry of largest magnitude decides the sign
+        const double* z = Zt + (size_t)i * n;
+        double best = -1.0; int bj = n;
+        for (int j = lane; j < n; j += 32) { const double a = fabs(z[j]); if (a > best) { best = a; bj = j; } }
+#pragma unroll
+        for (int q = 16; q > 0; q >>= 1) {
+            const double ob = __shfl_xor_sync(0xffffffffu, best, q);
+            const int oj = __shfl_xor_sync(0xffffffffu, bj, q);
+            if (ob > best || (ob == best && oj < bj)) { best = ob; bj = oj; }
+        }
+        const double sg = z[bj] > 0 ? 1.0 : (z[bj] < 0 ? -1.0 : 0.0);
+        const int r = s_rank[i];
+        for (int j = lane; j < n; j += 32) o_comp[(size_t)r * n + j] = sg * z[j];
+        if (lane == 0) o_ev[r] = s_d[i] < 0.0 ? 0.0 : s_d[i];
+    }
+    __syncthreads();
+    double tv = 0;
+    for (int i = tid; i < n; i += PT) tv += o_ev[i];
+    const double total = block_sum_pt(tv, s_red);
+    for (int i = tid; i < n; i += PT) {
+        o_ratio[i] = o_ev[i] / total;
+        o_sv[i] = sqrt(o_ev[i] * (double)(N - 1));
+        double a = 0;
+        for (int j = 0; j < n; ++j) a = fma(s_mean[j], o_comp[(size_t)i * n + j], a);
+        o_mproj[i] = a;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int nc = n_req;
+        if (nc <= 0) {   // searchsorted(cumsum(ratio), coef, side='right') + 1
+            double cs = 0; nc = 0;
+            for (int i = 0; i < n; ++i) { cs += o_ratio[i]; if (cs <= coef) ++nc; else break; }
+            nc += 1;
+        }
+        nc = max(1, min(nc, n));
+        double noise = 0.0;
+        if (nc < min(n, N)) { for (int i = nc; i < n; ++i) noise += o_ev[i]; noise /= (n - nc); }
+        o_tail[0] = nc; o_tail[1] = noise; o_tail[2] = N; o_tail[3] = s_fail ? 0.0 : 1.0;
+        if (n_comp_out) *n_comp_out = nc;
+    }
+}
+
+static size_t carve_pca(PcaWs& p, void* ws, size_t bytes, int N, int D)
+{
+    WsCarver c(ws, bytes);
+    p.xs = c.take<double>((size_t)N * D);
+    p.scale = c.take<double>(2 * (size_t)D);
+    p.gram = c.take<double>((size_t)KS * D * D);
+    p.A = c.take<double>((size_t)D * D);
+    p.Zt = c.take<double>((size_t)D * D);
+    p.Hv = c.take<double>((size_t)D * D);
+    p.hs = c.take<double>((size_t)D);
     return isb_align(c.off);
 }
 
@@ -1239,46 +1720,32 @@ extern "C" int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, con
                                    double tol, double reg_covar, int use_scaler, unsigned long long seed, const int32_t* init_labels,
                                    double* proba, double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream)
 {
-    ISB_REQUIRE(feat && proba && ws, "null pointer");
-    ISB_REQUIRE(N > 0 && D > 0 && ld >= D && K > 0 && n_init > 0 && max_iter > 0, "bad sizes");
-    if (D > DBIG || K > KMAX) { isb_set_error("device GMM handles D <= %d and K <= %d (got D=%d K=%d)", DBIG, KMAX, D, K); return ISB_ERR_UNSUPPORTED; }
+    return mixture_fit_predict<MIX_GMM>(feat, N, D, ld, n_dev, K, n_init, max_iter, tol, reg_covar, use_scaler, seed, init_labels, proba,
+                                        params_out, ws, ws_bytes, stream);
+}
+
+extern "C" size_t isb_mixture_fit_workspace_bytes(int kind, int N, int D, int K, int n_init)
+{
     GmmWs w;
-    size_t need = carve_gmm(w, ws, ws_bytes, N, D, K, n_init);
-    ISB_REQUIRE(need <= ws_bytes, "workspace too small");
-    cudaStream_t st = (cudaStream_t)stream;
-    ProfScope prof(ISB_PROF_GMM, st);
-    if (D > DMAX) {
-        int best = -1;
-        k_big_scale<<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
-        ISB_LAUNCH_CHECK();
-        if (int rc = fit_big(N, n_dev, D, K, n_init, max_iter, tol, reg_covar, seed, init_labels, w, st, &best)) return rc;
-        if (best >= 0) {
-            k_big_proba<<<(N + 7) / 8, 256, 0, st>>>(N, n_dev, D, K, best, w, proba, params_out);
-            ISB_LAUNCH_CHECK();
-            return ISB_OK;
-        }
-        // every restart failed: fall through to k_gmm_predict, which reports it (NaN probabilities, ok = 0)
-    } else {
-        k_gmm_scale<<<D, GT, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
-        ISB_LAUNCH_CHECK();
-        // one thread-block cluster per restart; the cluster size follows the (upper bound of the) sample count
-        const int CL = N <= 1024 ? 1 : (N <= 4096 ? 2 : (N <= 16384 ? 4 : 8));
-        const size_t par_bytes = sizeof(double) * (size_t)pstride(K, D);
-        ISB_CUDA_CHECK(cudaFuncSetAttribute(k_gmm_fit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)par_bytes));
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(n_init * CL); cfg.blockDim = dim3(GT); cfg.dynamicSmemBytes = par_bytes; cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        ISB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_gmm_fit, N, n_dev, D, K, max_iter, tol, reg_covar, seed, init_labels, CL, w));
-        ISB_LAUNCH_CHECK();
-    }
-    int blocks = (N + 255) / 256;
-    if (blocks > 132) blocks = 132;
-    k_gmm_predict<<<blocks, 256, 0, st>>>(N, n_dev, D, K, n_init, w, proba, params_out);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
+    return carve_gmm(w, nullptr, 0, N, D, K, n_init, kind == MIX_BGM ? MIX_BGM : MIX_GMM);
+}
+
+extern "C" int isb_mixture_fit_params_len(int kind, int D, int K)
+{
+    return 2 * D + pstride(K, D) + 1 + (kind == MIX_BGM ? D + D * D : 0);
+}
+
+extern "C" int isb_mixture_fit_predict(int kind, const double* feat, int N, int D, int ld, const int32_t* n_dev, int K, int n_init,
+                                       int max_iter, double tol, double reg_covar, int use_scaler, unsigned long long seed,
+                                       const int32_t* init_labels, double* proba, double* params_out, void* ws, size_t ws_bytes,
+                                       isb_stream_t stream)
+{
+    if (kind == MIX_GMM)
+        return mixture_fit_predict<MIX_GMM>(feat, N, D, ld, n_dev, K, n_init, max_iter, tol, reg_covar, use_scaler, seed, init_labels, proba,
+                                            params_out, ws, ws_bytes, stream);
+    ISB_REQUIRE(kind == MIX_BGM, "unknown mixture kind");
+    return mixture_fit_predict<MIX_BGM>(feat, N, D, ld, n_dev, K, n_init, max_iter, tol, reg_covar, use_scaler, seed, init_labels, proba,
+                                        params_out, ws, ws_bytes, stream);
 }
 
 extern "C" size_t isb_mixture_predict_workspace_bytes(int N, int D, int K)
@@ -1315,6 +1782,38 @@ extern "C" int isb_mixture_predict_proba(const double* x, int N, const int32_t* 
         x, D, prec_chol, D, w.big, D, bs, N, D, D, n_dev, 1, nullptr, K, 0, 1, 0, FuseW());
     ISB_LAUNCH_CHECK();
     k_big_proba<<<(N + 7) / 8, 256, 0, st>>>(N, n_dev, D, K, 0, w, proba, nullptr);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" size_t isb_pca_workspace_bytes(int N, int D)
+{
+    PcaWs p;
+    return carve_pca(p, nullptr, 0, N > 0 ? N : 0, D > 0 ? D : 0);
+}
+
+extern "C" int isb_pca_params_len(int D) { return D * D + 7 * D + 4; }
+
+extern "C" int isb_pca_fit(const double* feat, int N, int D, int ld, const int32_t* n_dev, int use_scaler, double coef, int n_components,
+                           double* params_out, int32_t* n_components_out, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    ISB_REQUIRE(feat && params_out && ws, "null pointer");
+    ISB_REQUIRE(N > 1 && D > 0 && ld >= D, "bad sizes");
+    ISB_REQUIRE(n_components > 0 ? n_components <= D : (coef > 0.0 && coef < 1.0), "n_components must be in [1, D] or coef in (0, 1)");
+    if (D > DBIG) { isb_set_error("device PCA handles D <= %d (got D=%d)", DBIG, D); return ISB_ERR_UNSUPPORTED; }
+    PcaWs p;
+    ISB_REQUIRE(carve_pca(p, ws, ws_bytes, N, D) <= ws_bytes, "workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfScope prof(ISB_PROF_GMM, st);
+    GmmWs w = {};
+    w.xs = p.xs; w.scale = p.scale;
+    k_big_scale<<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
+    ISB_LAUNCH_CHECK();
+    const BatchStride bs = { 0, 0, 0, 0, 0, 0, (size_t)D * D };
+    k_dgemm_batched<true, false><<<dim3((D + TN - 1) / TN, (D + TM - 1) / TM, KS), 256, 0, st>>>(
+        p.xs, D, p.xs, D, p.gram, D, bs, D, D, N, n_dev, 0, nullptr, 1, 1, KS, 0, FuseW());
+    ISB_LAUNCH_CHECK();
+    k_pca_eig<<<1, PT, 0, st>>>(N, n_dev, D, coef, n_components, p, params_out, n_components_out);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }

@@ -437,6 +437,57 @@ class Engine(object):
                                          _lib.ptr(proba), _lib.ptr(params), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
         return proba, params
 
+    #: isb_mixture_fit_predict kinds
+    MIXTURE_KINDS = {'GMM': 0, 'BGM': 1}
+
+    def mixture_fit_predict(self, d_feat, K, n_init, max_iter, use_scaler=True, seed=0, d_n=None, init_labels=None, tol=1e-3,
+                            reg_covar=1e-6, kind='GMM'):
+        """device class model of either kind ('GMM' = :meth:`gmm_fit_predict`, 'BGM' = BayesianGaussianMixture): returns
+        (proba [N,K] device, params device vector; see isb_mixture_fit_predict)"""
+        if kind == 'GMM':
+            return self.gmm_fit_predict(d_feat, K, n_init, max_iter, use_scaler, seed, d_n, init_labels, tol, reg_covar)
+        torch, lib = self.torch, self.lib
+        code = self.MIXTURE_KINDS[kind]
+        N, D = int(d_feat.shape[0]), int(d_feat.shape[1])
+        proba = self.buf('proba', (N, K), torch.float64)
+        params = self.buf('mixture_params', (lib.isb_mixture_fit_params_len(code, D, K),), torch.float64)
+        wsb = lib.isb_mixture_fit_workspace_bytes(code, N, D, int(K), int(n_init))
+        ws = self.buf('ws_gmm', (wsb,), torch.uint8)
+        d_init = None
+        if init_labels is not None:
+            d_init = self.to_device(np.ascontiguousarray(init_labels, dtype=np.int32), 'gmm_init')
+        self._ck(lib.isb_mixture_fit_predict(code, _lib.ptr(d_feat), N, D, int(d_feat.stride(0)), _lib.ptr(d_n), int(K), int(n_init),
+                                             int(max_iter), C.c_double(tol), C.c_double(reg_covar), int(bool(use_scaler)),
+                                             C.c_ulonglong(int(seed)), _lib.ptr(d_init), _lib.ptr(proba), _lib.ptr(params), _lib.ptr(ws),
+                                             C.c_size_t(wsb), _lib.stream_ptr()))
+        return proba, params
+
+    def pca_fit_transform(self, d_feat, use_scaler, pca_coef, d_n=None):
+        """scaler + PCA(pca_coef) fitted on features [N, D] (device; isb_pca_fit) and applied to them by isb_class_transform: returns
+        (transformed [N, D'] device, params device vector, D').  A float ``pca_coef`` makes D' depend on the data: it is read back
+        (4 bytes, one synchronisation); an int fixes it."""
+        torch, lib = self.torch, self.lib
+        N, D = int(d_feat.shape[0]), int(d_feat.shape[1])
+        ld = int(d_feat.stride(0))
+        params = self.buf('pca_params', (lib.isb_pca_params_len(D),), torch.float64)
+        n_comp = self.buf('pca_n_comp', (1,), torch.int32)
+        wsb = lib.isb_pca_workspace_bytes(N, D)
+        ws = self.buf('ws_pca', (wsb,), torch.uint8)
+        is_int = isinstance(pca_coef, (int, np.integer))
+        st = _lib.stream_ptr()
+        self._ck(lib.isb_pca_fit(_lib.ptr(d_feat), N, D, ld, _lib.ptr(d_n), int(bool(use_scaler)), C.c_double(0.0 if is_int else pca_coef),
+                                 int(pca_coef) if is_int else 0, _lib.ptr(params), _lib.ptr(n_comp), _lib.ptr(ws), C.c_size_t(wsb), st))
+        dims = int(pca_coef) if is_int else int(self.to_host(n_comp)[0])
+        comp = params[3 * D:3 * D + dims * D]
+        mproj = params[3 * D + D * D + 3 * D:3 * D + D * D + 3 * D + dims]
+        x = self.buf('pca_x', (N, dims), torch.float64)
+        twsb = lib.isb_class_transform_workspace_bytes(N, D, 1)
+        tws = self.buf('ws_pca_transform', (twsb,), torch.uint8)
+        self._ck(lib.isb_class_transform(_lib.ptr(d_feat), N, ld, _lib.ptr(d_n), D, _lib.ptr(params[:D]) if use_scaler else None,
+                                         _lib.ptr(params[D:2 * D]) if use_scaler else None, _lib.ptr(comp), _lib.ptr(mproj), None, dims,
+                                         _lib.ptr(x), _lib.ptr(tws), C.c_size_t(twsb), st))
+        return x, params, dims
+
     def class_model_predict(self, d_feat, cm, d_n=None):
         """predict_proba of a compiled caller-fitted model (class_models.CompiledModel) on features [N, >= n_features_in] (device):
         returns proba [N, K] device, asynchronous; the model's tables are device constants keyed on its digest"""

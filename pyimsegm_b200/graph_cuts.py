@@ -3,8 +3,9 @@ GraphCut on the superpixel graph, on the GPU.
 
 Mirror of the reference module ``imsegm/graph_cuts.py`` (same public names, arguments, error types).  The graph,
 the energies and the alpha-expansion itself run in CUDA behind ``include/imsegm_b200.h``
-(``isb_adjacency_edges`` / ``isb_gc_energies`` / ``isb_alpha_expansion``); the class model stays scikit-learn
-exactly as in the reference (``estim_class_model``, reference graph_cuts.py:73-163).
+(``isb_adjacency_edges`` / ``isb_gc_energies`` / ``isb_alpha_expansion``); the class model (``estim_class_model``, reference
+graph_cuts.py:73-163) is fitted on the device for every ``estim_model`` variant and ``pca_coef`` (``class_model_spec``) and returned
+as the reference's scikit-learn Pipeline; K > 8 and ``pca_coef='mle'`` fit with scikit-learn on the host.
 """
 import logging
 
@@ -26,8 +27,9 @@ MIN_UNARY_PROB = 0.01
 MAX_PAIRWISE_COST = 1e5
 #: edge weights are clamped to [1 / val, val] (reference graph_cuts.py:40)
 MIN_MAX_EDGE_WEIGHT = 1e3
-#: the default 'GMM' class model is fitted on the GPU (isb_gmm_fit_predict) when it fits the device kernel
-#: (<= 16 features, <= 8 classes, no PCA); set False to force scikit-learn on the host
+#: the class model of every estim_model variant, with or without PCA, is fitted on the GPU (isb_gmm_fit_predict /
+#: isb_mixture_fit_predict / isb_pca_fit) when it fits the device kernels (<= 232 features, <= 8 classes, pca_coef None, in (0, 1)
+#: or a component count); set False to force scikit-learn on the host
 USE_DEVICE_GMM = True
 #: a caller-fitted model (segment_color2d_slic_features_model_graphcut, segment_images_batch(model_pipeline=...), segment_resident)
 #: that class_models.compile_model supports runs its predict_proba on the device; set False to force the host round trip
@@ -112,14 +114,74 @@ def estim_class_model_kmeans(features, nb_classes, init_type='k-means++', max_it
     return gmm, y
 
 
+def class_model_spec(estim_model, nb_classes, max_iter=99):
+    """ (kind, n_init, max_iter) of the mixture that :func:`estim_class_model` fits for ``estim_model`` (reference
+    graph_cuts.py:107-163).  The reference's ``Pipeline.fit(X, y)`` hands the k-means / Otsu labels it computes to
+    ``GaussianMixture.fit``, which ignores them, so every variant but 'BGM' is a plain GaussianMixture with its own restart and
+    iteration counts.  This is the one place that interprets ``estim_model`` for the device fit.
+
+    :return tuple(str,int,int): kind 'GMM' (GaussianMixture) or 'BGM' (BayesianGaussianMixture), n_init, max_iter
+    """
+    nb_inits = max(1, int(np.sqrt(max_iter)))
+    name, init_type = estim_model, ''
+    if '_' in estim_model:
+        name, init_type = estim_model.split('_')[0], estim_model.split('_')[-1]
+    if name == 'GMM' and init_type in ('kmeans', 'Otsu'):
+        return 'GMM', 1, max_iter
+    if name == 'kmeans':
+        return 'GMM', nb_inits, 1
+    if name == 'BGM':
+        return 'BGM', nb_inits, max_iter
+    if name == 'Otsu' and nb_classes == 2:
+        return 'GMM', 1, 1
+    return 'GMM', nb_inits, max_iter
+
+
+def _device_pca_coef(pca_coef, nb_features):
+    """whether the device PCA takes this ``pca_coef``: None, a float in (0, 1) or a component count in [1, nb_features]"""
+    if pca_coef is None:
+        return True
+    if isinstance(pca_coef, (bool, np.bool_)):
+        return False
+    if isinstance(pca_coef, (int, np.integer)):
+        return 1 <= pca_coef <= nb_features
+    return isinstance(pca_coef, (float, np.floating)) and 0. < pca_coef < 1.
+
+
 def device_gmm_applicable(nb_features, nb_classes, estim_model='GMM', pca_coef=None):
-    return (USE_DEVICE_GMM and estim_model == 'GMM' and pca_coef is None and nb_features <= DEVICE_GMM_MAX_FEATURES
-            and nb_classes <= DEVICE_GMM_MAX_CLASSES)
+    """ whether :func:`estim_class_model` fits on the device: any ``estim_model`` string, ``pca_coef`` as in
+    :func:`_device_pca_coef`, <= 232 features and <= 8 classes ('mle' PCA and K > 8 stay on the host) """
+    return (USE_DEVICE_GMM and isinstance(estim_model, str) and _device_pca_coef(pca_coef, nb_features)
+            and nb_features <= DEVICE_GMM_MAX_FEATURES and nb_classes <= DEVICE_GMM_MAX_CLASSES)
 
 
-def sklearn_pipeline_from_device(params, nb_features, nb_classes, nb_samples, use_scaler=True, n_init=1, max_iter=99):
-    """ wrap the parameters fitted by ``isb_gmm_fit_predict`` into the scikit-learn objects the reference returns
-    (Pipeline[StandardScaler?, GaussianMixture]) so that ``predict_proba`` & co. keep working on the host """
+def _pca_from_device(params, nb_features, pca_coef):
+    """the fitted sklearn PCA of isb_pca_fit's parameters (host copy)"""
+    from sklearn import decomposition
+    p, D = np.asarray(params, dtype=np.float64), int(nb_features)
+    o = 3 * D
+    comp = p[o:o + D * D].reshape(D, D)
+    o += D * D
+    ev, ratio, sv = p[o:o + D], p[o + D:o + 2 * D], p[o + 2 * D:o + 3 * D]
+    nc, noise, n_samples, ok = p[o + 4 * D:o + 4 * D + 4]
+    if not ok:
+        raise np.linalg.LinAlgError('the device eigensolver of the PCA did not converge')
+    nc = int(nc)
+    pca = decomposition.PCA(pca_coef)
+    pca.mean_ = p[2 * D:3 * D].copy()
+    pca.components_ = comp[:nc].copy()
+    pca.explained_variance_, pca.explained_variance_ratio_, pca.singular_values_ = ev[:nc].copy(), ratio[:nc].copy(), sv[:nc].copy()
+    pca.n_components_, pca.noise_variance_, pca.n_samples_, pca.n_features_in_ = nc, float(noise), int(n_samples), D
+    pca._fit_svd_solver = 'covariance_eigh'
+    return pca
+
+
+def sklearn_pipeline_from_device(params, nb_features, nb_classes, nb_samples, use_scaler=True, n_init=1, max_iter=99, kind='GMM',
+                                 pca_params=None, pca_coef=None, nb_features_in=None):
+    """ wrap the parameters fitted by ``isb_gmm_fit_predict`` / ``isb_mixture_fit_predict`` (and ``isb_pca_fit``) into the
+    scikit-learn objects the reference returns (Pipeline[StandardScaler?, PCA?, GaussianMixture | BayesianGaussianMixture]) so that
+    ``predict_proba`` & co. keep working on the host.  With ``pca_params`` the scaler is the PCA fit's and ``nb_features`` counts
+    the PCA components the mixture saw; ``nb_features_in`` is then the width of the raw features. """
     from sklearn import mixture, pipeline, preprocessing
     p = np.asarray(params, dtype=np.float64)
     D, K = int(nb_features), int(nb_classes)
@@ -138,28 +200,73 @@ def sklearn_pipeline_from_device(params, nb_features, nb_classes, nb_samples, us
         raise ValueError('Fitting the mixture model failed because some components have ill-defined empirical covariance '
                          '(for instance caused by singleton or collapsed samples). Try to decrease the number of components')
     steps = []
+    if pca_params is not None:
+        D_in = int(nb_features_in)
+        if use_scaler:
+            pp = np.asarray(pca_params, dtype=np.float64)
+            mean, scale = pp[:D_in].copy(), pp[D_in:2 * D_in].copy()
+        pca = _pca_from_device(pca_params, D_in, pca_coef)
+    else:
+        D_in = D
     if use_scaler:
         sc = preprocessing.StandardScaler()
         sc.mean_, sc.scale_, sc.var_ = mean, scale, scale ** 2
-        sc.n_features_in_, sc.n_samples_seen_ = D, int(nb_samples)
+        sc.n_features_in_, sc.n_samples_seen_ = D_in, int(nb_samples)
         steps.append(('std_scaler', sc))
-    mm = mixture.GaussianMixture(n_components=K, covariance_type='full', n_init=n_init, max_iter=max_iter)
-    mm.weights_, mm.means_, mm.covariances_, mm.precisions_cholesky_ = weights, means, covs, prec_chol
-    mm.precisions_ = np.array([u @ u.T for u in prec_chol])
+    if pca_params is not None:
+        steps.append(('reduce_dim', pca))
+    if kind == 'BGM':
+        nk = weights
+        mm = mixture.BayesianGaussianMixture(n_components=K, covariance_type='full', n_init=n_init, max_iter=max_iter)
+        o += 5   # lower_bound | n_iter | converged | ok | best_init, then the priors
+        mm.weight_concentration_prior_, mm.mean_precision_prior_, mm.degrees_of_freedom_prior_ = 1. / K, 1., float(D)
+        mm.mean_prior_, mm.covariance_prior_ = p[o:o + D].copy(), p[o + D:o + D + D * D].reshape(D, D).copy()
+        # _estimate_weights / _estimate_means / _estimate_wishart_full from nk, then sklearn's own weights_ and precisions_
+        wc = (1. + nk, 1. / K + np.hstack((np.cumsum(nk[::-1])[-2::-1], 0)))
+        mm._set_parameters((wc, 1. + nk, means, D + nk, covs, prec_chol))
+    else:
+        mm = mixture.GaussianMixture(n_components=K, covariance_type='full', n_init=n_init, max_iter=max_iter)
+        mm.weights_, mm.means_, mm.covariances_, mm.precisions_cholesky_ = weights, means, covs, prec_chol
+        mm.precisions_ = np.array([u @ u.T for u in prec_chol])
     mm.converged_, mm.n_iter_, mm.lower_bound_, mm.n_features_in_ = bool(converged), int(n_iter), float(lower), D
     steps.append(('model', mm))
     return pipeline.Pipeline(steps)
 
 
-def estim_class_model_device(features, nb_classes, use_scaler=True, max_iter=99, init_labels=None, seed=None):
-    """ the default 'GMM' model fitted on the GPU; returns the same kind of object as :func:`estim_class_model` """
+def device_fit_predict(eng, d_feat, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef=None, seed=None, d_n=None, init_labels=None):
+    """ the class model fitted on device features [N, D] and evaluated on them, nothing leaves the device (a float ``pca_coef``
+    reads its component count back): returns (proba [N, K] device, mixture params, PCA params or None, dimensions the mixture saw) """
+    seed = RANDOM_SEED if seed is None else seed
+    d_pca, dims = None, int(d_feat.shape[1])
+    if pca_coef is not None:
+        d_feat, d_pca, dims = eng.pca_fit_transform(d_feat, use_scaler, pca_coef, d_n=d_n)
+        use_scaler = False   # the PCA fit owns the scaler
+    proba, params = eng.mixture_fit_predict(d_feat, nb_classes, n_init, max_iter, use_scaler, seed, d_n=d_n, init_labels=init_labels,
+                                            kind=kind)
+    return proba, params, d_pca, dims
+
+
+def fit_class_model_device(features, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef=None, init_labels=None, seed=None):
+    """ the class model of a :func:`class_model_spec` triple fitted on the GPU: the same kind of object as :func:`estim_class_model` """
     features = np.ascontiguousarray(features, dtype=np.float64)
     eng = get_engine()
-    n_init = max(1, int(np.sqrt(max_iter))) if init_labels is None else len(np.atleast_2d(init_labels))
     d_feat = eng.to_device(features, 'feat_in')
-    _, params = eng.gmm_fit_predict(d_feat, nb_classes, n_init, max_iter, use_scaler, RANDOM_SEED if seed is None else seed,
-                                    init_labels=None if init_labels is None else np.atleast_2d(init_labels))
-    return sklearn_pipeline_from_device(eng.to_host(params), features.shape[1], nb_classes, len(features), use_scaler, n_init, max_iter)
+    if init_labels is not None:
+        init_labels = np.atleast_2d(init_labels)
+    _, params, d_pca, dims = device_fit_predict(eng, d_feat, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef, seed,
+                                                init_labels=init_labels)
+    return sklearn_pipeline_from_device(eng.to_host(params), dims, nb_classes, len(features), use_scaler, n_init, max_iter, kind,
+                                        None if d_pca is None else eng.to_host(d_pca), pca_coef, features.shape[1])
+
+
+def estim_class_model_device(features, nb_classes, use_scaler=True, max_iter=99, init_labels=None, seed=None, estim_model='GMM',
+                             pca_coef=None):
+    """ :func:`estim_class_model` fitted on the GPU (every ``estim_model`` variant, optional PCA); ``init_labels`` [n_init, N]
+    replaces the device k-means++ start (one restart per row) """
+    kind, n_init, max_iter = class_model_spec(estim_model, nb_classes, max_iter)
+    if init_labels is not None:
+        n_init = len(np.atleast_2d(init_labels))
+    return fit_class_model_device(features, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef, init_labels, seed)
 
 
 def estim_class_model(features, nb_classes, estim_model='GMM', pca_coef=None, use_scaler=True, max_iter=99):
@@ -174,7 +281,7 @@ def estim_class_model(features, nb_classes, estim_model='GMM', pca_coef=None, us
     if device_gmm_applicable(features.shape[1], nb_classes, estim_model, pca_coef):
         import torch
         if torch.cuda.is_available():
-            return estim_class_model_device(features, nb_classes, use_scaler, max_iter)
+            return estim_class_model_device(features, nb_classes, use_scaler, max_iter, estim_model=estim_model, pca_coef=pca_coef)
     from sklearn import cluster, decomposition, mixture, pipeline, preprocessing
     steps = []
     if use_scaler:

@@ -21,7 +21,7 @@ import numpy as np
 from .class_models import CompiledModel, compile_model
 from .descriptors import FEATURES_SET_COLOR, compute_selected_features_img2d, flags_are_native, native_feature_layout
 from .engine import edge_capacity, edges_fit, get_engine
-from .graph_cuts import device_gmm_applicable, estim_class_model, segment_graph_cut_general
+from .graph_cuts import class_model_spec, device_gmm_applicable, estim_class_model, segment_graph_cut_general
 from .superpixels import _as_rgb_like, _supported_dtype, slic_params
 
 #: basic features extracted from superpixels (reference pipelines.py:35)
@@ -151,9 +151,27 @@ def _compiled_model(model, dict_features):
     return cm
 
 
+def _fit_model(nb_classes, use_scaler, estim_model='GMM', pca_coef=None):
+    """the resident model tuple of a device-fitted class model: ('fit', nb_classes, use_scaler, max_iter) for the default 'GMM',
+    ('fit', nb_classes, use_scaler, max_iter, kind, n_init, pca_coef) for any other variant (graph_cuts.class_model_spec).  It is
+    part of the CUDA-graph key, so a configuration never replays the graph of another."""
+    kind, n_init, max_iter = class_model_spec(estim_model, nb_classes)
+    if kind == 'GMM' and n_init == max(1, int(np.sqrt(max_iter))) and max_iter == 99 and pca_coef is None:
+        return ('fit', nb_classes, use_scaler, max_iter)
+    return ('fit', nb_classes, use_scaler, max_iter, kind, n_init, pca_coef)
+
+
+def _fit_spec(model):
+    """(nb_classes, use_scaler, max_iter, kind, n_init, pca_coef) of a resident model tuple (:func:`_fit_model`)"""
+    _, nb_classes, use_scaler, max_iter, *rest = model
+    kind, n_init, pca_coef = rest if rest else ('GMM', max(1, int(np.sqrt(max_iter))), None)
+    return nb_classes, use_scaler, max_iter, kind, n_init, pca_coef
+
+
 def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, early_soft=False):
-    """the whole hot path on the device.  ``model`` is either ('fit', nb_classes, use_scaler, max_iter) -> the default
-    GMM is fitted on the GPU and NOTHING syncs with the host until the results are ready; or a
+    """the whole hot path on the device.  ``model`` is either ('fit', nb_classes, use_scaler, max_iter[, kind, n_init, pca_coef])
+    (:func:`_fit_model`) -> the class model is fitted on the GPU and NOTHING syncs with the host until the results are ready (a
+    float pca_coef reads its component count back, and D > 16 features read one flag per EM iteration); or a
     :class:`~.class_models.CompiledModel` -> a caller-fitted model evaluated on the device, again without a sync; or a callable
     proba_fn(features) -> one round trip (features down, probabilities up) as in the reference.
     With a device-fitted or compiled model and colour features the two halves -- image -> class probabilities, probabilities -> cut
@@ -174,13 +192,14 @@ def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul,
         def predict(res):
             return eng.class_model_predict(res.d_feat, model, d_n=res.d_n_labels)
     elif on_device:
-        _, nb_classes, use_scaler, max_iter = model
+        nb_classes, use_scaler, max_iter, kind, n_init, pca_coef = _fit_spec(model)
         model_key = model
-        n_init = max(1, int(np.sqrt(max_iter)))
-        graphable = graphable and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES
+        graphable = (graphable and pca_coef is None
+                     and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES)
 
         def predict(res):
-            return eng.gmm_fit_predict(res.d_feat, nb_classes, n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED, d_n=res.d_n_labels)[0]
+            return graph_cuts.device_fit_predict(eng, res.d_feat, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef,
+                                                 d_n=res.d_n_labels)[0]
 
     proba = None
     if on_device:
@@ -227,8 +246,13 @@ def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_t
             proba_fn = model.predict_proba
         elif callable(model):
             proba_fn = model
-        else:
+        elif len(model) == 4:
             proba_fn = lambda f: estim_class_model(f, model[1], 'GMM', None, model[2], model[3]).predict_proba(f)  # noqa: E731
+        else:
+            from .graph_cuts import fit_class_model_device
+            nb_classes, use_scaler, max_iter, kind, n_init, pca_coef = _fit_spec(model)
+            proba_fn = lambda f: fit_class_model_device(f, nb_classes, use_scaler, kind, n_init, max_iter,  # noqa: E731
+                                                        pca_coef).predict_proba(f)
         slic, features = compute_color2d_superpixels_features(image, dict_features, sp_size=sp_size, sp_regul=sp_regul)
         if debug_visual is not None:
             img3 = image if image.ndim == 3 else np.stack([image] * 3, axis=-1)
@@ -301,12 +325,14 @@ def _over_streams(list_images, nb_streams, max_in_flight, launch, finish):
 
 
 def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIMPLE, sp_size=30, sp_regul=0.2, use_scaler=True,
-                         gc_regul=1., gc_edge_type='model', model_pipeline=None, nb_streams=3, max_in_flight=6):
+                         gc_regul=1., gc_edge_type='model', model_pipeline=None, nb_streams=3, max_in_flight=6, estim_model='GMM',
+                         pca_coef=None):
     """ the hot path over a LIST of images, the way the reference's experiment scripts run it through a process pool
     (``run_segm_slic_model_graphcut.py:461-466``): here consecutive images alternate over ``nb_streams`` CUDA streams with
     their own buffers, so the upload of image i+1 and the download of image i-1 overlap the kernels of image i.
 
-    :param int nb_classes: fit the default GMM per image on the GPU (as ``pipe_color2d_slic_features_model_graphcut``), or
+    :param int nb_classes: fit the class model per image on the GPU (as ``pipe_color2d_slic_features_model_graphcut``, with its
+        ``estim_model`` and ``pca_coef``), or
     :param model_pipeline: a fitted model used for every image (as ``segment_color2d_slic_features_model_graphcut``)
     :return list(tuple(ndarray,ndarray)): (segm, segm_soft) per image, in input order
     """
@@ -314,14 +340,14 @@ def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIM
         raise ValueError('give either nb_classes (per-image GMM) or model_pipeline')
     native = flags_are_native(dict_features) and gc_edge_type not in ('color', 'features')
     nb_fts = native_feature_layout(dict_features)[1] if native else 10 ** 6
-    if model_pipeline is None and not (native and device_gmm_applicable(nb_fts, nb_classes)):
-        return [pipe_color2d_slic_features_model_graphcut(im, nb_classes, dict_features, sp_size, sp_regul, None, use_scaler, 'GMM',
-                                                          gc_regul, gc_edge_type) for im in list_images]
+    if model_pipeline is None and not (native and device_gmm_applicable(nb_fts, nb_classes, estim_model, pca_coef)):
+        return [pipe_color2d_slic_features_model_graphcut(im, nb_classes, dict_features, sp_size, sp_regul, pca_coef, use_scaler,
+                                                          estim_model, gc_regul, gc_edge_type) for im in list_images]
     if not native:
         return [segment_color2d_slic_features_model_graphcut(im, model_pipeline, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)
                 for im in list_images]
     if model_pipeline is None:
-        model = ('fit', nb_classes, use_scaler, 99)
+        model = _fit_model(nb_classes, use_scaler, estim_model, pca_coef)
     else:
         model = _compiled_model(model_pipeline, dict_features) or model_pipeline.predict_proba
     classes = getattr(model_pipeline, 'classes_', None)
@@ -424,7 +450,8 @@ def segment_resident(d_image, model, dict_features, sp_size=30, sp_regul=0.2, gc
     """ the same hot path with the image ALREADY on the device (a cuda tensor [H, W, 3]) and the results left
     there: returns (segm int32 [H, W], segm_soft float64 [H, W, K]) device tensors.  ``model`` is a callable
     proba_fn(features), a fitted model (or its bound ``predict_proba``) -- evaluated on the device when
-    :func:`~.class_models.compile_model` supports it -- or ('fit', nb_classes, use_scaler, max_iter) for the GPU-fitted default GMM.
+    :func:`~.class_models.compile_model` supports it -- or ('fit', nb_classes, use_scaler, max_iter) for the GPU-fitted default GMM
+    (``_fit_model`` gives the tuple of the other ``estim_model`` variants and of ``pca_coef``).
     The indices in ``segm`` are not mapped through the model's ``classes_``.
     Nothing here waits for the device, so the edge count of the graph cut is not checked against its table as the host-facing
     pipelines do: after the connectivity pass every superpixel is connected, the region graph of a 2-D map is planar with at most
@@ -449,7 +476,7 @@ def pipe_color2d_slic_features_model_graphcut(image, nb_classes, dict_features, 
     logging.info('PIPELINE Superpixels-Features-GMM-GraphCut')
     nb_fts = native_feature_layout(dict_features)[1] if flags_are_native(dict_features) else 10 ** 6
     if flags_are_native(dict_features) and device_gmm_applicable(nb_fts, nb_classes, estim_model, pca_coef):
-        model = ('fit', nb_classes, use_scaler, 99)
+        model = _fit_model(nb_classes, use_scaler, estim_model, pca_coef)
     else:
         def model(features):
             return estim_class_model(features, nb_classes, estim_model, pca_coef, use_scaler).predict_proba(features)
