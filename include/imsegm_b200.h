@@ -190,6 +190,37 @@ int isb_filter_response_2d(const double* img, int n_slices, int H, int W, const 
 int isb_gaussian_filter_2d(const double* img, int n_slices, int H, int W, const double* w_half, int radius, double* tmp, double* out,
                            isb_stream_t stream);
 
+/* Inputs of the colour-space groups and of the median / meanGrad statistics of compute_selected_features_color2d, for the
+ * resident feature table.  Every launch below is capturable in a CUDA graph (no host read, no allocation). */
+enum isb_color_space { ISB_COLOR_HSV = 0, ISB_COLOR_LUV = 1, ISB_COLOR_LAB = 2, ISB_COLOR_HED = 3, ISB_COLOR_XYZ = 4 };
+/* convert_img_color_from_rgb (pyimsegm_b200/color.py): img [n_px, 3] interleaved RGB of any isb_dtype (u8 / 255, u16 / 65535,
+ * floats as they are) -> out [n_px, 3] f64 in the given isb_color_space.  IEEE pow / cbrt / log; hsv is bit-exact, a NaN pixel
+ * gives (0, 0, 0) in hsv. */
+int isb_color_convert(const void* img, int dtype, long long n_px, int space, double* out, isb_stream_t stream);
+/* np.sum(np.gradient(np.nan_to_num(img[..., c])), axis=0) of every channel of img [H, W, channels] interleaved: one-sided
+ * differences at the borders, central halves inside.  out [H, W, channels] is f32 for an f32 image (f32 arithmetic), f64 otherwise
+ * (integers are promoted as numpy does).  H < 2 or W < 2 is an argument error, as np.gradient raises. */
+int isb_gradient_sum_2d(const void* img, int dtype, int H, int W, int channels, void* out, isb_stream_t stream);
+/* isb_segment_median of an [H, W, channels] image into columns col0 .. col0 + channels of the feature table feat [nb, ld]; pixels
+ * go through np.nan_to_num first and the result through the table's rules (inf -> largest finite value, -0 -> +0); NaN for a
+ * label without pixels.  Workspace: isb_segment_median_workspace_bytes(H * W, nb). */
+int isb_segment_median_2d(const void* img, int dtype, const int32_t* seg, int H, int W, int channels, int nb, double* feat, int ld,
+                          int col0, void* ws, size_t ws_bytes, isb_stream_t stream);
+
+/* The Leung-Malik route of the statistics the fused kernel does not produce (median, meanGrad): every filter response in memory
+ * (texture.py _texture_desc_lm_materialised).
+ * background: planar [3, H, W] f64 = the image [H, W, 3] (any isb_dtype, values as they are) minus its background --
+ *   isb_gaussian_filter_2d (w_half DEVICE, radius) of every channel, mixed across the channels by mix [3][3] (HOST, row-major);
+ *   tmp and smooth: scratch [3, H, W] f64 */
+int isb_lm_background(const void* img, int dtype, int H, int W, const double* w_half, int radius, const double* mix, double* planar,
+                      double* tmp, double* smooth, isb_stream_t stream);
+/* one battery: resp [3, H, W] = isb_filter_response_2d(planar, kernels [n_kernels, kh, kw]); then clipped at max_signal, its norm
+ * |r| = sqrt(sum r^2) summed in a fixed order, and out [H, W, 3] f64 = (r * (log(1 + |r|) / 0.03)) / |r|, or zeros when |r| is 0
+ * or infinite */
+size_t isb_lm_battery_workspace_bytes(void);
+int isb_lm_battery_response(const double* planar, int H, int W, const double* kernels, int n_kernels, int kh, int kw, double max_signal,
+                            double* resp, double* out, void* ws, size_t ws_bytes, isb_stream_t stream);
+
 /* compute_label_histograms_positions (imsegm/descriptors.py:1288-1352) in one launch: for every position (row, col) and every
  * diameter d the histogram of the labels under the disc dy^2 + dx^2 <= d^2 (skimage.morphology.disk(d)) clipped to the image,
  * i.e. what compute_label_hist_segm (:1396) returns for the pair, and the pixel count of the clipped disc.

@@ -105,6 +105,12 @@ SIGNATURES = {
     'isb_segment_median_workspace_bytes': (_sz, [_ll, _i]),
     'isb_segment_median': (_i, [_vp, _i, _vp, _ll, _i, _i, _vp, _vp, _sz, _vp]),
     'isb_binary_opening_disk': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
+    'isb_color_convert': (_i, [_vp, _i, _ll, _i, _vp, _vp]),
+    'isb_gradient_sum_2d': (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    'isb_segment_median_2d': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _sz, _vp]),
+    'isb_lm_background': (_i, [_vp, _i, _i, _i, _vp, _i, C.POINTER(_d), _vp, _vp, _vp, _vp]),
+    'isb_lm_battery_workspace_bytes': (_sz, []),
+    'isb_lm_battery_response': (_i, [_vp, _i, _i, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

@@ -915,12 +915,26 @@ def flags_are_native(dict_features):
                                        for k, v in dict_features.items())
 
 
+#: feature groups of the resident single-GPU path: the image, its colour spaces (pyimsegm_b200.color) and the two Leung-Malik banks
+RESIDENT_FEATURE_GROUPS = ('color', 'color_hsv', 'color_luv', 'color_lab', 'color_hed', 'color_xyz', 'tLM', 'tLM_short')
+
+
+def flags_are_resident(dict_features):
+    """True when the resident single-GPU path computes every requested group and statistic: any of
+    :data:`RESIDENT_FEATURE_GROUPS` with any subset of :data:`NAMES_FEATURE_FLAGS`.  Anything else takes the general path, which
+    warns about what it does not recognise."""
+    return bool(dict_features) and all(k in RESIDENT_FEATURE_GROUPS and all(f in NAMES_FEATURE_FLAGS for f in v)
+                                       for k, v in dict_features.items())
+
+
 def native_feature_layout(dict_features):
-    """[(key, flags, first column, n columns)] in the reference's column order: colour groups first, then texture"""
+    """[(key, flags, first column, n columns)] in the column order of :func:`compute_selected_features_color2d`: colour groups
+    first, then texture groups, each in dict order; a group's flags in NAMES_FEATURE_FLAGS order (statistic-major, channel-minor
+    columns), a texture group battery-major"""
     layout, col = [], 0
     for k in [k for k in dict_features if k.startswith('color')] + [k for k in dict_features if k.startswith('tLM')]:
-        flags = [f for f in ('mean', 'std', 'energy') if f in dict_features[k]]
-        n = 3 * len(flags) * (1 if k == 'color' else (15 if k.endswith('_short') else 20))
+        flags = [f for f in NAMES_FEATURE_FLAGS if f in dict_features[k]]
+        n = 3 * len(flags) * (1 if k.startswith('color') else (15 if k.endswith('_short') else 20))
         layout.append((k, flags, col, n))
         col += n
     return layout, col

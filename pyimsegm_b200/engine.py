@@ -372,6 +372,58 @@ class Engine(object):
                                           _lib.ptr(centres), _lib.ptr(counts), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
         return feat, centres, counts
 
+    #: isb_color_space codes of the ``color_<space>`` feature groups
+    COLOR_SPACES = {'hsv': 0, 'luv': 1, 'lab': 2, 'hed': 3, 'xyz': 4}
+
+    def color_convert(self, d_img, space):
+        """a [H,W,3] device RGB image in ``space`` (pyimsegm_b200.color), f64 [H,W,3] in one cached buffer that the next conversion
+        overwrites"""
+        H, W = int(d_img.shape[0]), int(d_img.shape[1])
+        out = self.buf('color_conv', (H, W, 3), self.torch.float64)
+        self._ck(self.lib.isb_color_convert(_lib.ptr(d_img), _lib.dtype_code(d_img.dtype), C.c_longlong(H * W), self.COLOR_SPACES[space],
+                                            _lib.ptr(out), _lib.stream_ptr()))
+        return out
+
+    def gradient_sum(self, d_img):
+        """np.sum(np.gradient(np.nan_to_num(channel)), axis=0) of every channel of a [H,W,C] device image: f32 for an f32 image, f64
+        otherwise (cached buffer)"""
+        torch = self.torch
+        H, W, Cn = (int(v) for v in d_img.shape)
+        dtype = torch.float32 if d_img.dtype == torch.float32 else torch.float64
+        out = self.buf('grad_' + str(dtype)[6:], (H, W, Cn), dtype)
+        self._ck(self.lib.isb_gradient_sum_2d(_lib.ptr(d_img), _lib.dtype_code(d_img.dtype), H, W, Cn, _lib.ptr(out), _lib.stream_ptr()))
+        return out
+
+    def segment_median(self, d_img, d_seg, nb, feat, col0=0):
+        """per-label median of every channel of a [H,W,C] device image (np.nan_to_num'd pixels) into feat[:nb, col0:col0 + C]"""
+        torch, lib = self.torch, self.lib
+        H, W, Cn = (int(v) for v in d_img.shape)
+        wsb = lib.isb_segment_median_workspace_bytes(C.c_longlong(H * W), int(nb))
+        ws = self.buf('ws_median', (wsb,), torch.uint8)
+        self._ck(lib.isb_segment_median_2d(_lib.ptr(d_img), _lib.dtype_code(d_img.dtype), _lib.ptr(d_seg), H, W, Cn, int(nb), _lib.ptr(feat),
+                                           int(feat.shape[1]), int(col0), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
+        return feat
+
+    def group_stats(self, d_src, d_seg, nb, flags, feat, col0, want_centres=False):
+        """the statistics ``flags`` of one feature group over a [H,W,3] device source into feat[:, col0:], statistic-major in the
+        order mean, std, energy, median, meanGrad and channel-minor, as compute_image2d_color_statistic lays them out.  With
+        ``want_centres`` the first stats launch of the group also forms the centroids: returns them, or None when the group has no
+        such launch"""
+        native = [f for f in ('mean', 'std', 'energy') if f in flags]
+        centres = None
+        col = col0
+        if native:
+            _, centres, _ = self.segment_stats(d_src, d_seg, nb, native, feat=feat, col0=col, want_centres=want_centres)
+            col += 3 * len(native)
+        if 'median' in flags:
+            self.segment_median(d_src, d_seg, nb, feat, col)
+            col += 3
+        if 'meanGrad' in flags:
+            _, grad_centres, _ = self.segment_stats(self.gradient_sum(d_src), d_seg, nb, ('mean', ), feat=feat, col0=col,
+                                                    want_centres=want_centres and centres is None)
+            centres = grad_centres if centres is None else centres
+        return centres
+
     # -- (iii) graph, energies, alpha-expansion ---------------------------------------------------------------------
     def adjacency(self, d_seg, nb, cap):
         """unique 4-connected label pairs; returns (edges int32 [cap,2] device, n_edges device int32[1], cap)"""

@@ -19,7 +19,7 @@ import logging
 import numpy as np
 
 from .class_models import CompiledModel, compile_model
-from .descriptors import FEATURES_SET_COLOR, compute_selected_features_img2d, flags_are_native, native_feature_layout
+from .descriptors import FEATURES_SET_COLOR, compute_selected_features_img2d, flags_are_resident, native_feature_layout
 from .engine import edge_capacity, edges_fit, get_engine
 from .graph_cuts import class_model_spec, device_gmm_applicable, estim_class_model, segment_graph_cut_general
 from .superpixels import _as_rgb_like, _supported_dtype, slic_params
@@ -43,13 +43,15 @@ class DeviceSuperpixels(object):
 
 
 def _device_slic_features(eng, image, dict_features, sp_size, sp_regul):
-    """H2D, SLIC, fused colour statistics + centroids; everything stays on the device"""
+    """H2D, SLIC, the feature table of ``native_feature_layout`` + centroids; everything stays on the device"""
     if sp_regul <= 0.:
         raise ValueError('slic. regularisation must be positive')
     on_device = hasattr(image, 'is_cuda')
     if not on_device:
         image = _supported_dtype(_as_rgb_like(image))
     H, W = int(image.shape[0]), int(image.shape[1])
+    if min(H, W) < 2 and any('meanGrad' in flags for flags in dict_features.values()):
+        raise ValueError('Shape of array too small to calculate a numerical gradient, at least (edge_order + 1) elements are required.')
     n_seg, compact = slic_params((H, W), sp_size, sp_regul)
     if n_seg < 1:
         raise ValueError('superpixel size %r is larger than the image %r' % (sp_size, tuple(image.shape)))
@@ -62,13 +64,17 @@ def _device_slic_features(eng, image, dict_features, sp_size, sp_regul):
     res.d_feat = eng.buf('feat', (res.nb_bound, max(ncol, 1)), eng.torch.float64)
     res.d_centres = None
     for key, flags, col0, _ in layout:
-        if key == 'color':
-            _, res.d_centres, _ = eng.segment_stats(res.d_img, res.d_seg, res.nb_bound, flags, feat=res.d_feat, col0=col0,
-                                                    want_centres=True)
+        if key.startswith('color'):
+            src = res.d_img if key == 'color' else eng.color_convert(res.d_img, key.split('_')[-1])
+            centres = eng.group_stats(src, res.d_seg, res.nb_bound, flags, res.d_feat, col0, want_centres=res.d_centres is None)
+            res.d_centres = res.d_centres if centres is None else centres
         else:
-            from .texture import device_lm_features
-            device_lm_features(eng, res.d_img, res.d_seg, res.nb_bound, flags, 'short' if key.endswith('_short') else 'normal',
-                               feat=res.d_feat, col0=col0)
+            from .texture import device_lm_features, device_lm_materialised
+            bank = 'short' if key.endswith('_short') else 'normal'
+            if 'median' in flags or 'meanGrad' in flags:
+                device_lm_materialised(eng, res.d_img, res.d_seg, res.nb_bound, flags, bank, res.d_feat, col0)
+            else:
+                device_lm_features(eng, res.d_img, res.d_seg, res.nb_bound, flags, bank, feat=res.d_feat, col0=col0)
     if res.d_centres is None:
         _, res.d_centres, _ = eng.segment_stats(None, res.d_seg, res.nb_bound, (), want_centres=True)
     return res
@@ -83,7 +89,7 @@ def compute_color2d_superpixels_features(image, dict_features, sp_size=30, sp_re
         raise ValueError('slic. regularisation must be positive')
     image = np.asarray(image)
     eng = get_engine()
-    if image.ndim == 3 and flags_are_native(dict_features):
+    if image.ndim == 3 and flags_are_resident(dict_features):
         res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
         nb = int(eng.to_host(res.d_n_labels)[0])
         slic = eng.to_host(res.d_seg).astype(np.int64)
@@ -143,7 +149,7 @@ def _compiled_model(model, dict_features):
     """the device form of a caller-fitted model for the native path (its feature count has to match the native feature layout), or
     None: then its predict_proba runs on the host"""
     from . import graph_cuts
-    if not graph_cuts.USE_DEVICE_PREDICT or not flags_are_native(dict_features):
+    if not graph_cuts.USE_DEVICE_PREDICT or not flags_are_resident(dict_features):
         return None
     cm = compile_model(model)
     if cm is None or cm.n_features_in != native_feature_layout(dict_features)[1]:
@@ -184,8 +190,8 @@ def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul,
     if not hasattr(image, 'is_cuda'):
         image = eng.to_device(_supported_dtype(_as_rgb_like(np.asarray(image))), 'image')
     on_device = isinstance(model, (tuple, CompiledModel))
-    graphable = (on_device and USE_CUDA_GRAPHS and not no_cut and all(k == 'color' for k in dict_features)
-                 and flags_are_native(dict_features))
+    graphable = (on_device and USE_CUDA_GRAPHS and not no_cut and all(k.startswith('color') for k in dict_features)
+                 and flags_are_resident(dict_features))
     if isinstance(model, CompiledModel):
         model_key = ('compiled', model.digest)
 
@@ -239,7 +245,7 @@ def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul,
 def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, debug_visual, classes=None):
     image = np.asarray(image)
     eng = get_engine()
-    native = image.ndim == 3 and flags_are_native(dict_features) and gc_edge_type not in ('color', 'features')
+    native = image.ndim == 3 and flags_are_resident(dict_features) and gc_edge_type not in ('color', 'features')
     if not native or debug_visual is not None:
         # general path: every stage still runs on the device, but through the numpy-facing stage functions
         if isinstance(model, CompiledModel):
@@ -338,7 +344,7 @@ def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIM
     """
     if (nb_classes is None) == (model_pipeline is None):
         raise ValueError('give either nb_classes (per-image GMM) or model_pipeline')
-    native = flags_are_native(dict_features) and gc_edge_type not in ('color', 'features')
+    native = flags_are_resident(dict_features) and gc_edge_type not in ('color', 'features')
     nb_fts = native_feature_layout(dict_features)[1] if native else 10 ** 6
     if model_pipeline is None and not (native and device_gmm_applicable(nb_fts, nb_classes, estim_model, pca_coef)):
         return [pipe_color2d_slic_features_model_graphcut(im, nb_classes, dict_features, sp_size, sp_regul, pca_coef, use_scaler,
@@ -373,7 +379,7 @@ def compute_features_batch(list_images, dict_features, sp_size=30, sp_regul=0.2,
 
     :return list(ndarray): features [N_i, D] per image, in input order
     """
-    if not flags_are_native(dict_features) or any(np.ndim(im) != 3 for im in list_images):
+    if not flags_are_resident(dict_features) or any(np.ndim(im) != 3 for im in list_images):
         return [compute_color2d_superpixels_features(im, dict_features, sp_size=sp_size, sp_regul=sp_regul)[1] for im in list_images]
     def launch(eng, image):
         res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
@@ -474,8 +480,8 @@ def pipe_color2d_slic_features_model_graphcut(image, nb_classes, dict_features, 
     :return tuple(ndarray,ndarray): segmentation [H, W] int32, soft segmentation [H, W, nb_classes] float64
     """
     logging.info('PIPELINE Superpixels-Features-GMM-GraphCut')
-    nb_fts = native_feature_layout(dict_features)[1] if flags_are_native(dict_features) else 10 ** 6
-    if flags_are_native(dict_features) and device_gmm_applicable(nb_fts, nb_classes, estim_model, pca_coef):
+    nb_fts = native_feature_layout(dict_features)[1] if flags_are_resident(dict_features) else 10 ** 6
+    if flags_are_resident(dict_features) and device_gmm_applicable(nb_fts, nb_classes, estim_model, pca_coef):
         model = _fit_model(nb_classes, use_scaler, estim_model, pca_coef)
     else:
         def model(features):

@@ -151,6 +151,43 @@ def device_lm_features(eng, d_img, d_seg, nb, flags, bank_type='normal', feat=No
     return feat, names, ncol
 
 
+def _device_batteries(eng, bank_type):
+    """the batteries of :func:`create_filter_bank_lm_2d` for 'normal' / 'short' as f64 device tensors, uploaded once per device"""
+    key = ('batteries', bank_type, eng.device.index)
+    if key not in _BANK_CACHE:
+        from .descriptors import SHORT_FILTERS_SIGMAS
+        filters, _ = create_filter_bank_lm_2d(sigmas=SHORT_FILTERS_SIGMAS, nb_orient=4) if bank_type == 'short' else create_filter_bank_lm_2d()
+        _BANK_CACHE[key] = [eng.torch.from_numpy(np.ascontiguousarray(f, dtype=np.float64)).to(eng.device) for f in filters]
+    return _BANK_CACHE[key]
+
+
+def device_lm_materialised(eng, d_img, d_seg, nb, flags, bank_type, feat, col0):
+    """the device form of :func:`_texture_desc_lm_materialised` into feat[:, col0:] (battery-major): background subtraction
+    (``isb_lm_background``), then per battery the clipped, log-norm scaled responses (``isb_lm_battery_response``) and their group
+    statistics (:meth:`~.engine.Engine.group_stats`).  Nothing is read back; the buffers are the engine's."""
+    from .descriptors import MAX_SIGNAL_RESPONSE
+    from .engine import gaussian_half_kernel
+    torch, lib = eng.torch, eng.lib
+    H, W = int(d_img.shape[0]), int(d_img.shape[1])
+    st = _lib.stream_ptr()
+    w_half, radius = gaussian_half_kernel(BACKGROUND_SIGMA)
+    d_w = eng.const_device(w_half, 'lm_bg_half')
+    _, _, mix = background_kernel()
+    planar, tmp, smooth = (eng.buf(name, (3, H, W), torch.float64) for name in ('lmm_planar', 'lmm_tmp', 'lmm_smooth'))
+    _lib.check(lib.isb_lm_background(_lib.ptr(d_img), _lib.dtype_code(d_img.dtype), H, W, _lib.ptr(d_w), radius,
+                                     mix.ctypes.data_as(C.POINTER(C.c_double)), _lib.ptr(planar), _lib.ptr(tmp), _lib.ptr(smooth), st))
+    out = eng.buf('lmm_out', (H, W, 3), torch.float64)
+    wsb = lib.isb_lm_battery_workspace_bytes()
+    ws = eng.buf('ws_lmm', (wsb,), torch.uint8)
+    per_battery = 3 * len(flags)
+    for b, d_k in enumerate(_device_batteries(eng, bank_type)):
+        nk, kh, kw = (int(v) for v in d_k.shape)
+        _lib.check(lib.isb_lm_battery_response(_lib.ptr(planar), H, W, _lib.ptr(d_k), nk, kh, kw, C.c_double(MAX_SIGNAL_RESPONSE),
+                                               _lib.ptr(tmp), _lib.ptr(out), _lib.ptr(ws), C.c_size_t(wsb), st))
+        eng.group_stats(out, d_seg, nb, flags, feat, col0 + b * per_battery)
+    return feat
+
+
 def _texture_desc_lm_materialised(img, seg, feature_flags, bank_type):
     """ the reference's own sequence (descriptors.py:1078-1098) with every array in memory: background (sigma 150 on all three
     axes), per battery the strongest response per channel (FP64 on the device, ``isb_filter_response_2d``), clip, log-norm
