@@ -6,9 +6,9 @@ region growing (RG2SP) built on it.  Modules of the reference outside that path 
 import sys
 
 import pyimsegm_b200
-from pyimsegm_b200 import descriptors, graph_cuts, labeling, pipelines, region_growing, superpixels, tiled, utilities
+from pyimsegm_b200 import descriptors, ellipse_fitting, graph_cuts, labeling, pipelines, region_growing, superpixels, tiled, utilities
 
-for _name in ('descriptors', 'graph_cuts', 'labeling', 'pipelines', 'region_growing', 'superpixels', 'tiled', 'utilities'):
+for _name in ('descriptors', 'ellipse_fitting', 'graph_cuts', 'labeling', 'pipelines', 'region_growing', 'superpixels', 'tiled', 'utilities'):
     sys.modules[__name__ + '.' + _name] = getattr(pyimsegm_b200, _name)
 
 __version__ = '0.1.9+b200'

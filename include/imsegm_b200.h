@@ -400,6 +400,33 @@ int isb_segment_median(const void* img, int dtype, const int32_t* seg, long long
  * features: erosion then dilation with a disc, borders reflected.  mask / tmp / out : [H, W] uint8 (0 / 1) */
 int isb_binary_opening_disk(const uint8_t* mask, int H, int W, int radius, uint8_t* tmp, uint8_t* out, isb_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * (x) ellipse fitting -- imsegm/ellipse_fitting.py: EllipseModelSegm (skimage.measure.EllipseModel + criterion :76-139),
+ *     ransac_segm :142-261 and add_overlap_ellipse :282-349
+ * ------------------------------------------------------------------------------------------------------------------ */
+
+/* T trials in one launch, one CTA each.  Trial t belongs to centre trial_centre[t] (< C), whose boundary points are
+ * pts[pt_off[c] .. pt_off[c+1]) ([P, 2] f64).  Without params_in the trial fits an ellipse (Halir-Flusser direct fit) to the points
+ * samp_idx[samp_off[t] .. samp_off[t+1]) (indices into its centre's points, in drawn order); with params_in [T, 5] it takes those
+ * parameters.  Then: residuals of every point of the centre (stationary distance from the skimage start angle), n_inl = count of
+ * residuals < thr, crit = sum of lab_term[sp_lab[j]] over the N superpixel points sp_pts [N, 2] inside the ellipse, added in a fixed
+ * order.  ok [T]: 1 fitted, 0 not exactly one admissible eigenvector, -1 singular S3 (numpy's LinAlgError).  params_out [T, 5];
+ * resid_out (optional): residuals of trial t at resid_out[resid_off[t] ..].  The caller validates sample indices. */
+int isb_ellipse_ransac(int T, const int32_t* trial_centre, const int32_t* samp_off, const int32_t* samp_idx, const double* params_in,
+                       int C, const double* pts, const int32_t* pt_off, double thr, const double* sp_pts, const int32_t* sp_lab,
+                       const double* lab_term, int N, int32_t* ok, double* params_out, int32_t* n_inl, double* crit,
+                       double* resid_out, const long long* resid_off, isb_stream_t stream);
+/* skimage.draw.ellipse raster of one ellipse into mask [H, W] u8 and, in the same pass over segm [H, W] i32, counts [2 * n_labels + 1]
+ * u64: pixels per label | pixels per label inside the ellipse | ellipse area.  bbox_host (HOST, 4 ints): clipped bounding box
+ * r0, c0, r1, c1 (inclusive); geom_host (HOST, 6 doubles): centre relative to (r0, c0), the two radii, sin and cos of the rotation.
+ * Labels outside [0, n_labels) are not counted; up to 4096 labels are counted in shared memory, more directly in counts. */
+int isb_ellipse_overlap(const int32_t* segm, int H, int W, int n_labels, const int32_t* bbox_host, const double* geom_host,
+                        uint8_t* mask, unsigned long long* counts, isb_stream_t stream);
+/* grey erosion (op 0) or dilation (op 1) of a 0/1 mask [H, W] u8 over n_offsets (dy, dx) footprint offsets (device i32 [n, 2]),
+ * borders as scipy.ndimage's 'reflect'.  The footprints of skimage.morphology.disk(r) for a non-integer r. */
+int isb_binary_morph_footprint(const uint8_t* in, int H, int W, const int32_t* offsets, int n_offsets, int op, uint8_t* out,
+                               isb_stream_t stream);
+
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);
 
