@@ -208,7 +208,7 @@ int isb_segment_median_2d(const void* img, int dtype, const int32_t* seg, int H,
                           int col0, void* ws, size_t ws_bytes, isb_stream_t stream);
 
 /* The Leung-Malik route of the statistics the fused kernel does not produce (median, meanGrad): every filter response in memory
- * (texture.py _texture_desc_lm_materialised).
+ * (texture.py device_lm_materialised).
  * background: planar [3, H, W] f64 = the image [H, W, 3] (any isb_dtype, values as they are) minus its background --
  *   isb_gaussian_filter_2d (w_half DEVICE, radius) of every channel, mixed across the channels by mix [3][3] (HOST, row-major);
  *   tmp and smooth: scratch [3, H, W] f64 */

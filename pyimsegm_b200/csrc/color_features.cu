@@ -4,7 +4,7 @@
 //                            pow / cbrt / log (NOT the division-free forms of slic_prepare.cu, which define SLIC's own rgb2lab)
 //   isb_gradient_sum_2d      np.sum(np.gradient(np.nan_to_num(ch)), axis=0) per channel, in the image's float type (descriptors.py
 //                            compute_image2d_color_statistic, 'meanGrad')
-//   isb_lm_background        the materialised Leung-Malik route (texture.py _texture_desc_lm_materialised): planar copy of the image
+//   isb_lm_background        the materialised Leung-Malik route (texture.py device_lm_materialised): planar copy of the image
 //   isb_lm_battery_response  minus its sigma-150 background, then per battery the strongest response, clip, sum of squares in a fixed
 //                            order (block partials, every CTA of the second kernel re-adds them in the same order: no floating atomics,
 //                            a rerun gives the same bits) and the log-norm scaling, written interleaved [H, W, 3]

@@ -6,7 +6,6 @@ SLIC -> features -> GraphCut pipeline uses (same public names, feature-dictionar
 error types).  The reference computes them in its only native module ``imsegm/features_cython.pyx``; here
 they come from ``isb_segment_stats_2d`` (``include/imsegm_b200.h``).
 """
-import itertools
 import logging
 
 import numpy as np
@@ -75,14 +74,17 @@ def _device_dtype(img):
     return img.astype(np.float64)
 
 
+def _upload(img, seg):
+    """(engine, device image, device int32 labels, max label + 1) of an image already in a device dtype and its label map"""
+    eng = get_engine()
+    return eng, eng.to_device(img, 'image'), eng.to_device(seg.astype(np.int32, copy=False), 'seg_in'), int(seg.max()) + 1
+
+
 def _device_stats(img, seg, flags):
     """[nb, 3 * len(flags)] statistics in the order mean, std, energy (only those requested)"""
     img, seg = _device_dtype(img), np.asarray(seg)
     _check_color_image_segm(img, seg)
-    eng = get_engine()
-    nb = int(seg.max()) + 1
-    d_img = eng.to_device(img, 'image')
-    d_seg = eng.to_device(seg.astype(np.int32, copy=False), 'seg_in')
+    eng, d_img, d_seg, nb = _upload(img, seg)
     feat, _, _ = eng.segment_stats(d_img, d_seg, nb, flags)
     return eng.to_host(feat).copy()
 
@@ -807,38 +809,22 @@ def reduce_close_points(points, dist_thr):
 
 def compute_image2d_color_statistic(image, segm, feature_flags=NAMES_FEATURE_FLAGS, color_name='color'):
     """ statistics of a colour image over the segments; columns are statistic-major, channel-minor
-    (reference descriptors.py:787-863)
+    (reference descriptors.py:787-863), all of them from one upload (:meth:`~.engine.Engine.group_stats`).  An image of another
+    dtype than u8 / u16 / f32 / f64 (float16, say) is widened to f64 for every statistic, ``meanGrad`` included: the reference
+    takes that gradient in the image's own dtype.
 
     :return tuple(ndarray,list(str)): features [nb_segments, 3 * nb_statistics], column names
     """
-    image, segm = np.asarray(image), np.asarray(segm)
+    image, segm = _device_dtype(image), np.asarray(segm)
     _check_color_image(image)
     _check_color_image_segm(image, segm)
-    ch_names = ['%s-ch%i' % (color_name, i + 1) for i in range(3)]
-    native = [f for f in ('mean', 'std', 'energy') if f in feature_flags]
-    blocks = {}
-    if native:
-        stats = _device_stats(image, segm, native)
-        for i, f in enumerate(native):
-            blocks[f] = stats[:, 3 * i:3 * i + 3]
-    if 'median' in feature_flags:
-        blocks['median'] = numpy_img2d_color_median(np.nan_to_num(image), segm)
-    if 'meanGrad' in feature_flags:
-        clean = np.nan_to_num(image)
-        grad = np.zeros(clean.shape, dtype=clean.dtype if clean.dtype.kind == 'f' else float)
-        for i in range(3):
-            grad[:, :, i] = np.sum(np.gradient(clean[:, :, i]), axis=0)
-        blocks['meanGrad'] = _device_stats(grad, segm, ('mean', ))
-    order = [f for f in NAMES_FEATURE_FLAGS if f in feature_flags]
-    nb = int(segm.max()) + 1
-    features = np.hstack([blocks[f] for f in order]) if order else np.empty((nb, 0))
-    names = list(itertools.chain.from_iterable(['%s_%s' % (n, f) for n in ch_names] for f in order))
     _check_unrecognised_feature_names(feature_flags)
-    features = np.nan_to_num(features)
-    features[features == 0] = 0
-    if features.shape[1] != len(names):
-        raise ValueError('features: %r and names %r' % (features.shape, names))
-    return features, names
+    flags = [f for f in NAMES_FEATURE_FLAGS if f in feature_flags]
+    _check_gradient_size(image.shape[:2], [flags])
+    eng, d_img, d_seg, nb = _upload(image, segm)
+    feat = eng.buf('feat', (nb, max(3 * len(flags), 1)), eng.torch.float64)
+    eng.group_stats(d_img, d_seg, nb, flags, feat, 0)
+    return _finish_features(eng.to_host(feat[:, :3 * len(flags)]), _stat_names(color_name, flags))
 
 
 def norm_features(features, scaler=None):
@@ -852,35 +838,24 @@ def norm_features(features, scaler=None):
 
 def compute_selected_features_color2d(img, segments, feature_flags=FEATURES_SET_ALL):
     """ features of a colour image selected by the dictionary grammar ``{'color[_<space>]': flags, 'tLM[_short]': flags}``
-    (reference descriptors.py:1207-1270)
+    (reference descriptors.py:1207-1270): the table of :func:`device_feature_table` over the given label map, from one upload of the
+    image and one of the labels.  Other groups and statistics are dropped with a warning.
     """
-    img = np.asarray(img)
+    img, segments = _device_dtype(img), np.asarray(segments)
     _check_color_image(img)
-    features, names = [], []
-    for k in [k for k in feature_flags if k.startswith('color')]:
-        clr = k.split('_')[-1] if '_' in k else 'rgb'
-        if '_' in k:
-            from .color import convert_img_color_from_rgb
-            img_color = convert_img_color_from_rgb(img, clr)
-        else:
-            img_color = img
-        fts, ns = compute_image2d_color_statistic(img_color, segments, feature_flags[k], color_name=clr)
-        features.append(fts)
-        names += ns
-    for k in [k for k in feature_flags if k.startswith('tLM')]:
-        bank_type = k.split('_')[-1] if '_' in k else 'normal'
-        from .texture import compute_texture_desc_lm_img2d_clr
-        fts, ns = compute_texture_desc_lm_img2d_clr(img, segments, feature_flags[k], bank_type)
-        features.append(fts)
-        names += ns
+    layout, ncol = native_feature_layout(feature_flags)
     _check_unrecognised_feature_group(feature_flags)
-    features = np.concatenate(tuple(features), axis=1)
-    features = np.nan_to_num(features)
-    features[features == 0] = 0
+    if not layout:
+        raise ValueError('no colour or texture feature group in %r' % (feature_flags, ))
+    for key, _, _, _ in layout:
+        _check_unrecognised_feature_names(feature_flags[key])
+    _check_color_image_segm(img, segments)
+    eng, d_img, d_seg, nb = _upload(img, segments)
+    feat = eng.buf('feat', (nb, max(ncol, 1)), eng.torch.float64)
+    device_feature_table(eng, d_img, d_seg, nb, feature_flags, feat)
+    features, names = _finish_features(eng.to_host(feat[:, :ncol]), native_feature_names(feature_flags))
     if not features.size:
         logging.error('not supported features: %r', feature_flags)
-    if features.shape[1] != len(names):
-        raise ValueError('features: %r and names %r' % (features.shape, names))
     return features, names
 
 
@@ -938,6 +913,68 @@ def native_feature_layout(dict_features):
         layout.append((k, flags, col, n))
         col += n
     return layout, col
+
+
+def _lm_bank(key):
+    """the bank type of a texture group"""
+    return 'short' if key.endswith('_short') else 'normal'
+
+
+def _stat_names(prefix, flags):
+    """'<prefix>-chN_<statistic>' of a three-channel source, statistic-major and channel-minor"""
+    return ['%s-ch%i_%s' % (prefix, c + 1, f) for f in flags for c in range(3)]
+
+
+def native_feature_names(dict_features):
+    """the column names of the :func:`native_feature_layout` table: '<space>-chN_<statistic>' for a colour group (space 'rgb' for a
+    key without '_'), 'tLM_<battery>-chN_<statistic>' battery-major for a texture group"""
+    from .texture import bank_names
+    names = []
+    for key, flags, _, _ in native_feature_layout(dict_features)[0]:
+        if key.startswith('color'):
+            names += _stat_names(key.split('_')[-1] if '_' in key else 'rgb', flags)
+        else:
+            names += [n for battery in bank_names(_lm_bank(key)) for n in _stat_names('tLM_' + battery, flags)]
+    return names
+
+
+def _check_gradient_size(shape_hw, group_flags):
+    """``meanGrad`` of an image less than two pixels high or wide: numpy's own error for a gradient of such an array"""
+    if min(shape_hw) < 2 and any('meanGrad' in flags for flags in group_flags):
+        raise ValueError('Shape of array too small to calculate a numerical gradient, at least (edge_order + 1) elements are required.')
+
+
+def _finish_features(features, names):
+    """NaN / inf -> finite, -0 -> +0, one name per column (the reference's closing steps of a feature table)"""
+    features = np.nan_to_num(features)
+    features[features == 0] = 0
+    if features.shape[1] != len(names):
+        raise ValueError('features: %r and names %r' % (features.shape, names))
+    return features, names
+
+
+def device_feature_table(eng, d_img, d_seg, nb, dict_features, feat, want_centres=False):
+    """the :func:`native_feature_layout` table of a [H,W,3] device image over device labels [H,W] int32 in [0, nb), into ``feat``
+    (at least nb rows and the layout's columns).  A colour group takes the image, or its device conversion when the key ends in
+    '_<space>' of :data:`~.color.DICT_CONVERT_COLOR_FROM_RGB`; a texture group takes the fused Leung-Malik kernel, or the materialised
+    responses when it asks for median or meanGrad.  Nothing is read back.  With ``want_centres`` the first statistics launch of a
+    colour group also forms the centroids: returns them, or None when no group has such a launch."""
+    from .color import DICT_CONVERT_COLOR_FROM_RGB
+    from .texture import device_lm_features, device_lm_materialised
+    layout, _ = native_feature_layout(dict_features)
+    _check_gradient_size(d_seg.shape, [flags for _, flags, _, _ in layout])
+    centres = None
+    for key, flags, col0, _ in layout:
+        if key.startswith('color'):
+            space = key.split('_')[-1]
+            src = eng.color_convert(d_img, space) if space in DICT_CONVERT_COLOR_FROM_RGB else d_img
+            got = eng.group_stats(src, d_seg, nb, flags, feat, col0, want_centres=want_centres and centres is None)
+            centres = centres if got is None else got
+        elif 'median' in flags or 'meanGrad' in flags:
+            device_lm_materialised(eng, d_img, d_seg, nb, flags, _lm_bank(key), feat, col0)
+        else:
+            device_lm_features(eng, d_img, d_seg, nb, flags, _lm_bank(key), feat=feat, col0=col0)
+    return centres
 
 
 # the Leung-Malik bank lives in texture.py (it shares the device layout code); the reference keeps it in this module

@@ -19,7 +19,8 @@ import logging
 import numpy as np
 
 from .class_models import CompiledModel, compile_model
-from .descriptors import FEATURES_SET_COLOR, compute_selected_features_img2d, flags_are_resident, native_feature_layout
+from .descriptors import (FEATURES_SET_COLOR, _check_gradient_size, compute_selected_features_img2d, device_feature_table,
+                          flags_are_resident, native_feature_layout)
 from .engine import edge_capacity, edges_fit, get_engine
 from .graph_cuts import class_model_spec, device_gmm_applicable, estim_class_model, segment_graph_cut_general
 from .superpixels import _as_rgb_like, _supported_dtype, slic_params
@@ -50,8 +51,7 @@ def _device_slic_features(eng, image, dict_features, sp_size, sp_regul):
     if not on_device:
         image = _supported_dtype(_as_rgb_like(image))
     H, W = int(image.shape[0]), int(image.shape[1])
-    if min(H, W) < 2 and any('meanGrad' in flags for flags in dict_features.values()):
-        raise ValueError('Shape of array too small to calculate a numerical gradient, at least (edge_order + 1) elements are required.')
+    _check_gradient_size((H, W), dict_features.values())      # before SLIC: the feature table would refuse this image
     n_seg, compact = slic_params((H, W), sp_size, sp_regul)
     if n_seg < 1:
         raise ValueError('superpixel size %r is larger than the image %r' % (sp_size, tuple(image.shape)))
@@ -60,21 +60,8 @@ def _device_slic_features(eng, image, dict_features, sp_size, sp_regul):
     res.d_img = image if on_device else eng.to_device(image, 'image')
     res.d_seg, res.d_n_labels = eng.slic(res.d_img, n_seg, compact, sigma=1.0)
     res.nb_bound = eng.slic_label_bound(H, W, n_seg)
-    layout, ncol = native_feature_layout(dict_features)
-    res.d_feat = eng.buf('feat', (res.nb_bound, max(ncol, 1)), eng.torch.float64)
-    res.d_centres = None
-    for key, flags, col0, _ in layout:
-        if key.startswith('color'):
-            src = res.d_img if key == 'color' else eng.color_convert(res.d_img, key.split('_')[-1])
-            centres = eng.group_stats(src, res.d_seg, res.nb_bound, flags, res.d_feat, col0, want_centres=res.d_centres is None)
-            res.d_centres = res.d_centres if centres is None else centres
-        else:
-            from .texture import device_lm_features, device_lm_materialised
-            bank = 'short' if key.endswith('_short') else 'normal'
-            if 'median' in flags or 'meanGrad' in flags:
-                device_lm_materialised(eng, res.d_img, res.d_seg, res.nb_bound, flags, bank, res.d_feat, col0)
-            else:
-                device_lm_features(eng, res.d_img, res.d_seg, res.nb_bound, flags, bank, feat=res.d_feat, col0=col0)
+    res.d_feat = eng.buf('feat', (res.nb_bound, max(native_feature_layout(dict_features)[1], 1)), eng.torch.float64)
+    res.d_centres = device_feature_table(eng, res.d_img, res.d_seg, res.nb_bound, dict_features, res.d_feat, want_centres=True)
     if res.d_centres is None:
         _, res.d_centres, _ = eng.segment_stats(None, res.d_seg, res.nb_bound, (), want_centres=True)
     return res

@@ -7,7 +7,7 @@ Host side: the filter bank is built with numpy/scipy exactly like the reference 
 the log-norm scaling and the per-superpixel statistics run in CUDA (``csrc/lm_texture.cu``).
 """
 import ctypes as C
-import itertools
+import functools
 
 import numpy as np
 
@@ -67,6 +67,19 @@ def create_filter_bank_lm_2d(radius=16, sigmas=None, nb_orient=8):
     return filters, names
 
 
+def lm_bank(bank_type):
+    """:func:`create_filter_bank_lm_2d` of the 'short' bank (3 sigmas x 4 orientations, 15 batteries) or, for any other bank type,
+    of the full one (4 x 8, 20 batteries)"""
+    from .descriptors import SHORT_FILTERS_SIGMAS
+    return create_filter_bank_lm_2d(sigmas=SHORT_FILTERS_SIGMAS, nb_orient=4) if bank_type == 'short' else create_filter_bank_lm_2d()
+
+
+@functools.lru_cache(maxsize=None)
+def bank_names(bank_type):
+    """the battery names of :func:`lm_bank`, built once per bank type"""
+    return tuple(lm_bank(bank_type)[1])
+
+
 def _round_tf32(x):
     """cvt.rna.tf32.f32: round a float32 to 10 explicit mantissa bits, ties away from zero"""
     bits = np.ascontiguousarray(x, dtype=np.float32).view(np.uint32)
@@ -78,13 +91,8 @@ def bank_operand_layout(bank_type):
     """(names, w_tc, NP, orient, n_batt) for 'normal' / 'short' on the HOST.  ``w_tc`` holds, per kernel row, the weights in the operand
     layout of the tensor-core contraction (see isb_lm_texture): float32 [33 kernel rows][hi | lo][10 k-chunks][NP / 8][8 filters][4 taps],
     correlation form (kernels flipped), tf32-rounded value and tf32-rounded remainder, taps 33..39 and the padding filters zero"""
-    from .descriptors import SHORT_FILTERS_SIGMAS
-    if bank_type == 'short':
-        filters, names = create_filter_bank_lm_2d(sigmas=SHORT_FILTERS_SIGMAS, nb_orient=4)
-        orient, NP = 4, 48
-    else:
-        filters, names = create_filter_bank_lm_2d()
-        orient, NP = 8, 80
+    filters, names = lm_bank(bank_type)
+    orient, NP = (4, 48) if bank_type == 'short' else (8, 80)
     n_sig = len(filters) // 5
     cols = []
     for s in range(n_sig):      # oriented batteries first: edge s0 | bar s0 | edge s1 | ...
@@ -155,16 +163,16 @@ def _device_batteries(eng, bank_type):
     """the batteries of :func:`create_filter_bank_lm_2d` for 'normal' / 'short' as f64 device tensors, uploaded once per device"""
     key = ('batteries', bank_type, eng.device.index)
     if key not in _BANK_CACHE:
-        from .descriptors import SHORT_FILTERS_SIGMAS
-        filters, _ = create_filter_bank_lm_2d(sigmas=SHORT_FILTERS_SIGMAS, nb_orient=4) if bank_type == 'short' else create_filter_bank_lm_2d()
+        filters, _ = lm_bank(bank_type)
         _BANK_CACHE[key] = [eng.torch.from_numpy(np.ascontiguousarray(f, dtype=np.float64)).to(eng.device) for f in filters]
     return _BANK_CACHE[key]
 
 
 def device_lm_materialised(eng, d_img, d_seg, nb, flags, bank_type, feat, col0):
-    """the device form of :func:`_texture_desc_lm_materialised` into feat[:, col0:] (battery-major): background subtraction
-    (``isb_lm_background``), then per battery the clipped, log-norm scaled responses (``isb_lm_battery_response``) and their group
-    statistics (:meth:`~.engine.Engine.group_stats`).  Nothing is read back; the buffers are the engine's."""
+    """the reference's own sequence (descriptors.py:1078-1098) with every response in memory, into feat[:, col0:] (battery-major):
+    background subtraction (``isb_lm_background``), then per battery the clipped, log-norm scaled responses
+    (``isb_lm_battery_response``) and their group statistics (:meth:`~.engine.Engine.group_stats`) -- the route for the statistics
+    the fused kernel does not produce (``median``, ``meanGrad``).  Nothing is read back; the buffers are the engine's."""
     from .descriptors import MAX_SIGNAL_RESPONSE
     from .engine import gaussian_half_kernel
     torch, lib = eng.torch, eng.lib
@@ -188,72 +196,15 @@ def device_lm_materialised(eng, d_img, d_seg, nb, flags, bank_type, feat, col0):
     return feat
 
 
-def _texture_desc_lm_materialised(img, seg, feature_flags, bank_type):
-    """ the reference's own sequence (descriptors.py:1078-1098) with every array in memory: background (sigma 150 on all three
-    axes), per battery the strongest response per channel (FP64 on the device, ``isb_filter_response_2d``), clip, log-norm
-    scaling, then :func:`compute_image2d_color_statistic` -- the route for the statistics the fused kernel does not produce
-    (``median``, ``meanGrad``) """
-    from .descriptors import (MAX_SIGNAL_RESPONSE, SHORT_FILTERS_SIGMAS, _gauss_smooth_slices, compute_image2d_color_statistic,
-                              compute_img_filter_response3d)
-    img = np.asarray(img, dtype=np.float64)
-    _, _, mix = background_kernel()
-    roll = np.ascontiguousarray(np.rollaxis(img, -1, 0))
-    smooth = _gauss_smooth_slices(roll, BACKGROUND_SIGMA)          # the two image axes ...
-    roll = roll - np.tensordot(mix, smooth, axes=(1, 0))           # ... and the reflected length-3 channel axis
-    if bank_type == 'short':
-        filters, fl_names = create_filter_bank_lm_2d(sigmas=SHORT_FILTERS_SIGMAS, nb_orient=4)
-    else:
-        filters, fl_names = create_filter_bank_lm_2d()
-    features, names = [], []
-    for battery, fl_name in zip(filters, fl_names):
-        resp = compute_img_filter_response3d(roll, battery)
-        resp[resp > MAX_SIGNAL_RESPONSE] = MAX_SIGNAL_RESPONSE
-        norm = np.sqrt(np.sum(resp ** 2))
-        if norm == 0 or abs(norm) == np.inf:
-            resp = np.zeros(resp.shape)
-        else:
-            resp = (resp * (np.log(1 + norm) / 0.03)) / norm
-        fts, ns = compute_image2d_color_statistic(np.rollaxis(resp, 0, 3), seg, feature_flags, fl_name)
-        features.append(fts)
-        names += ns
-    features = np.nan_to_num(np.concatenate(tuple(features), axis=1))
-    features[features == 0] = 0
-    names = ['tLM_%s' % n for n in names]
-    if features.shape[1] != len(names):
-        raise ValueError('features: %r and names %r' % (features.shape, names))
-    return features, names
-
-
 def compute_texture_desc_lm_img2d_clr(img, seg, feature_flags, bank_type='normal'):
     """ texture descriptors of a colour image: statistics of the Leung-Malik filter-bank responses per segment
-    (reference descriptors.py:1041-1106)
+    (reference descriptors.py:1041-1106), the texture group of :func:`~.descriptors.compute_selected_features_color2d`
 
     :param ndarray img: image [H, W, 3]
     :param ndarray seg: segmentation [H, W]
-    :param list(str) feature_flags: subset of ('mean', 'std', 'energy') -- the statistics the device computes
+    :param list(str) feature_flags: subset of ('mean', 'std', 'energy', 'median', 'meanGrad')
     :param str bank_type: 'normal' (4 sigmas x 8 orientations, 20 batteries) or 'short' (3 x 4, 15 batteries)
     :return tuple(ndarray,list(str)): features [nb_segments, n_batteries * 3 * n_flags], names
     """
-    from .descriptors import NAMES_FEATURE_FLAGS, _check_color_image, _check_color_image_segm, _check_unrecognised_feature_names, _device_dtype
-    img, seg = _device_dtype(img), np.asarray(seg)
-    _check_color_image(img)
-    _check_color_image_segm(img, seg)
-    if any(f in ('median', 'meanGrad') for f in feature_flags):
-        # these two statistics need the filter responses in memory: per-battery path, exactly the reference's sequence
-        return _texture_desc_lm_materialised(img, seg, feature_flags, bank_type)
-    flags = [f for f in ('mean', 'std', 'energy') if f in feature_flags]
-    _check_unrecognised_feature_names(feature_flags)
-    eng = get_engine()
-    nb = int(seg.max()) + 1
-    d_img = eng.to_device(img, 'image')
-    d_seg = eng.to_device(seg.astype(np.int32, copy=False), 'seg_in')
-    feat, fl_names, ncol = device_lm_features(eng, d_img, d_seg, nb, flags, bank_type)
-    features = eng.to_host(feat).copy()
-    order = [f for f in NAMES_FEATURE_FLAGS if f in flags]
-    names = list(itertools.chain.from_iterable(
-        ['tLM_%s-ch%i_%s' % (n, c + 1, f) for f in order for c in range(3)] for n in fl_names))
-    features = np.nan_to_num(features)
-    features[features == 0] = 0
-    if features.shape[1] != len(names):
-        raise ValueError('features: %r and names %r' % (features.shape, names))
-    return features, names
+    from .descriptors import compute_selected_features_color2d
+    return compute_selected_features_color2d(img, seg, {'tLM_short' if bank_type == 'short' else 'tLM': feature_flags})

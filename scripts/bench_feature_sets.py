@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """
 bench_feature_sets.py -- the feature sets the reference's users run (median, meanGrad, colour-space groups) on the resident device
-path against the general path they took before.  Prints one JSON line.
+path against the general path and the numpy API.  Prints one JSON line.
 
     python scripts/bench_feature_sets.py --steps K --warmup W [--texture]
 
@@ -12,8 +12,10 @@ descriptors.FEATURES_SET_ALL (colour and tLM with all five statistics).  Legs, a
   pipe_resident / pipe_general   pipe_color2d_slic_features_model_graphcut (self-fitted GMM), resident vs. debug_visual={} -- the
                                  general path through the numpy-facing stages (which also fills the small debug_visual arrays; its
                                  features come from compute_color2d_superpixels_features, so from the resident feature table too)
-  features_resident / features_host   compute_color2d_superpixels_features vs. segment_slic_img2d + compute_selected_features_img2d
-Parity: max |features resident - host route| per set on the same superpixels, and segm equality of the two pipeline paths under
+  features_resident / features_numpy  compute_color2d_superpixels_features vs. segment_slic_img2d + compute_selected_features_img2d
+                                       -- the numpy API on the label map SLIC gave (the same device feature driver, with one
+                                       upload of the image and of the labels and one download of the table)
+Parity: max |features resident - numpy API| per set on the same superpixels, and segm equality of the two pipeline paths under
 one caller-fitted StandardScaler + GaussianMixture.
 """
 import argparse
@@ -62,8 +64,8 @@ def run(steps, warmup, texture):
                 ('pipe_general', lambda: pipelines.pipe_color2d_slic_features_model_graphcut(img, K, feats, SP, REG, gc_regul=GC,
                                                                                                debug_visual={})),
                 ('features_resident', lambda: pipelines.compute_color2d_superpixels_features(img, feats, SP, REG)),
-                ('features_host', lambda: compute_selected_features_img2d(img, segment_slic_img2d(img, sp_size=SP, relative_compact=REG),
-                                                                          feats))]
+                ('features_numpy', lambda: compute_selected_features_img2d(img, segment_slic_img2d(img, sp_size=SP, relative_compact=REG),
+                                                                           feats))]
 
     nstage = lib.isb_profile_stage_count()
     stage_ids = {lib.isb_profile_stage_name(i).decode(): i for i in range(nstage)}
@@ -75,14 +77,14 @@ def run(steps, warmup, texture):
                 fn()
         # parity: features on the same superpixels, and one caller-fitted model through both pipeline paths
         slic, fts = pipelines.compute_color2d_superpixels_features(img, feats, SP, REG)
-        host_fts, _ = compute_selected_features_img2d(img, slic, feats)
+        api_fts, _ = compute_selected_features_img2d(img, slic, feats)
         model = pipeline.Pipeline([('scaler', preprocessing.StandardScaler()),
-                                   ('model', mixture.GaussianMixture(K, covariance_type='full', random_state=0))]).fit(host_fts)
+                                   ('model', mixture.GaussianMixture(K, covariance_type='full', random_state=0))]).fit(api_fts)
         seg_res, _ = pipelines.segment_color2d_slic_features_model_graphcut(img, model, feats, SP, REG, GC)
         seg_gen, _ = pipelines.segment_color2d_slic_features_model_graphcut(img, model, feats, SP, REG, GC, debug_visual={})
-        parity = {'features_max_abs_diff': float(np.max(np.abs(fts - host_fts))), 'n_features': int(fts.shape[1]),
+        parity = {'features_max_abs_diff': float(np.max(np.abs(fts - api_fts))), 'n_features': int(fts.shape[1]),
                   'shared_model_segm_identical': bool(np.array_equal(seg_res, seg_gen))}
-        del seg_res, seg_gen, fts, host_fts
+        del seg_res, seg_gen, fts, api_fts
         per_step = {name: [] for name, _ in legs}
         for _ in range(steps):           # the legs alternate inside every step (the host shares the machine with other work)
             for name, fn in legs:
@@ -106,8 +108,8 @@ def run(steps, warmup, texture):
                               'segment_stats_stage_ms': ms_arr[stage_ids['segment_stats']], 'lm_stage_ms': ms_arr[stage_ids['lm_texture']]}
         result[set_name] = {'features': {k: list(v) for k, v in feats.items()}, 'legs': legs_out, 'parity': parity,
                             'speedup_pipe': legs_out['pipe_general']['ms_per_image'] / legs_out['pipe_resident']['ms_per_image'],
-                            'speedup_features': legs_out['features_host']['ms_per_image'] / legs_out['features_resident']['ms_per_image']}
-    return {'metric': 'ms per image, feature sets with median / meanGrad / colour spaces: resident path vs general path',
+                            'speedup_features': legs_out['features_numpy']['ms_per_image'] / legs_out['features_resident']['ms_per_image']}
+    return {'metric': 'ms per image, feature sets with median / meanGrad / colour spaces: resident path vs general path and numpy API',
             'unit': 'ms', 'n_gpus': 1, 'steps': steps, 'warmup': warmup, 'higher_is_better': False, 'dtype': 'f64', 'data': 'synthetic',
             'config': {'workload': 'one config-2 image (%dx%d RGB f64), SLIC sp_size=%d, %d-class GMM, GraphCut gc_regul %g'
                                    % (bench.H, bench.W, SP, K, GC),

@@ -19,6 +19,35 @@ def test_native_feature_layout_mixed_dict():
         [('color', ['mean', 'std', 'energy'], 0, 9), ('tLM', ['mean'], 9, 60)], 69)
 
 
+def test_native_feature_names():
+    from pyimsegm_b200.descriptors import NAMES_FEATURE_FLAGS, _stat_names, native_feature_names
+
+    def chans(prefix, flags):
+        return ['%s-ch%i_%s' % (prefix, c, f) for f in flags for c in (1, 2, 3)]
+
+    # compute_image2d_color_statistic's default color_name: the reference doctest (descriptors.py:804-808)
+    assert _stat_names('color', NAMES_FEATURE_FLAGS) == [
+        'color-ch1_mean', 'color-ch2_mean', 'color-ch3_mean', 'color-ch1_std', 'color-ch2_std', 'color-ch3_std',
+        'color-ch1_energy', 'color-ch2_energy', 'color-ch3_energy', 'color-ch1_median', 'color-ch2_median', 'color-ch3_median',
+        'color-ch1_meanGrad', 'color-ch2_meanGrad', 'color-ch3_meanGrad']
+    # 'color' and keys without '_' are 'rgb', a known or unknown space names itself; duplicate and unknown flags drop out
+    assert native_feature_names({'color': ('std', 'mean', 'std', 'foo')}) == chans('rgb', ('mean', 'std'))
+    assert native_feature_names({'colorX': ('energy', )}) == chans('rgb', ('energy', ))
+    assert native_feature_names({'color_hsv': ('meanGrad', 'median')}) == chans('hsv', ('median', 'meanGrad'))
+    assert native_feature_names({'color_foo': ('mean', )}) == chans('foo', ('mean', ))
+    # colour groups first, then texture groups, each in dict order; other groups contribute nothing
+    assert native_feature_names({'tLM_short': ('mean', ), 'gray': ('mean', ), 'color_lab': ('std', ), 'color': ('mean', )}) == (
+        chans('lab', ('std', )) + chans('rgb', ('mean', ))
+        + [n for s in ('1.4', '2.0', '4.0') for b in ('edge', 'bar', 'Gauss', 'GaussLap', 'GaussLap2')
+           for n in chans('tLM_sigma%s-%s' % (s, b), ('mean', ))])
+    # the full bank for 'tLM' and any suffix other than 'short', battery-major (reference descriptors.py:1066-1074)
+    full = [n for s in ('1.4', '2.0', '2.8', '4.0') for b in ('edge', 'bar', 'Gauss', 'GaussLap', 'GaussLap2')
+            for n in chans('tLM_sigma%s-%s' % (s, b), ('mean', 'std', 'median'))]
+    assert native_feature_names({'tLM': ('median', 'mean', 'std')}) == full
+    assert native_feature_names({'tLM_long': ('median', 'mean', 'std')}) == full
+    assert native_feature_names({}) == [] and native_feature_names({'color': ()}) == []
+
+
 def test_resident_predicate():
     from pyimsegm_b200.descriptors import FEATURES_SET_ALL, NAMES_FEATURE_FLAGS, flags_are_native, flags_are_resident
     admitted = [{'color': ['mean', 'std', 'median']}, {'color': ['mean', 'median']}, {'color': NAMES_FEATURE_FLAGS}, FEATURES_SET_ALL,
