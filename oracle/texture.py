@@ -72,6 +72,50 @@ def battery_responses(img, bank_type='normal', background_sigma=150):
     return np.array(out), names
 
 
+def reflect_index(n, pad):
+    """indices of an axis of length n padded by ``pad`` on both sides in ndimage's mode 'reflect' (d c b a | a b c d | d c b a), for
+    any pad: the 2n-periodic reflection.  np.pad(mode='symmetric') differs from it once the pad is wider than the axis."""
+    i = np.arange(-pad, n + pad) % (2 * n)
+    return np.where(i < n, i, 2 * n - 1 - i)
+
+
+def convolve_reflect(planes, kernels):
+    """ndimage.convolve(plane, kernel) (mode 'reflect') of every plane [..., H, W] with every odd square kernel [K, k, k], in float64
+    by FFT: reflect-pad, then fftconvolve 'valid'.  Returns [K, ..., H, W]."""
+    from scipy import signal
+    planes = np.asarray(planes, dtype=np.float64)
+    kernels = np.asarray(kernels, dtype=np.float64)
+    r = kernels.shape[-1] // 2
+    H, W = planes.shape[-2:]
+    padded = planes[..., reflect_index(H, r)[:, None], reflect_index(W, r)[None, :]]
+    kern = kernels.reshape(kernels.shape[:1] + (1, ) * (planes.ndim - 2) + kernels.shape[1:])
+    return signal.fftconvolve(padded[None], kern, mode='valid', axes=(-2, -1))
+
+
+def clipped_responses(img, bank_type='normal', background_sigma=150):
+    """the reference's responses before their log-norm scaling (descriptors.py:1078-1092), by FFT in float64:
+    (img - background [3, H, W], clipped battery responses [n_batteries, 3, H, W], battery norms [n_batteries]).
+    A battery's scaled response is ``a * resp`` with ``a = log(1 + norm) / 0.03 / norm`` (0 when the norm is 0 or infinite)."""
+    img = np.asarray(img)
+    sub = img - ndimage.gaussian_filter(img.astype(float), background_sigma)
+    roll = np.rollaxis(sub, -1, 0)
+    bank, _ = filter_bank(sigmas=SIGMAS_SHORT, nb_orient=4) if bank_type == 'short' else filter_bank()
+    out = np.empty((len(bank), ) + roll.shape)
+    for b, battery in enumerate(bank):
+        resp = np.max(convolve_reflect(roll, battery), axis=0)
+        resp[resp > MAX_RESPONSE] = MAX_RESPONSE
+        out[b] = resp
+    return roll, out, np.sqrt(np.sum(out ** 2, axis=(1, 2, 3)))
+
+
+def norm_scale(norms):
+    """the log-norm factor a of every battery (descriptors.py:1090-1094); 0 for a norm of 0, inf or NaN, whose features are 0"""
+    norms = np.asarray(norms, dtype=np.float64)
+    ok = (norms != 0) & np.isfinite(norms)
+    safe = np.where(ok, norms, 1.)
+    return np.where(ok, np.log(1 + safe) / 0.03 / safe, 0.)
+
+
 def texture_desc_lm(img, seg, flags, bank_type='normal', stat_fn=None):
     """features [N, n_batteries * 3 * len(flags)] in the reference's column order, names"""
     import oracle

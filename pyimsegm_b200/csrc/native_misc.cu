@@ -287,7 +287,9 @@ __global__ void __launch_bounds__(256) k_conv_battery_max(const double* __restri
             const int yy = reflect_at(y + kh / 2 - a, H);
             for (int b = kw - 1; b >= 0; --b) acc = __dadd_rn(acc, __dmul_rn(k[a * kw + b], im[(size_t)yy * W + reflect_at(x + kw / 2 - b, W)]));
         }
-        best = (f == 0 || acc > best) ? acc : best;   // np.max over the battery (NaN handling is not needed: inputs are finite)
+        // np.max over the battery, which returns NaN when any kernel's response is NaN: the Leung-Malik route feeds this kernel an
+        // image minus its background, NaN wherever the image has a NaN or an infinity within the background's reach
+        best = (f == 0 || acc > best || isnan(acc)) ? acc : best;
     }
     out[i] = best;
 }
