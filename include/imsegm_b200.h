@@ -77,8 +77,15 @@ int isb_slic_kmeans(const double* lab_planar, int H, int W, const double* seeds_
                     double step, int max_iter, int slic_zero, int32_t* labels, double* centroids, void* ws, size_t ws_bytes,
                     isb_stream_t stream);
 
+/* Test hooks of the sweeps' per-tile candidate lists.  isb_slic_set_tile_cap(cap > 0) caps the list of every tile at cap
+ * records for workspaces sized afterwards (0 restores the default sizing) and returns the previous cap; a tile whose list
+ * overflows is assigned by scanning every cluster, with the same result.  isb_slic_full_scan_tiles counts those tile
+ * assignments on the current device since the library was loaded. */
+int isb_slic_set_tile_cap(int cap);
+long long isb_slic_full_scan_tiles(void);
+
 /* Row-band form of the sweeps: one image taller than a GPU wants to hold (BASELINE config 5, SURVEY.md section 8e) is cut into
- * row bands, one per GPU.  The cluster state (centres, windows, bins) is replicated in every band's workspace and lives in
+ * row bands, one per GPU.  The cluster state (centres, windows) is replicated in every band's workspace and lives in
  * the coordinates of the whole image; a band holds pixel memory for its owned rows plus a halo of >= 2*step_y rows on either
  * side, assigns every row of that slab and sums the clusters whose centre row it owns (all their members are inside the slab;
  * a member further away -- an orphan that no window covers -- is counted in xchg[6 n_seeds] and the caller must then fall back

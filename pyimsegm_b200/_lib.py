@@ -52,6 +52,8 @@ SIGNATURES = {
     'isb_segment_stats_finish': (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     'isb_slic_kmeans_workspace_bytes': (_sz, [_i, _i, _i, _i, _i]),
     'isb_slic_kmeans': (_i, [_vp, _i, _i, _vp, _i, _i, _i, _d, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    'isb_slic_set_tile_cap': (_i, [_i]),
+    'isb_slic_full_scan_tiles': (_ll, []),
     'isb_slic3d_prepare': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _d, _vp, _vp, _vp]),
     'isb_slic3d_kmeans_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'isb_slic3d_kmeans': (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _d, C.POINTER(_d), _i, _vp, _vp, _sz, _vp]),

@@ -5,8 +5,8 @@
 // The original is cluster-centric: for k ascending, scan the +-2*step window and take the pixel when
 // `distance > d` (strict) -- i.e. every pixel ends with argmin over {clusters whose window holds it} of
 // (d, k) in lexicographic order.  That per-pixel minimum is order-independent, so it is evaluated here
-// pixel-centric: one CTA per 32x32 pixel tile gathers the clusters whose integer window intersects the tile
-// (from a uniform bin grid over the current centroids), every pixel loops over that list in shared memory.
+// pixel-centric: one CTA per 32x32 pixel tile takes the list of the clusters whose integer window intersects the tile
+// (written by whoever last set the cluster's centre), every pixel loops over that list in shared memory.
 // The distance is computed with the oracle's exact operation order in IEEE double (no FMA).
 //
 // The centroid update of the original is a raster-order SEQUENTIAL double sum per cluster; a tree/atomic
@@ -43,18 +43,16 @@ struct KmState {
     double* cy; double* cx; double* c0; double* c1; double* c2;
     int4* win;       // [n] (y0, y1, x0, x1); empty (0,0,0,0) when dead
     int4* obb;       // [n] bbox of the cluster's member pixels (ymin, ymax, xmin, xmax), empty = (INT_MAX, -1, INT_MAX, -1)
-    int* bin_start;  // [nbins + 1]
-    int* bin_fill;   // [nbins]
-    int* bin_of;     // [n]
-    int* pack_done;  // [1] CTA counter of k_pack
-    Cand* packed;    // [n] cluster records in bin order (what k_assign streams)
-    double* packed_maxdc; // [n] SLICO: the maxima in bin order, beside `packed`
+    // per 32x32 tile of the pixel memory: the records of the clusters whose window meets it, in no particular order.  A tile whose
+    // count exceeds tcap has overflowed (its list is incomplete) and k_assign scans every cluster for it instead.
+    int* tile_cnt;   // [tiles]
+    Cand* tile_cand; // [tiles * tcap]
     unsigned long long* maxdc; // [n] SLICO colour-distance maxima as raw double bits (non-negative doubles order like their bits)
     int slico;
-    int n, H, W, step_y, step_x, B, nby, nbx;
+    int n, H, W, step_y, step_x, ntx, tcap;   // ntx: tiles per row
     double sw;       // spatial weight 1/step^2
     // Row-band mode (one band of a taller image per GPU, isb_slic_band_*): pixel memory is a slab of H rows whose row 0 is
-    // global row y_off of an image Hg rows tall; cluster geometry (centres, windows, bins) is always global.  The
+    // global row y_off of an image Hg rows tall; cluster geometry (centres, windows) is always global.  The
     // monolithic path is the band [0, H) of itself: y_off = 0, Hg = H, pstride = H * W.
     int Hg, y_off, own_lo, own_hi, halo;
     size_t pstride;  // distance between the Lab planes, in doubles
@@ -74,129 +72,110 @@ __device__ __forceinline__ int4 make_window(double cy, double cx, int step_y, in
     return w;
 }
 
-// Between two sweeps the clusters are re-binned in three small launches:
-//   k_seed (first sweep only) or k_update / k_import : centres, windows, bin_of, and a count per bin in bin_fill
-//   k_scan_bins (one CTA)  : exclusive scan of the counts -> bin_start; the counts are zeroed (they become the fill cursors)
-//   k_pack (many CTAs)     : the packed, bin-ordered cluster records that k_assign streams; order inside a bin is irrelevant
-//   (k_assign leaves bin_fill alone; k_update / k_import need it zero again, k_pack's last CTA does that)
+// Between two sweeps nothing is re-binned: whoever sets a cluster's centre -- k_seed (first sweep), k_update<false> or k_import
+// (band mode) -- appends its record to the list of every tile its window meets, and k_assign zeroes its tile's count once it
+// has read it, so that the next appends start from zero.  Dead clusters append nothing.
+__device__ __forceinline__ Cand make_cand(int k, double cy, double cx, double c0, double c1, double c2, int4 w)
+{
+    Cand c;
+    c.cy = cy; c.cx = cx; c.c0 = c0; c.c1 = c1; c.c2 = c2;
+    c.y0 = w.x; c.y1 = w.y; c.x0 = w.z; c.x1 = w.w; c.k = k; c.pad = 0;
+    return c;
+}
+
+// append c to the tiles of this slab that its window meets; thread t of nt takes every nt-th of those tiles
+__device__ __forceinline__ void append_tiles(const KmState& s, const Cand& c, int t, int nt)
+{
+    const int ya = max(c.y0 - s.y_off, 0), yb = min(c.y1 - s.y_off, s.H);   // the window's rows in the slab
+    if (ya >= yb || c.x0 >= c.x1) return;
+    const int ty0 = ya / TILE, tx0 = c.x0 / TILE;
+    const int nx = (c.x1 - 1) / TILE - tx0 + 1, nxy = ((yb - 1) / TILE - ty0 + 1) * nx;
+    for (int i = t; i < nxy; i += nt) {
+        const int tile = (ty0 + i / nx) * s.ntx + tx0 + i % nx;
+        const int pos = atomicAdd(&s.tile_cnt[tile], 1);
+        if (pos < s.tcap) s.tile_cand[(size_t)tile * s.tcap + pos] = c;
+    }
+}
+
 __global__ void k_seed(KmState s, const double* __restrict__ seeds_yx)
 {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= s.n) return;
     const double cy = seeds_yx[2 * k], cx = seeds_yx[2 * k + 1];
     s.cy[k] = cy; s.cx[k] = cx; s.c0[k] = 0.0; s.c1[k] = 0.0; s.c2[k] = 0.0;
-    s.win[k] = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
-    const int by = min(max((int)cy / s.B, 0), s.nby - 1), bx = min(max((int)cx / s.B, 0), s.nbx - 1);
-    s.bin_of[k] = by * s.nbx + bx;
-    atomicAdd(&s.bin_fill[by * s.nbx + bx], 1);
+    const int4 w = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
+    s.win[k] = w;
     s.obb[k] = make_int4(INT_MAX, -1, INT_MAX, -1);
     s.maxdc[k] = (unsigned long long)__double_as_longlong(1.0);
-}
-
-__global__ void __launch_bounds__(1024) k_scan_bins(KmState s)
-{
-    const int nbins = s.nby * s.nbx;
-    // exclusive scan of bin counts: warp shuffles + one partial per warp, chunks of blockDim
-    __shared__ int s_wsum[32];
-    __shared__ int s_part_total;
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) { s_carry = 0; *s.pack_done = 0; }
-    __syncthreads();
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    for (int base = 0; base < nbins; base += blockDim.x) {
-        int b = base + threadIdx.x;
-        int v = b < nbins ? s.bin_fill[b] : 0;
-        int incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-        if (lane == 31) s_wsum[wid] = incl;
-        __syncthreads();
-        if (wid == 0) {
-            int t = lane < nw ? s_wsum[lane] : 0, ti = t;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { int u = __shfl_up_sync(0xffffffffu, ti, o); if (lane >= o) ti += u; }
-            s_wsum[lane] = ti - t; // exclusive prefix of the warp sums
-            if (lane == 31) s_part_total = ti;
-        }
-        __syncthreads();
-        const int carry = s_carry;
-        if (b < nbins) { s.bin_start[b] = carry + s_wsum[wid] + incl - v; s.bin_fill[b] = 0; }
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry = carry + s_part_total;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) s.bin_start[nbins] = s_carry;
-}
-
-__global__ void __launch_bounds__(256) k_pack(KmState s)
-{
-    const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k < s.n) {
-        const int bin = s.bin_of[k];
-        if (bin >= 0) {
-            const int pos = s.bin_start[bin] + atomicAdd(&s.bin_fill[bin], 1);
-            const int4 w = s.win[k];
-            Cand c;
-            c.cy = s.cy[k]; c.cx = s.cx[k]; c.c0 = s.c0[k]; c.c1 = s.c1[k]; c.c2 = s.c2[k];
-            c.y0 = w.x; c.y1 = w.y; c.x0 = w.z; c.x1 = w.w; c.k = k; c.pad = 0;
-            s.packed[pos] = c;
-            if (s.slico) s.packed_maxdc[pos] = __longlong_as_double((long long)s.maxdc[k]);
-        }
-    }
-    // the last CTA to finish zeroes the fill cursors: k_update / k_import count the next sweep's bins from zero
-    __shared__ int s_last;
-    __syncthreads();
-    if (threadIdx.x == 0) { __threadfence(); s_last = atomicAdd(s.pack_done, 1) == (int)gridDim.x - 1; }
-    __syncthreads();
-    if (s_last) {
-        const int nbins = s.nby * s.nbx;
-        for (int b = threadIdx.x; b < nbins; b += blockDim.x) s.bin_fill[b] = 0;
-    }
+    append_tiles(s, make_cand(k, cy, cx, 0.0, 0.0, 0.0, w), 0, 1);
 }
 
 // non-negative doubles order like their bit patterns: compare on the integer pipe instead of the FP64 pipe
 // (unsigned, so that a NaN of either sign ranks above every number and can never win)
 __device__ __forceinline__ unsigned long long dbits(double v) { return (unsigned long long)__double_as_longlong(v); }
 
+// tile assignments that scanned every cluster because their list overflowed (isb_slic_full_scan_tiles)
+__device__ unsigned long long d_full_scans;
+
+// per-candidate floats of the per-thread lower bounds: the centre, every colour channel rounded down (lo) and up (hi), and for
+// SLICO 1 / maxdc rounded down
+struct __align__(16) CandF {
+    float cy, cx, inv, pad0;
+    float lo0, lo1, lo2, pad1;
+    float hi0, hi1, hi2, pad2;
+};
+
 // assignment: one CTA (128 threads) per 32x32 tile; a thread owns one column and AROWS = 8 consecutive rows.
-// The tile's Lab values are staged in shared memory, candidates are visited nearest-first and the loop stops as soon as
-// the spatial lower bound of every remaining candidate exceeds the worst of the thread's current minima.
+// The tile's Lab values arrive in shared memory by a TMA load while the candidate list is staged and sorted, candidates are
+// visited nearest-first and the loop stops as soon as the spatial lower bound of every remaining candidate exceeds the worst of
+// the thread's current minima.
 template <bool SLICO>
 __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ CUtensorMap lab_map, int use_tma, KmState s,
                                                         const double* __restrict__ lab, int* __restrict__ labels)
 {
-    __shared__ Cand cand[ACAP];
+    __shared__ __align__(16) Cand cand[ACAP];
     __shared__ double s_maxdc[SLICO ? ACAP : 1];
     __shared__ float s_key[ACAP];
-    __shared__ float2 s_cf[ACAP];         // (cy, cx) of the candidate as floats, for the per-thread spatial lower bound
+    __shared__ CandF s_cf[ACAP];
     __shared__ double s_lb[ACAP];          // lower bound of the spatial term of the candidate at sorted position i, and of all later ones
     __shared__ unsigned char s_order[ACAP];
     __shared__ __align__(128) double s_px[3][TILE][TILE]; // Lab of the tile
     __shared__ __align__(8) unsigned long long s_bar;     // mbarrier of the TMA tile load
-    __shared__ int s_ncand, s_done, s_row, s_off, s_total;
+    __shared__ int s_ncand, s_done;
     const int tx0 = blockIdx.x * TILE, ty0 = blockIdx.y * TILE;
     const int tx1 = min(tx0 + TILE, s.W);
     const int gy0 = ty0 + s.y_off, gy1 = min(ty0 + TILE, s.H) + s.y_off; // the tile's rows in global coordinates
+    const int tile = blockIdx.y * s.ntx + blockIdx.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const size_t HW = s.pstride;
     const int x = tx0 + lane;
     const bool xin = x < s.W;
     const int yb = ty0 + warp * AROWS; // first row of this thread
+    const uint32_t bar = wgmma::smem_u32(&s_bar);
 
     double best[AROWS];
     int bestk[AROWS];
 #pragma unroll
     for (int j = 0; j < AROWS; ++j) { best[j] = DBL_MAX; bestk[j] = -1; }
-    if (use_tma) {
+    if (threadIdx.x == 0 && use_tma) {
         // the three Lab planes of the tile arrive as ONE 3-D tensor-map load (32 x 32 x 3 doubles, out-of-image elements read as 0)
-        // while every warp gathers the candidate clusters; the distance loop waits on the mbarrier
-        if (threadIdx.x == 0) {
-            wgmma::mbar_init(wgmma::smem_u32(&s_bar), 1);
-            wgmma::fence_mbar_init();
-            wgmma::mbar_arrive_expect_tx(wgmma::smem_u32(&s_bar), 3 * TILE * TILE * 8);
-            wgmma::tma_load_3d(wgmma::smem_u32(&s_px[0][0][0]), &lab_map, tx0, ty0, 0, wgmma::smem_u32(&s_bar));
-        }
-    } else {
+        // while the candidates are staged and sorted; the distance loop waits for it
+        wgmma::mbar_init(bar, 1);
+        wgmma::fence_mbar_init();
+        wgmma::mbar_arrive_expect_tx(bar, 3 * TILE * TILE * 8);
+        wgmma::tma_load_3d(wgmma::smem_u32(&s_px[0][0][0]), &lab_map, tx0, ty0, 0, bar);
+    }
+    // the tile's list: every thread reads the count (one broadcast load); a complete list of one round is staged by 16-byte loads
+    // spread over the CTA, a longer or overflowed one in rounds below
+    const int total = s.tile_cnt[tile];
+    const bool scan_all = total > s.tcap;   // the list overflowed: every cluster's window is tested instead
+    const bool fast = total <= ACAP && !scan_all;
+    if (fast) {
+        const int4* src = reinterpret_cast<const int4*>(s.tile_cand + (size_t)tile * s.tcap);
+        int4* dst = reinterpret_cast<int4*>(cand);
+        for (int i = threadIdx.x; i < total * (int)(sizeof(Cand) / sizeof(int4)); i += ATHREADS) dst[i] = src[i];
+    }
+    if (!use_tma) {
         double v[3][AROWS];
 #pragma unroll
         for (int j = 0; j < AROWS; ++j) {
@@ -211,77 +190,62 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
             s_px[0][warp * AROWS + j][lane] = v[0][j]; s_px[1][warp * AROWS + j][lane] = v[1][j]; s_px[2][warp * AROWS + j][lane] = v[2][j];
         }
     }
-    // bins that can hold a centroid whose window reaches this tile (superset; the exact window test follows)
-    const int by0 = max(gy0 - 2 * s.step_y - 2, 0) / s.B, by1 = min(gy1 + 2 * s.step_y + 1, s.Hg - 1) / s.B;
-    const int bx0 = max(tx0 - 2 * s.step_x - 2, 0) / s.B, bx1 = min(tx1 + 2 * s.step_x + 1, s.W - 1) / s.B;
     const float tcy = 0.5f * (gy0 + gy1 - 1), tcx = 0.5f * (tx0 + tx1 - 1);
-    const int byl = min(by1, s.nby - 1), bxl = min(bx1, s.nbx - 1);
-    // how many clusters sit in the bin rows that can reach this tile (bins of one row are contiguous in bin order)
-    if (threadIdx.x == 0) { s_row = by0; s_off = 0; s_done = 0; s_ncand = 0; s_total = 0; }
     __syncthreads();
-    if (warp == 0) {
-        int t = 0;
-        for (int row = by0 + lane; row <= byl; row += 32) t += s.bin_start[row * s.nbx + bxl + 1] - s.bin_start[row * s.nbx + bx0];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-        if (lane == 0) s_total = t;
+    if (threadIdx.x == 0) {
+        s.tile_cnt[tile] = 0;   // read by every thread before the barrier; the next sweep's appends start from zero
+        if (scan_all) atomicAdd(&d_full_scans, 1ull);
     }
-    __syncthreads();
-    const bool fast = s_total <= ACAP; // everything fits in one round: all warps build the list together
 
+    int off = 0;   // warp 0, rounds: where the next round resumes
     while (true) {
-        if (fast) {
-            for (int row = by0 + warp; row <= byl; row += AWARPS) {
-                const int beg = s.bin_start[row * s.nbx + bx0], end = s.bin_start[row * s.nbx + bxl + 1];
-                for (int i = beg + lane; i < end; i += 32) {
-                    const Cand c = s.packed[i];
-                    if ((c.y0 < gy1) && (c.y1 > gy0) && (c.x0 < tx1) && (c.x1 > tx0)) {
-                        const int pos = atomicAdd(&s_ncand, 1);
-                        cand[pos] = c;
-                        if (SLICO) s_maxdc[pos] = s.packed_maxdc[i];
-                        const float fy = (float)c.cy - tcy, fx = (float)c.cx - tcx;
-                        s_key[pos] = fy * fy + fx * fx;
-                        s_cf[pos] = make_float2((float)c.cy, (float)c.cx);
-                    }
-                }
-            }
-            if (threadIdx.x == 0) s_done = 1;
-        } else if (warp == 0) {
-            // deterministic, resumable scan of the bin rows: fill up to ACAP candidates per round
+        if (!fast && warp == 0) {
+            // deterministic, resumable scan: up to ACAP candidates per round, from the tile's list while it is complete, else from
+            // every cluster whose window meets the tile
+            const int end = scan_all ? s.n : total;
             int n = 0;
-            int row = s_row, off = s_off;
-            while (row <= byl && n < ACAP) {
-                int beg = s.bin_start[row * s.nbx + bx0] + off;
-                int end = s.bin_start[row * s.nbx + bxl + 1];
-                while (beg < end && n < ACAP) {
-                    int room = ACAP - n;
-                    int i = beg + lane;
-                    bool ok = false;
-                    Cand c;
-                    if (i < end && lane < room) {
-                        c = s.packed[i];
-                        ok = (c.y0 < gy1) && (c.y1 > gy0) && (c.x0 < tx1) && (c.x1 > tx0);
+            while (off < end && n < ACAP) {
+                const int room = ACAP - n;
+                const int i = off + lane;
+                bool ok = false;
+                Cand c;
+                if (i < end && lane < room) {
+                    if (scan_all) {
+                        const int4 w = s.win[i];
+                        ok = (w.x < gy1) && (w.y > gy0) && (w.z < tx1) && (w.w > tx0);
+                        if (ok) c = make_cand(i, s.cy[i], s.cx[i], s.c0[i], s.c1[i], s.c2[i], w);
+                    } else {
+                        c = s.tile_cand[(size_t)tile * s.tcap + i];
+                        ok = true;
                     }
-                    unsigned m = __ballot_sync(0xffffffffu, ok);
-                    if (ok) {
-                        int pos = n + __popc(m & ((1u << lane) - 1u));
-                        cand[pos] = c;
-                        if (SLICO) s_maxdc[pos] = s.packed_maxdc[i];
-                        const float fy = (float)c.cy - tcy, fx = (float)c.cx - tcx;
-                        s_key[pos] = fy * fy + fx * fx;
-                        s_cf[pos] = make_float2((float)c.cy, (float)c.cx);
-                    }
-                    n += __popc(m);
-                    int adv = min(min(32, room), end - beg);
-                    beg += adv; off += adv;
                 }
-                if (beg >= end) { ++row; off = 0; }
+                const unsigned m = __ballot_sync(0xffffffffu, ok);
+                if (ok) cand[n + __popc(m & ((1u << lane) - 1u))] = c;
+                n += __popc(m);
+                off += min(min(32, room), end - off);
             }
-            if (lane == 0) { s_ncand = n; s_row = row; s_off = off; s_done = row > byl; }
+            if (lane == 0) { s_ncand = n; s_done = off >= end; }
+        }
+        if (!fast) __syncthreads();   // the round is staged
+        const int nc = fast ? total : s_ncand;
+        const int done = fast || s_done;
+        for (int t = threadIdx.x; t < nc; t += ATHREADS) {
+            const Cand& c = cand[t];
+            const float fy = (float)c.cy - tcy, fx = (float)c.cx - tcx;
+            s_key[t] = fy * fy + fx * fx;
+            CandF f;
+            f.cy = (float)c.cy; f.cx = (float)c.cx; f.inv = 1.f; f.pad0 = f.pad1 = f.pad2 = 0.f;
+            f.lo0 = __double2float_rd(c.c0); f.lo1 = __double2float_rd(c.c1); f.lo2 = __double2float_rd(c.c2);
+            f.hi0 = __double2float_ru(c.c0); f.hi1 = __double2float_ru(c.c1); f.hi2 = __double2float_ru(c.c2);
+            if (SLICO) {
+                // the maximum as it is now: k_slico_max raised it after the record was written
+                const double m = __longlong_as_double((long long)s.maxdc[c.k]);
+                s_maxdc[t] = m;
+                f.inv = __frcp_rd(__double2float_ru(m));
+            }
+            s_cf[t] = f;
         }
         __syncthreads();
-        const int nc = s_ncand;
-        const int done = s_done;
         // nearest-first evaluation order (rank sort by distance of the centroid to the tile centre).  Any order gives the
         // same result -- the minimum over (distance, index) is order independent.
         for (int t = threadIdx.x; t < nc; t += ATHREADS) {
@@ -299,7 +263,19 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
             s_lb[rank] = r > 0.f ? (double)(r * r * 0.999f) * s.sw * 0.999 : 0.0;
         }
         __syncthreads();
-        if (use_tma) wgmma::mbar_wait(wgmma::smem_u32(&s_bar), 0);   // phase 0 completes once; later rounds pass immediately
+        if (use_tma) wgmma::mbar_wait(bar, 0);   // phase 0 completes once; later rounds pass immediately
+        // the colour box of this thread's pixels (the rows inside the image), every bound rounded outwards
+        float plo0 = INFINITY, plo1 = INFINITY, plo2 = INFINITY, phi0 = -INFINITY, phi1 = -INFINITY, phi2 = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < AROWS; ++j) {
+            if (yb + j < s.H) {
+                const int ry = warp * AROWS + j;
+                const double v0 = s_px[0][ry][lane], v1 = s_px[1][ry][lane], v2 = s_px[2][ry][lane];
+                plo0 = fminf(plo0, __double2float_rd(v0)); phi0 = fmaxf(phi0, __double2float_ru(v0));
+                plo1 = fminf(plo1, __double2float_rd(v1)); phi1 = fmaxf(phi1, __double2float_ru(v1));
+                plo2 = fminf(plo2, __double2float_rd(v2)); phi2 = fmaxf(phi2, __double2float_ru(v2));
+            }
+        }
         if (xin) {
             const double xd = (double)x;
             // this thread's pixels: column x, AROWS consecutive rows: the float form of the column and the centre of the run
@@ -312,13 +288,24 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
                 if (dbits(s_lb[ci]) > worst) break; // sorted by key: nobody further down the list can win either
                 const int c = s_order[ci];
                 {
-                    // spatial lower bound of this candidate for ALL of the thread's pixels, in float: the centre is at least
-                    // |cx - x| away in x and |cy - ymid| - (AROWS-1)/2 in y.  2e-3 px absorbs the float conversion of coordinates
-                    // up to 16k, the factor 0.998 the rounding of the few float operations: the bound can only come out smaller
-                    // than the exact double distance term, so it never rejects a candidate that could win or tie
-                    const float2 cf = s_cf[c];
-                    const float ax = fmaxf(fabsf(cf.y - xf) - 2e-3f, 0.f), ay = fmaxf(fabsf(cf.x - ymid) - (0.5f * (AROWS - 1) + 2e-3f), 0.f);
-                    if ((ax * ax + ay * ay) * swf > worstf) continue;
+                    // lower bound of this candidate's distance for ALL of the thread's pixels, in float.  Spatial term: the centre is
+                    // at least |cx - x| away in x and |cy - ymid| - (AROWS-1)/2 in y; 2e-3 px absorbs the float conversion of
+                    // coordinates up to 16k, the factor 0.998 the rounding of the few float operations.  Colour term: each channel
+                    // is at least the gap between the pixels' box and the centre; the box, the centre and every operation round
+                    // towards a smaller result, so the term is at most the exact sum of squares, and the factor 0.998 leaves room
+                    // for the rounding of the double chain (the double distance is at least the exact one times 1 - 2^-50).
+                    // Both terms can only come out smaller than the exact double distance, and fl(a + b) >= a for b >= 0, so a
+                    // candidate whose bound exceeds every row's minimum cannot win or tie any row
+                    const CandF f = s_cf[c];
+                    const float ax = fmaxf(fabsf(f.cx - xf) - 2e-3f, 0.f), ay = fmaxf(fabsf(f.cy - ymid) - (0.5f * (AROWS - 1) + 2e-3f), 0.f);
+                    const float lbs = (ax * ax + ay * ay) * swf;
+                    if (lbs > worstf) continue;
+                    const float g0 = fmaxf(fmaxf(__fsub_rd(plo0, f.hi0), __fsub_rd(f.lo0, phi0)), 0.f);
+                    const float g1 = fmaxf(fmaxf(__fsub_rd(plo1, f.hi1), __fsub_rd(f.lo1, phi1)), 0.f);
+                    const float g2 = fmaxf(fmaxf(__fsub_rd(plo2, f.hi2), __fsub_rd(f.lo2, phi2)), 0.f);
+                    float lbc = __fadd_rd(__fadd_rd(__fmul_rd(g0, g0), __fmul_rd(g1, g1)), __fmul_rd(g2, g2));
+                    if (SLICO) lbc = __fmul_rd(lbc, f.inv);
+                    if (__fmaf_rd(lbc, 0.998f, lbs) > worstf) continue;
                 }
                 const int cx0 = cand[c].x0, cx1 = cand[c].x1;
                 if (x < cx0 || x >= cx1) continue;
@@ -447,6 +434,7 @@ __global__ void __launch_bounds__(UTHREADS, UBLOCKS) k_update(KmState s, const d
     __shared__ double s_acc[3];
     __shared__ int4 s_box;
     __shared__ int s_skip;
+    __shared__ Cand s_rec;             // the new record of the cluster
     const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
     const int k = s.n - 1 - blockIdx.x;   // last cluster first (see above)
     if (threadIdx.x == 0) {
@@ -454,7 +442,8 @@ __global__ void __launch_bounds__(UTHREADS, UBLOCKS) k_update(KmState s, const d
         const int4 o = s.obb[k];
         int skip = 0;
         if (BAND) {
-            const bool alive = s.bin_of[k] >= 0;
+            const int4 w = s.win[k];
+            const bool alive = w.y > w.x;   // an alive cluster's window holds its centre row; a dead one's is empty
             const int cr = alive ? (int)s.cy[k] : 0;   // row of the centre the assignment used
             if (o.y >= o.x && (!alive || o.x + s.y_off < cr - s.halo || o.y + s.y_off > cr + s.halo))
                 atomicAdd((unsigned long long*)&xchg[6 * (size_t)s.n], 1ull);
@@ -564,39 +553,42 @@ __global__ void __launch_bounds__(UTHREADS, UBLOCKS) k_update(KmState s, const d
         if (lane < 3) s_acc[lane] = acc;
     }
     __syncthreads();
-    if (threadIdx.x != 0) return;
-    long long cnt = 0, sy = 0, sx = 0;
+    if (wl != 0) return;
+    if (lane == 0) {
+        long long cnt = 0, sy = 0, sx = 0;
 #pragma unroll
-    for (int w = 0; w < UGATHER; ++w) { cnt += s_int[w][0]; sy += s_int[w][1]; sx += s_int[w][2]; }
-    // centroid = sums / count with IEEE divisions (the original divides every feature by the element count), new window,
-    // bin of the new centre; a cluster without pixels is dead for good
-    const double a0 = s_acc[0], a1 = s_acc[1], a2 = s_acc[2];
-    if (BAND) {
-        long long* r = xchg + 6 * (size_t)k;
-        if (cnt > 0) {
-            const double dn = (double)cnt;
-            r[0] = __double_as_longlong(__ddiv_rn((double)sy, dn)); r[1] = __double_as_longlong(__ddiv_rn((double)sx, dn));
-            r[2] = __double_as_longlong(__ddiv_rn(a0, dn)); r[3] = __double_as_longlong(__ddiv_rn(a1, dn));
-            r[4] = __double_as_longlong(__ddiv_rn(a2, dn));
-            r[5] = 1;
-        } else r[5] = 2;
-        return;
+        for (int w = 0; w < UGATHER; ++w) { cnt += s_int[w][0]; sy += s_int[w][1]; sx += s_int[w][2]; }
+        // centroid = sums / count with IEEE divisions (the original divides every feature by the element count), new window;
+        // a cluster without pixels is dead for good
+        const double a0 = s_acc[0], a1 = s_acc[1], a2 = s_acc[2];
+        if (BAND) {
+            long long* r = xchg + 6 * (size_t)k;
+            if (cnt > 0) {
+                const double dn = (double)cnt;
+                r[0] = __double_as_longlong(__ddiv_rn((double)sy, dn)); r[1] = __double_as_longlong(__ddiv_rn((double)sx, dn));
+                r[2] = __double_as_longlong(__ddiv_rn(a0, dn)); r[3] = __double_as_longlong(__ddiv_rn(a1, dn));
+                r[4] = __double_as_longlong(__ddiv_rn(a2, dn));
+                r[5] = 1;
+            } else r[5] = 2;
+        } else {
+            int4 w = make_int4(0, 0, 0, 0);
+            if (cnt > 0) {
+                const double dn = (double)cnt;
+                const double cy = __ddiv_rn((double)sy, dn), cx = __ddiv_rn((double)sx, dn);
+                const double c0 = __ddiv_rn(a0, dn), c1 = __ddiv_rn(a1, dn), c2 = __ddiv_rn(a2, dn);
+                s.cy[k] = cy; s.cx[k] = cx; s.c0[k] = c0; s.c1[k] = c1; s.c2[k] = c2;
+                w = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
+                s_rec = make_cand(k, cy, cx, c0, c1, c2, w);
+            } else s_rec.y0 = s_rec.y1 = 0;   // dead: an empty window, no tile
+            s.win[k] = w;
+            s.obb[k] = make_int4(INT_MAX, -1, INT_MAX, -1);
+        }
     }
-    int4 w = make_int4(0, 0, 0, 0);
-    int bin = -1;
-    if (cnt > 0) {
-        const double dn = (double)cnt;
-        const double cy = __ddiv_rn((double)sy, dn), cx = __ddiv_rn((double)sx, dn);
-        s.cy[k] = cy; s.cx[k] = cx;
-        s.c0[k] = __ddiv_rn(a0, dn); s.c1[k] = __ddiv_rn(a1, dn); s.c2[k] = __ddiv_rn(a2, dn);
-        w = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
-        const int by = min(max((int)cy / s.B, 0), s.nby - 1), bx = min(max((int)cx / s.B, 0), s.nbx - 1);
-        bin = by * s.nbx + bx;
-        atomicAdd(&s.bin_fill[bin], 1);
-    }
-    s.win[k] = w;
-    s.bin_of[k] = bin;
-    s.obb[k] = make_int4(INT_MAX, -1, INT_MAX, -1);
+    if (BAND) return;   // band mode: k_import appends the merged centres
+    // the next k_assign's candidate lists: the new record goes to every tile its window meets (up to 5 x 5 tiles at step 29),
+    // one tile per lane of the first warp
+    __syncwarp();
+    append_tiles(s, s_rec, lane, 32);
 }
 
 // band mode: take the merged exchange records (see k_update<true>) into the replicated cluster state
@@ -610,15 +602,13 @@ __global__ void k_import(KmState s, const long long* __restrict__ xchg)
         const double cy = __longlong_as_double(r[0]), cx = __longlong_as_double(r[1]);
         s.cy[k] = cy; s.cx[k] = cx;
         s.c0[k] = __longlong_as_double(r[2]); s.c1[k] = __longlong_as_double(r[3]); s.c2[k] = __longlong_as_double(r[4]);
-        s.win[k] = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
-        const int by = min(max((int)cy / s.B, 0), s.nby - 1), bx = min(max((int)cx / s.B, 0), s.nbx - 1);
-        s.bin_of[k] = by * s.nbx + bx;
-        atomicAdd(&s.bin_fill[by * s.nbx + bx], 1);
+        const int4 w = make_window(cy, cx, s.step_y, s.step_x, s.Hg, s.W);
+        s.win[k] = w;
+        append_tiles(s, make_cand(k, cy, cx, __longlong_as_double(r[2]), __longlong_as_double(r[3]), __longlong_as_double(r[4]), w), 0, 1);
     } else {
         // 2: the owner found no member, the cluster is dead for good; 0: it was dead already.  (An alive cluster always has
         // exactly one owner, so 0 cannot occur for it.)
         s.win[k] = make_int4(0, 0, 0, 0);
-        s.bin_of[k] = -1;
     }
 }
 
@@ -647,39 +637,36 @@ __global__ void k_export_centroids(KmState s, double* out)
     out[5 * k + 2] = s.c0[k]; out[5 * k + 3] = s.c1[k]; out[5 * k + 4] = s.c2[k];
 }
 
+// > 0: cap on the tile lists below the sizing of carve (isb_slic_set_tile_cap), so that tests can force the full-scan path
+static int g_tile_cap = 0;
+
 static size_t carve(KmState& s, void* ws, size_t bytes, int H, int W, int n, int step_y, int step_x)
 {
     WsCarver c(ws, bytes);
     // H here is the height the cluster geometry lives in (the whole image); band callers overwrite the slab fields afterwards
     s.n = n; s.H = H; s.W = W; s.step_y = step_y; s.step_x = step_x;
     s.Hg = H; s.y_off = 0; s.own_lo = 0; s.own_hi = H; s.halo = 0; s.pstride = (size_t)H * W;
-    s.B = 2 * (step_y > step_x ? step_y : step_x); // bin edge: coarse enough that the per-sweep scan over the bins is short
-    if (s.B < 16) s.B = 16;
-    s.nby = (H + s.B - 1) / s.B; s.nbx = (W + s.B - 1) / s.B;
     s.cy = c.take<double>(n); s.cx = c.take<double>(n);
     s.c0 = c.take<double>(n); s.c1 = c.take<double>(n); s.c2 = c.take<double>(n);
     s.win = c.take<int4>(n); s.obb = c.take<int4>(n);
-    s.bin_start = c.take<int>((size_t)s.nby * s.nbx + 1);
-    s.bin_fill = c.take<int>((size_t)s.nby * s.nbx);
-    s.bin_of = c.take<int>(n);
-    s.pack_done = c.take<int>(1);
-    s.packed = c.take<Cand>(n);
     s.maxdc = c.take<unsigned long long>(n);
-    s.packed_maxdc = c.take<double>(n);
+    // a window is 4 step + 1 wide, so about (TILE + 4 step + 2) / step + 1 centres of the seed grid per axis have a window that
+    // meets a tile; one more per axis is the margin for clusters that drift together.  More than that is still exact (k_assign
+    // then scans every cluster for the tile), only slower.
+    s.ntx = (W + TILE - 1) / TILE;
+    s.tcap = ((TILE + 4 * step_y + 2) / step_y + 2) * ((TILE + 4 * step_x + 2) / step_x + 2);
+    if (g_tile_cap > 0 && g_tile_cap < s.tcap) s.tcap = g_tile_cap;
+    const size_t tiles = (size_t)((H + TILE - 1) / TILE) * s.ntx;   // a band's slab has at most as many tile rows as the image
+    s.tile_cnt = c.take<int>(tiles);
+    s.tile_cand = c.take<Cand>(tiles * s.tcap);
     return isb_align(c.off);
 }
 
-// seeds != nullptr: first binning (centres from the seed grid); else re-binning after k_update / k_import
-static int rebin(KmState& s, const double* seeds_yx, cudaStream_t st)
+// first sweep: centres from the seed grid, and their records in empty tile lists
+static int seed(KmState& s, const double* seeds_yx, cudaStream_t st)
 {
-    if (seeds_yx) {
-        ISB_CUDA_CHECK(cudaMemsetAsync(s.bin_fill, 0, sizeof(int) * (size_t)s.nby * s.nbx, st));
-        k_seed<<<(s.n + 255) / 256, 256, 0, st>>>(s, seeds_yx);
-        ISB_LAUNCH_CHECK();
-    }
-    k_scan_bins<<<1, 1024, 0, st>>>(s);
-    ISB_LAUNCH_CHECK();
-    k_pack<<<(s.n + 255) / 256, 256, 0, st>>>(s);
+    ISB_CUDA_CHECK(cudaMemsetAsync(s.tile_cnt, 0, sizeof(int) * (size_t)((s.Hg + TILE - 1) / TILE) * s.ntx, st));
+    k_seed<<<(s.n + 255) / 256, 256, 0, st>>>(s, seeds_yx);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }
@@ -726,7 +713,7 @@ extern "C" int isb_slic_kmeans(const double* lab_planar, int H, int W, const dou
     s.slico = slic_zero ? 1 : 0;
     cudaStream_t st = (cudaStream_t)stream;
     ISB_CUDA_CHECK(cudaMemsetAsync(labels, 0, sizeof(int32_t) * (size_t)H * W, st));
-    if (int rc = rebin(s, seeds_yx, st)) return rc;
+    if (int rc = seed(s, seeds_yx, st)) return rc;
     CUtensorMap lab_map;
     memset(&lab_map, 0, sizeof(lab_map));
     const int use_tma = make_lab_map(lab_map, lab_planar, H, W, s.pstride) ? 1 : 0;
@@ -743,7 +730,6 @@ extern "C" int isb_slic_kmeans(const double* lab_planar, int H, int W, const dou
             k_slico_max<<<(unsigned)((npx + 255) / 256), 256, 0, st>>>(s, lab_planar, labels);
             ISB_LAUNCH_CHECK();
         }
-        { ProfScope p(ISB_PROF_FINALIZE, st); if (int rc = rebin(s, nullptr, st)) return rc; }
     }
     if (centroids) {
         k_export_centroids<<<(n_seeds + 255) / 256, 256, 0, st>>>(s, centroids);
@@ -787,7 +773,7 @@ extern "C" int isb_slic_band_begin(const isb_slic_band_t* b, isb_stream_t stream
     if (int rc = band_state(b, s)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     ISB_CUDA_CHECK(cudaMemsetAsync(b->labels_slab, 0, sizeof(int32_t) * (size_t)b->slab_rows * b->width, st));
-    return rebin(s, b->seeds_yx, st);
+    return seed(s, b->seeds_yx, st);
 }
 
 extern "C" int isb_slic_band_assign(const isb_slic_band_t* b, isb_stream_t stream)
@@ -843,6 +829,20 @@ extern "C" int isb_slic_band_finalize(const isb_slic_band_t* b, const uint64_t* 
         ISB_REQUIRE(maxdc_xchg, "null pointer");
         ISB_CUDA_CHECK(cudaMemcpyAsync(s.maxdc, maxdc_xchg, sizeof(uint64_t) * (size_t)s.n, cudaMemcpyDeviceToDevice, st));
     }
-    ProfScope p(ISB_PROF_FINALIZE, st);
-    return rebin(s, nullptr, st);
+    return ISB_OK;
+}
+
+extern "C" int isb_slic_set_tile_cap(int cap)
+{
+    ISB_REQUIRE(cap >= 0, "bad tile cap");
+    const int prev = g_tile_cap;
+    g_tile_cap = cap;
+    return prev;
+}
+
+extern "C" long long isb_slic_full_scan_tiles(void)
+{
+    unsigned long long v = 0;
+    ISB_CUDA_CHECK(cudaMemcpyFromSymbol(&v, d_full_scans, sizeof(v)));
+    return (long long)v;
 }
