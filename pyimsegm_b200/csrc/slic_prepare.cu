@@ -11,7 +11,7 @@
 
 namespace {
 
-struct GaussW { double w[9]; int r; };
+struct GaussW { double w[9]; };
 
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
@@ -89,8 +89,10 @@ __device__ __forceinline__ void rgb2lab_px(double r, double g, double b, double&
     B = dmul(200.0, dsub(f[1], f[2]));
 }
 
+// scipy.ndimage 'reflect' for any i, including images smaller than the radius that reflect more than once
 __device__ __forceinline__ int reflect_idx(int i, int n)
 {
+    if ((unsigned)i < (unsigned)n) return i;
     if (n == 1) return 0;
     int p = 2 * n;
     i %= p;
@@ -137,77 +139,140 @@ __global__ void k_minmax_decode(const unsigned long long* mm, double* out)
     out[1] = f64_unordered(mm[1]);
 }
 
-constexpr int TY = 16, TX = 32;
+// k_blur_lab: one CTA = TX output columns x SH output rows, walked down in chunks of K rows.
+//   stage 1  load + rescale + depth axis of the K new input rows into a ring of 2R+K haloed rows (the first chunk fills all 2R+K)
+//   stage 2  rows axis: one thread per (channel, haloed column) reads its 2R+K ring samples once into registers, writes K outputs
+//   stage 3  cols axis + rgb2lab + ratio for the K x TX output pixels
+// Rescale and depth work per output pixel is (SH+2R)(TX+2R)/(SH TX) (1.19x at R=4), the rows axis (TX+2R)/TX (1.06x at R=4).
+// The radius is a template parameter so every tap loop unrolls and the weights are read from parameter space.
+constexpr int TX = 128, SH = 64, KR = 8, NT = 256;
 
-// one CTA = TY x TX output pixels; smem: input tile with halo r (after rescale + depth pass), then row-blurred strip
-__global__ void __launch_bounds__(256) k_blur_lab(const void* img, int dtype, int H, int W, int C, const double* minmax,
-                                                  int rescale, GaussW gw, double ratio, double* out)
+template <int R>
+struct BlurShape {
+    static constexpr int IW = TX + 2 * R;   // haloed tile width
+    static constexpr int RING = 2 * R + KR; // input rows held at once
+    static constexpr size_t smem = sizeof(double) * 3 * ((size_t)RING * IW + (size_t)KR * IW) + sizeof(int) * IW;
+};
+
+template <int R>
+__global__ void __launch_bounds__(NT, 2) k_blur_lab(const void* __restrict__ img, int dtype, int H, int W, int C,
+                                                    const double* __restrict__ minmax, int rescale, GaussW gw, double ratio,
+                                                    double* __restrict__ out)
 {
+    using S = BlurShape<R>;
+    constexpr int IW = S::IW, RING = S::RING;
     extern __shared__ double smem[];
-    const int r = gw.r;
-    const int IW = TX + 2 * r, IH = TY + 2 * r;
-    double* s_in = smem;               // [3][IH][IW]
-    double* s_v = smem + 3 * IH * IW;  // [3][TY][IW]
-    const int x0 = blockIdx.x * TX, y0 = blockIdx.y * TY;
+    double* s_in = smem;                     // [3][RING][IW]
+    double* s_v = smem + 3 * RING * IW;      // [3][KR][IW]
+    int* s_gx = (int*)(s_v + 3 * KR * IW);   // [IW] reflected source column of each haloed column
+    const int x0 = blockIdx.x * TX, y0 = blockIdx.y * SH;
+    const int y_end = min(y0 + SH, H);
     const double mn = minmax[0], mx = minmax[1];
     const bool do_rescale = rescale && (mn != 0.0 || mx != 1.0);
     const double span = dsub(mx, mn);
-
-    for (int i = threadIdx.x; i < IH * IW; i += blockDim.x) {
-        int iy = i / IW, ix = i - iy * IW;
-        int gy = reflect_idx(y0 + iy - r, H), gx = reflect_idx(x0 + ix - r, W);
-        size_t base = ((size_t)gy * W + gx) * C;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            double v = load_as_f64(img, dtype, base + (C == 3 ? c : 0));
-            if (do_rescale) v = ddiv(dsub(v, mn), span);
-            if (r > 0) {
-                // depth axis of skimage's [1,H,W,3] array: all taps reflect onto the same sample
-                double t = dmul(v, gw.w[0]);
-                for (int j = r; j >= 1; --j) t = dadd(t, dmul(dadd(v, v), gw.w[j]));
-                v = t;
-            }
-            s_in[(c * IH + iy) * IW + ix] = v;
-        }
-    }
-    __syncthreads();
-    // rows axis (vertical), for every column of the haloed tile
-    for (int i = threadIdx.x; i < 3 * TY * IW; i += blockDim.x) {
-        int c = i / (TY * IW), rem = i - c * TY * IW;
-        int ty = rem / IW, ix = rem - ty * IW;
-        const double* col = s_in + (c * IH + ty + r) * IW + ix;
-        double t;
-        if (r > 0) {
-            t = dmul(col[0], gw.w[0]);
-            for (int j = r; j >= 1; --j) t = dadd(t, dmul(dadd(col[-j * IW], col[j * IW]), gw.w[j]));
-        } else t = col[0];
-        s_v[(c * TY + ty) * IW + ix] = t;
-    }
-    __syncthreads();
-    // cols axis (horizontal) + rgb2lab + scale
     const size_t HW = (size_t)H * W;
-    for (int i = threadIdx.x; i < TY * TX; i += blockDim.x) {
-        int ty = i / TX, tx = i - ty * TX;
-        int gy = y0 + ty, gx = x0 + tx;
-        if (gy >= H || gx >= W) continue;
-        double v[3];
+
+    for (int ix = threadIdx.x; ix < IW; ix += NT) s_gx[ix] = reflect_idx(x0 + ix - R, W);
+    __syncthreads();
+
+    // rescale, then the depth axis of skimage's [1,H,W,3] array: all its taps reflect onto the same sample
+    auto prep = [&](double v) {
+        if (do_rescale) v = ddiv(dsub(v, mn), span);
+        if (R > 0) {
+            double t = dmul(v, gw.w[0]);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const double* row = s_v + (c * TY + ty) * IW + tx + r;
-            double t;
-            if (r > 0) {
-                t = dmul(row[0], gw.w[0]);
-                for (int j = r; j >= 1; --j) t = dadd(t, dmul(dadd(row[-j], row[j]), gw.w[j]));
-            } else t = row[0];
-            v[c] = t;
+            for (int j = R; j >= 1; --j) t = dadd(t, dmul(dadd(v, v), gw.w[j]));
+            v = t;
         }
-        double L, A, B;
-        rgb2lab_px(v[0], v[1], v[2], L, A, B);
-        size_t p = (size_t)gy * W + gx;
-        out[p] = dmul(L, ratio);
-        out[HW + p] = dmul(A, ratio);
-        out[2 * HW + p] = dmul(B, ratio);
+        return v;
+    };
+
+    int slot0 = 0; // ring slot of the chunk's first input row
+    for (int cy = y0; cy < y_end; cy += KR) {
+        // stage 1: input rows [lo, lo + nrow) relative to y0 - R
+        const int first = cy == y0;
+        const int lo = first ? 0 : cy - y0 + 2 * R, nrow = first ? RING : KR;
+        for (int i = threadIdx.x; i < nrow * IW; i += NT) {
+            const int row = i / IW, ix = i - row * IW;
+            const int ir = lo + row;
+            const int gy = reflect_idx(y0 - R + ir, H);
+            const size_t base = ((size_t)gy * W + s_gx[ix]) * C;
+            double* dst = s_in + (ir % RING) * IW + ix;
+            if (C == 3) {
+#pragma unroll
+                for (int c = 0; c < 3; ++c) dst[c * RING * IW] = prep(load_as_f64(img, dtype, base + c));
+            } else {
+                const double v = prep(load_as_f64(img, dtype, base));
+#pragma unroll
+                for (int c = 0; c < 3; ++c) dst[c * RING * IW] = v;
+            }
+        }
+        __syncthreads();
+        // stage 2: rows axis
+        for (int i = threadIdx.x; i < 3 * IW; i += NT) {
+            const int c = i / IW, ix = i - c * IW;
+            const double* col = s_in + c * RING * IW + ix;
+            double w[RING];
+#pragma unroll
+            for (int k = 0; k < RING; ++k) {
+                int s = slot0 + k;
+                if (s >= RING) s -= RING;
+                w[k] = col[s * IW];
+            }
+            double* dst = s_v + c * KR * IW + ix;
+#pragma unroll
+            for (int k = 0; k < KR; ++k) {
+                double t = w[k + R];
+                if (R > 0) {
+                    t = dmul(w[k + R], gw.w[0]);
+#pragma unroll
+                    for (int j = R; j >= 1; --j) t = dadd(t, dmul(dadd(w[k + R - j], w[k + R + j]), gw.w[j]));
+                }
+                dst[k * IW] = t;
+            }
+        }
+        __syncthreads();
+        // stage 3: cols axis + rgb2lab + scale
+        for (int i = threadIdx.x; i < KR * TX; i += NT) {
+            const int ty = i / TX, tx = i - ty * TX;
+            const int gy = cy + ty, gx = x0 + tx;
+            if (gy >= y_end || gx >= W) continue;
+            double v[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const double* row = s_v + (c * KR + ty) * IW + tx + R;
+                double t = row[0];
+                if (R > 0) {
+                    t = dmul(row[0], gw.w[0]);
+#pragma unroll
+                    for (int j = R; j >= 1; --j) t = dadd(t, dmul(dadd(row[-j], row[j]), gw.w[j]));
+                }
+                v[c] = t;
+            }
+            double L, A, B;
+            rgb2lab_px(v[0], v[1], v[2], L, A, B);
+            const size_t p = (size_t)gy * W + gx;
+            out[p] = dmul(L, ratio);
+            out[HW + p] = dmul(A, ratio);
+            out[2 * HW + p] = dmul(B, ratio);
+        }
+        // the next stage 1 overwrites only ring rows this chunk's stage 2 has finished with (a barrier ago), and the next
+        // stage 2 writes s_v only after the barrier that follows the next stage 1
+        slot0 += KR;
+        if (slot0 >= RING) slot0 -= RING;
     }
+}
+
+template <int R>
+static int blur_lab_launch(const void* img, int dtype, int H, int W, int C, const double* minmax, int rescale, const GaussW& gw,
+                           double ratio, double* out, cudaStream_t st)
+{
+    const size_t smem = BlurShape<R>::smem;
+    if (smem > 48 * 1024) ISB_CUDA_CHECK(cudaFuncSetAttribute(k_blur_lab<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid((W + TX - 1) / TX, (H + SH - 1) / SH);
+    k_blur_lab<R><<<grid, NT, smem, st>>>(img, dtype, H, W, C, minmax, rescale, gw, ratio, out);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
 }
 
 static int minmax_launch(const void* img, int dtype, size_t n, double* minmax_out, cudaStream_t st)
@@ -248,13 +313,16 @@ extern "C" int isb_slic_prepare(const void* img, int dtype, int H, int W, int C,
     if (rescale != 2)
         if (int rc = minmax_launch(img, dtype, (size_t)H * W * C, minmax_out, st)) return rc;
     GaussW gw;
-    gw.r = radius;
     for (int i = 0; i < 9; ++i) gw.w[i] = (i <= radius && w_half) ? w_half[i] : 0.0;
-    dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY);
-    size_t smem = sizeof(double) * 3 * ((size_t)(TY + 2 * radius) * (TX + 2 * radius) + (size_t)TY * (TX + 2 * radius));
-    if (smem > 48 * 1024)
-        ISB_CUDA_CHECK(cudaFuncSetAttribute(k_blur_lab, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_blur_lab<<<grid, 256, smem, st>>>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
+    switch (radius) {
+        case 0: return blur_lab_launch<0>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        case 1: return blur_lab_launch<1>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        case 2: return blur_lab_launch<2>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        case 3: return blur_lab_launch<3>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        case 4: return blur_lab_launch<4>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        case 5: return blur_lab_launch<5>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        case 6: return blur_lab_launch<6>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        case 7: return blur_lab_launch<7>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+        default: return blur_lab_launch<8>(img, dtype, H, W, C, minmax_out, rescale, gw, ratio, lab_planar, st);
+    }
 }
