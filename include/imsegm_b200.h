@@ -181,7 +181,8 @@ int isb_label_hist_2d(const int16_t* segm_select, const int16_t* struc_elem, int
                       isb_stream_t stream);
 
 /* histogram_regions_labels_counts (imsegm/labeling.py:208-240, a per-pixel Python loop in the reference): joint histogram
- * hist[a][b] = #{p : slic[p] == a and annot[p] == b}, hist is [nb_slic, nb_annot] u32; labels must be in range */
+ * hist[a][b] = #{p : slic[p] == a and annot[p] == b}, hist is [nb_slic, nb_annot] u32; labels must be below nb_slic / nb_annot.
+ * A pixel with a negative label in either map is skipped, as compute_labels_overlap_matrix (labeling.py:490-523) does. */
 int isb_region_label_hist(const int32_t* slic, const int32_t* annot, int H, int W, int nb_slic, int nb_annot, uint32_t* hist,
                           isb_stream_t stream);
 
@@ -433,6 +434,37 @@ int isb_ellipse_overlap(const int32_t* segm, int H, int W, int n_labels, const i
  * borders as scipy.ndimage's 'reflect'.  The footprints of skimage.morphology.disk(r) for a non-integer r. */
 int isb_binary_morph_footprint(const uint8_t* in, int H, int W, const int32_t* offsets, int n_offsets, int op, uint8_t* out,
                                isb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * (xi) labeling -- imsegm/labeling.py: boundary and contour maps, the exact Euclidean distance transform, the (row, col)
+ *      lists of contour_coords / compute_boundary_distances, and the final relabel gather.  Label maps are [H, W] i32.
+ * ------------------------------------------------------------------------------------------------------------------ */
+
+/* skimage.segmentation.find_boundaries(seg, mode='thick', connectivity=1) of compute_boundary_distances (labeling.py:708,710):
+ * out [H, W] u8 is 1 where one of the pixel's in-image 4-neighbours has another label (pixels outside the image never count,
+ * negative labels are ordinary values). */
+int isb_label_boundary_map(const int32_t* seg, int H, int W, uint8_t* out, isb_stream_t stream);
+/* contour_binary_map (labeling.py:34-79) as 0 / 1 u8: rows 1..H-2 and columns 1..W-2 are 1 where seg == label and a 4-neighbour
+ * differs from label; include_boundary != 0 also sets every frame pixel with seg == label. */
+int isb_label_contour_map(const int32_t* seg, int H, int W, int32_t label, int include_boundary, uint8_t* out, isb_stream_t stream);
+/* scipy.ndimage.distance_transform_edt of an input whose zeros are the nonzero pixels of sites [H, W] u8 (compute_distance_map
+ * labeling.py:167, compute_boundary_distances :711): dist [H, W] f64 = sqrt((double)d2), d2 the integer squared distance to the
+ * nearest site -- bit-identical to scipy.  Without any site every pixel is measured from (-1, 0), as scipy's feature transform
+ * does: dist = sqrt((y + 1)^2 + x^2).  H, W <= 32768 (d2 fits int32), else ISB_ERR_ARG.  ws: isb_edt_workspace_bytes(H, W). */
+size_t isb_edt_workspace_bytes(int H, int W);
+int isb_edt_2d(const uint8_t* sites, int H, int W, double* dist, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* order-preserving compaction of a mask [H, W] u8 (contour_coords labeling.py:101-105, the point list of
+ * compute_boundary_distances :707-712): isb_mask_compact_count scans the per-tile counts into ws and writes the number P of set
+ * pixels to the DEVICE int64 total; isb_mask_compact_write (same ws, after the count) writes points [P, 2] i64 (row, col) in raster
+ * order and, when values [H, W] f64 is given, values_out [P] = values at those pixels.  ws: isb_mask_compact_workspace_bytes. */
+size_t isb_mask_compact_workspace_bytes(int H, int W);
+int isb_mask_compact_count(const uint8_t* mask, int H, int W, void* ws, size_t ws_bytes, long long* total, isb_stream_t stream);
+int isb_mask_compact_write(const uint8_t* mask, int H, int W, const double* values, const void* ws, size_t ws_bytes, int64_t* points,
+                           double* values_out, isb_stream_t stream);
+/* the final step of relabel_max_overlap_unique (labeling.py:611-613), relabel_max_overlap_merge (:678-680) and
+ * assume_bg_on_boundary (:753): out = lut[seg] where 0 <= seg < n_lut, out = seg elsewhere (negative labels pass through).
+ * isb_gather below indexes its table unguarded. */
+int isb_relabel_gather(const int32_t* seg, long long npx, const int32_t* lut, int n_lut, int32_t* out, isb_stream_t stream);
 
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);

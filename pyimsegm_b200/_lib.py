@@ -116,6 +116,14 @@ SIGNATURES = {
     'isb_ellipse_ransac': (_i, [_i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _d, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'isb_ellipse_overlap': (_i, [_vp, _i, _i, _i, C.POINTER(C.c_int32), C.POINTER(_d), _vp, _vp, _vp]),
     'isb_binary_morph_footprint': (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
+    'isb_label_boundary_map': (_i, [_vp, _i, _i, _vp, _vp]),
+    'isb_label_contour_map': (_i, [_vp, _i, _i, C.c_int32, _i, _vp, _vp]),
+    'isb_edt_workspace_bytes': (_sz, [_i, _i]),
+    'isb_edt_2d': (_i, [_vp, _i, _i, _vp, _vp, _sz, _vp]),
+    'isb_mask_compact_workspace_bytes': (_sz, [_i, _i]),
+    'isb_mask_compact_count': (_i, [_vp, _i, _i, _vp, _sz, _vp, _vp]),
+    'isb_mask_compact_write': (_i, [_vp, _i, _i, _vp, _vp, _sz, _vp, _vp, _vp]),
+    'isb_relabel_gather': (_i, [_vp, _ll, _vp, _i, _vp, _vp]),
 }
 
 

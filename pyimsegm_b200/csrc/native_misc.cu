@@ -106,7 +106,8 @@ __global__ void k_ray_features(const signed char* __restrict__ seg, int H, int W
 }
 
 // joint histogram of two label maps: hist[a][b] = #{p : slic[p] == a, annot[p] == b}; a thread walks a short column strip so
-// that runs of equal (a, b) cost one atomic
+// that runs of equal (a, b) cost one atomic.  A pixel with a negative label in either map is not counted
+// (compute_labels_overlap_matrix, imsegm/labeling.py:519-521).
 __global__ void __launch_bounds__(256) k_region_label_hist(const int* __restrict__ slic, const int* __restrict__ annot, int H, int W, int nb_annot,
                                                            unsigned* hist)
 {
@@ -119,7 +120,7 @@ __global__ void __launch_bounds__(256) k_region_label_hist(const int* __restrict
         int a = -1, b = -1;
         if (y < y1) { a = slic[(size_t)y * W + x]; b = annot[(size_t)y * W + x]; }
         if (a != ca || b != cb) {
-            if (run) atomicAdd(&hist[(size_t)ca * nb_annot + cb], run);
+            if (run && ca >= 0 && cb >= 0) atomicAdd(&hist[(size_t)ca * nb_annot + cb], run);
             ca = a; cb = b; run = 0;
         }
         if (y < y1) ++run;
