@@ -453,6 +453,12 @@ int isb_label_contour_map(const int32_t* seg, int H, int W, int32_t label, int i
  * does: dist = sqrt((y + 1)^2 + x^2).  H, W <= 32768 (d2 fits int32), else ISB_ERR_ARG.  ws: isb_edt_workspace_bytes(H, W). */
 size_t isb_edt_workspace_bytes(int H, int W);
 int isb_edt_2d(const uint8_t* sites, int H, int W, double* dist, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* the same transform giving, instead of the distance, the flat index (row * W + column) of a nearest site (image_inpaint_pixels,
+ * annotation.py:279-286): index [H, W] i32, -1 everywhere when there is no site.  Of equidistant sites it takes the one of smallest
+ * column, then of smallest row -- the choice of scipy.ndimage.distance_transform_edt(..., return_indices=True).  Same kernels as
+ * isb_edt_2d plus one byte per pixel; ws: isb_edt_index_workspace_bytes(H, W). */
+size_t isb_edt_index_workspace_bytes(int H, int W);
+int isb_edt_2d_indices(const uint8_t* sites, int H, int W, int32_t* index, void* ws, size_t ws_bytes, isb_stream_t stream);
 /* order-preserving compaction of a mask [H, W] u8 (contour_coords labeling.py:101-105, the point list of
  * compute_boundary_distances :707-712): isb_mask_compact_count scans the per-tile counts into ws and writes the number P of set
  * pixels to the DEVICE int64 total; isb_mask_compact_write (same ws, after the count) writes points [P, 2] i64 (row, col) in raster
@@ -465,6 +471,43 @@ int isb_mask_compact_write(const uint8_t* mask, int H, int W, const double* valu
  * assume_bg_on_boundary (:753): out = lut[seg] where 0 <= seg < n_lut, out = seg elsewhere (negative labels pass through).
  * isb_gather below indexes its table unguarded. */
 int isb_relabel_gather(const int32_t* seg, long long npx, const int32_t* lut, int n_lut, int32_t* out, isb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * (xii) annotation -- imsegm/annotation.py: colour histograms, palette lookups and nearest-pixel quantisation.  Pixels are
+ *       interleaved [n_px, channels]; label maps are i64.
+ * ------------------------------------------------------------------------------------------------------------------ */
+
+/* colour histogram of unique_image_colors / image_frequent_colors (annotation.py:46-68, :163-193): hist [2^24] u64 gets +1 at
+ * r << 16 | g << 8 | b for every pixel of img [n_px, channels] u8; channels 3 or 4 (only the first three count), 1 = grey (v, v, v).
+ * accumulate = 0 zeroes hist first, 1 adds to what it holds (several images into one histogram). */
+int isb_color_hist(const uint8_t* img, long long n_px, int channels, int accumulate, unsigned long long* hist, isb_stream_t stream);
+/* the nonzero bins of hist in ascending packed order, as isb_mask_compact_count / _write: the count writes their number P to the
+ * DEVICE int64 total, the write (same ws, after the count) colors [P] i32 (packed RGB) and counts [P] i64.
+ * ws: isb_color_hist_workspace_bytes(). */
+size_t isb_color_hist_workspace_bytes(void);
+int isb_color_hist_compact_count(const unsigned long long* hist, void* ws, size_t ws_bytes, long long* total, isb_stream_t stream);
+int isb_color_hist_compact_write(const unsigned long long* hist, const void* ws, size_t ws_bytes, int32_t* colors, int64_t* counts,
+                                 isb_stream_t stream);
+/* palette index of every pixel of img [n_px, channels] (channels 1 .. 4) against palette [n_colors, channels] of the same dtype
+ * (ISB_U8 or ISB_F64; n_colors <= 1024, else ISB_ERR_UNSUPPORTED):
+ *   mode 0, exact (convert_img_colors_to_labels_reverted :94-125, quantize_image_nearest_pixel :308-316): the LAST entry equal to the
+ *           pixel in every channel, -1 when none; unmatched (optional DEVICE u64) gets the number of -1 pixels, matched (optional
+ *           [n_px] u8) 1 / 0 per pixel;
+ *   mode 1, L1-nearest (image_color_2_labels :245-247, quantize_image_nearest_color :271-273): the FIRST entry of least sum of
+ *           |pixel - entry| over the channels (np.argmin); uint8 sums are exact integers, float64 sums add the channels in order from
+ *           0 as numpy does, and a NaN distance wins at its first occurrence.
+ * labels [n_px] i64 = values[index] when values [n_colors] i64 is given, the index otherwise. */
+int isb_palette_map(const void* img, int dtype, long long n_px, int channels, const void* palette, int n_colors, int mode,
+                    const int64_t* values, int64_t* labels, uint8_t* matched, unsigned long long* unmatched, isb_stream_t stream);
+/* label -> colour gather (convert_img_labels_to_colors :128-160): out [n_px] rows of row_bytes (1 .. 32) bytes = the row of table
+ * [n_colors, row_bytes] for each label -- with keys [n_colors] i64 (ascending, unique) the row whose key equals the label, without
+ * them row = label for 0 <= label < n_colors.  A label without a row writes zeros and is counted in missing (optional DEVICE u64).
+ * n_colors <= 1024, else ISB_ERR_UNSUPPORTED. */
+int isb_palette_gather(const int64_t* labels, long long n_px, const int64_t* keys, int n_colors, const void* table, int row_bytes,
+                       void* out, unsigned long long* missing, isb_stream_t stream);
+/* out[i] = src[index[i]] for n elements of elem_bytes (1, 2, 4 or 8) bytes: the values at the sites of isb_edt_2d_indices
+ * (image_inpaint_pixels :279-286).  Indices are not checked. */
+int isb_gather_at_index(const void* src, int elem_bytes, const int32_t* index, long long n, void* out, isb_stream_t stream);
 
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);

@@ -124,6 +124,15 @@ SIGNATURES = {
     'isb_mask_compact_count': (_i, [_vp, _i, _i, _vp, _sz, _vp, _vp]),
     'isb_mask_compact_write': (_i, [_vp, _i, _i, _vp, _vp, _sz, _vp, _vp, _vp]),
     'isb_relabel_gather': (_i, [_vp, _ll, _vp, _i, _vp, _vp]),
+    'isb_edt_index_workspace_bytes': (_sz, [_i, _i]),
+    'isb_edt_2d_indices': (_i, [_vp, _i, _i, _vp, _vp, _sz, _vp]),
+    'isb_color_hist': (_i, [_vp, _ll, _i, _i, _vp, _vp]),
+    'isb_color_hist_workspace_bytes': (_sz, []),
+    'isb_color_hist_compact_count': (_i, [_vp, _vp, _sz, _vp, _vp]),
+    'isb_color_hist_compact_write': (_i, [_vp, _vp, _sz, _vp, _vp, _vp]),
+    'isb_palette_map': (_i, [_vp, _i, _ll, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    'isb_palette_gather': (_i, [_vp, _ll, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    'isb_gather_at_index': (_i, [_vp, _i, _vp, _ll, _vp, _vp]),
 }
 
 

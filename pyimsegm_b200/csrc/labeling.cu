@@ -1,11 +1,12 @@
 // labeling.cu -- the label-map kernels of the reference's imsegm/labeling.py:
 //   thick boundary map   (skimage find_boundaries(mode='thick') inside compute_boundary_distances :684-716)
 //   interior contour map (contour_binary_map :34-79, contour_coords :82-117)
-//   exact 2-D Euclidean distance transform (scipy.ndimage.distance_transform_edt, compute_distance_map :146-169)
+//   exact 2-D Euclidean distance transform (scipy.ndimage.distance_transform_edt, compute_distance_map :146-169), and the same transform
+//   giving the index of a nearest site (distance_transform_edt(..., return_indices=True); image_inpaint_pixels of annotation.py)
 //   order-preserving mask compaction (the (row, col) lists of contour_coords and compute_boundary_distances)
 //   relabel gather with negative pass-through (relabel_max_overlap_unique :611-613, relabel_max_overlap_merge :678-680)
 // The overlap matrix (compute_labels_overlap_matrix :490-523) is isb_region_label_hist (native_misc.cu).
-#include "common.cuh"
+#include "compact.cuh"
 
 namespace {
 
@@ -90,11 +91,15 @@ __global__ void __launch_bounds__(256) k_edt_links(const unsigned* __restrict__ 
 }
 
 // 1c: gT[x][y] = distance from (y, x) to the nearest site in column x (EDT_NONE for a column without one), transposed through
-// shared memory so that both the reads and the writes are coalesced
+// shared memory so that both the reads and the writes are coalesced.  IDX (the nearest-site variant) also writes upT[x][y] = 1 when
+// that site lies above (row y - gT), 0 when below (row y + gT); equidistant sites above and below give the upper one.
+template <bool IDX>
 __global__ void __launch_bounds__(256) k_edt_cols(const unsigned* __restrict__ bits, const int* __restrict__ above,
-                                                  const int* __restrict__ below, int H, int W, int* __restrict__ gT)
+                                                  const int* __restrict__ below, int H, int W, int* __restrict__ gT,
+                                                  uint8_t* __restrict__ upT)
 {
     __shared__ int tile[EDT_BAND][256 + 1];
+    __shared__ uint8_t up_tile[IDX ? EDT_BAND : 1][IDX ? 256 + 4 : 1];
     const int xb = blockIdx.x * 256, x = xb + threadIdx.x, b = blockIdx.y;
     const int y0 = b * EDT_BAND, y1 = min(y0 + EDT_BAND, H);
     if (x < W) {
@@ -111,12 +116,16 @@ __global__ void __launch_bounds__(256) k_edt_cols(const unsigned* __restrict__ b
             if (a >= 0) d = y - a;
             if (c != EDT_NONE) d = min(d, c - y);
             tile[r][threadIdx.x] = d;
+            if constexpr (IDX) up_tile[r][threadIdx.x] = a >= 0 && y - a == d;
         }
     }
     __syncthreads();
     for (int e = threadIdx.x; e < 256 * EDT_BAND; e += 256) {
         const int xx = e / EDT_BAND, r = e % EDT_BAND;
-        if (xb + xx < W && y0 + r < y1) gT[(size_t)(xb + xx) * H + y0 + r] = tile[r][xx];
+        if (xb + xx < W && y0 + r < y1) {
+            gT[(size_t)(xb + xx) * H + y0 + r] = tile[r][xx];
+            if constexpr (IDX) upT[(size_t)(xb + xx) * H + y0 + r] = up_tile[r][xx];
+        }
     }
 }
 
@@ -245,10 +254,15 @@ __global__ void __launch_bounds__(EDT_ROWS) k_edt_carry(const int* __restrict__ 
 
 // 2e: the nearest site of every pixel is the running maximum of the marks; dist = sqrt((double)d2) as scipy forms it, written row-major
 // through shared memory.  A row without marks has no site anywhere in the image: scipy then measures every pixel from (-1, 0).
+// IDX writes instead the flat index (row * W + column) of that site, its row from upT, or -1 when the image has no site.
+template <bool IDX> struct EdtOut { using T = double; };
+template <> struct EdtOut<true> { using T = int; };
+
+template <bool IDX>
 __global__ void __launch_bounds__(EDT_ROWS) k_edt_fill(const int* __restrict__ gT, const int* __restrict__ mark, const int* __restrict__ carry,
-                                                       int H, int W, double* __restrict__ dist)
+                                                       const uint8_t* __restrict__ upT, int H, int W, typename EdtOut<IDX>::T* __restrict__ out)
 {
-    __shared__ double tile[EDT_ROWS][EDT_COLS + 1];
+    __shared__ typename EdtOut<IDX>::T tile[EDT_ROWS][EDT_COLS + 1];
     const int b = blockIdx.x, y0 = blockIdx.y * EDT_ROWS, x0 = b * EDT_COLS, y = y0 + threadIdx.x;
     if (y < H) {
         int owner = carry[(size_t)b * H + y];
@@ -256,87 +270,24 @@ __global__ void __launch_bounds__(EDT_ROWS) k_edt_fill(const int* __restrict__ g
         for (int c = 0; c < EDT_COLS && x0 + c < W; ++c) {
             const int x = x0 + c, m = mark[(size_t)x * H + y];
             if (m > owner) { owner = m; gown = gT[(size_t)m * H + y]; }
-            tile[threadIdx.x][c] = owner >= 0 ? sqrt((double)parab(x, owner, gown))
-                                              : sqrt((double)((long long)(y + 1) * (y + 1) + (long long)x * x));
+            if constexpr (IDX) {
+                tile[threadIdx.x][c] = owner >= 0 ? (upT[(size_t)owner * H + y] ? y - gown : y + gown) * W + owner : -1;
+            } else {
+                tile[threadIdx.x][c] = owner >= 0 ? sqrt((double)parab(x, owner, gown))
+                                                  : sqrt((double)((long long)(y + 1) * (y + 1) + (long long)x * x));
+            }
         }
     }
     __syncthreads();
     for (int e = threadIdx.x; e < EDT_ROWS * EDT_COLS; e += EDT_ROWS) {
         const int r = e / EDT_COLS, c = e % EDT_COLS;
-        if (y0 + r < H && x0 + c < W) dist[(size_t)(y0 + r) * W + x0 + c] = tile[r][c];
+        if (y0 + r < H && x0 + c < W) out[(size_t)(y0 + r) * W + x0 + c] = tile[r][c];
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// order-preserving compaction of a [H, W] mask: per tile counts, one scan, then the writes in raster order
+// order-preserving compaction of a [H, W] mask (compact.cuh): the writes in raster order
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int CPT_THREADS = 256, CPT_PER = 16, CPT_TILE = CPT_THREADS * CPT_PER;
-
-__device__ __forceinline__ int thread_count(const uint8_t* __restrict__ mask, long long beg, long long n)
-{
-    int c = 0;
-    for (int k = 0; k < CPT_PER; ++k) {
-        const long long i = beg + k;
-        if (i < n && mask[i]) ++c;
-    }
-    return c;
-}
-
-// exclusive prefix of v over the block; *total = block sum
-__device__ __forceinline__ int block_exclusive_scan(int v, int* total)
-{
-    __shared__ int warp_sum[CPT_THREADS / 32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    int inc = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-    }
-    if (lane == 31) warp_sum[wid] = inc;
-    __syncthreads();
-    if (wid == 0) {
-        int w = lane < CPT_THREADS / 32 ? warp_sum[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += u;
-        }
-        if (lane < CPT_THREADS / 32) warp_sum[lane] = w;   // inclusive over warps
-    }
-    __syncthreads();
-    const int before = wid ? warp_sum[wid - 1] : 0;
-    *total = warp_sum[CPT_THREADS / 32 - 1];
-    return before + inc - v;
-}
-
-__global__ void __launch_bounds__(CPT_THREADS) k_compact_count(const uint8_t* __restrict__ mask, long long n, long long* __restrict__ tile_count)
-{
-    const long long beg = (long long)blockIdx.x * CPT_TILE + (long long)threadIdx.x * CPT_PER;
-    int total;
-    block_exclusive_scan(thread_count(mask, beg, n), &total);
-    if (threadIdx.x == 0) tile_count[blockIdx.x] = total;
-}
-
-// exclusive scan of the tile counts in one CTA (tiles are few: 16 384 for an 8192^2 map); total -> tile_off[n_tiles]
-__global__ void __launch_bounds__(1024) k_compact_scan(const long long* __restrict__ tile_count, int n_tiles, long long* __restrict__ tile_off)
-{
-    __shared__ long long part[1024];
-    const int per = (n_tiles + 1023) / 1024, t = threadIdx.x;
-    const int b0 = min(t * per, n_tiles), b1 = min(b0 + per, n_tiles);
-    long long s = 0;
-    for (int b = b0; b < b1; ++b) s += tile_count[b];
-    part[t] = s;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) {
-        const long long u = t >= o ? part[t - o] : 0;
-        __syncthreads();
-        part[t] += u;
-        __syncthreads();
-    }
-    long long run = t ? part[t - 1] : 0;
-    for (int b = b0; b < b1; ++b) { tile_off[b] = run; run += tile_count[b]; }
-    if (t == 1023) tile_off[n_tiles] = part[1023];
-}
-
 __global__ void __launch_bounds__(CPT_THREADS) k_compact_write(const uint8_t* __restrict__ mask, long long n, int W, const double* __restrict__ values,
                                                                const long long* __restrict__ tile_off, int64_t* __restrict__ points,
                                                                double* __restrict__ values_out)
@@ -365,7 +316,6 @@ __global__ void __launch_bounds__(256) k_relabel(const int* __restrict__ seg, lo
 
 inline int edt_bands(int H) { return (H + EDT_BAND - 1) / EDT_BAND; }
 inline int edt_col_bands(int W) { return (W + EDT_COLS - 1) / EDT_COLS; }
-inline int compact_tiles(long long n) { return (int)((n + CPT_TILE - 1) / CPT_TILE); }
 
 } // namespace
 
@@ -396,12 +346,10 @@ extern "C" size_t isb_edt_workspace_bytes(int H, int W)
     return isb_align(sizeof(unsigned) * bw) + 2 * isb_align(sizeof(int) * bw) + 4 * isb_align(sizeof(int) * px) + 5 * isb_align(sizeof(int) * bh);
 }
 
-extern "C" int isb_edt_2d(const uint8_t* sites, int H, int W, double* dist, void* ws, size_t ws_bytes, isb_stream_t stream)
+// both transforms share every kernel; IDX adds the above / below flags of the column pass and writes site indices instead of distances
+template <bool IDX>
+int edt_run(const uint8_t* sites, int H, int W, typename EdtOut<IDX>::T* out, void* ws, size_t ws_bytes, cudaStream_t st)
 {
-    ISB_REQUIRE(sites && dist && ws, "null pointer");
-    ISB_REQUIRE(H > 0 && W > 0, "bad sizes");
-    ISB_REQUIRE(H <= 32768 && W <= 32768, "the squared distances of an image larger than 32768 x 32768 overflow int32");
-    ISB_REQUIRE(ws_bytes >= isb_edt_workspace_bytes(H, W), "workspace too small");
     const int nb = edt_bands(H), nc = edt_col_bands(W);
     WsCarver c(ws, ws_bytes);
     unsigned* bits = c.take<unsigned>((size_t)nb * W);
@@ -415,13 +363,13 @@ extern "C" int isb_edt_2d(const uint8_t* sites, int H, int W, double* dist, void
     int* tail = c.take<int>((size_t)nc * H);
     int* bmax = c.take<int>((size_t)nc * H);
     int* carry = c.take<int>((size_t)nc * H);
-    cudaStream_t st = (cudaStream_t)stream;
+    uint8_t* upT = IDX ? c.take<uint8_t>((size_t)H * W) : nullptr;
     const unsigned gx = (unsigned)((W + 255) / 256), gy = (unsigned)((H + EDT_ROWS - 1) / EDT_ROWS);
     k_edt_bits<<<dim3(gx, nb), 256, 0, st>>>(sites, H, W, bits);
     ISB_LAUNCH_CHECK();
     k_edt_links<<<gx, 256, 0, st>>>(bits, nb, W, above, below);
     ISB_LAUNCH_CHECK();
-    k_edt_cols<<<dim3(gx, nb), 256, 0, st>>>(bits, above, below, H, W, gT);
+    k_edt_cols<IDX><<<dim3(gx, nb), 256, 0, st>>>(bits, above, below, H, W, gT, upT);
     ISB_LAUNCH_CHECK();
     k_edt_local<<<dim3(gy, nc), EDT_ROWS, 0, st>>>(gT, H, W, prev, next, head, tail);
     ISB_LAUNCH_CHECK();
@@ -436,16 +384,39 @@ extern "C" int isb_edt_2d(const uint8_t* sites, int H, int W, double* dist, void
     ISB_LAUNCH_CHECK();
     k_edt_carry<<<gy, EDT_ROWS, 0, st>>>(bmax, H, nc, carry);
     ISB_LAUNCH_CHECK();
-    k_edt_fill<<<dim3(nc, gy), EDT_ROWS, 0, st>>>(gT, mark, carry, H, W, dist);
+    k_edt_fill<IDX><<<dim3(nc, gy), EDT_ROWS, 0, st>>>(gT, mark, carry, upT, H, W, out);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
+}
+
+extern "C" int isb_edt_2d(const uint8_t* sites, int H, int W, double* dist, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    ISB_REQUIRE(sites && dist && ws, "null pointer");
+    ISB_REQUIRE(H > 0 && W > 0, "bad sizes");
+    ISB_REQUIRE(H <= 32768 && W <= 32768, "the squared distances of an image larger than 32768 x 32768 overflow int32");
+    ISB_REQUIRE(ws_bytes >= isb_edt_workspace_bytes(H, W), "workspace too small");
+    return edt_run<false>(sites, H, W, dist, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t isb_edt_index_workspace_bytes(int H, int W)
+{
+    if (H <= 0 || W <= 0) return 0;
+    return isb_edt_workspace_bytes(H, W) + isb_align((size_t)H * W);
+}
+
+extern "C" int isb_edt_2d_indices(const uint8_t* sites, int H, int W, int32_t* index, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    ISB_REQUIRE(sites && index && ws, "null pointer");
+    ISB_REQUIRE(H > 0 && W > 0, "bad sizes");
+    ISB_REQUIRE(H <= 32768 && W <= 32768, "the squared distances of an image larger than 32768 x 32768 overflow int32");
+    ISB_REQUIRE(ws_bytes >= isb_edt_index_workspace_bytes(H, W), "workspace too small");
+    return edt_run<true>(sites, H, W, index, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 extern "C" size_t isb_mask_compact_workspace_bytes(int H, int W)
 {
     if (H <= 0 || W <= 0) return 0;
-    const int nt = compact_tiles((long long)H * W);
-    return isb_align(sizeof(long long) * (size_t)nt) + isb_align(sizeof(long long) * ((size_t)nt + 1));
+    return compact_workspace_bytes((long long)H * W);
 }
 
 extern "C" int isb_mask_compact_count(const uint8_t* mask, int H, int W, void* ws, size_t ws_bytes, long long* total, isb_stream_t stream)
@@ -453,18 +424,7 @@ extern "C" int isb_mask_compact_count(const uint8_t* mask, int H, int W, void* w
     ISB_REQUIRE(mask && ws && total, "null pointer");
     ISB_REQUIRE(H > 0 && W > 0, "bad sizes");
     ISB_REQUIRE(ws_bytes >= isb_mask_compact_workspace_bytes(H, W), "workspace too small");
-    const long long n = (long long)H * W;
-    const int nt = compact_tiles(n);
-    WsCarver c(ws, ws_bytes);
-    long long* tile_count = c.take<long long>(nt);
-    long long* tile_off = c.take<long long>((size_t)nt + 1);
-    cudaStream_t st = (cudaStream_t)stream;
-    k_compact_count<<<nt, CPT_THREADS, 0, st>>>(mask, n, tile_count);
-    ISB_LAUNCH_CHECK();
-    k_compact_scan<<<1, 1024, 0, st>>>(tile_count, nt, tile_off);
-    ISB_LAUNCH_CHECK();
-    ISB_CUDA_CHECK(cudaMemcpyAsync(total, tile_off + nt, sizeof(long long), cudaMemcpyDeviceToDevice, st));
-    return ISB_OK;
+    return compact_count(mask, (long long)H * W, ws, (cudaStream_t)stream, total);
 }
 
 extern "C" int isb_mask_compact_write(const uint8_t* mask, int H, int W, const double* values, const void* ws, size_t ws_bytes, int64_t* points,
@@ -476,9 +436,7 @@ extern "C" int isb_mask_compact_write(const uint8_t* mask, int H, int W, const d
     ISB_REQUIRE(ws_bytes >= isb_mask_compact_workspace_bytes(H, W), "workspace too small");
     const long long n = (long long)H * W;
     const int nt = compact_tiles(n);
-    WsCarver c(const_cast<void*>(ws), ws_bytes);
-    c.take<long long>(nt);
-    const long long* tile_off = c.take<long long>((size_t)nt + 1);
+    const long long* tile_off = compact_tile_offsets(ws, n);
     k_compact_write<<<nt, CPT_THREADS, 0, (cudaStream_t)stream>>>(mask, n, W, values, tile_off, points, values_out);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
