@@ -295,24 +295,18 @@ int isb_alpha_expansion(int N, const int32_t* n_nodes_dev /* optional device N *
 
 /* ------------------------------------------------------------------------------------------------------------------
  * class model -- replaces the host round trip of estim_class_model / predict_proba (imsegm/graph_cuts.py:73-163 default
- * 'GMM', imsegm/pipelines.py:95-96): StandardScaler + sklearn-style full-covariance GaussianMixture EM, n_init
- * restarts run concurrently (one CTA each), best lower bound wins.
+ * 'GMM', imsegm/pipelines.py:95-96) for either mixture of the reference's estim_model variants: StandardScaler +
+ * sklearn-style full-covariance EM, n_init restarts run concurrently (one CTA each), best lower bound wins.
+ *   kind 0 = GaussianMixture, 1 = BayesianGaussianMixture (full covariance, dirichlet_process, default priors: weight
+ *   concentration 1/K, mean precision 1, mean = mean of the scaled features, degrees of freedom D, covariance = their np.cov)
  *   feat [N, ld] f64 (first D columns used), n_dev: optional device int32 with the real row count (<= N)
  *   init_labels: optional [n_init, N] i32 hard assignments (deterministic start); else k-means++/Lloyd from `seed`
- *   proba: out [N, K];  params_out: optional, isb_gmm_params_len(D, K) doubles:
+ *   proba: out [N, K];  params_out: optional, isb_mixture_fit_params_len(kind, D, K) doubles:
  *     scaler mean[D] | scaler scale[D] | weights[K] | means[K,D] | covariances[K,D,D] | precisions_cholesky[K,D,D] |
  *     lower_bound | n_iter | converged | ok | best_init
+ *   For kind 1 the layout has nk (responsibility sums + 10 eps) in place of the weights, the posterior means and (normalised)
+ *   covariances, the ELBO as lower_bound, followed by mean_prior[D] | covariance_prior[D,D].
  * ------------------------------------------------------------------------------------------------------------------ */
-size_t isb_gmm_workspace_bytes(int N, int D, int K, int n_init);
-int isb_gmm_params_len(int D, int K);
-int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, const int32_t* n_dev, int K, int n_init, int max_iter, double tol,
-                        double reg_covar, int use_scaler, unsigned long long seed, const int32_t* init_labels, double* proba,
-                        double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream);
-/* the same fit for either mixture of the reference's estim_model variants: kind 0 = GaussianMixture (exactly isb_gmm_fit_predict),
- * kind 1 = BayesianGaussianMixture (full covariance, dirichlet_process, default priors: weight concentration 1/K, mean precision 1,
- * mean = mean of the scaled features, degrees of freedom D, covariance = their np.cov).  For kind 1 the params_out layout is the GMM
- * one with nk (responsibility sums + 10 eps) in place of the weights, the posterior means and (normalised) covariances, the ELBO as
- * lower_bound, followed by mean_prior[D] | covariance_prior[D,D].  Same limits and errors as isb_gmm_fit_predict. */
 size_t isb_mixture_fit_workspace_bytes(int kind, int N, int D, int K, int n_init);
 int isb_mixture_fit_params_len(int kind, int D, int K);
 int isb_mixture_fit_predict(int kind, const double* feat, int N, int D, int ld, const int32_t* n_dev, int K, int n_init, int max_iter,
@@ -390,11 +384,9 @@ int isb_lm_texture_finish(int nb, int n_batt, int flags, const double* acc, cons
 
 /* known-answer test of the tensor-core plumbing (tests/test_gpu_umma.py): D[128, N] = A[128, K] * B[N, K]^T with wgmma.mma_async
  * (TF32 inputs, FP32 accumulators) in one CTA of two warpgroups; A, B row-major f32 holding tf32-representable values,
- * N in {16, 48, 80, 240, 256}, K % 8 == 0 (<= 64).  variant 0 = A and B from K-major unswizzled shared memory, 1 = the same with the
- * descriptor's LBO / SBO fields swapped (diagnostic), 2 = A from registers (the form the contraction uses). */
+ * N in {48, 80} (the widths of the contraction), K % 8 == 0 (<= 64).  A comes from registers and B from K-major unswizzled shared
+ * memory, the form the contraction uses; variant must be 2 (the shared-memory A operands 0 / 1 are gone). */
 int isb_wgmma_selftest(const float* A, const float* B, int N, int K, int variant, float* D, isb_stream_t stream);
-/* profiling aid: clocks per dependent FP64 add / multiply / fma (one warp, chains of n operations); out: device, 4 doubles */
-int isb_fp64_latency(int n, double* out, isb_stream_t stream);
 
 /* per-segment, per-channel median -- numpy_img2d_color_median (imsegm/descriptors.py:420-455, channels = 3, n_px = H*W) and
  * numpy_img3d_gray_median (:651-676, channels = 1, n_px = D*H*W); np.median semantics (mean of the two middle values for an even
@@ -403,10 +395,6 @@ int isb_fp64_latency(int n, double* out, isb_stream_t stream);
 size_t isb_segment_median_workspace_bytes(long long n_px, int nb);
 int isb_segment_median(const void* img, int dtype, const int32_t* seg, long long n_px, int channels, int nb, double* out, void* ws,
                        size_t ws_bytes, isb_stream_t stream);
-
-/* skimage.morphology.opening(mask, disk(radius)) of a binary mask as imsegm/descriptors.py:1873-1876 applies it before tracing Ray
- * features: erosion then dilation with a disc, borders reflected.  mask / tmp / out : [H, W] uint8 (0 / 1) */
-int isb_binary_opening_disk(const uint8_t* mask, int H, int W, int radius, uint8_t* tmp, uint8_t* out, isb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * (x) ellipse fitting -- imsegm/ellipse_fitting.py: EllipseModelSegm (skimage.measure.EllipseModel + criterion :76-139),
@@ -431,7 +419,8 @@ int isb_ellipse_ransac(int T, const int32_t* trial_centre, const int32_t* samp_o
 int isb_ellipse_overlap(const int32_t* segm, int H, int W, int n_labels, const int32_t* bbox_host, const double* geom_host,
                         uint8_t* mask, unsigned long long* counts, isb_stream_t stream);
 /* grey erosion (op 0) or dilation (op 1) of a 0/1 mask [H, W] u8 over n_offsets (dy, dx) footprint offsets (device i32 [n, 2]),
- * borders as scipy.ndimage's 'reflect'.  The footprints of skimage.morphology.disk(r) for a non-integer r. */
+ * borders as scipy.ndimage's 'reflect'.  Two calls with the offsets of skimage.morphology.disk(r) make the opening that
+ * imsegm/descriptors.py:1873-1876 and imsegm/ellipse_fitting.py apply to a binary mask. */
 int isb_binary_morph_footprint(const uint8_t* in, int H, int W, const int32_t* offsets, int n_offsets, int op, uint8_t* out,
                                isb_stream_t stream);
 

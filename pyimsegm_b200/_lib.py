@@ -71,9 +71,6 @@ SIGNATURES = {
     'isb_gc_energies': (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _d, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     'isb_alpha_expansion_workspace_bytes': (_sz, [_i, _i, _i]),
     'isb_alpha_expansion': (_i, [_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
-    'isb_gmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
-    'isb_gmm_params_len': (_i, [_i, _i]),
-    'isb_gmm_fit_predict': (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _d, _d, _i, C.c_ulonglong, _vp, _vp, _vp, _vp, _sz, _vp]),
     'isb_mixture_fit_workspace_bytes': (_sz, [_i, _i, _i, _i, _i]),
     'isb_mixture_fit_params_len': (_i, [_i, _i, _i]),
     'isb_mixture_fit_predict': (_i, [_i, _vp, _i, _i, _i, _vp, _i, _i, _i, _d, _d, _i, C.c_ulonglong, _vp, _vp, _vp, _vp, _sz, _vp]),
@@ -92,7 +89,6 @@ SIGNATURES = {
     'isb_lm_texture_finish': (_i, [_i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     'isb_lm_texture': (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _i, C.POINTER(_d), _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _sz, _vp]),
     'isb_wgmma_selftest': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
-    'isb_fp64_latency': (_i, [_i, _vp, _vp]),
     'isb_fill_i32': (_i, [_vp, _ll, _i, _vp]),
     'isb_combine': (_i, [_vp, _vp, _ll, _i, _vp]),
     'isb_gray_stats_workspace_bytes': (_sz, [_i]),
@@ -106,7 +102,6 @@ SIGNATURES = {
     'isb_gather': (_i, [_vp, _ll, _vp, _vp, _i, _vp, _vp, _vp]),
     'isb_segment_median_workspace_bytes': (_sz, [_ll, _i]),
     'isb_segment_median': (_i, [_vp, _i, _vp, _ll, _i, _i, _vp, _vp, _sz, _vp]),
-    'isb_binary_opening_disk': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     'isb_color_convert': (_i, [_vp, _i, _ll, _i, _vp, _vp]),
     'isb_gradient_sum_2d': (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     'isb_segment_median_2d': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _sz, _vp]),

@@ -37,12 +37,13 @@ def build(force=False, verbose=False):
     build_dir = os.path.join(HERE, 'build')
     os.makedirs(build_dir, exist_ok=True)
     procs = []
+    # any source may include any header, so an object is stale once it is older than its .cu or than the newest header
+    headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith('.cuh')] + [os.path.join(HERE, '..', 'include', 'imsegm_b200.h')]
+    newest_header = max(os.path.getmtime(h) for h in headers)
     for src in sources():
         obj = os.path.join(build_dir, os.path.basename(src)[:-3] + '.o')
         objs.append(obj)
-        if (not force) and os.path.isfile(obj) and os.path.getmtime(obj) > max(
-                os.path.getmtime(src), os.path.getmtime(os.path.join(CSRC, 'common.cuh')),
-                os.path.getmtime(os.path.join(HERE, '..', 'include', 'imsegm_b200.h'))):
+        if (not force) and os.path.isfile(obj) and os.path.getmtime(obj) > max(os.path.getmtime(src), newest_header):
             continue
         cmd = [nvcc] + ARCH + FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-c', src, '-o', obj]
         procs.append((cmd, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))

@@ -15,7 +15,7 @@ void isb_set_error(const char* fmt, ...)
 }
 
 extern "C" const char* isb_last_error(void) { return g_err; }
-extern "C" int isb_abi_version(void) { return 7; }  // 7: device predict_proba of caller-fitted models (class transform, mixture, forest); 6: Hopper port: wgmma contraction, isb_wgmma_selftest replaces isb_umma_selftest, no issue-rate probe; 5: banded Leung-Malik statistics (accumulate / finish), tcgen05 issue-rate probe; 4: tcgen05 operand layout (w_tc), UMMA self-test, graph replay accounting, segment median
+extern "C" int isb_abi_version(void) { return 8; }  // 8: one entry point per operation: the GMM-only fit removed (isb_mixture_fit_* kind 0), the disc-only opening removed (isb_binary_morph_footprint), no FP64 latency probe, isb_wgmma_selftest for N in {48, 80} with A from registers; 7: device predict_proba of caller-fitted models (class transform, mixture, forest); 6: Hopper port: wgmma contraction, isb_wgmma_selftest replaces isb_umma_selftest, no issue-rate probe; 5: banded Leung-Malik statistics (accumulate / finish), tcgen05 issue-rate probe; 4: tcgen05 operand layout (w_tc), UMMA self-test, graph replay accounting, segment median
 extern "C" long long isb_launch_count(void) { return g_isb_launches; }
 extern "C" int isb_note_graph_replay(long long n_kernels) { g_isb_launches += n_kernels; return ISB_OK; }
 

@@ -95,3 +95,14 @@ __device__ __forceinline__ double f64_unordered(unsigned long long u)
     u = (u & 0x8000000000000000ull) ? (u & 0x7FFFFFFFFFFFFFFFull) : ~u;
     return __longlong_as_double((long long)u);
 }
+
+// scipy.ndimage 'reflect' for any i, including images smaller than the radius that reflect more than once
+__device__ __forceinline__ int reflect_index(int i, int n)
+{
+    if ((unsigned)i < (unsigned)n) return i;
+    if (n == 1) return 0;
+    int p = 2 * n;
+    i %= p;
+    if (i < 0) i += p;
+    return (i < n) ? i : (p - 1 - i);
+}

@@ -359,10 +359,7 @@ __global__ void k_binary_morph(const uint8_t* __restrict__ in, int H, int W, con
     const int y = (int)(i / W), x = (int)(i % W);
     uint8_t v = op == 0 ? 1 : 0;
     for (int k = 0; k < n_offs; ++k) {
-        int yy = y + offs[2 * k], xx = x + offs[2 * k + 1];
-        const int ph = 2 * H, pw = 2 * W;
-        yy = ((yy % ph) + ph) % ph; if (yy >= H) yy = ph - 1 - yy;
-        xx = ((xx % pw) + pw) % pw; if (xx >= W) xx = pw - 1 - xx;
+        const int yy = reflect_index(y + offs[2 * k], H), xx = reflect_index(x + offs[2 * k + 1], W);
         const uint8_t s = in[(size_t)yy * W + xx] != 0;
         v = op == 0 ? (v & s) : (v | s);
     }

@@ -1708,22 +1708,6 @@ static size_t carve_pca(PcaWs& p, void* ws, size_t bytes, int N, int D)
 
 } // namespace
 
-extern "C" size_t isb_gmm_workspace_bytes(int N, int D, int K, int n_init)
-{
-    GmmWs w;
-    return carve_gmm(w, nullptr, 0, N, D, K, n_init);
-}
-
-extern "C" int isb_gmm_params_len(int D, int K) { return 2 * D + pstride(K, D) + 1; }
-
-extern "C" int isb_gmm_fit_predict(const double* feat, int N, int D, int ld, const int32_t* n_dev, int K, int n_init, int max_iter,
-                                   double tol, double reg_covar, int use_scaler, unsigned long long seed, const int32_t* init_labels,
-                                   double* proba, double* params_out, void* ws, size_t ws_bytes, isb_stream_t stream)
-{
-    return mixture_fit_predict<MIX_GMM>(feat, N, D, ld, n_dev, K, n_init, max_iter, tol, reg_covar, use_scaler, seed, init_labels, proba,
-                                        params_out, ws, ws_bytes, stream);
-}
-
 extern "C" size_t isb_mixture_fit_workspace_bytes(int kind, int N, int D, int K, int n_init)
 {
     GmmWs w;

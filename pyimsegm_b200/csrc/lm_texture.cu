@@ -30,15 +30,6 @@ namespace {
 constexpr int VB_R = 32;      // output rows per thread
 constexpr int VB_T = 128;     // threads (columns) per CTA
 
-__device__ __forceinline__ int reflect_idx(int i, int n)
-{
-    if (n == 1) return 0;
-    int p = 2 * n;
-    i %= p;
-    if (i < 0) i += p;
-    return (i < n) ? i : (p - 1 - i);
-}
-
 __global__ void __launch_bounds__(256) k_lm_to_planar(const void* __restrict__ img, int dtype, size_t npx, double* __restrict__ out)
 {
     size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -87,7 +78,7 @@ __global__ void __launch_bounds__(VB_T) k_lm_vblur(const double* __restrict__ in
             int i = y0 + db + t;
             // one reflection is enough when radius + 2R <= n0 (FAST_REFLECT); the general form handles images smaller than the kernel
             if (FAST_REFLECT) i = i < 0 ? -1 - i : (i >= n0 ? 2 * n0 - 1 - i : i);
-            else i = reflect_idx(i, n0);
+            else i = reflect_index(i, n0);
             const double v = col[(size_t)i * n1];
 #pragma unroll
             for (int r = 0; r < R; ++r) acc[r] = fma(w[R - 1 + t - r], v, acc[r]);
@@ -443,7 +434,7 @@ __global__ void __launch_bounds__(256) k_lm_pad_split(const float* __restrict__ 
 {
     const int xp = blockIdx.x * blockDim.x + threadIdx.x, yp = blockIdx.y, c = blockIdx.z;
     if (xp >= Wp) return;
-    const float v = img[(size_t)c * H * W + (size_t)reflect_idx(yp - KRAD, H) * W + reflect_idx(xp - KRAD, W)];
+    const float v = img[(size_t)c * H * W + (size_t)reflect_index(yp - KRAD, H) * W + reflect_index(xp - KRAD, W)];
     unsigned hb, lb;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(v));
     const float hi = __uint_as_float(hb);

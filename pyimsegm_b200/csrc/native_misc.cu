@@ -262,15 +262,6 @@ extern "C" int isb_disc_label_hist(const int32_t* segm, const double* proba, int
 // ---------------------------------------------------------------------------------------------------------------------
 namespace {
 
-__device__ __forceinline__ int reflect_at(int i, int n)
-{
-    if (n == 1) return 0;
-    const int p = 2 * n;
-    i %= p;
-    if (i < 0) i += p;
-    return i < n ? i : p - 1 - i;
-}
-
 // out[s][y][x] = max_f sum_{a,b} K[f][a][b] img[s][reflect(y + kh/2 - a)][reflect(x + kw/2 - b)]
 __global__ void __launch_bounds__(256) k_conv_battery_max(const double* __restrict__ img, int S, int H, int W, const double* __restrict__ kern,
                                                           int nf, int kh, int kw, double* __restrict__ out)
@@ -285,8 +276,8 @@ __global__ void __launch_bounds__(256) k_conv_battery_max(const double* __restri
         double acc = 0.0;
         // ndimage.convolve == correlate with the flipped kernel: walk the flipped kernel in C order
         for (int a = kh - 1; a >= 0; --a) {
-            const int yy = reflect_at(y + kh / 2 - a, H);
-            for (int b = kw - 1; b >= 0; --b) acc = __dadd_rn(acc, __dmul_rn(k[a * kw + b], im[(size_t)yy * W + reflect_at(x + kw / 2 - b, W)]));
+            const int yy = reflect_index(y + kh / 2 - a, H);
+            for (int b = kw - 1; b >= 0; --b) acc = __dadd_rn(acc, __dmul_rn(k[a * kw + b], im[(size_t)yy * W + reflect_index(x + kw / 2 - b, W)]));
         }
         // np.max over the battery, which returns NaN when any kernel's response is NaN: the Leung-Malik route feeds this kernel an
         // image minus its background, NaN wherever the image has a NaN or an infinity within the background's reach
@@ -306,8 +297,8 @@ __global__ void __launch_bounds__(256) k_gauss_axis(const double* __restrict__ i
     double t = __dmul_rn(im[(size_t)y * W + x], w_half[0]);
     for (int j = r; j >= 1; --j) {
         double a, b;
-        if (axis == 0) { a = im[(size_t)reflect_at(y - j, H) * W + x]; b = im[(size_t)reflect_at(y + j, H) * W + x]; }
-        else { a = im[(size_t)y * W + reflect_at(x - j, W)]; b = im[(size_t)y * W + reflect_at(x + j, W)]; }
+        if (axis == 0) { a = im[(size_t)reflect_index(y - j, H) * W + x]; b = im[(size_t)reflect_index(y + j, H) * W + x]; }
+        else { a = im[(size_t)y * W + reflect_index(x - j, W)]; b = im[(size_t)y * W + reflect_index(x + j, W)]; }
         t = __dadd_rn(t, __dmul_rn(__dadd_rn(a, b), w_half[j]));
     }
     out[i] = t;

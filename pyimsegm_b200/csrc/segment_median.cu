@@ -176,33 +176,6 @@ static size_t carve_med(MedWs& w, void* ws, size_t bytes, size_t n, int nb)
     return isb_align(c.off);
 }
 
-__device__ __forceinline__ int reflect_px(int i, int n)
-{
-    if (n == 1) return 0;
-    const int p = 2 * n;
-    i %= p;
-    if (i < 0) i += p;
-    return i < n ? i : p - 1 - i;
-}
-
-// op 0: erosion (all pixels under the disc set), op 1: dilation (any pixel under the disc set); borders reflected
-__global__ void __launch_bounds__(256) k_morph_disk(const unsigned char* __restrict__ src, int H, int W, int radius, int op, unsigned char* __restrict__ dst)
-{
-    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
-    if (x >= W || y >= H) return;
-    const int r2 = radius * radius;
-    bool acc = op == 0;
-    for (int dy = -radius; dy <= radius; ++dy) {
-        const int yy = reflect_px(y + dy, H);
-        for (int dx = -radius; dx <= radius; ++dx) {
-            if (dy * dy + dx * dx > r2) continue;
-            const bool v = src[(size_t)yy * W + reflect_px(x + dx, W)] != 0;
-            if (op == 0) acc = acc && v; else acc = acc || v;
-        }
-    }
-    dst[(size_t)y * W + x] = acc ? 1 : 0;
-}
-
 } // namespace
 
 extern "C" size_t isb_segment_median_workspace_bytes(long long n_px, int nb)
@@ -256,17 +229,4 @@ extern "C" int isb_segment_median_2d(const void* img, int dtype, const int32_t* 
 {
     ISB_REQUIRE(H > 0 && W > 0, "bad sizes");
     return segment_median(img, dtype, seg, (long long)H * W, channels, nb, feat, ld, col0, true, ws, ws_bytes, stream);
-}
-
-extern "C" int isb_binary_opening_disk(const uint8_t* mask, int H, int W, int radius, uint8_t* tmp, uint8_t* out, isb_stream_t stream)
-{
-    ISB_REQUIRE(mask && tmp && out, "null pointer");
-    ISB_REQUIRE(H > 0 && W > 0 && radius >= 0 && radius <= 512, "bad sizes");
-    cudaStream_t st = (cudaStream_t)stream;
-    const dim3 grid((W + 31) / 32, (H + 7) / 8);
-    k_morph_disk<<<grid, 256, 0, st>>>(mask, H, W, radius, 0, tmp);
-    ISB_LAUNCH_CHECK();
-    k_morph_disk<<<grid, 256, 0, st>>>(tmp, H, W, radius, 1, out);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
 }

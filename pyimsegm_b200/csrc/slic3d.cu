@@ -21,15 +21,6 @@
 
 namespace {
 
-__device__ __forceinline__ int reflect3(int i, int n)
-{
-    if (n == 1) return 0;
-    const int p = 2 * n;
-    i %= p;
-    if (i < 0) i += p;
-    return i < n ? i : p - 1 - i;
-}
-
 // dtype -> f64 with skimage's img_as_float scale (1/255, 1/65535 for the integer types; floats unchanged)
 __global__ void k3_load(const void* __restrict__ vol, int dtype, size_t n, double* __restrict__ out)
 {
@@ -51,8 +42,8 @@ __global__ void k3_blur_axis(const double* __restrict__ in, double* __restrict__
     const long st = axis == 0 ? (long)H * W : (axis == 1 ? W : 1);
     double t = __dmul_rn(in[i], w[0]);
     for (int j = r; j >= 1; --j) {
-        const double a = in[i + (long)(reflect3(c - j, n) - c) * st];
-        const double b = in[i + (long)(reflect3(c + j, n) - c) * st];
+        const double a = in[i + (long)(reflect_index(c - j, n) - c) * st];
+        const double b = in[i + (long)(reflect_index(c + j, n) - c) * st];
         t = __dadd_rn(t, __dmul_rn(__dadd_rn(a, b), w[j]));
     }
     out[i] = t;

@@ -89,17 +89,6 @@ __device__ __forceinline__ void rgb2lab_px(double r, double g, double b, double&
     B = dmul(200.0, dsub(f[1], f[2]));
 }
 
-// scipy.ndimage 'reflect' for any i, including images smaller than the radius that reflect more than once
-__device__ __forceinline__ int reflect_idx(int i, int n)
-{
-    if ((unsigned)i < (unsigned)n) return i;
-    if (n == 1) return 0;
-    int p = 2 * n;
-    i %= p;
-    if (i < 0) i += p;
-    return (i < n) ? i : (p - 1 - i);
-}
-
 __global__ void k_minmax(const void* img, int dtype, size_t n, unsigned long long* mm)
 {
     double lo = 1.0 / 0.0, hi = -1.0 / 0.0;
@@ -172,7 +161,7 @@ __global__ void __launch_bounds__(NT, 2) k_blur_lab(const void* __restrict__ img
     const double span = dsub(mx, mn);
     const size_t HW = (size_t)H * W;
 
-    for (int ix = threadIdx.x; ix < IW; ix += NT) s_gx[ix] = reflect_idx(x0 + ix - R, W);
+    for (int ix = threadIdx.x; ix < IW; ix += NT) s_gx[ix] = reflect_index(x0 + ix - R, W);
     __syncthreads();
 
     // rescale, then the depth axis of skimage's [1,H,W,3] array: all its taps reflect onto the same sample
@@ -195,7 +184,7 @@ __global__ void __launch_bounds__(NT, 2) k_blur_lab(const void* __restrict__ img
         for (int i = threadIdx.x; i < nrow * IW; i += NT) {
             const int row = i / IW, ix = i - row * IW;
             const int ir = lo + row;
-            const int gy = reflect_idx(y0 - R + ir, H);
+            const int gy = reflect_index(y0 - R + ir, H);
             const size_t base = ((size_t)gy * W + s_gx[ix]) * C;
             double* dst = s_in + (ir % RING) * IW + ix;
             if (C == 3) {

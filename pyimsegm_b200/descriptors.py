@@ -680,20 +680,44 @@ def compute_ray_features_positions(segm, list_positions, angle_step=5., border_l
     return pos_rays, pos_shift, feature_names
 
 
+def _disk_offsets(radius, shift):
+    """(dy, dx) offsets of skimage.morphology.disk(radius) as skimage's erosion (shift False) and dilation (shift True) apply an
+    even-sized footprint: padded by a zero row / column before (erosion) or after (dilation) it"""
+    L = np.arange(-radius, radius + 1)
+    X, Y = np.meshgrid(L, L)
+    selem = (X ** 2 + Y ** 2) <= radius ** 2
+    rows, cols = np.nonzero(selem)
+    m, n = selem.shape
+    rows = rows + (1 if (m % 2 == 0 and not shift) else 0)
+    cols = cols + (1 if (n % 2 == 0 and not shift) else 0)
+    cy, cx = (m + (m % 2 == 0)) // 2, (n + (n % 2 == 0)) // 2
+    return np.stack([rows - cy, cols - cx], axis=1).astype(np.int32), (m % 2 == 0 or n % 2 == 0)
+
+
 def binary_opening_disk(mask, radius):
     """ morphological opening of a binary 2-D mask with a disc of ``radius`` pixels, borders reflected -- what the reference gets
-    from ``skimage.morphology.opening(mask, morphology.disk(radius))`` (descriptors.py:1873-1876); ``isb_binary_opening_disk`` """
+    from ``skimage.morphology.opening(mask, morphology.disk(radius))`` (descriptors.py:1873-1876, ellipse_fitting.py:412-433), as
+    two launches of ``isb_binary_morph_footprint``.  A non-integer radius gives a disc with an even side, which skimage (0.16-0.18
+    as recalled) applies to the image padded by side - 1 with its edge values; an integer radius needs no padding."""
     from . import _lib
-    mask = np.ascontiguousarray(mask, dtype=np.uint8)
+    mask = np.asarray(mask, dtype=np.uint8)
     if mask.ndim != 2:
         raise ValueError('expected a 2-D mask, got shape %r' % (mask.shape, ))
+    ero, even = _disk_offsets(radius, False)
+    dil, _ = _disk_offsets(radius, True)
+    pad = len(np.arange(-radius, radius + 1)) - 1 if even else 0
+    if pad:
+        mask = np.pad(mask, pad, mode='edge')
+    H, W = mask.shape
     eng = get_engine()
     d_in = eng.to_device(mask, 'morph_in')
     tmp = eng.buf('morph_tmp', mask.shape, eng.torch.uint8)
     out = eng.buf('morph_out', mask.shape, eng.torch.uint8)
-    _lib.check(eng.lib.isb_binary_opening_disk(_lib.ptr(d_in), mask.shape[0], mask.shape[1], int(radius), _lib.ptr(tmp), _lib.ptr(out),
-                                               _lib.stream_ptr()))
-    return eng.to_host(out).astype(bool)
+    for src, offs, op, dst in ((d_in, ero, 0, tmp), (tmp, dil, 1, out)):
+        d_off = eng.const_device(offs, 'morph_offsets')
+        _lib.check(eng.lib.isb_binary_morph_footprint(_lib.ptr(src), H, W, _lib.ptr(d_off), len(offs), op, _lib.ptr(dst),
+                                                      _lib.stream_ptr()))
+    return eng.to_host(out)[pad:H - pad, pad:W - pad].astype(bool)
 
 
 def compute_ray_features_segm_2d_vectors(seg_binary, position, angle_step=5., smooth_coef=0, edge='up'):

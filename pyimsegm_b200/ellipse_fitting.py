@@ -374,46 +374,6 @@ def add_overlap_ellipse(segm, ellipse_params, label, thr_overlap=1.):
     return segm
 
 
-def _disk_offsets(radius, shift):
-    """(dy, dx) offsets of skimage.morphology.disk(radius) as skimage's erosion (shift False) and dilation (shift True) apply an
-    even-sized footprint: padded by a zero row / column before (erosion) or after (dilation) it"""
-    L = np.arange(-radius, radius + 1)
-    X, Y = np.meshgrid(L, L)
-    selem = (X ** 2 + Y ** 2) <= radius ** 2
-    rows, cols = np.nonzero(selem)
-    m, n = selem.shape
-    rows = rows + (1 if (m % 2 == 0 and not shift) else 0)
-    cols = cols + (1 if (n % 2 == 0 and not shift) else 0)
-    cy, cx = (m + (m % 2 == 0)) // 2, (n + (n % 2 == 0)) // 2
-    return np.stack([rows - cy, cols - cx], axis=1).astype(np.int32), (m % 2 == 0 or n % 2 == 0)
-
-
-def _opening_disk_float(mask, radius):
-    """skimage.morphology.opening(mask, disk(radius)) for a non-integer radius (0.16-0.18 as recalled: a footprint with an even side
-    first pads the image by side - 1 with its edge values), as two launches of isb_binary_morph_footprint"""
-    ero, even = _disk_offsets(radius, False)
-    dil, _ = _disk_offsets(radius, True)
-    pad = len(np.arange(-radius, radius + 1)) - 1 if even else 0
-    mask = np.ascontiguousarray(np.pad(np.asarray(mask, dtype=np.uint8), pad, mode='edge'))
-    eng = get_engine()
-    torch = eng.torch
-    H, W = mask.shape
-    d_in = eng.to_device(mask)
-    tmp = torch.empty((H, W), dtype=torch.uint8, device=eng.device)
-    out = torch.empty((H, W), dtype=torch.uint8, device=eng.device)
-    for src, offs, op, dst in ((d_in, ero, 0, tmp), (tmp, dil, 1, out)):
-        d_off = eng.to_device(offs)
-        _lib.check(eng.lib.isb_binary_morph_footprint(_lib.ptr(src), H, W, _lib.ptr(d_off), len(offs), op, _lib.ptr(dst),
-                                                      _lib.stream_ptr()))
-    return eng.to_host(out)[pad:H - pad, pad:W - pad].astype(bool)
-
-
-def _opening(mask, radius):
-    if float(radius) == int(radius):
-        return binary_opening_disk(mask, int(radius))
-    return _opening_disk_float(mask, radius)
-
-
 def split_segm_background_foreground(seg, sel_bg=STRUC_ELEM_BG, sel_fg=STRUC_ELEM_FG):
     """ smoothing segmentation with morphological operation
 
@@ -425,10 +385,10 @@ def split_segm_background_foreground(seg, sel_bg=STRUC_ELEM_BG, sel_fg=STRUC_ELE
     seg_bg = (seg > 0)
     seg_bg = 1 - ndimage.binary_fill_holes(seg_bg)
     if sel_bg > 0:
-        seg_bg = _opening(seg_bg, sel_bg).astype(seg_bg.dtype)
+        seg_bg = binary_opening_disk(seg_bg, sel_bg).astype(seg_bg.dtype)
     seg_fg = (seg == 1)
     if sel_fg > 0:
-        seg_fg = _opening(seg_fg, sel_fg)
+        seg_fg = binary_opening_disk(seg_fg, sel_fg)
     return seg_bg, seg_fg
 
 

@@ -471,38 +471,21 @@ class Engine(object):
                                          _lib.ptr(stats), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
         return labels, energy, stats
 
-    def gmm_fit_predict(self, d_feat, K, n_init, max_iter, use_scaler=True, seed=0, d_n=None, init_labels=None, tol=1e-3,
-                        reg_covar=1e-6):
-        """device class model: returns (proba [N,K] device, params device vector; see isb_gmm_fit_predict)"""
-        torch, lib = self.torch, self.lib
-        N, D = int(d_feat.shape[0]), int(d_feat.shape[1])
-        ld = int(d_feat.stride(0))
-        proba = self.buf('proba', (N, K), torch.float64)
-        params = self.buf('gmm_params', (lib.isb_gmm_params_len(D, K),), torch.float64)
-        wsb = lib.isb_gmm_workspace_bytes(N, D, int(K), int(n_init))
-        ws = self.buf('ws_gmm', (wsb,), torch.uint8)
-        d_init = None
-        if init_labels is not None:
-            d_init = self.to_device(np.ascontiguousarray(init_labels, dtype=np.int32), 'gmm_init')
-        self._ck(lib.isb_gmm_fit_predict(_lib.ptr(d_feat), N, D, ld, _lib.ptr(d_n), int(K), int(n_init), int(max_iter), C.c_double(tol),
-                                         C.c_double(reg_covar), int(bool(use_scaler)), C.c_ulonglong(int(seed)), _lib.ptr(d_init),
-                                         _lib.ptr(proba), _lib.ptr(params), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
-        return proba, params
-
     #: isb_mixture_fit_predict kinds
     MIXTURE_KINDS = {'GMM': 0, 'BGM': 1}
+    #: the params buffer of each kind: a captured CUDA graph holds the address of the one it writes, so a fit of the other kind
+    #: (with a longer params vector) must not grow it
+    _MIXTURE_PARAMS = {'GMM': 'gmm_params', 'BGM': 'mixture_params'}
 
     def mixture_fit_predict(self, d_feat, K, n_init, max_iter, use_scaler=True, seed=0, d_n=None, init_labels=None, tol=1e-3,
                             reg_covar=1e-6, kind='GMM'):
-        """device class model of either kind ('GMM' = :meth:`gmm_fit_predict`, 'BGM' = BayesianGaussianMixture): returns
+        """device class model of either kind ('GMM' = GaussianMixture, 'BGM' = BayesianGaussianMixture): returns
         (proba [N,K] device, params device vector; see isb_mixture_fit_predict)"""
-        if kind == 'GMM':
-            return self.gmm_fit_predict(d_feat, K, n_init, max_iter, use_scaler, seed, d_n, init_labels, tol, reg_covar)
         torch, lib = self.torch, self.lib
         code = self.MIXTURE_KINDS[kind]
         N, D = int(d_feat.shape[0]), int(d_feat.shape[1])
         proba = self.buf('proba', (N, K), torch.float64)
-        params = self.buf('mixture_params', (lib.isb_mixture_fit_params_len(code, D, K),), torch.float64)
+        params = self.buf(self._MIXTURE_PARAMS[kind], (lib.isb_mixture_fit_params_len(code, D, K),), torch.float64)
         wsb = lib.isb_mixture_fit_workspace_bytes(code, N, D, int(K), int(n_init))
         ws = self.buf('ws_gmm', (wsb,), torch.uint8)
         d_init = None

@@ -27,8 +27,8 @@ MIN_UNARY_PROB = 0.01
 MAX_PAIRWISE_COST = 1e5
 #: edge weights are clamped to [1 / val, val] (reference graph_cuts.py:40)
 MIN_MAX_EDGE_WEIGHT = 1e3
-#: the class model of every estim_model variant, with or without PCA, is fitted on the GPU (isb_gmm_fit_predict /
-#: isb_mixture_fit_predict / isb_pca_fit) when it fits the device kernels (<= 232 features, <= 8 classes, pca_coef None, in (0, 1)
+#: the class model of every estim_model variant, with or without PCA, is fitted on the GPU (isb_mixture_fit_predict /
+#: isb_pca_fit) when it fits the device kernels (<= 232 features, <= 8 classes, pca_coef None, in (0, 1)
 #: or a component count); set False to force scikit-learn on the host
 USE_DEVICE_GMM = True
 #: a caller-fitted model (segment_color2d_slic_features_model_graphcut, segment_images_batch(model_pipeline=...), segment_resident)
@@ -178,7 +178,7 @@ def _pca_from_device(params, nb_features, pca_coef):
 
 def sklearn_pipeline_from_device(params, nb_features, nb_classes, nb_samples, use_scaler=True, n_init=1, max_iter=99, kind='GMM',
                                  pca_params=None, pca_coef=None, nb_features_in=None):
-    """ wrap the parameters fitted by ``isb_gmm_fit_predict`` / ``isb_mixture_fit_predict`` (and ``isb_pca_fit``) into the
+    """ wrap the parameters fitted by ``isb_mixture_fit_predict`` (and ``isb_pca_fit``) into the
     scikit-learn objects the reference returns (Pipeline[StandardScaler?, PCA?, GaussianMixture | BayesianGaussianMixture]) so that
     ``predict_proba`` & co. keep working on the host.  With ``pca_params`` the scaler is the PCA fit's and ``nb_features`` counts
     the PCA components the mixture saw; ``nb_features_in`` is then the width of the raw features. """

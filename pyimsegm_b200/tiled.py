@@ -383,8 +383,8 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
             res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
                              force_whole=force_whole, raw_margin=margin)
             features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
-            d_proba, _ = eng.gmm_fit_predict(res.d_feat, int(nb_classes), n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED,
-                                             d_n=res.d_n_labels)
+            d_proba, _ = eng.mixture_fit_predict(res.d_feat, int(nb_classes), n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED,
+                                                 d_n=res.d_n_labels)
             redo_front = False
         lo, hi = res.bands[res.local[0]].own_lo, res.bands[res.local[-1]].own_hi
         soft = eng.early_soft(res.d_seg[lo:hi], d_proba) if want_soft else None

@@ -124,7 +124,7 @@ def test_annotation_entry_points_reject_bad_arguments():
     from pyimsegm_b200 import _lib
     lib = _lib.lib()
     p = C.c_void_p(16)
-    assert lib.isb_abi_version() == 7
+    assert lib.isb_abi_version() == 8
     assert lib.isb_color_hist(None, 4, 3, 0, p, None) == _lib.ISB_ERR_ARG
     assert lib.isb_color_hist(p, 4, 2, 0, p, None) == _lib.ISB_ERR_ARG and b'channels' in lib.isb_last_error()
     assert lib.isb_color_hist(p, 0, 3, 0, p, None) == _lib.ISB_ERR_ARG

@@ -27,7 +27,7 @@ def test_null_pointers_and_bad_sizes_are_reported(lib):
         lambda: lib.isb_segment_stats_2d(None, 3, None, 8, 8, 4, 1, None, 3, 0, None, None, None, 0, None),
         lambda: lib.isb_adjacency_edges(None, 8, 8, 4, None, 16, None, None, 0, None),
         lambda: lib.isb_alpha_expansion(4, None, 2, 3, None, None, None, None, None, -1, None, None, None, None, 0, None),
-        lambda: lib.isb_gmm_fit_predict(None, 10, 3, 3, None, 2, 1, 10, 1e-3, 1e-6, 1, 0, None, None, None, None, 0, None),
+        lambda: lib.isb_mixture_fit_predict(0, None, 10, 3, 3, None, 2, 1, 10, 1e-3, 1e-6, 1, 0, None, None, None, None, 0, None),
         lambda: lib.isb_slic3d_kmeans(None, 2, 8, 8, None, 4, 1, 2, 2, 2.0, None, 10, None, None, 0, None),
         lambda: lib.isb_enforce_connectivity3d(None, 2, 8, 8, 1, 10, None, None, None, 0, None),
         lambda: lib.isb_disc_label_hist(None, None, 8, 8, None, 1, None, 1, None, 0, 0, 3, None, None, None),
@@ -50,7 +50,7 @@ def test_messages_name_the_problem(lib):
     assert 'C must be 1 or 3' in _err(lib)
     assert lib.isb_filter_response_2d(p, 1, 8, 8, p, 1, 4, 3, p, None) == _lib.ISB_ERR_ARG
     assert 'odd' in _err(lib)
-    assert lib.isb_gmm_fit_predict(p, 10, 300, 300, None, 2, 1, 10, 1e-3, 1e-6, 1, 0, None, p, None, p, 1 << 40, None) == _lib.ISB_ERR_UNSUPPORTED
+    assert lib.isb_mixture_fit_predict(0, p, 10, 300, 300, None, 2, 1, 10, 1e-3, 1e-6, 1, 0, None, p, None, p, 1 << 40, None) == _lib.ISB_ERR_UNSUPPORTED
     assert 'D <=' in _err(lib)
     with pytest.raises(NotImplementedError):
         _lib.check(_lib.ISB_ERR_UNSUPPORTED)

@@ -69,7 +69,7 @@ def test_fit_entries_reject_bad_arguments_without_a_gpu():
     buf = (C.c_double * 64)()
     p = C.cast(buf, C.c_void_p)
     err = lambda: lib.isb_last_error().decode()  # noqa: E731
-    assert lib.isb_abi_version() == 7
+    assert lib.isb_abi_version() == 8
     big = 1 << 40
     # isb_mixture_fit_predict(kind, feat, N, D, ld, n_dev, K, n_init, max_iter, tol, reg, use_scaler, seed, init, proba, params, ws, ws_bytes, st)
     fa = [1, p, 100, 3, 3, None, 2, 1, 10, 1e-3, 1e-6, 1, 0, None, p, p, p, big, None]
@@ -89,11 +89,9 @@ def test_fit_entries_reject_bad_arguments_without_a_gpu():
     args = list(fa)
     args[17] = 64
     assert lib.isb_mixture_fit_predict(*args) == _lib.ISB_ERR_ARG and 'workspace' in err()
-    # kind 0 is the GMM entry: same workspace and parameter layout; kind 1 adds its priors
-    assert lib.isb_mixture_fit_workspace_bytes(0, 5000, 6, 3, 9) == lib.isb_gmm_workspace_bytes(5000, 6, 3, 9)
-    assert lib.isb_mixture_fit_workspace_bytes(1, 5000, 6, 3, 9) > lib.isb_gmm_workspace_bytes(5000, 6, 3, 9)
-    assert lib.isb_mixture_fit_params_len(0, 6, 3) == lib.isb_gmm_params_len(6, 3)
-    assert lib.isb_mixture_fit_params_len(1, 6, 3) == lib.isb_gmm_params_len(6, 3) + 6 + 36
+    # kind 1 adds its priors to the GMM workspace and parameter layout
+    assert lib.isb_mixture_fit_workspace_bytes(1, 5000, 6, 3, 9) > lib.isb_mixture_fit_workspace_bytes(0, 5000, 6, 3, 9)
+    assert lib.isb_mixture_fit_params_len(1, 6, 3) == lib.isb_mixture_fit_params_len(0, 6, 3) + 6 + 36
     # isb_pca_fit(feat, N, D, ld, n_dev, use_scaler, coef, n_components, params, n_comp_out, ws, ws_bytes, st)
     pa = [p, 100, 3, 3, None, 1, 0.95, 0, p, None, p, big, None]
     for i, bad in ((0, None), (8, None), (10, None), (1, 1), (2, 0), (3, 2), (6, 1.0), (6, 0.0), (7, 4), (11, 64)):

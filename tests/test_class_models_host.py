@@ -205,7 +205,7 @@ def test_new_cabi_entries_reject_bad_arguments_without_a_gpu():
     buf = (C.c_double * 64)()
     p = C.cast(buf, C.c_void_p)
     err = lambda: lib.isb_last_error().decode()  # noqa: E731
-    assert lib.isb_abi_version() == 7
+    assert lib.isb_abi_version() == 8
     assert lib.isb_class_transform(None, 4, 3, None, 3, None, None, None, None, None, 3, p, None, 0, None) == _lib.ISB_ERR_ARG
     assert 'null' in err()
     assert lib.isb_class_transform(p, 4, 2, None, 3, None, None, None, None, None, 3, p, None, 0, None) == _lib.ISB_ERR_ARG

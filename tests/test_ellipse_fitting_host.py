@@ -149,9 +149,13 @@ def test_ransac_and_criterion_validation():
     ef._check_criteria([1, 0], [1.5, np.nan], term, 2)
     with pytest.raises(IndexError):
         ef._check_criteria([1, 0], [np.nan, 0.], term, 2)
-    offs, even = ef._disk_offsets(1.5, False)
+
+
+def test_disk_offsets_of_an_even_footprint():
+    from pyimsegm_b200 import descriptors as ds
+    offs, even = ds._disk_offsets(1.5, False)
     assert even and sorted(map(tuple, offs.tolist())) == [(0, 0), (0, 1), (1, 0), (1, 1)]
-    offs, _ = ef._disk_offsets(1.5, True)
+    offs, _ = ds._disk_offsets(1.5, True)
     assert sorted(map(tuple, offs.tolist())) == [(-1, -1), (-1, 0), (0, -1), (0, 0)]
 
 
@@ -170,7 +174,7 @@ def test_ellipse_entries_reject_bad_arguments():
     p = C.cast(buf, C.c_void_p)
     assert lib.isb_binary_morph_footprint(p, 8, 8, p, 4, 2, C.cast((C.c_double * 16)(), C.c_void_p), None) == _lib.ISB_ERR_ARG
     assert 'op' in lib.isb_last_error().decode()
-    assert lib.isb_abi_version() == 7
+    assert lib.isb_abi_version() == 8
 
 
 def test_ransac_draws_the_reference_sample_sequence(monkeypatch):

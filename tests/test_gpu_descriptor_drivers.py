@@ -163,9 +163,10 @@ def test_supervised_data_step_labels_follow_the_annotation():
 
 
 def test_binary_opening_equals_scipy_grey_opening():
-    """isb_binary_opening_disk: erosion then dilation with a disc, reflected borders (what skimage.morphology.opening does on a
-    boolean image through scipy.ndimage.grey_erosion / grey_dilation)"""
+    """binary_opening_disk: erosion then dilation with a disc, reflected borders (what skimage.morphology.opening does on a
+    boolean image through scipy.ndimage.grey_erosion / grey_dilation); a non-integer radius against the oracle's opening"""
     from scipy import ndimage
+    from oracle import ellipse as oe
     from pyimsegm_b200 import descriptors as ds
     rng = np.random.RandomState(3)
     mask = ndimage.gaussian_filter(rng.random_sample((70, 95)), 2) > 0.5
@@ -174,6 +175,7 @@ def test_binary_opening_equals_scipy_grey_opening():
         disk = (yy ** 2 + xx ** 2) <= radius ** 2
         want = ndimage.grey_dilation(ndimage.grey_erosion(mask.astype(np.uint8), footprint=disk), footprint=disk).astype(bool)
         assert np.array_equal(ds.binary_opening_disk(mask, radius), want)
+    assert np.array_equal(ds.binary_opening_disk(mask, 1.5), oe.opening(mask.astype(np.uint8), oe.disk(1.5)).astype(bool))
 
 
 def test_segment_median_on_the_device(oracle):

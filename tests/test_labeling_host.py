@@ -239,7 +239,7 @@ def test_labeling_entry_points_reject_bad_arguments():
     from pyimsegm_b200 import _lib
     lib = _lib.lib()
     p = C.c_void_p(16)
-    assert lib.isb_abi_version() == 7
+    assert lib.isb_abi_version() == 8
     assert lib.isb_label_boundary_map(None, 4, 4, p, None) == _lib.ISB_ERR_ARG
     assert lib.isb_label_contour_map(p, 0, 4, 1, 0, p, None) == _lib.ISB_ERR_ARG
     assert lib.isb_edt_workspace_bytes(0, 4) == 0
