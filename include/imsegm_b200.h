@@ -389,8 +389,9 @@ int isb_lm_texture_finish(int nb, int n_batt, int flags, const double* acc, cons
 int isb_wgmma_selftest(const float* A, const float* B, int N, int K, int variant, float* D, isb_stream_t stream);
 
 /* per-segment, per-channel median -- numpy_img2d_color_median (imsegm/descriptors.py:420-455, channels = 3, n_px = H*W) and
- * numpy_img3d_gray_median (:651-676, channels = 1, n_px = D*H*W); np.median semantics (mean of the two middle values for an even
- * count), NaN for a label without pixels.
+ * numpy_img3d_gray_median (:651-676, channels = 1, n_px = D*H*W); np.median semantics in the image's own type: an odd count gives
+ * the middle value, an even count the mean of the two middle values taken in float32 for an ISB_F32 image (sum rounded to float32,
+ * then halved) and in float64 otherwise; NaN for a label with a NaN pixel and for a label without pixels.
  *   img : [n_px, channels] interleaved, dtype = isb_dtype;  seg : [n_px] labels in [0, nb);  out : [nb, channels] f64 */
 size_t isb_segment_median_workspace_bytes(long long n_px, int nb);
 int isb_segment_median(const void* img, int dtype, const int32_t* seg, long long n_px, int channels, int nb, double* out, void* ws,

@@ -220,8 +220,10 @@ def color2d_std(img, seg, means=None):
 
 
 def color2d_median(img, seg):
-    """imsegm/descriptors.py:420-455 numpy_img2d_color_median: per label and channel, np.median of the member pixels"""
-    img, seg = np.asarray(img, dtype=np.float64), np.asarray(seg)
+    """imsegm/descriptors.py:420-455 numpy_img2d_color_median: per label and channel, np.median of the member pixels in the image's
+    own dtype (a float32 image averages its two middle values in float32, as np.median of the reference's list of float32 values
+    does); NaN for a label without pixels and for a label with a NaN pixel"""
+    img, seg = np.asarray(img), np.asarray(seg)
     nb = int(seg.max()) + 1
     out = np.full((nb, 3), np.nan)
     for lb in range(nb):

@@ -83,26 +83,35 @@ struct SelShared {
     unsigned long long next;   // smallest key above the selected one
     int k;
     int le;                    // how many keys are <= the selected one
+    int nan;                   // how many keys are NaN
 };
 
-// np.median of the n keys key_at(0..n): 8-bit MSB-first radix select of the lower middle rank, one more pass for the upper middle
-// one.  Every thread of the CTA calls it and gets the result.
+// the keys of +inf and -inf: a NaN key lies above the first (sign bit clear) or below the second (sign bit set)
+constexpr unsigned long long KEY_PINF = 0xFFF0000000000000ull, KEY_NINF = 0x000FFFFFFFFFFFFFull;
+
+// np.median of the n keys key_at(0..n) in the float type of the image (float32 when ``f32``): 8-bit MSB-first radix select of the
+// lower middle rank, one more pass for the upper middle one; NaN when any key is NaN.  Every thread of the CTA calls it and gets
+// the result.
 template <class KeyAt>
-__device__ double med_select(const KeyAt& key_at, int n, SelShared& s)
+__device__ double med_select(const KeyAt& key_at, int n, bool f32, SelShared& s)
 {
     const int k_lo = (n - 1) / 2, k_hi = n / 2;
     __syncthreads();                       // the previous call's readers are done with s
-    if (threadIdx.x == 0) { s.prefix = 0ull; s.k = k_lo; }
+    if (threadIdx.x == 0) { s.prefix = 0ull; s.k = k_lo; s.nan = 0; }
     for (int pass = 0; pass < 8; ++pass) {
         const int shift = 56 - 8 * pass;
         for (int i = threadIdx.x; i < 256; i += MT) s.hist[i] = 0;
         __syncthreads();
         const unsigned long long prefix = s.prefix;
+        int n_nan = 0;
         for (int i = threadIdx.x; i < n; i += MT) {
             const unsigned long long key = key_at(i);
+            if (pass == 0) n_nan += key > KEY_PINF || key < KEY_NINF;
             if (pass == 0 || (key >> (shift + 8)) == (prefix >> (shift + 8))) atomicAdd(&s.hist[(int)((key >> shift) & 255ull)], 1);
         }
+        if (pass == 0 && n_nan) atomicAdd(&s.nan, n_nan);
         __syncthreads();
+        if (s.nan) return nan("");         // np.median propagates NaN; s.nan is final after the barrier, so every thread returns here
         if (threadIdx.x == 0) {
             int k = s.k, d = 0;
             for (; d < 255; ++d) { if (k < s.hist[d]) break; k -= s.hist[d]; }
@@ -112,7 +121,8 @@ __device__ double med_select(const KeyAt& key_at, int n, SelShared& s)
         __syncthreads();
     }
     const unsigned long long sel = s.prefix;    // key of the element of rank k_lo
-    double hi = f64_unordered(sel);
+    const double lo = f64_unordered(sel);
+    double hi = lo;
     if (k_hi != k_lo) {
         if (threadIdx.x == 0) { s.next = ~0ull; s.le = 0; }
         __syncthreads();
@@ -127,7 +137,10 @@ __device__ double med_select(const KeyAt& key_at, int n, SelShared& s)
         __syncthreads();
         if (s.le < k_hi + 1) hi = f64_unordered(s.next);   // the upper middle element is the next larger value
     }
-    return 0.5 * (f64_unordered(sel) + hi);
+    if (k_hi == k_lo) return lo;           // odd count: the middle value itself (no 0.5 * (v + v), which overflows near DBL_MAX)
+    // np.mean of the two middles: summed and halved in the image's float type (u8 / u16 middles add exactly in float64)
+    if (f32) return (double)__fmul_rn(__fadd_rn((float)lo, (float)hi), 0.5f);
+    return 0.5 * (lo + hi);
 }
 
 // one CTA per label serves every channel.  A label of at most ``cap`` pixels stages its C keys per pixel in shared memory once
@@ -143,6 +156,7 @@ __global__ void __launch_bounds__(MT) k_med_select(const void* __restrict__ img,
     double* row = out + (size_t)lb * ld + col0;
     if (n <= 0) { for (int c = threadIdx.x; c < C; c += MT) row[c] = nan(""); return; }
     const unsigned* ord = order + beg;
+    const bool f32 = dtype == ISB_F32;
     if (n <= cap) {
         for (int i = threadIdx.x; i < n; i += MT) {
             const size_t p = (size_t)ord[i] * C;
@@ -153,11 +167,11 @@ __global__ void __launch_bounds__(MT) k_med_select(const void* __restrict__ img,
         double m;
         if (n <= cap) {
             const unsigned long long* keys = s_keys + (size_t)c * cap;
-            m = med_select([&](int i) { return keys[i]; }, n, s);      // the first barrier inside also publishes the staged keys
+            m = med_select([&](int i) { return keys[i]; }, n, f32, s);      // the first barrier inside also publishes the staged keys
         } else {
-            m = med_select([&](int i) { return f64_ordered(med_load(img, dtype, (size_t)ord[i] * C + c, clean)); }, n, s);
+            m = med_select([&](int i) { return f64_ordered(med_load(img, dtype, (size_t)ord[i] * C + c, clean)); }, n, f32, s);
         }
-        if (clean) {   // the feature table's rules: an infinite mean of two middles -> the largest finite value, -0 -> +0
+        if (clean) {   // the feature table's rules: an infinite median (FLT_MAX + FLT_MAX in float32) -> the largest finite value, -0 -> +0
             if (isinf(m)) m = m > 0 ? DBL_MAX : -DBL_MAX;
             if (m == 0.) m = 0.;
         }
