@@ -1,15 +1,15 @@
 """
 Drop-in alias: ``import imsegm.pipelines`` (``superpixels``, ``descriptors``, ``graph_cuts``) resolves to the
 H100-native implementation in ``pyimsegm_b200`` for the SLIC -> features -> GraphCut hot path of Borda/pyImSegm and for the
-region growing (RG2SP) built on it, and for ``labeling``, ``ellipse_fitting`` and ``annotation``.  The reference's ``classification``
-(supervised training) is not provided.
+region growing (RG2SP) built on it, and for ``labeling``, ``ellipse_fitting``, ``annotation`` and ``classification``.  Of
+``classification`` only the scoring half is provided (segmentations against annotations); its supervised training is not.
 """
 import sys
 
 import pyimsegm_b200
-from pyimsegm_b200 import annotation, descriptors, ellipse_fitting, graph_cuts, labeling, pipelines, region_growing, superpixels, tiled, utilities
+from pyimsegm_b200 import annotation, classification, descriptors, ellipse_fitting, graph_cuts, labeling, pipelines, region_growing, superpixels, tiled, utilities
 
-for _name in ('annotation', 'descriptors', 'ellipse_fitting', 'graph_cuts', 'labeling', 'pipelines', 'region_growing', 'superpixels', 'tiled', 'utilities'):
+for _name in ('annotation', 'classification', 'descriptors', 'ellipse_fitting', 'graph_cuts', 'labeling', 'pipelines', 'region_growing', 'superpixels', 'tiled', 'utilities'):
     sys.modules[__name__ + '.' + _name] = getattr(pyimsegm_b200, _name)
 
 __version__ = '0.1.9+b200'

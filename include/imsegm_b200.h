@@ -29,7 +29,8 @@ enum isb_status {
     ISB_ERR_UNSUPPORTED = -4
 };
 
-enum isb_dtype { ISB_U8 = 0, ISB_U16 = 1, ISB_F32 = 2, ISB_F64 = 3 };
+/* ISB_I8 .. ISB_BOOL are taken by the label maps of isb_contingency_count / _write only */
+enum isb_dtype { ISB_U8 = 0, ISB_U16 = 1, ISB_F32 = 2, ISB_F64 = 3, ISB_I8 = 4, ISB_I16 = 5, ISB_I32 = 6, ISB_U32 = 7, ISB_I64 = 8, ISB_BOOL = 9 };
 
 const char* isb_last_error(void);
 int isb_abi_version(void);
@@ -498,6 +499,26 @@ int isb_palette_gather(const int64_t* labels, long long n_px, const int64_t* key
 /* out[i] = src[index[i]] for n elements of elem_bytes (1, 2, 4 or 8) bytes: the values at the sites of isb_edt_2d_indices
  * (image_inpaint_pixels :279-286).  Indices are not checked. */
 int isb_gather_at_index(const void* src, int elem_bytes, const int32_t* index, long long n, void* out, isb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * (xiii) classification -- the scoring half of imsegm/classification.py: every metric derives from one contingency table.
+ * ------------------------------------------------------------------------------------------------------------------ */
+
+/* contingency table of two label maps y_true, y_pred [n] of dtypes ISB_BOOL, ISB_U8, ISB_I8, ISB_U16, ISB_I16, ISB_I32, ISB_U32 or
+ * ISB_I64 (the two may differ): the pixels of every (true value, pred value) pair, leaving out every pixel whose value in either map
+ * is one of drop [n_drop] i64 (ascending; optional when n_drop = 0) -- compute_classif_stat_segm_annot :404-410.
+ * The count (synchronises the stream twice, to read 4 and 2 values back) writes to the HOST info [6]:
+ *   K_true, K_pred (distinct kept values of each map; 0, 0 when every pixel is dropped), min_true, range_true, min_pred, range_pred.
+ * The kept values of a map of 32 or 64 bits must span fewer than 2^26 values, else ISB_ERR_UNSUPPORTED.
+ * The write (same arguments, info and ws, after the count) writes values_true [K_true] and values_pred [K_pred] i64 ascending and
+ * counts [K_true * K_pred] i64, row-major over (true, pred); K_true * K_pred <= 2^28, else ISB_ERR_UNSUPPORTED.
+ * ws: isb_contingency_workspace_bytes(dtype_true, dtype_pred) (0 for an unsupported dtype). */
+size_t isb_contingency_workspace_bytes(int dtype_true, int dtype_pred);
+int isb_contingency_count(const void* y_true, int dtype_true, const void* y_pred, int dtype_pred, long long n, const int64_t* drop, int n_drop,
+                          void* ws, size_t ws_bytes, long long* info, isb_stream_t stream);
+int isb_contingency_write(const void* y_true, int dtype_true, const void* y_pred, int dtype_pred, long long n, const int64_t* drop, int n_drop,
+                          const long long* info, void* ws, size_t ws_bytes, int64_t* values_true, int64_t* values_pred, int64_t* counts,
+                          isb_stream_t stream);
 
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);

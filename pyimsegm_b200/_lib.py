@@ -128,6 +128,9 @@ SIGNATURES = {
     'isb_palette_map': (_i, [_vp, _i, _ll, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'isb_palette_gather': (_i, [_vp, _ll, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     'isb_gather_at_index': (_i, [_vp, _i, _vp, _ll, _vp, _vp]),
+    'isb_contingency_workspace_bytes': (_sz, [_i, _i]),
+    'isb_contingency_count': (_i, [_vp, _i, _vp, _i, _ll, _vp, _i, _vp, _sz, C.POINTER(_ll), _vp]),
+    'isb_contingency_write': (_i, [_vp, _i, _vp, _i, _ll, _vp, _i, C.POINTER(_ll), _vp, _sz, _vp, _vp, _vp, _vp]),
 }
 
 

@@ -1,0 +1,543 @@
+"""
+The scoring half of the reference's ``imsegm/classification.py``: the metrics between annotations and segmentations.
+
+Every number comes from one contingency table -- the pixels of every (annotation value, segmentation value) pair after the
+``drop_labels`` mask -- counted on the device (``csrc/classification.cu``, one upload of the two maps and three passes over them).
+Everything else runs on the host over the table's nonzero cells, never over the pixels again: the confusion matrix, the accuracy,
+the adjusted Rand score (scikit-learn's pair-confusion formula in integers), precision / recall / F1 / support (scikit-learn's own
+``precision_recall_fscore_support`` on the cells weighted by their counts, which gives the same float64 divisions, warnings and
+exceptions as on the pixel arrays), the ``relabel=True`` table of ``labeling.relabel_max_overlap_unique`` and the binary ratios.
+There is no CPU fallback.
+
+Label maps are integer or bool arrays of any shape; float arrays holding integers are cast on the host, other floats raise the
+``ValueError`` scikit-learn raises for continuous targets.  The values of a map of 32 or 64 bits must span fewer than 2^26 values
+(``NotImplementedError`` above), and a table of more than 2^28 cells raises ``MemoryError``.
+
+Behaviour of the reference that is kept:
+
+- With two or fewer distinct labels, ``compute_classif_metrics`` renumbers them as the reference's ``relabel_sequential`` does,
+  including its wrap of a negative label into the end of its look-up table, so -1 and 0 become one class:
+  ``compute_classif_metrics([-1, 0, 0, -1, 0], [0, 0, -1, -1, 0])`` has accuracy 1.0 and confusion ``[[5]]``.  In that case float
+  maps raise ``TypeError`` (the reference sizes its table with a float), and so does ``relabel=True`` on float maps.
+- An average that scikit-learn rejects (``'binary'`` on more than two labels, ``'samples'``) gives -1 for its four entries.
+
+Differences from the reference:
+
+- Bool maps count as 0 / 1 integers; the reference's ``relabel_sequential`` indexes with them as masks and raises ``IndexError``.
+- ``relabel=True`` keeps negative labels as ``labeling.relabel_max_overlap_unique`` of this package does.
+- ``compute_stat_per_image`` runs the pairs one after the other on the device (the upload of a pair overlaps the counting of the
+  previous one) and ignores ``nb_workers``; it shows no progress bar.
+
+Not provided: the training half of the module (the classifier zoo and its pipelines, parameter searches, cross-validation,
+feature selection, saving and loading classifiers, dataset balancing and down-sampling).  Those wrap scikit-learn estimators
+and have no pixel work to move to the device.  This is the one module of the package in which not every public name of the
+reference exists.
+"""
+import ctypes as C
+import logging
+
+import numpy as np
+from sklearn import metrics
+
+from . import _lib
+from .engine import get_engine
+from .utilities import ImageDimensionError
+
+#: name template for exporting trained classifier (adding classifier name and version)
+TEMPLATE_NAME_CLF = 'classifier_{}.pkl'
+#: default (recommended) classifier for supervised segmentation
+DEFAULT_CLASSIF_NAME = 'RandForest'
+#: default (recommended) clustering for unsupervised segmentation
+DEFAULT_CLUSTERING = 'kMeans'
+#: default types of computed metrics
+METRIC_AVERAGES = ('macro', 'weighted')
+#: default computed metrics
+METRIC_SCORING = ('f1_macro', 'accuracy', 'precision_macro', 'recall_macro')
+#: mapping of metrics names to used functions
+DICT_SCORING = {
+    'f1': metrics.f1_score,
+    'accuracy': metrics.accuracy_score,
+    'precision': metrics.precision_score,
+    'recall': metrics.recall_score,
+}
+
+#: largest contingency table (cells)
+TABLE_MAX_CELLS = 1 << 28
+# enum isb_dtype of include/imsegm_b200.h for the label maps
+_LABEL_DTYPES = {'bool': 9, 'uint8': 0, 'int8': 4, 'uint16': 1, 'int16': 5, 'int32': 6, 'uint32': 7, 'int64': 8}
+_I64 = np.iinfo(np.int64)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# contingency table (device)
+# ---------------------------------------------------------------------------------------------------------------------
+
+def _labels(arr):
+    """(flat contiguous label array of a device dtype, whether it was float) of a map"""
+    arr = np.asarray(arr)
+    kind = arr.dtype.kind
+    if kind == 'f':
+        if arr.size and not (np.all(np.isfinite(arr)) and np.all(np.floor(arr) == arr)):
+            raise ValueError("Classification metrics can't handle continuous targets")
+        if arr.size and (arr.min() < _I64.min or arr.max() >= 2.0 ** 63):
+            raise ValueError('labels must fit in int64')
+        return arr.astype(np.int64).ravel(), True
+    if kind not in 'biu':
+        raise TypeError('label maps must hold integers, got %s' % arr.dtype)
+    if arr.dtype.name not in _LABEL_DTYPES:
+        if arr.size and arr.max() > _I64.max:
+            raise ValueError('labels must fit in int64')
+        arr = arr.astype(np.int64)
+    return np.ascontiguousarray(arr).ravel(), False
+
+
+def _drop_list(drop_labels):
+    """ascending int64 values of ``drop_labels`` that an integer map can hold"""
+    ints = set()
+    for v in ([] if drop_labels is None else np.asarray(list(drop_labels), dtype=object).ravel().tolist()):
+        try:
+            iv = int(v)
+        except (TypeError, ValueError, OverflowError):
+            continue
+        if iv == v and _I64.min <= iv <= _I64.max:
+            ints.add(iv)
+    return np.array(sorted(ints), dtype=np.int64)
+
+
+class _Pending(object):
+    """one contingency table in flight on an engine's current stream: the count has run, the write and download are enqueued"""
+
+    def __init__(self, eng, y_true, y_pred, drop):
+        torch, lib, st = eng.torch, eng.lib, _lib.stream_ptr()
+        self.dtypes = (_LABEL_DTYPES[y_true.dtype.name], _LABEL_DTYPES[y_pred.dtype.name])
+        n = y_true.size
+        d_true = eng.to_device(y_true.view(np.uint8) if y_true.dtype == bool else y_true, 'clf_true')
+        d_pred = eng.to_device(y_pred.view(np.uint8) if y_pred.dtype == bool else y_pred, 'clf_pred')
+        d_drop = eng.to_device(drop, 'clf_drop') if len(drop) else None
+        ws_bytes = lib.isb_contingency_workspace_bytes(*self.dtypes)
+        ws = eng.buf('clf_ws', ws_bytes, torch.uint8)
+        info = (C.c_longlong * 6)()
+        args = (_lib.ptr(d_true), self.dtypes[0], _lib.ptr(d_pred), self.dtypes[1], C.c_longlong(n), _lib.ptr(d_drop), len(drop))
+        _lib.check(lib.isb_contingency_count(*args, _lib.ptr(ws), C.c_size_t(ws_bytes), info, st))
+        self.k = (int(info[0]), int(info[1]))
+        if self.k[0] * self.k[1] > TABLE_MAX_CELLS:
+            raise MemoryError('a contingency table of %d x %d cells is above the limit of %d' % (self.k + (TABLE_MAX_CELLS, )))
+        self.done = None
+        if self.k[0] and self.k[1]:
+            v_true = eng.buf('clf_values_true', self.k[0], torch.int64)
+            v_pred = eng.buf('clf_values_pred', self.k[1], torch.int64)
+            counts = eng.buf('clf_counts', self.k, torch.int64)
+            _lib.check(lib.isb_contingency_write(*args, info, _lib.ptr(ws), C.c_size_t(ws_bytes), _lib.ptr(v_true), _lib.ptr(v_pred),
+                                                 _lib.ptr(counts), st))
+            self.hosts, self.done = eng.download([v_true[:self.k[0]], v_pred[:self.k[1]], counts[:self.k[0], :self.k[1]]])
+
+    def result(self):
+        """(true values [K_true], pred values [K_pred], counts [K_true, K_pred]) int64"""
+        if self.done is None:
+            return np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros((0, 0), np.int64)
+        self.done.synchronize()
+        return tuple(h.numpy().copy() for h in self.hosts)
+
+
+def _contingency(y_true, y_pred, drop=()):
+    """(true values, pred values, counts [K_true, K_pred]) of two flat label arrays of device dtypes, pixels with a value in the
+    ascending int64 ``drop`` in either map left out"""
+    drop = np.ascontiguousarray(drop, dtype=np.int64)
+    if y_true.size == 0:
+        return np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros((0, 0), np.int64)
+    return _Pending(get_engine(), y_true, y_pred, drop).result()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# metrics from the table (host)
+# ---------------------------------------------------------------------------------------------------------------------
+
+class _Table(object):
+    """the nonzero cells of a contingency table: true value a, pred value b, pixel count w (int64 arrays)"""
+
+    def __init__(self, a, b, w, is_float=False):
+        self.a, self.b, self.w, self.is_float = a, b, w, is_float
+
+    @classmethod
+    def from_dense(cls, v_true, v_pred, counts, is_float=False):
+        r, c = np.nonzero(counts)
+        return cls(v_true[r], v_pred[c], counts[r, c], is_float)
+
+    def merged(self, a, b):
+        """the cells with their values replaced by a, b and equal pairs summed"""
+        if len(a) == 0:
+            return _Table(a, b, self.w, self.is_float)
+        pairs, inv = np.unique(np.stack([a, b], 1), axis=0, return_inverse=True)
+        w = np.bincount(inv.ravel(), weights=self.w, minlength=len(pairs)).astype(np.int64)
+        return _Table(pairs[:, 0], pairs[:, 1], w, self.is_float)
+
+    def labels(self):
+        return np.union1d(self.a, self.b)
+
+
+def _sequential(table):
+    """the cells renumbered as the reference's relabel_sequential over the union of labels (at most two): a table of max + 1 entries
+    filled in order, negative labels wrapping as numpy indices do"""
+    uq = table.labels()
+    if len(uq) == 0:
+        raise ValueError('zero-size array to reduction operation maximum which has no identity')
+    if table.is_float:
+        raise TypeError("'numpy.float64' object cannot be interpreted as an integer")
+    size = int(uq.max()) + 1
+
+    def slot(v):
+        if not -size <= v < size:
+            raise IndexError('index %d is out of bounds for axis 0 with size %d' % (v, size))
+        return v % size
+
+    lut = {}
+    for i, lb in enumerate(uq.tolist()):
+        lut[slot(lb)] = i
+    remap = {lb: lut[slot(lb)] for lb in uq.tolist()}
+    get = np.vectorize(remap.__getitem__, otypes=[np.int64])
+    return table.merged(get(table.a), get(table.b))
+
+
+def _adjusted_rand(table):
+    """scikit-learn's adjusted_rand_score from the pair confusion of the table, in integers"""
+    w = table.w
+    n = int(w.sum())
+    _, ia = np.unique(table.a, return_inverse=True)
+    _, ib = np.unique(table.b, return_inverse=True)
+    n_c = np.bincount(ia.ravel(), weights=w).astype(np.int64)
+    n_k = np.bincount(ib.ravel(), weights=w).astype(np.int64)
+    sum_squares = int((w * w).sum())
+    tp = sum_squares - n
+    fp = int((w * n_k[ib.ravel()]).sum()) - sum_squares
+    fn = int((w * n_c[ia.ravel()]).sum()) - sum_squares
+    tn = n * n - fp - fn - sum_squares
+    if fn == 0 and fp == 0:
+        return 1.0
+    return 2.0 * (tp * tn - fn * fp) / ((tp + fn) * (fn + tn) + (tp + fp) * (fp + tn))
+
+
+def _confusion(table):
+    """confusion matrix over the sorted union of labels, as lists of Python ints"""
+    uq = table.labels()
+    conf = np.zeros((len(uq), len(uq)), dtype=np.int64)
+    np.add.at(conf, (np.searchsorted(uq, table.a), np.searchsorted(uq, table.b)), table.w)
+    return conf.tolist()
+
+
+def _classif_metrics(table, metric_averages, ndim=1):
+    """compute_classif_metrics of the pixels the table counts, taken from arrays of ``ndim`` dimensions"""
+    if len(table.labels()) <= 2:
+        table = _sequential(table)
+    if ndim != 1:                                   # scikit-learn's clustering scores take label vectors
+        raise ValueError('labels_true must be 1D: %d dimensions given' % ndim)
+    y_true, y_pred, weight = table.a, table.b, table.w
+    eval_str = 'EVALUATION: {:<2} PRE: {:.3f} REC: {:.3f} F1: {:.3f} S: {:>6}'
+    try:
+        p, r, f, s = metrics.precision_recall_fscore_support(y_true, y_pred, sample_weight=weight)
+        for lb, _ in enumerate(p):
+            logging.debug(eval_str.format(lb, p[lb], r[lb], f[lb], s[lb]))
+    except Exception:
+        logging.exception('metrics.precision_recall_fscore_support')
+    n = int(weight.sum())
+    dict_metrics = {
+        'ARS': _adjusted_rand(table),
+        'accuracy': float(np.float64(int(weight[y_true == y_pred].sum())) / np.float64(n)),
+        'confusion': _confusion(table),
+    }
+    names = ['precision', 'recall', 'f1', 'support']
+    for avg in metric_averages:
+        try:
+            mtr = metrics.precision_recall_fscore_support(y_true, y_pred, average=avg, sample_weight=weight)
+            res = dict(zip(['{}_{}'.format(nm, avg) for nm in names], mtr))
+        except Exception:
+            logging.exception('metrics.precision_recall_fscore_support')
+            res = dict(zip(['{}_{}'.format(nm, avg) for nm in names], [-1] * 4))
+        dict_metrics.update(res)
+    return dict_metrics
+
+
+def _tp_tn_fp_fn(table, label_positive=None):
+    """compute_tp_tn_fp_fn of the pixels the table counts"""
+    uq_labels = table.labels().tolist()
+    if len(uq_labels) > 2:
+        logging.debug('too many labels: %r', uq_labels)
+        return np.nan, np.nan, np.nan, np.nan
+    if len(uq_labels) < 2:
+        logging.debug('only one label: %r', uq_labels)
+        return int(table.w.sum()), 0, 0, 0
+    if label_positive is None or label_positive not in uq_labels:
+        label_positive = uq_labels[-1]
+    uq_labels.remove(label_positive)
+    neg = uq_labels[0]
+
+    def count(a, b):
+        return np.int64(table.w[(table.a == a) & (table.b == b)].sum())
+    # the reference's orientation: FP is annotated positive and segmented negative
+    return count(label_positive, label_positive), count(neg, neg), count(label_positive, neg), count(neg, label_positive)
+
+
+def _ratio_fpfn_tpfn(tp, fp, fn):
+    if (fp + fn) == 0:
+        return 0.
+    return float(fp + fn) / float(tp + fn)
+
+
+def _ratio_tpfp_tpfn(tp, fp, fn):
+    if (tp + fn) == 0:
+        return 0.
+    return float(tp + fp) / float(tp + fn)
+
+
+def _unique_lut(rows, cols, counts, n_lut, keep_bg, query):
+    """the look-up table of labeling.max_overlap_unique_lut at the columns ``query`` from the positive cells (rows, cols, counts) of
+    the overlap matrix, without building the matrix:
+    - greedy: cells by count descending, ties by row then column (row-major order), skipping a used row or column;
+    - first fill: an unmatched column i takes i when no matched row is i;
+    - second fill: the unmatched columns that are also matched rows, ascending, take the matched columns that are not matched rows,
+      descending (the largest free value first); once those run out the rest stay -1."""
+    rows, cols, counts = (np.asarray(x, dtype=np.int64) for x in (rows, cols, counts))
+    match = {}
+    if keep_bg:
+        if n_lut == 0:
+            raise IndexError('list assignment index out of range')
+        match[0] = 0
+        keep = (rows != 0) & (cols != 0)
+        rows, cols, counts = rows[keep], cols[keep], counts[keep]
+    keep = counts > 0
+    rows, cols, counts = rows[keep], cols[keep], counts[keep]
+    order = np.lexsort((cols, rows, -counts))
+    used_r = set(match.values())
+    n_r, n_c = len(np.unique(rows)), len(np.unique(cols))
+    for r, c in zip(rows[order].tolist(), cols[order].tolist()):
+        if r in used_r or c in match:
+            continue
+        used_r.add(r)
+        match[c] = r
+        if len(used_r) >= n_r + keep_bg or len(match) >= n_c + keep_bg:
+            break
+    matched_rows = set(match.values())
+    pending = sorted(r for r in matched_rows if 0 <= r < n_lut and r not in match)
+    free = sorted((c for c in match if c not in matched_rows), reverse=True)
+    second = dict(zip(pending, free))
+    out = []
+    for q in np.asarray(query, dtype=np.int64).tolist():
+        if q in match:
+            out.append(match[q])
+        elif q not in matched_rows:
+            out.append(q)
+        else:
+            out.append(second.get(q, -1))
+    return np.array(out, dtype=np.int64)
+
+
+def _relabel_unique(table):
+    """the table after ``y_pred = relabel_max_overlap_unique(y_true, y_pred, keep_bg=False)`` (labeling.py of this package):
+    negative labels kept"""
+    if table.is_float:
+        raise TypeError('label maps must be integer arrays, got float64')
+    a, b, w = table.a, table.b, table.w
+    if len(a) == 0:
+        raise ValueError('zero-size array to reduction operation maximum which has no identity')
+    n_rows, n_lut = int(a.max()) + 1, int(b.max()) + 1
+    if n_rows < 0 or n_lut < 0:                     # numpy's ValueError of the overlap matrix's np.zeros
+        raise ValueError('negative dimensions are not allowed')
+    lo = int(b.min())
+    if lo < -n_lut:                                 # numpy's IndexError of lut[seg] in labeling.relabel_max_overlap_unique
+        raise IndexError('index %d is out of bounds for axis 0 with size %d' % (lo, n_lut))
+    pos = (a >= 0) & (b >= 0)
+    uq_b = np.unique(b[b >= 0])
+    lut = _unique_lut(a[pos], b[pos], w[pos], n_lut, False, uq_b)
+    new_b = b.copy()
+    sel = b >= 0
+    new_b[sel] = lut[np.searchsorted(uq_b, b[sel])]
+    return table.merged(a, new_b)
+
+
+def _stat_segm_annot(table, name, relabel):
+    """compute_classif_stat_segm_annot of the pixels the table counts (after the drop mask)"""
+    if relabel:
+        table = _relabel_unique(table)
+    dict_stat = _classif_metrics(table, ['macro'])
+    if len(np.unique(table.b)) == 2:
+        tp, _, fp, fn = _tp_tn_fp_fn(table)
+        dict_stat['(FP+FN)/(TP+FN)'] = _ratio_fpfn_tpfn(tp, fp, fn)
+        dict_stat['(TP+FP)/(TP+FN)'] = _ratio_tpfp_tpfn(tp, fp, fn)
+    dict_stat['name'] = name
+    return dict_stat
+
+
+def _table_of(y_true, y_pred, drop=()):
+    (t, ft), (p, fp) = _labels(y_true), _labels(y_pred)
+    return _Table.from_dense(*_contingency(t, p, drop), is_float=ft or fp)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# public functions
+# ---------------------------------------------------------------------------------------------------------------------
+
+def compute_classif_metrics(y_true, y_pred, metric_averages=METRIC_AVERAGES):
+    """ standard metrics of a multi-class classification (reference classification.py:305-371): ARS, accuracy, confusion matrix
+    and precision / recall / F1 / support for every average of ``metric_averages`` (-1 each when scikit-learn rejects the average)
+
+    >>> np.random.seed(0)
+    >>> y_true = np.random.randint(0, 3, 25) * 2
+    >>> y_pred = np.random.randint(0, 2, 25) * 2
+    >>> d = compute_classif_metrics(y_true, y_true)
+    >>> d['accuracy']
+    1.0
+    >>> d['confusion']
+    [[10, 0, 0], [0, 10, 0], [0, 0, 5]]
+    >>> d = compute_classif_metrics(y_true, y_pred)
+    >>> d['accuracy']  # doctest: +ELLIPSIS
+    0.32...
+    >>> d['confusion']
+    [[3, 7, 0], [5, 5, 0], [1, 4, 0]]
+    """
+    y_true, y_pred = np.array(y_true), np.array(y_pred)
+    if y_true.shape != y_pred.shape:
+        raise ValueError('prediction (%i) and annotation (%i) should be equal' % (len(y_true), len(y_pred)))
+    return _classif_metrics(_table_of(y_true, y_pred), metric_averages, y_true.ndim)
+
+
+def compute_classif_stat_segm_annot(annot_segm_name, drop_labels=None, relabel=False):
+    """ classification statistic between an annotation and a segmentation (reference classification.py:374-421): the pixels with a
+    value of ``drop_labels`` in either map are left out, ``relabel`` matches the segmentation's classes to the annotation's first
+    (``labeling.relabel_max_overlap_unique``), and a segmentation of two classes adds the two binary ratios
+
+    >>> np.random.seed(0)
+    >>> annot = np.random.randint(0, 2, (5, 10))
+    >>> segm = np.random.randint(0, 2, (5, 10))
+    >>> d = compute_classif_stat_segm_annot((annot, segm, 'ttt'), relabel=True, drop_labels=[5])
+    >>> d['(FP+FN)/(TP+FN)']  # doctest: +ELLIPSIS
+    0.846...
+    >>> d = compute_classif_stat_segm_annot((annot, segm + 1, 'ttt'), relabel=False, drop_labels=[0])
+    >>> d['confusion']
+    [[13, 17], [0, 0]]
+    """
+    annot, segm, name = annot_segm_name
+    annot, segm = np.asarray(annot), np.asarray(segm)
+    if segm.shape != annot.shape:
+        raise ImageDimensionError('dimension do not match for segm: %r - annot: %r' % (segm.shape, annot.shape))
+    return _stat_segm_annot(_table_of(annot, segm, _drop_list(drop_labels)), name, relabel)
+
+
+def compute_stat_per_image(segms, annots, names=None, nb_workers=2, drop_labels=None, relabel=False):
+    """ ``compute_classif_stat_segm_annot`` of every (annotation, segmentation) pair as a DataFrame indexed by ``name`` (reference
+    classification.py:424-471).  The pairs alternate over two CUDA streams: the upload and counting passes of pair i + 1 overlap
+    the final counting pass of pair i.  ``nb_workers`` is accepted and ignored.
+
+    >>> np.random.seed(0)
+    >>> img_true = np.random.randint(0, 3, (50, 100))
+    >>> img_pred = np.random.randint(0, 2, (50, 100))
+    >>> df = compute_stat_per_image([img_true], [img_pred], drop_labels=[-1])
+    >>> df.round(4).iloc[0]['accuracy']
+    0.3384
+    """
+    import pandas as pd
+    from .pipelines import _batch_engines
+    if len(segms) != len(annots):
+        raise RuntimeError('size of segment. (%i) amd annot. (%i) should be equal' % (len(segms), len(annots)))
+    if not names:
+        names = map(str, range(len(segms)))
+    drop = _drop_list(drop_labels)
+    engines = _batch_engines(2)
+    torch = engines[0][0].torch
+    caller = torch.cuda.current_stream()
+    list_stat, prev = [], None
+
+    def finish(job):
+        kind, payload, name = job
+        if kind == 'error':
+            raise payload
+        table = payload[0] if kind == 'host' else _Table.from_dense(*payload[0].result(), is_float=payload[1])
+        list_stat.append(_stat_segm_annot(table, name, relabel))
+
+    for i, (annot, segm, name) in enumerate(zip(annots, segms, names)):
+        annot, segm = np.asarray(annot), np.asarray(segm)
+        if segm.shape != annot.shape:
+            job = ('error', ImageDimensionError('dimension do not match for segm: %r - annot: %r' % (segm.shape, annot.shape)), name)
+        else:
+            (t, ft), (p, fp) = _labels(annot), _labels(segm)
+            if t.size == 0:
+                job = ('host', (_Table(t.astype(np.int64), p.astype(np.int64), np.zeros(0, np.int64), ft or fp), ), name)
+            else:
+                eng, stream = engines[i % 2]
+                stream.wait_stream(caller)
+                with torch.cuda.stream(stream):
+                    job = ('device', (_Pending(eng, t, p, drop), ft or fp), name)
+        if prev is not None:
+            finish(prev)
+        prev = job
+    if prev is not None:
+        finish(prev)
+    for _, stream in engines:
+        caller.wait_stream(stream)
+    df_stat = pd.DataFrame(list_stat)
+    df_stat.set_index('name', inplace=True)
+    return df_stat
+
+
+def relabel_sequential(labels, uq_labels=None):
+    """ labels renumbered 0, 1, ... in the order of ``uq_labels`` (default: the sorted unique labels), as a list (reference
+    classification.py:635-653); the table has max(uq_labels) + 1 entries, so a negative label wraps as a numpy index
+
+    >>> relabel_sequential([0, 0, 0, 5, 5, 5, 0, 5])
+    [0, 0, 0, 1, 1, 1, 0, 1]
+    """
+    labels = np.asarray(labels)
+    uq = np.unique(labels) if uq_labels is None else np.asarray(uq_labels)
+    lut = np.zeros(np.max(uq) + 1)
+    lut[uq] = np.arange(len(uq))
+    return lut[labels].astype(labels.dtype).tolist()
+
+
+def compute_tp_tn_fp_fn(annot, segm, label_positive=None):
+    """ (TP, TN, FP, FN) of two binary maps (reference classification.py:1265-1310): NaN each for more than two labels, (pixels, 0, 0,
+    0) for one; FP counts annotated-positive pixels segmented negative, as in the reference
+
+    >>> np.random.seed(0)
+    >>> annot = np.random.randint(0, 2, (5, 7)) * 9
+    >>> segm = np.random.randint(0, 2, (5, 7)) * 9
+    >>> compute_tp_tn_fp_fn(annot, annot)
+    (20, 15, 0, 0)
+    >>> compute_tp_tn_fp_fn(annot, segm)
+    (9, 5, 11, 10)
+    >>> compute_tp_tn_fp_fn(annot, np.ones((5, 7)))
+    (nan, nan, nan, nan)
+    """
+    annot, segm = np.asarray(annot), np.asarray(segm)
+    if annot.size != segm.size:
+        raise ValueError('annotation (%i) and segmentation (%i) should have the same size' % (annot.size, segm.size))
+    if annot.size == 0:
+        return 0, 0, 0, 0
+    return _tp_tn_fp_fn(_table_of(annot, segm), label_positive)
+
+
+def compute_metric_fpfn_tpfn(annot, segm, label_positive=None):
+    """ (FP + FN) / (TP + FN) (reference classification.py:1313-1337)
+
+    >>> np.random.seed(0)
+    >>> annot = np.random.randint(0, 2, (50, 75)) * 3
+    >>> segm = np.random.randint(0, 2, (50, 75)) * 3
+    >>> compute_metric_fpfn_tpfn(annot, segm)  # doctest: +ELLIPSIS
+    1.02...
+    >>> compute_metric_fpfn_tpfn(annot, annot)
+    0.0
+    """
+    tp, _, fp, fn = compute_tp_tn_fp_fn(annot, segm, label_positive)
+    return _ratio_fpfn_tpfn(tp, fp, fn)
+
+
+def compute_metric_tpfp_tpfn(annot, segm, label_positive=None):
+    """ (TP + FP) / (TP + FN) (reference classification.py:1340-1366)
+
+    >>> np.random.seed(0)
+    >>> annot = np.random.randint(0, 2, (50, 75)) * 3
+    >>> segm = np.random.randint(0, 2, (50, 75)) * 3
+    >>> compute_metric_tpfp_tpfn(annot, segm)  # doctest: +ELLIPSIS
+    1.03...
+    >>> compute_metric_tpfp_tpfn(annot, annot)
+    1.0
+    """
+    tp, _, fp, fn = compute_tp_tn_fp_fn(annot, segm, label_positive)
+    return _ratio_tpfp_tpfn(tp, fp, fn)

@@ -9,6 +9,7 @@
 #include <type_traits>
 
 #include "compact.cuh"
+#include "run_flush.cuh"
 
 namespace {
 
@@ -25,33 +26,23 @@ __device__ __forceinline__ unsigned pixel_key(const uint8_t* __restrict__ img, l
     return ((unsigned)p[0] << 16) | ((unsigned)p[1] << 8) | p[2];   // the alpha of RGBA does not count
 }
 
-// Every lane keeps a run (colour, count) over its pixels, which lie 32 apart; a run is flushed when the colour changes and at the
-// end.  A flush first sums the runs of all flushing lanes with the same colour (__match_any_sync), so one global atomic serves a
-// whole warp: a single-colour image issues one atomic per 32 * HIST_PER pixels.
-__device__ __forceinline__ void flush_run(bool flush, unsigned key, unsigned cnt, unsigned long long* __restrict__ hist)
-{
-    const unsigned fl = __ballot_sync(FULL, flush);
-    if (flush) {
-        const unsigned peers = __match_any_sync(fl, key);
-        const unsigned s = __reduce_add_sync(peers, cnt);
-        if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(hist + key, (unsigned long long)s);
-    }
-}
-
+// every lane keeps a run of one colour over its pixels, which lie 32 apart (flush_run): a single-colour image issues one atomic per
+// 32 * HIST_PER pixels
 __global__ void __launch_bounds__(256) k_color_hist(const uint8_t* __restrict__ img, long long n, int C, unsigned long long* __restrict__ hist)
 {
     const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long long base = warp * 32LL * HIST_PER + (threadIdx.x & 31);
     if (warp * 32LL * HIST_PER >= n) return;                         // uniform over the warp
+    const auto add = [hist](unsigned key, unsigned s) { atomicAdd(hist + key, (unsigned long long)s); };
     unsigned cur = NO_KEY, cnt = 0;
     for (int k = 0; k < HIST_PER; ++k) {
         const long long i = base + 32LL * k;
         const unsigned key = i < n ? pixel_key(img, i, C) : NO_KEY;
-        flush_run(key != cur && cnt != 0, cur, cnt, hist);
+        flush_run(key != cur && cnt != 0, cur, cnt, add);
         if (key != cur) { cur = key; cnt = 0; }
         if (key != NO_KEY) ++cnt;
     }
-    flush_run(cnt != 0, cur, cnt, hist);
+    flush_run(cnt != 0, cur, cnt, add);
 }
 
 __global__ void __launch_bounds__(CPT_THREADS) k_hist_write(const unsigned long long* __restrict__ hist, long long n,
