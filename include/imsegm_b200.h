@@ -229,6 +229,18 @@ int isb_lm_background(const void* img, int dtype, int H, int W, const double* w_
 size_t isb_lm_battery_workspace_bytes(void);
 int isb_lm_battery_response(const double* planar, int H, int W, const double* kernels, int n_kernels, int kh, int kw, double max_signal,
                             double* resp, double* out, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* The same battery step split in two for row bands of one image (pyimsegm_b200/tiled.py), whose norm is summed over the bands in
+ * between.  planar [3, H, W] is a slab of the background-subtracted image.
+ * partial: resp [3, H, W] = isb_filter_response_2d(planar, kernels), and *sumsq (DEVICE, one f64) = the sum of the squared responses
+ *   clipped at max_signal over the slab rows [row_lo, row_hi) only -- the rows the band owns -- in the fixed block-partial order of
+ *   isb_lm_battery_response (a slab that owns all its rows gets that call's sum bit for bit).  Workspace:
+ *   isb_lm_battery_workspace_bytes().
+ * scale: out [row_hi - row_lo, W, 3] f64 = (r * (log(1 + |r|) / 0.03)) / |r| of the clipped responses resp [3, H, W] of the slab rows
+ *   [row_lo, row_hi), with |r| = sqrt(*sumsq) (DEVICE), or zeros when |r| is 0 or infinite */
+int isb_lm_battery_partial(const double* planar, int H, int W, const double* kernels, int n_kernels, int kh, int kw, double max_signal,
+                           int row_lo, int row_hi, double* resp, double* sumsq, void* ws, size_t ws_bytes, isb_stream_t stream);
+int isb_lm_battery_scale(const double* resp, int H, int W, int row_lo, int row_hi, double max_signal, const double* sumsq, double* out,
+                         isb_stream_t stream);
 
 /* compute_label_histograms_positions (imsegm/descriptors.py:1288-1352) in one launch: for every position (row, col) and every
  * diameter d the histogram of the labels under the disc dy^2 + dx^2 <= d^2 (skimage.morphology.disk(d)) clipped to the image,

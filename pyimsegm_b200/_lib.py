@@ -108,6 +108,8 @@ SIGNATURES = {
     'isb_lm_background': (_i, [_vp, _i, _i, _i, _vp, _i, C.POINTER(_d), _vp, _vp, _vp, _vp]),
     'isb_lm_battery_workspace_bytes': (_sz, []),
     'isb_lm_battery_response': (_i, [_vp, _i, _i, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _sz, _vp]),
+    'isb_lm_battery_partial': (_i, [_vp, _i, _i, _vp, _i, _i, _i, _d, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    'isb_lm_battery_scale': (_i, [_vp, _i, _i, _i, _i, _d, _vp, _vp, _vp]),
     'isb_ellipse_ransac': (_i, [_i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _d, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'isb_ellipse_overlap': (_i, [_vp, _i, _i, _i, C.POINTER(C.c_int32), C.POINTER(_d), _vp, _vp, _vp]),
     'isb_binary_morph_footprint': (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),

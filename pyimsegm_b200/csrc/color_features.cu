@@ -8,6 +8,8 @@
 //   isb_lm_battery_response  minus its sigma-150 background, then per battery the strongest response, clip, sum of squares in a fixed
 //                            order (block partials, every CTA of the second kernel re-adds them in the same order: no floating atomics,
 //                            a rerun gives the same bits) and the log-norm scaling, written interleaved [H, W, 3]
+//   isb_lm_battery_partial   the same battery step split for row bands (tiled.py): the responses of a slab and the sum of squares of
+//   isb_lm_battery_scale     its owned rows, then -- once the bands' sums are added -- the scaling of a row range with that norm
 // Built with -fmad=false like every source here; the gradient spells its rounding out with the _rn intrinsics as well.
 #include <float.h>
 #include <algorithm>
@@ -196,16 +198,42 @@ __device__ __forceinline__ double block_sum(double v, double* s)
     return t;
 }
 
-__global__ void __launch_bounds__(NORM_THREADS) k_resp_sumsq(const double* __restrict__ resp, size_t n, double vmax, double* __restrict__ partial)
+// NORM_BLOCKS partial sums of the squared clipped responses resp [3][hw]: of every element (kWhole), or of the pixels [p0, p0 + np)
+// of each plane -- the owned rows of a slab.  Both visit the elements in the same order, so a slab that owns all its rows gets the
+// whole-image partials.
+template <bool kWhole>
+__global__ void __launch_bounds__(NORM_THREADS) k_resp_sumsq(const double* __restrict__ resp, size_t n, size_t hw, size_t p0, size_t np,
+                                                             double vmax, double* __restrict__ partial)
 {
     __shared__ double s[NORM_THREADS];
     double acc = 0.;
     for (size_t i = (size_t)blockIdx.x * NORM_THREADS + threadIdx.x; i < n; i += (size_t)NORM_BLOCKS * NORM_THREADS) {
-        const double v = clip_resp(resp[i], vmax);
+        const double v = clip_resp(resp[kWhole ? i : (i / np) * hw + p0 + i % np], vmax);
         acc = __dadd_rn(acc, __dmul_rn(v, v));
     }
     const double t = block_sum(acc, s);
     if (threadIdx.x == 0) partial[blockIdx.x] = t;
+}
+
+// the sum of the NORM_BLOCKS partials, in one fixed order; every thread gets it
+__device__ __forceinline__ double partials_total(const double* __restrict__ partial, double* s)
+{
+    double acc = 0.;
+    for (int j = threadIdx.x; j < NORM_BLOCKS; j += NORM_THREADS) acc = __dadd_rn(acc, partial[j]);
+    return block_sum(acc, s);
+}
+
+__global__ void __launch_bounds__(NORM_THREADS) k_partials_total(const double* __restrict__ partial, double* __restrict__ total)
+{
+    __shared__ double s[NORM_THREADS];
+    const double t = partials_total(partial, s);
+    if (threadIdx.x == 0) *total = t;
+}
+
+// (clip(r) * scale) / |r| with scale = log(1 + |r|) / 0.03, or 0 when |r| is 0 or infinite
+__device__ __forceinline__ double scaled_resp(double r, double vmax, double scale, double norm, bool zero)
+{
+    return zero ? 0. : __ddiv_rn(__dmul_rn(clip_resp(r, vmax), scale), norm);
 }
 
 // (clip(r) * (log(1 + |r|) / 0.03)) / |r|, or 0 everywhere when |r| is 0 or infinite; planar [3, hw] -> interleaved [hw, 3]
@@ -213,14 +241,26 @@ __global__ void __launch_bounds__(NORM_THREADS) k_resp_scale(const double* __res
                                                              const double* __restrict__ partial, double* __restrict__ out)
 {
     __shared__ double s[NORM_THREADS];
-    double acc = 0.;
-    for (int j = threadIdx.x; j < NORM_BLOCKS; j += NORM_THREADS) acc = __dadd_rn(acc, partial[j]);
-    const double norm = sqrt(block_sum(acc, s));
+    const double norm = sqrt(partials_total(partial, s));
     const bool zero = norm == 0. || isinf(norm);
     const double scale = __ddiv_rn(log(__dadd_rn(1., norm)), 0.03);
     for (size_t i = (size_t)blockIdx.x * NORM_THREADS + threadIdx.x; i < 3 * hw; i += (size_t)gridDim.x * NORM_THREADS) {
         const size_t c = i / hw, p = i % hw;
-        out[3 * p + c] = zero ? 0. : __ddiv_rn(__dmul_rn(clip_resp(resp[i], vmax), scale), norm);
+        out[3 * p + c] = scaled_resp(resp[i], vmax, scale, norm, zero);
+    }
+}
+
+// the same scaling with the norm's square given (summed over the bands of an image): the pixels [p0, p0 + np) of every plane of
+// resp [3, hw] -> interleaved out [np, 3]
+__global__ void __launch_bounds__(NORM_THREADS) k_resp_scale_rows(const double* __restrict__ resp, size_t hw, size_t p0, size_t np,
+                                                                  double vmax, const double* __restrict__ sumsq, double* __restrict__ out)
+{
+    const double norm = sqrt(*sumsq);
+    const bool zero = norm == 0. || isinf(norm);
+    const double scale = __ddiv_rn(log(__dadd_rn(1., norm)), 0.03);
+    for (size_t i = (size_t)blockIdx.x * NORM_THREADS + threadIdx.x; i < 3 * np; i += (size_t)gridDim.x * NORM_THREADS) {
+        const size_t c = i / np, q = i % np;
+        out[3 * q + c] = scaled_resp(resp[c * hw + p0 + q], vmax, scale, norm, zero);
     }
 }
 
@@ -289,10 +329,45 @@ extern "C" int isb_lm_battery_response(const double* planar, int H, int W, const
     const int rc = isb_filter_response_2d(planar, 3, H, W, kernels, n_kernels, kh, kw, resp, stream);
     if (rc != ISB_OK) return rc;
     const size_t hw = (size_t)H * W;
-    k_resp_sumsq<<<NORM_BLOCKS, NORM_THREADS, 0, st>>>(resp, 3 * hw, max_signal, (double*)ws);
+    k_resp_sumsq<true><<<NORM_BLOCKS, NORM_THREADS, 0, st>>>(resp, 3 * hw, hw, 0, hw, max_signal, (double*)ws);
     ISB_LAUNCH_CHECK();
     const unsigned grid = (unsigned)std::min<size_t>((3 * hw + NORM_THREADS - 1) / NORM_THREADS, 4096);
     k_resp_scale<<<grid, NORM_THREADS, 0, st>>>(resp, hw, max_signal, (const double*)ws, out);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+// ---- the same battery step split for row bands: the norm is summed over the bands between the two calls ------------------------
+
+extern "C" int isb_lm_battery_partial(const double* planar, int H, int W, const double* kernels, int n_kernels, int kh, int kw,
+                                      double max_signal, int row_lo, int row_hi, double* resp, double* sumsq, void* ws, size_t ws_bytes,
+                                      isb_stream_t stream)
+{
+    ISB_REQUIRE(planar && kernels && resp && sumsq && ws, "null pointer");
+    ISB_REQUIRE(H > 0 && W > 0 && row_lo >= 0 && row_lo < row_hi && row_hi <= H, "bad sizes");
+    ISB_REQUIRE(ws_bytes >= isb_lm_battery_workspace_bytes(), "workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfScope prof(ISB_PROF_LM, st);
+    const int rc = isb_filter_response_2d(planar, 3, H, W, kernels, n_kernels, kh, kw, resp, stream);
+    if (rc != ISB_OK) return rc;
+    const size_t hw = (size_t)H * W, np = (size_t)(row_hi - row_lo) * W;
+    k_resp_sumsq<false><<<NORM_BLOCKS, NORM_THREADS, 0, st>>>(resp, 3 * np, hw, (size_t)row_lo * W, np, max_signal, (double*)ws);
+    ISB_LAUNCH_CHECK();
+    k_partials_total<<<1, NORM_THREADS, 0, st>>>((const double*)ws, sumsq);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_lm_battery_scale(const double* resp, int H, int W, int row_lo, int row_hi, double max_signal, const double* sumsq,
+                                    double* out, isb_stream_t stream)
+{
+    ISB_REQUIRE(resp && sumsq && out, "null pointer");
+    ISB_REQUIRE(H > 0 && W > 0 && row_lo >= 0 && row_lo < row_hi && row_hi <= H, "bad sizes");
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfScope prof(ISB_PROF_LM, st);
+    const size_t np = (size_t)(row_hi - row_lo) * W;
+    const unsigned grid = (unsigned)std::min<size_t>((3 * np + NORM_THREADS - 1) / NORM_THREADS, 4096);
+    k_resp_scale_rows<<<grid, NORM_THREADS, 0, st>>>(resp, (size_t)H * W, (size_t)row_lo * W, np, max_signal, sumsq, out);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }

@@ -926,6 +926,12 @@ def flags_are_resident(dict_features):
                                        for k, v in dict_features.items())
 
 
+def flags_are_banded(dict_features):
+    """True when the banded path (pyimsegm_b200.tiled) computes every requested group and statistic: any of
+    :data:`RESIDENT_FEATURE_GROUPS` with any of :data:`NAMES_FEATURE_FLAGS` but 'median', which does not decompose over row bands"""
+    return flags_are_resident(dict_features) and not any('median' in v for v in dict_features.values())
+
+
 def native_feature_layout(dict_features):
     """[(key, flags, first column, n columns)] in the column order of :func:`compute_selected_features_color2d`: colour groups
     first, then texture groups, each in dict order; a group's flags in NAMES_FEATURE_FLAGS order (statistic-major, channel-minor

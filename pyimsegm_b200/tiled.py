@@ -19,6 +19,13 @@ back to the whole image on its own GPU).
 
 Several bands may live on one GPU (``bands_per_rank``); the merge between them is the same integer sum done by
 ``isb_combine`` -- that is also how the single-GPU tests exercise every code path of the exchange.
+
+Features: any group of ``descriptors.RESIDENT_FEATURE_GROUPS`` (the image, its colour spaces, the two Leung-Malik banks) with mean /
+std / energy / meanGrad (``descriptors.flags_are_banded``); a median does not decompose over bands and is refused.  ``meanGrad``
+takes the gradient of the owned rows +- 1 and keeps the owned rows; the Leung-Malik responses' norms are summed over the bands in
+band order between the two halves of the battery step.  Models: :func:`pipe_color2d_slic_features_model_graphcut_tiled` fits any
+device ``estim_model`` / ``pca_coef`` on the replicated feature table, :func:`segment_color2d_slic_features_model_graphcut_tiled`
+applies a caller-fitted one (on the device when ``class_models.compile_model`` takes it, on every rank's host otherwise).
 """
 import ctypes as C
 import logging
@@ -232,20 +239,16 @@ def slic_tiled(image, n_segments, compactness, sigma=1.0, max_iter=10, slic_zero
     return res
 
 
-def color_stats_tiled(res, image_dtype, channels, flags, comm=None, eng=None, feat=None, col0=0):
-    """colour statistics + centroids of the banded image over ``res.d_seg``: every band accumulates its owned rows, the
-    accumulators are summed over the GPUs, every GPU finishes the same [nb, 3*len(flags)] table"""
-    eng = eng or get_engine()
+def _stats_banded(res, source, flags, feat, col0, centres, comm, eng):
+    """statistics ``flags`` (of mean / std / energy) of a banded 3-channel source over ``res.d_seg`` into feat[:, col0:] (and the
+    centroids into ``centres`` unless it is None): every band accumulates its owned rows, the accumulators are summed over the GPUs
+    between the calls, every GPU finishes the same table.  ``source(i)`` -> (device pointer to the owned rows [rows, W, 3] of local
+    band i, isb dtype code); it is called right before each pass over the band, so it may fill a buffer the bands share."""
     torch, lib = eng.torch, eng.lib
-    comm = comm or default_comm()
-    H, W = res.shape
-    if channels != 3:
-        raise ValueError('the colour statistics need a 3-channel image')
-    code = _lib.dtype_code(np.dtype(image_dtype))
-    itemsize = np.dtype(image_dtype).itemsize
+    W = res.shape[1]
     nb = int(res.nb_bound)
     st = _lib.stream_ptr()
-    bits, ncol = flag_bits(flags)
+    bits, _ = flag_bits(flags)
     acc = eng.buf('tb_acc', (nb, 6), torch.float64)
     iacc = eng.buf('tb_iacc', (nb, 3), torch.int64)
     acc.zero_()
@@ -253,12 +256,11 @@ def color_stats_tiled(res, image_dtype, channels, flags, comm=None, eng=None, fe
 
     def rows(i, b):
         bd = res.bands[b]
-        img_ptr = res.d_raw[i].data_ptr() + (bd.own_lo - bd.up_lo) * W * 3 * itemsize
-        seg_ptr = res.d_seg.data_ptr() + bd.own_lo * W * 4
-        return bd, C.c_void_p(img_ptr), C.c_void_p(seg_ptr)
+        ptr, code = source(i)
+        return bd, C.c_void_p(ptr), code, C.c_void_p(res.d_seg.data_ptr() + bd.own_lo * W * 4)
 
     for i, b in enumerate(res.local):
-        bd, img_ptr, seg_ptr = rows(i, b)
+        bd, img_ptr, code, seg_ptr = rows(i, b)
         _lib.check(lib.isb_segment_stats_accumulate(img_ptr, code, seg_ptr, bd.own_hi - bd.own_lo, W, bd.own_lo, nb, _lib.ptr(acc),
                                                     _lib.ptr(iacc), st))
     comm.all_reduce(acc, 'sum')
@@ -269,17 +271,100 @@ def color_stats_tiled(res, image_dtype, channels, flags, comm=None, eng=None, fe
         meanf = eng.buf('tb_meanf', (nb, 3), torch.float32)
         var.zero_()
         for i, b in enumerate(res.local):
-            bd, img_ptr, seg_ptr = rows(i, b)
+            bd, img_ptr, code, seg_ptr = rows(i, b)
             _lib.check(lib.isb_segment_stats_deviation(img_ptr, code, seg_ptr, bd.own_hi - bd.own_lo, W, nb, _lib.ptr(acc), _lib.ptr(iacc),
                                                        _lib.ptr(meanf), _lib.ptr(var), st))
         comm.all_reduce(var, 'sum')
-    if feat is None:
-        feat = eng.buf('feat', (nb, max(ncol, 1)), torch.float64)
-    centres = eng.buf('centres', (nb, 2), torch.float64)
     _lib.check(lib.isb_segment_stats_finish(nb, bits, _lib.ptr(acc), _lib.ptr(var), _lib.ptr(iacc), _lib.ptr(feat), int(feat.shape[1]),
                                             int(col0), _lib.ptr(centres), None, st))
+
+
+def _raw_rows(res, i, lo, hi, itemsize, what):
+    """device pointer to the raw image rows [lo, hi) of local band i; ValueError when the band did not keep them"""
+    bd = res.bands[res.local[i]]
+    if lo < bd.up_lo or hi > bd.up_hi:
+        raise ValueError('the band keeps the raw rows %d:%d, %s needs %d:%d (slic_tiled raw_margin)' % (bd.up_lo, bd.up_hi, what, lo, hi))
+    return res.d_raw[i].data_ptr() + (lo - bd.up_lo) * res.shape[1] * 3 * itemsize
+
+
+def color_stats_tiled(res, image_dtype, channels, flags, comm=None, eng=None, feat=None, col0=0):
+    """colour statistics + centroids of the banded image over ``res.d_seg``: every band accumulates its owned rows, the
+    accumulators are summed over the GPUs, every GPU finishes the same [nb, 3*len(flags)] table"""
+    eng = eng or get_engine()
+    comm = comm or default_comm()
+    if channels != 3:
+        raise ValueError('the colour statistics need a 3-channel image')
+    code = _lib.dtype_code(np.dtype(image_dtype))
+    itemsize = np.dtype(image_dtype).itemsize
+    nb = int(res.nb_bound)
+    if feat is None:
+        feat = eng.buf('feat', (nb, max(flag_bits(flags)[1], 1)), eng.torch.float64)
+    centres = eng.buf('centres', (nb, 2), eng.torch.float64)
+
+    def source(i):
+        bd = res.bands[res.local[i]]
+        return _raw_rows(res, i, bd.own_lo, bd.own_hi, itemsize, 'the colour statistics'), code
+
+    _stats_banded(res, source, flags, feat, col0, centres, comm, eng)
     res.d_feat, res.d_centres = feat, centres
     return feat, centres
+
+
+def gradient_rows(bd, H):
+    """the rows [lo, hi) whose np.gradient gives the owned rows of band ``bd`` their whole-image values: one more row on each side
+    that is not an image border (there the gradient is one-sided, as it is for the whole image)"""
+    return max(bd.own_lo - 1, 0), min(bd.own_hi + 1, H)
+
+
+def color_group_tiled(res, image_dtype, key, flags, comm=None, eng=None, feat=None, col0=0, centres=None):
+    """the statistics ``flags`` (mean / std / energy / meanGrad) of one colour group of ``native_feature_layout`` -- the image, or
+    its conversion when ``key`` ends in '_<space>' of DICT_CONVERT_COLOR_FROM_RGB -- over ``res.d_seg`` into feat[:, col0:], the
+    centroids into ``centres`` when given.  A band converts its owned rows (plus the gradient's one row on each interior side)
+    into an f64 buffer of its own; ``meanGrad`` is the mean of ``isb_gradient_sum_2d`` of those rows (f32 for an f32 image that
+    is not converted, as on the single-image path), of which only the owned rows are accumulated."""
+    from .color import DICT_CONVERT_COLOR_FROM_RGB
+    eng = eng or get_engine()
+    torch, lib = eng.torch, eng.lib
+    comm = comm or default_comm()
+    H, W = res.shape
+    st = _lib.stream_ptr()
+    space = key.split('_')[-1]
+    convert = space in DICT_CONVERT_COLOR_FROM_RGB
+    grad = 'meanGrad' in flags
+    native = [f for f in ('mean', 'std', 'energy') if f in flags]
+    code, itemsize = _lib.dtype_code(np.dtype(image_dtype)), np.dtype(image_dtype).itemsize
+    srcs = []       # per local band: (pointer to rows [lo, hi), dtype code, item size, lo, hi)
+    for i, b in enumerate(res.local):
+        bd = res.bands[b]
+        lo, hi = gradient_rows(bd, H) if grad else (bd.own_lo, bd.own_hi)
+        ptr = _raw_rows(res, i, lo, hi, itemsize, 'the colour group %r' % key)
+        if convert:
+            conv = eng.buf('tb%d_conv' % i, (hi - lo, W, 3), torch.float64)
+            _lib.check(lib.isb_color_convert(C.c_void_p(ptr), code, C.c_longlong((hi - lo) * W), eng.COLOR_SPACES[space], _lib.ptr(conv), st))
+            srcs.append((conv.data_ptr(), _lib.dtype_code(np.dtype(np.float64)), 8, lo, hi))
+        else:
+            srcs.append((ptr, code, itemsize, lo, hi))
+
+    def owned(i, ptr, isz, lo):
+        return ptr + (res.bands[res.local[i]].own_lo - lo) * W * 3 * isz
+
+    col = col0
+    if native:
+        _stats_banded(res, lambda i: (owned(i, srcs[i][0], srcs[i][2], srcs[i][3]), srcs[i][1]), native, feat, col, centres, comm, eng)
+        centres = None
+        col += 3 * len(native)
+    if grad:
+        f32 = srcs[0][1] == _lib.dtype_code(np.dtype(np.float32))
+        gdtype, gcode, gsize = (torch.float32, srcs[0][1], 4) if f32 else (torch.float64, _lib.dtype_code(np.dtype(np.float64)), 8)
+
+        def gradient(i):
+            ptr, c, _, lo, hi = srcs[i]
+            out = eng.buf('tb_grad', (hi - lo, W, 3), gdtype)
+            _lib.check(lib.isb_gradient_sum_2d(C.c_void_p(ptr), c, hi - lo, W, 3, _lib.ptr(out), st))
+            return owned(i, out.data_ptr(), gsize, lo), gcode
+
+        _stats_banded(res, gradient, ('mean', ), feat, col, centres, comm, eng)
+    return feat
 
 
 LM_ROW_MARGIN = 616     # rows of the Leung-Malik descriptor's footprint: sigma-150 background (radius 600) + half a 33 x 33 kernel
@@ -330,61 +415,151 @@ def texture_stats_tiled(res, image_dtype, flags, bank_type='normal', comm=None, 
     return feat
 
 
-def features_tiled(res, image_dtype, channels, layout, ncol, comm=None, eng=None):
-    """the [nb, ncol] feature table of ``native_feature_layout`` over the banded image (``res.d_feat``) + the centroids"""
+def texture_gradient_tiled(res, image_dtype, bank_type='normal', comm=None, eng=None, feat=None, col0=0, stride=3):
+    """``meanGrad`` of every Leung-Malik battery of the banded image over ``res.d_seg``: battery b's three columns go to
+    feat[:, col0 + b * stride:].  The route of ``texture.device_lm_materialised`` split at the response norm: every band subtracts
+    the background of its rows + ``LM_ROW_MARGIN + 1`` rows of halo (``slic_tiled`` must have kept them, see
+    :func:`banded_raw_margin`); then per battery every band computes its responses and the sum of their squares over its owned rows
+    (``isb_lm_battery_partial``), the ranks exchange those sums and add them in band order -- the same bits on every rank and in
+    every run --, and every band scales its owned rows +- 1 with that norm (``isb_lm_battery_scale``), takes their gradient and
+    accumulates the owned rows."""
+    from .descriptors import MAX_SIGNAL_RESPONSE
+    from .texture import BACKGROUND_SIGMA, _device_batteries, background_kernel
     eng = eng or get_engine()
-    feat = eng.buf('feat', (int(res.nb_bound), max(ncol, 1)), eng.torch.float64)
+    torch, lib = eng.torch, eng.lib
+    comm = comm or default_comm()
+    H, W = res.shape
+    st = _lib.stream_ptr()
+    code, itemsize = _lib.dtype_code(np.dtype(image_dtype)), np.dtype(image_dtype).itemsize
+    f64 = _lib.dtype_code(np.dtype(np.float64))
+    margin = LM_ROW_MARGIN + 1
+    w_half, radius = gaussian_half_kernel(BACKGROUND_SIGMA)
+    d_w = eng.const_device(w_half, 'lm_bg_half')
+    _, _, mix = background_kernel()
+    slabs = []      # per local band: (slab rows [lo, hi), its background-subtracted planar copy, its responses)
+    for i, b in enumerate(res.local):
+        bd = res.bands[b]
+        lo, hi = max(bd.own_lo - margin, 0), min(bd.own_hi + margin, H)
+        ptr = _raw_rows(res, i, lo, hi, itemsize, 'the texture meanGrad')
+        planar = eng.buf('tb%d_lmm_planar' % i, (3, hi - lo, W), torch.float64)
+        tmp, smooth = (eng.buf(name, (3, hi - lo, W), torch.float64) for name in ('lmm_tmp', 'lmm_smooth'))
+        _lib.check(lib.isb_lm_background(C.c_void_p(ptr), code, hi - lo, W, _lib.ptr(d_w), radius, mix.ctypes.data_as(C.POINTER(C.c_double)),
+                                         _lib.ptr(planar), _lib.ptr(tmp), _lib.ptr(smooth), st))
+        slabs.append((lo, hi, planar, eng.buf('tb%d_lmm_resp' % i, (3, hi - lo, W), torch.float64)))
+    n_bands = len(res.bands)
+    sums = eng.buf('tb_lmm_sumsq', (n_bands + 1, ), torch.float64)     # one slot per band, then their total
+    wsb = lib.isb_lm_battery_workspace_bytes()
+    ws = eng.buf('ws_lmm', (wsb, ), torch.uint8)
+    for bt, d_k in enumerate(_device_batteries(eng, bank_type)):
+        nk, kh, kw = (int(v) for v in d_k.shape)
+        sums.zero_()
+        for i, b in enumerate(res.local):
+            bd, (lo, hi, planar, resp) = res.bands[b], slabs[i]
+            _lib.check(lib.isb_lm_battery_partial(_lib.ptr(planar), hi - lo, W, _lib.ptr(d_k), nk, kh, kw, C.c_double(MAX_SIGNAL_RESPONSE),
+                                                  bd.own_lo - lo, bd.own_hi - lo, _lib.ptr(resp), C.c_void_p(sums.data_ptr() + 8 * b),
+                                                  _lib.ptr(ws), C.c_size_t(wsb), st))
+        comm.all_reduce(sums, 'sum')    # an all-gather: every slot has one writer, the other ranks add +0
+        for b in range(n_bands):
+            _combine(lib, sums.data_ptr() + 8 * n_bands, sums.data_ptr() + 8 * b, 1, OP_SUM_F64)
+
+        def gradient(i):
+            bd, (lo, hi, planar, resp) = res.bands[res.local[i]], slabs[i]
+            g_lo, g_hi = gradient_rows(bd, H)
+            scaled = eng.buf('tb_lmm_out', (g_hi - g_lo, W, 3), torch.float64)
+            _lib.check(lib.isb_lm_battery_scale(_lib.ptr(resp), hi - lo, W, g_lo - lo, g_hi - lo, C.c_double(MAX_SIGNAL_RESPONSE),
+                                                C.c_void_p(sums.data_ptr() + 8 * n_bands), _lib.ptr(scaled), st))
+            grad = eng.buf('tb_grad', (g_hi - g_lo, W, 3), torch.float64)
+            _lib.check(lib.isb_gradient_sum_2d(_lib.ptr(scaled), f64, g_hi - g_lo, W, 3, _lib.ptr(grad), st))
+            return grad.data_ptr() + (bd.own_lo - g_lo) * W * 3 * 8, f64
+
+        _stats_banded(res, gradient, ('mean', ), feat, col0 + bt * stride, None, comm, eng)
+    return feat
+
+
+def banded_raw_margin(layout):
+    """raw rows a band keeps above and below its owned ones (``slic_tiled(raw_margin=...)``) for the feature groups of ``layout``
+    (``native_feature_layout``): none beyond the blur's for colour groups, whose gradient needs one row that the blur radius
+    already covers; the Leung-Malik footprint ``LM_ROW_MARGIN`` for a texture group, one row more when it asks for ``meanGrad``
+    (the gradient of the responses one row beyond the owned ones)"""
+    texture = [flags for key, flags, _, _ in layout if key.startswith('tLM')]
+    if not texture:
+        return 0
+    return LM_ROW_MARGIN + (1 if any('meanGrad' in flags for flags in texture) else 0)
+
+
+def features_tiled(res, image_dtype, channels, layout, ncol, comm=None, eng=None):
+    """the [nb, ncol] feature table of ``native_feature_layout`` over the banded image (``res.d_feat``) + the centroids, which come
+    from the first statistics of a colour group (or from a pass over the image when there is none).  ``layout`` may hold any group
+    of RESIDENT_FEATURE_GROUPS with any statistic but 'median' (``descriptors.flags_are_banded``)."""
+    eng = eng or get_engine()
+    torch = eng.torch
+    nb = int(res.nb_bound)
+    feat = eng.buf('feat', (nb, max(ncol, 1)), torch.float64)
     centres = None
-    for key, flags, col0, _ in layout:
-        if key == 'color':
-            _, centres = color_stats_tiled(res, image_dtype, channels, flags, comm=comm, eng=eng, feat=feat, col0=col0)
-        else:
-            texture_stats_tiled(res, image_dtype, flags, 'short' if key.endswith('_short') else 'normal', comm=comm, eng=eng, feat=feat,
-                                col0=col0)
+    for key, flags, col0, n in layout:
+        if key.startswith('color'):
+            if centres is None and flags:
+                centres = eng.buf('centres', (nb, 2), torch.float64)
+                color_group_tiled(res, image_dtype, key, flags, comm=comm, eng=eng, feat=feat, col0=col0, centres=centres)
+            else:
+                color_group_tiled(res, image_dtype, key, flags, comm=comm, eng=eng, feat=feat, col0=col0)
+            continue
+        bank = 'short' if key.endswith('_short') else 'normal'
+        if 'meanGrad' not in flags:
+            texture_stats_tiled(res, image_dtype, flags, bank, comm=comm, eng=eng, feat=feat, col0=col0)
+            continue
+        # battery-major columns: the fused kernel's mean / std / energy, then the gradient mean of the materialised responses
+        native = [f for f in ('mean', 'std', 'energy') if f in flags]
+        n_batt, per_battery = n // (3 * len(flags)), 3 * len(flags)
+        if native:
+            part = texture_stats_tiled(res, image_dtype, native, bank, comm=comm, eng=eng)
+            block = feat[:, col0:col0 + n].view(nb, n_batt, per_battery)
+            block[:, :, :3 * len(native)].copy_(part[:nb, :n_batt * 3 * len(native)].reshape(nb, n_batt, 3 * len(native)))
+        texture_gradient_tiled(res, image_dtype, bank, comm=comm, eng=eng, feat=feat, col0=col0 + 3 * len(native), stride=per_battery)
     if centres is None:
-        _, centres = color_stats_tiled(res, image_dtype, channels, (), comm=comm, eng=eng, feat=eng.buf('feat_none', (int(res.nb_bound), 1),
-                                                                                                         eng.torch.float64))
+        _, centres = color_stats_tiled(res, image_dtype, channels, (), comm=comm, eng=eng, feat=eng.buf('feat_none', (nb, 1), torch.float64))
     res.d_feat, res.d_centres = feat, centres
     return feat, centres
 
 
-def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_features=None, sp_size=30, sp_regul=0.2, use_scaler=True,
-                                                    gc_regul=1., gc_edge_type='model', max_iter=99, comm=None, bands_per_rank=1,
-                                                    want_soft=True, gather_segm=False):
-    """ ``pipe_color2d_slic_features_model_graphcut`` (reference pipelines.py:46-110) for one image banded over the GPUs of
-    ``comm``.  Every rank passes the same host image and gets the rows it owns:
 
-    :return tuple: (segm [rows, W] int32, segm_soft [rows, W, K] float64 or None, (row_lo, row_hi)); with ``gather_segm``
-        ``segm`` is the whole [H, W] map on every rank (``segm_soft`` stays banded: it is 8*K bytes per pixel)
-    """
-    from . import graph_cuts
-    from .descriptors import flags_are_native, native_feature_layout
-    from .superpixels import _as_rgb_like, _supported_dtype, slic_params
-    if sp_regul <= 0.:
-        raise ValueError('slic. regularisation must be positive')
-    dict_features = {'color': ['mean']} if dict_features is None else dict_features
+
+def _admit(dict_features):
+    """(layout, ncol, raw margin) of a feature dictionary the banded path takes; NotImplementedError for any other, before any
+    device work"""
+    from .descriptors import flags_are_banded, native_feature_layout
     layout, ncol = native_feature_layout(dict_features)
-    if not layout or not flags_are_native(dict_features):
-        raise NotImplementedError('the banded path computes mean / std / energy of the colours and of the Leung-Malik responses (got %r)'
-                                  % dict_features)
-    margin = LM_ROW_MARGIN if any(k.startswith('tLM') for k, _, _, _ in layout) else 0
-    eng = get_engine()
-    torch = eng.torch
-    comm = comm or default_comm()
+    if not layout or not flags_are_banded(dict_features):
+        raise NotImplementedError('the banded path computes mean / std / energy / meanGrad of the colour, colour-space and Leung-Malik '
+                                  'groups; a median does not decompose over row bands (got %r)' % (dict_features, ))
+    return layout, ncol, banded_raw_margin(layout)
+
+
+def _prepare_image(image, layout, sp_size, sp_regul):
+    """(host image in a device dtype, n_segments, compactness) with the single-image pipelines' argument errors"""
+    from .descriptors import _check_gradient_size
+    from .superpixels import _as_rgb_like, _supported_dtype, slic_params
     image = _supported_dtype(_as_rgb_like(np.asarray(image)))
     H, W = int(image.shape[0]), int(image.shape[1])
+    _check_gradient_size((H, W), [flags for _, flags, _, _ in layout])
     n_seg, compact = slic_params((H, W), sp_size, sp_regul)
     if n_seg < 1:
         raise ValueError('superpixel size %r is larger than the image %r' % (sp_size, tuple(image.shape)))
-    n_init = max(1, int(np.sqrt(max_iter)))
+    return image, n_seg, compact
+
+
+def _banded_segment(eng, shape, comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm):
+    """the tail both banded pipelines share: ``front(force_whole)`` -> (res, d_proba) runs the banded SLIC (``defer_check``), the
+    feature table and the class probabilities; then the soft segmentation of the owned rows, the graph cut on the replicated
+    superpixel graph, the LUT gather of the owned rows and one download.  Orphan pixels beyond the halo redo the front on the whole
+    image, an edge table that was too small redoes the cut.  Returns (segm, segm_soft or None, (row_lo, row_hi)) on the host."""
+    from . import graph_cuts
+    torch = eng.torch
+    H, W = shape
     force_whole, redo_front = False, True
     while True:
         if redo_front:
-            res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
-                             force_whole=force_whole, raw_margin=margin)
-            features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
-            d_proba, _ = eng.mixture_fit_predict(res.d_feat, int(nb_classes), n_init, max_iter, use_scaler, graph_cuts.RANDOM_SEED,
-                                                 d_n=res.d_n_labels)
+            res, d_proba = front(force_whole)
             redo_front = False
         lo, hi = res.bands[res.local[0]].own_lo, res.bands[res.local[-1]].own_hi
         soft = eng.early_soft(res.d_seg[lo:hi], d_proba) if want_soft else None
@@ -410,3 +585,81 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
         if edges_fit(n_edges[0], cap):
             break
     return h_segm.numpy(), (soft[0].numpy() if want_soft else None), (lo, hi)
+
+
+def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_features=None, sp_size=30, sp_regul=0.2, use_scaler=True,
+                                                    gc_regul=1., gc_edge_type='model', max_iter=99, comm=None, bands_per_rank=1,
+                                                    want_soft=True, gather_segm=False, estim_model='GMM', pca_coef=None):
+    """ ``pipe_color2d_slic_features_model_graphcut`` (reference pipelines.py:46-110) for one image banded over the GPUs of
+    ``comm``.  Every rank passes the same host image and gets the rows it owns.  The features may be any group of
+    RESIDENT_FEATURE_GROUPS with mean / std / energy / meanGrad (not median); the class model is fitted on the GPU on the
+    replicated feature table, every ``estim_model`` variant and ``pca_coef`` that ``graph_cuts.device_gmm_applicable`` takes.
+
+    :return tuple: (segm [rows, W] int32, segm_soft [rows, W, K] float64 or None, (row_lo, row_hi)); with ``gather_segm``
+        ``segm`` is the whole [H, W] map on every rank (``segm_soft`` stays banded: it is 8*K bytes per pixel)
+    """
+    from . import graph_cuts
+    if sp_regul <= 0.:
+        raise ValueError('slic. regularisation must be positive')
+    dict_features = {'color': ['mean']} if dict_features is None else dict_features
+    layout, ncol, margin = _admit(dict_features)
+    if not graph_cuts.device_gmm_applicable(ncol, nb_classes, estim_model, pca_coef):
+        raise NotImplementedError('the banded path fits the class model on the GPU, which does not take estim_model=%r, pca_coef=%r with '
+                                  '%d features and %d classes' % (estim_model, pca_coef, ncol, nb_classes))
+    # the default 'GMM' gives (GMM, sqrt(max_iter) restarts, max_iter): the mixture fit the banded path has always made
+    kind, n_init, n_iter = graph_cuts.class_model_spec(estim_model, nb_classes, max_iter)
+    image, n_seg, compact = _prepare_image(image, layout, sp_size, sp_regul)
+    eng = get_engine()
+    comm = comm or default_comm()
+
+    def front(force_whole):
+        res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
+                         force_whole=force_whole, raw_margin=margin)
+        features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
+        d_proba = graph_cuts.device_fit_predict(eng, res.d_feat, int(nb_classes), use_scaler, kind, n_init, n_iter, pca_coef,
+                                                graph_cuts.RANDOM_SEED, d_n=res.d_n_labels)[0]
+        return res, d_proba
+
+    return _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm)
+
+
+def segment_color2d_slic_features_model_graphcut_tiled(image, model_pipeline, dict_features, sp_size=30, sp_regul=0.2, gc_regul=1.,
+                                                       gc_edge_type='model', comm=None, bands_per_rank=1, want_soft=True,
+                                                       gather_segm=False):
+    """ ``segment_color2d_slic_features_model_graphcut`` (reference pipelines.py:160-241) for one image banded over the GPUs of
+    ``comm``: a caller-fitted model -- typically the group model of ``estim_model_classes_group`` -- applied to an image too large
+    for one pass.  A model that ``class_models.compile_model`` takes (and whose feature count matches the banded table) is evaluated
+    on the device on every rank; any other model's ``predict_proba`` runs on the host of every rank, on the same replicated feature
+    table, and its probabilities are uploaded.  The labels are mapped through the model's ``classes_``.
+
+    :return tuple: (segm [rows, W], segm_soft [rows, W, K] float64 or None, (row_lo, row_hi)) as
+        :func:`pipe_color2d_slic_features_model_graphcut_tiled`
+    """
+    from .pipelines import _compiled_model
+    if sp_regul <= 0.:
+        raise ValueError('slic. regularisation must be positive')
+    layout, ncol, margin = _admit(dict_features)
+    image, n_seg, compact = _prepare_image(image, layout, sp_size, sp_regul)
+    classes = getattr(model_pipeline, 'classes_', None)
+    eng = get_engine()
+    comm = comm or default_comm()
+    compiled = _compiled_model(model_pipeline, dict_features)
+
+    def front(force_whole):
+        res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
+                         force_whole=force_whole, raw_margin=margin)
+        features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
+        if compiled is not None:
+            return res, eng.class_model_predict(res.d_feat, compiled, d_n=res.d_n_labels)
+        nb = int(eng.to_host(res.d_n_labels)[0])
+        features = eng.to_host(res.d_feat[:nb, :ncol]).copy()
+        features[np.isnan(features)] = 0
+        proba = np.asarray(model_pipeline.predict_proba(features), dtype=np.float64)
+        padded = np.zeros((int(res.nb_bound), proba.shape[1]))      # the rows of the label bound, as a device model gives
+        padded[:nb] = proba
+        return res, eng.to_device(padded, 'proba')
+
+    segm, soft, rows = _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm)
+    if classes is not None:
+        segm = np.asarray(classes)[segm]
+    return segm, soft, rows
