@@ -365,6 +365,22 @@ size_t isb_forest_predict_workspace_bytes(int N, int n_trees);
 int isb_forest_predict_proba(const double* x, int N, const int32_t* n_dev, int D, int n_trees, const int32_t* roots, const int32_t* feature,
                              const double* threshold, const int32_t* left, const int32_t* right, int n_nodes, const double* value, int K,
                              int average, double* proba, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* k-nearest neighbours (KNeighborsClassifier, Euclidean metric): fit_x [N_t, D] the training rows (_fit_X), y [N_t] their class
+ * indices (_y, in [0, K)).  The squared distance of a query to a training row is sum_d (x_d - t_d)^2 in feature order, every step
+ * rounded (no FMA): the bits of a left-to-right float64 loop.  The neighbours are the k smallest by (squared distance, training
+ * index).  weights 0 (uniform): proba = class counts / k.  weights 1 (distance): w = 1 / sqrt(d^2), or the indicator d^2 == 0 when
+ * any neighbour is at distance 0 (_get_weights); the weights are added per class in ascending neighbour order and divided by their
+ * row sum.  1 <= k <= 64, k <= N_t, K <= 64.  ws: isb_knn_predict_workspace_bytes(N, N_t, k) (the per-split neighbour lists). */
+size_t isb_knn_predict_workspace_bytes(int N, int N_t, int k);
+int isb_knn_predict_proba(const double* x, int N, const int32_t* n_dev, int D, const double* fit_x, int N_t, const int32_t* y, int k, int K,
+                          int weights, double* proba, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* logistic regression: coef [n_coef, D], intercept [n_coef]; decision_c = x . coef_c + intercept_c.  n_coef == 1 (binary):
+ * proba [N, 2] = [1 - expit(d), expit(d)] (_predict_proba_lr); else proba [N, n_coef] = softmax(d) in sklearn.utils.extmath.softmax's
+ * order (subtract the row maximum, exp, divide by the row sum).  n_coef <= 64.  ws: isb_linear_predict_workspace_bytes (0 bytes;
+ * ws may be NULL). */
+size_t isb_linear_predict_workspace_bytes(int N, int n_coef);
+int isb_linear_predict_proba(const double* x, int N, const int32_t* n_dev, int D, const double* coef, const double* intercept, int n_coef,
+                             double* proba, void* ws, size_t ws_bytes, isb_stream_t stream);
 
 /* compute_texture_desc_lm_img2d_clr (imsegm/descriptors.py:1041-1106): sigma-150 background subtraction (reflect, all three
  * axes), Leung-Malik filter bank (33x33 kernels) as an implicit GEMM on the tensor cores (wgmma.mma_async with TF32 inputs and the 3xTF32

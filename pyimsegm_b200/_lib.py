@@ -83,6 +83,10 @@ SIGNATURES = {
     'isb_mixture_predict_proba': (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     'isb_forest_predict_workspace_bytes': (_sz, [_i, _i]),
     'isb_forest_predict_proba': (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
+    'isb_knn_predict_workspace_bytes': (_sz, [_i, _i, _i]),
+    'isb_knn_predict_proba': (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    'isb_linear_predict_workspace_bytes': (_sz, [_i, _i]),
+    'isb_linear_predict_proba': (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _sz, _vp]),
     'isb_lm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'isb_lm_acc_doubles': (_sz, [_i, _i]),
     'isb_lm_texture_accumulate': (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _i, C.POINTER(_d), _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),

@@ -4,16 +4,23 @@ Device ``predict_proba`` of a caller-fitted class model.
 The reference's shared-model entry point (``segment_color2d_slic_features_model_graphcut``, reference pipelines.py:160-241) takes
 a model fitted elsewhere: the group mixture of ``estim_model_classes_group`` (:113-157) or a trained classifier
 (``classification.py:101``, a random forest by default).  :func:`compile_model` turns such a model into flat tables that
-``isb_class_transform`` / ``isb_mixture_predict_proba`` / ``isb_forest_predict_proba`` (include/imsegm_b200.h) evaluate on the
-device, so the pipeline keeps its features on the GPU and never waits for the host.
+``isb_class_transform`` / ``isb_mixture_predict_proba`` / ``isb_forest_predict_proba`` / ``isb_knn_predict_proba`` /
+``isb_linear_predict_proba`` (include/imsegm_b200.h) evaluate on the device, so the pipeline keeps its features on the GPU and
+never waits for the host.
 
 Supported: a bare estimator or a ``Pipeline`` of an optional ``StandardScaler``, an optional ``PCA`` and one of
 ``GaussianMixture`` / ``BayesianGaussianMixture`` (any covariance type, <= 232 features after the transforms, <= 8 components) or
-``DecisionTreeClassifier`` / ``RandomForestClassifier`` / ``ExtraTreesClassifier`` (single output, <= 64 classes).  Anything else
-gives ``None`` and the caller keeps the host round trip.
+``DecisionTreeClassifier`` / ``RandomForestClassifier`` / ``ExtraTreesClassifier`` (single output, <= 64 classes) or
+``KNeighborsClassifier`` (single output, ``weights`` 'uniform' or 'distance', Euclidean metric -- 'euclidean', or 'minkowski' with
+p = 2 and no ``metric_params`` -- 1 <= n_neighbors <= 64 and <= the training rows, <= 64 classes; ``isb_knn_predict_proba``) or
+``LogisticRegression`` (``coef_`` [1 or K, D], <= 64 classes; ``isb_linear_predict_proba``).  Anything else gives ``None`` and the
+caller keeps the host round trip.
 
 Trees and forests are bit-identical to scikit-learn (``n_jobs=None``) when no PCA is involved; mixtures and PCA differ only by the
-order of floating-point sums.
+order of floating-point sums.  k-nearest neighbours take their squared distances as a left-to-right float64 loop and order ties by
+training index: with uniform weights the result is bit-identical to scikit-learn wherever scikit-learn's own distances (its kd-tree
+or its ||x||^2 - 2 x.t + ||t||^2 expansion) pick the same neighbours, i.e. away from near ties of the k-th and (k+1)-th distances;
+distance weights and logistic regression differ by the rounding of their sums.
 """
 import hashlib
 import weakref
@@ -26,9 +33,14 @@ FOREST_MAX_CLASSES = 64
 
 #: fitted attributes a refit replaces: a snapshot holds them, so an unchanged model is not compiled again
 _FITTED_ATTRS = ('mean_', 'scale_', 'components_', 'explained_variance_', 'weights_', 'means_', 'precisions_cholesky_',
-                 'weight_concentration_', 'degrees_of_freedom_', 'mean_precision_', 'tree_', 'estimators_')
+                 'weight_concentration_', 'degrees_of_freedom_', 'mean_precision_', 'tree_', 'estimators_', '_fit_X', '_y', 'coef_',
+                 'intercept_')
 #: parameters that change what predict_proba computes without a refit
-_PREDICT_PARAMS = ('with_mean', 'with_std', 'whiten', 'covariance_type', 'weight_concentration_prior_type')
+_PREDICT_PARAMS = ('with_mean', 'with_std', 'whiten', 'covariance_type', 'weight_concentration_prior_type', 'n_neighbors', 'weights', 'p',
+                   'metric', 'metric_params')
+#: isb_knn_predict_proba's weights codes
+KNN_WEIGHTS = {'uniform': 0, 'distance': 1}
+KNN_MAX_NEIGHBOURS = 64
 
 _CACHE = weakref.WeakKeyDictionary()
 
@@ -36,21 +48,24 @@ _CACHE = weakref.WeakKeyDictionary()
 class CompiledModel(object):
     """device tables of one fitted model.
 
-    :ivar str kind: 'mixture' or 'forest'
+    :ivar str kind: 'mixture', 'forest', 'knn' or 'linear'
     :ivar int n_features_in: feature columns the model takes
     :ivar int n_dims: dimensions after the transforms (what the final estimator sees)
     :ivar int n_classes: columns of ``predict_proba``
     :ivar classes_: ``getattr(model, 'classes_', None)`` of the source model
     :ivar dict tables: name -> contiguous ndarray (see the C-ABI for the layouts)
-    :ivar bytes digest: content digest of the tables (device constants and CUDA graphs are keyed on it)
+    :ivar dict params: scalar arguments of the evaluation ('knn': n_neighbors and the weights code)
+    :ivar bytes digest: content digest of the tables and parameters (device constants and CUDA graphs are keyed on it)
     """
 
-    def __init__(self, kind, n_features_in, n_dims, n_classes, classes, tables, average=False):
+    def __init__(self, kind, n_features_in, n_dims, n_classes, classes, tables, average=False, params=None):
         self.kind, self.n_features_in, self.n_dims, self.n_classes = kind, int(n_features_in), int(n_dims), int(n_classes)
         self.classes_ = classes
         self.average = bool(average)
+        self.params = {k: int(v) for k, v in (params or {}).items()}
         self.tables = {k: np.ascontiguousarray(v) for k, v in tables.items()}
-        h = hashlib.blake2b(repr((kind, self.n_features_in, self.n_dims, self.n_classes, self.average)).encode(), digest_size=16)
+        key = (kind, self.n_features_in, self.n_dims, self.n_classes, self.average) + ((sorted(self.params.items()), ) if self.params else ())
+        h = hashlib.blake2b(repr(key).encode(), digest_size=16)
         for name in sorted(self.tables):
             arr = self.tables[name]
             h.update(repr((name, arr.shape, arr.dtype.str)).encode())
@@ -119,7 +134,9 @@ def compile_model(model):
 def _compile(model):
     from sklearn.decomposition import PCA
     from sklearn.ensemble import ExtraTreesClassifier, RandomForestClassifier
+    from sklearn.linear_model import LogisticRegression
     from sklearn.mixture import BayesianGaussianMixture, GaussianMixture
+    from sklearn.neighbors import KNeighborsClassifier
     from sklearn.preprocessing import StandardScaler
     from sklearn.tree import DecisionTreeClassifier
     steps = _steps(model)
@@ -138,6 +155,10 @@ def _compile(model):
         kind = 'mixture'
     elif type(final) in (DecisionTreeClassifier, RandomForestClassifier, ExtraTreesClassifier):
         kind = 'forest'
+    elif type(final) is KNeighborsClassifier:
+        kind = 'knn'
+    elif type(final) is LogisticRegression:
+        kind = 'linear'
     else:
         return None
     first = transforms[0] if transforms else final
@@ -145,11 +166,15 @@ def _compile(model):
     tables, dims = _transform_tables(scaler, pca, n_in)
     if dims is None or int(final.n_features_in_) != dims:
         return None
+    average, params = False, None
     if kind == 'mixture':
         final_tables, n_classes = _mixture_tables(final, dims)
-        average = False
-    else:
+    elif kind == 'forest':
         final_tables, n_classes, average = _forest_tables(final, dims)
+    elif kind == 'knn':
+        final_tables, n_classes, params = _knn_tables(final, dims)
+    else:
+        final_tables, n_classes = _linear_tables(final, dims)
     if final_tables is None:
         return None
     tables.update(final_tables)
@@ -157,7 +182,7 @@ def _compile(model):
         classes = getattr(model, 'classes_', None)
     except Exception:  # noqa: BLE001 -- Pipeline.classes_ raises when the final step has none
         classes = None
-    return CompiledModel(kind, n_in, dims, n_classes, classes, tables, average)
+    return CompiledModel(kind, n_in, dims, n_classes, classes, tables, average, params)
 
 
 def _transform_tables(scaler, pca, n_in):
@@ -267,3 +292,40 @@ def _forest_tables(est, D):
               'threshold': np.concatenate(threshold), 'left': np.concatenate(left).astype(i32),
               'right': np.concatenate(right).astype(i32), 'value': np.ascontiguousarray(np.concatenate(value), dtype=np.float64)}
     return tables, K, type(est) is not DecisionTreeClassifier
+
+
+def _knn_tables(est, D):
+    """the training rows (_fit_X as float64) and their class indices (_y) of a Euclidean KNeighborsClassifier, with n_neighbors and
+    the weights code; (None, None, None) for anything isb_knn_predict_proba does not compute the same way"""
+    weights = est.weights
+    if not isinstance(weights, str) or weights not in KNN_WEIGHTS:
+        return None, None, None
+    p, metric = est.p, est.metric
+    if est.metric_params or not (metric == 'euclidean' or (metric == 'minkowski' and p == 2)):
+        return None, None, None
+    # the metric the model was fitted with (kneighbors uses it): a parameter change without a refit must agree with it
+    if getattr(est, 'effective_metric_', None) != 'euclidean' or getattr(est, 'effective_metric_params_', None):
+        return None, None, None
+    if getattr(est, 'outputs_2d_', True) or not isinstance(est._fit_X, np.ndarray):
+        return None, None, None
+    fit_x = np.asarray(est._fit_X, dtype=np.float64)
+    y = np.asarray(est._y)
+    K = len(est.classes_)
+    k = est.n_neighbors
+    if fit_x.ndim != 2 or fit_x.shape[1] != D or y.shape != (len(fit_x), ) or not isinstance(k, (int, np.integer)):
+        return None, None, None
+    if not (1 <= k <= min(KNN_MAX_NEIGHBOURS, len(fit_x))) or K > FOREST_MAX_CLASSES or len(fit_x) >= 2 ** 31:
+        return None, None, None
+    if len(y) and (y.min() < 0 or y.max() >= K):
+        return None, None, None
+    return {'fit_x': fit_x, 'y': y.astype(np.int32)}, K, {'n_neighbors': int(k), 'weights': KNN_WEIGHTS[weights]}
+
+
+def _linear_tables(est, D):
+    """coef_ [1 or K, D] and intercept_ of a LogisticRegression; (None, None) for any other layout"""
+    coef = np.asarray(est.coef_, dtype=np.float64)
+    K = len(est.classes_)
+    if coef.ndim != 2 or coef.shape[1] != D or coef.shape[0] != (1 if K == 2 else K) or K < 2 or K > FOREST_MAX_CLASSES:
+        return None, None
+    intercept = np.broadcast_to(np.asarray(est.intercept_, dtype=np.float64), (coef.shape[0], ))
+    return {'coef': coef, 'intercept': np.array(intercept)}, K

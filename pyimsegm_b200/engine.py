@@ -543,6 +543,17 @@ class Engine(object):
             ws = self.buf('ws_cm_predict', (max(wsb, 1),), torch.uint8)
             self._ck(lib.isb_mixture_predict_proba(_lib.ptr(x), N, _lib.ptr(d_n), cm.n_dims, K, _lib.ptr(t['prec_chol']), _lib.ptr(t['bvec']),
                                                    _lib.ptr(t['log_const']), _lib.ptr(proba), _lib.ptr(ws), C.c_size_t(wsb), st))
+        elif cm.kind == 'knn':
+            n_fit, k = len(cm.tables['y']), cm.params['n_neighbors']
+            wsb = lib.isb_knn_predict_workspace_bytes(N, n_fit, k)
+            ws = self.buf('ws_cm_predict', (max(wsb, 1),), torch.uint8)
+            self._ck(lib.isb_knn_predict_proba(_lib.ptr(x), N, _lib.ptr(d_n), cm.n_dims, _lib.ptr(t['fit_x']), n_fit, _lib.ptr(t['y']), k, K,
+                                               cm.params['weights'], _lib.ptr(proba), _lib.ptr(ws), C.c_size_t(wsb), st))
+        elif cm.kind == 'linear':
+            wsb = lib.isb_linear_predict_workspace_bytes(N, len(cm.tables['intercept']))
+            ws = self.buf('ws_cm_predict', (max(wsb, 1),), torch.uint8)
+            self._ck(lib.isb_linear_predict_proba(_lib.ptr(x), N, _lib.ptr(d_n), cm.n_dims, _lib.ptr(t['coef']), _lib.ptr(t['intercept']),
+                                                  len(cm.tables['intercept']), _lib.ptr(proba), _lib.ptr(ws), C.c_size_t(wsb), st))
         else:
             n_trees, n_nodes = len(cm.tables['roots']), len(cm.tables['left'])
             wsb = lib.isb_forest_predict_workspace_bytes(N, n_trees)
