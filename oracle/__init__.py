@@ -345,10 +345,13 @@ def pairwise_cost(gc_regul, nb_classes, max_cost=1e5):
 
 
 def integerise(edge_w, unary, pairwise):
-    """pyGCO cut_general_graph float path: returns int32 (w, unary, pairwise)"""
-    dwf = max(np.abs(unary).max(), np.abs(edge_w).max() * pairwise.max()) + 1e-10
+    """pyGCO cut_general_graph float path: returns int32 (w, unary, pairwise).  A NaN edge weight (degenerate edge model, DESIGN.md
+    section 2) is left out of the down-weight factor and becomes 0, where pyGCO's C cast is undefined; no edge at all is accepted"""
+    edge_w = np.asarray(edge_w, dtype=float)
+    ok = ~np.isnan(edge_w)
+    dwf = max(np.abs(unary).max(), (np.abs(edge_w[ok]).max() if ok.any() else 0.) * pairwise.max()) + 1e-10
     u = (unary / dwf * 100000).astype(np.intc)
-    w = (edge_w / dwf * 1000).astype(np.intc)
+    w = (np.where(ok, edge_w, 0.) / dwf * 1000).astype(np.intc)
     v = (pairwise * 100).astype(np.intc)
     return w, u, v
 

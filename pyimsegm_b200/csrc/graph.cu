@@ -286,7 +286,9 @@ __global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024) k_gc_energie
     // pyGCO: down_weight_factor = max(|unary|.max(), |w|.max() * pairwise.max()) + 1e-10
     const double dwf = fmax(umax, wmax * pmax) + 1e-10;
     for (int i = tid; i < N * K; i += nth) unary_i[i] = (int)((unary[i] / dwf) * 100000.0);
-    for (int e = tid; e < E; e += nth) edge_wi[e] = (int)((edge_w[e] / dwf) * 1000.0);
+    // a degenerate edge model (std(d) = 0 with d = 0, coincident centroids under a weight of 0) leaves a NaN weight: it stays NaN in
+    // edge_w as in the reference, fmax above kept it out of wmax, and its capacity is 0 (graph_cuts.integerise_energies on the host)
+    for (int e = tid; e < E; e += nth) { const double wv = edge_w[e]; edge_wi[e] = isnan(wv) ? 0 : (int)((wv / dwf) * 1000.0); }
     for (int i = tid; i < K * K; i += nth) smooth_i[i] = (int)(pairwise[i] * 100.0);
 }
 

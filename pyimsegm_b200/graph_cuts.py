@@ -592,6 +592,25 @@ def _canonical_int_edges(edges, w_i):
     return np.ascontiguousarray(out, dtype=np.int32), np.ascontiguousarray(np.minimum(merged_w[order], 2 ** 31 - 1), dtype=np.intc)
 
 
+def integerise_energies(edge_weights, unary_cost, pairwise_cost, down_weight_factor=None):
+    """ pyGCO's float -> int conversion of ``cut_general_graph``, as ``k_gc_energies`` (csrc/graph.cu) does it on the device:
+    truncation towards zero of ``unary / f * 1e5``, ``w / f * 1e3`` and ``pairwise * 100`` with
+    ``f = max(|unary|.max(), |w|.max() * pairwise.max()) + 1e-10``.  An edge weight that is NaN (a degenerate edge model: every
+    edge at the same distance, or coincident centroids under a weight that underflowed, DESIGN.md section 2) is left out of ``f``
+    and becomes capacity 0, where pyGCO's C cast of NaN is undefined; no edge (E = 0) counts as a largest weight of 0.
+
+    :return tuple(ndarray,ndarray,ndarray): int32 (edge weights [E], unary [N, K], pairwise [K, K])
+    """
+    w, un, pw = np.asarray(edge_weights), np.asarray(unary_cost), np.asarray(pairwise_cost)   # in their own types, as pyGCO does
+    nan_w = np.isnan(w)
+    if down_weight_factor is None:
+        w_max = np.abs(w[~nan_w]).max() if not nan_w.all() else 0.
+        down_weight_factor = max(np.abs(un).max(), w_max * pw.max()) + 1e-10
+    un_i = (un / down_weight_factor * 100000).astype(np.intc)
+    w_i = ((np.where(nan_w, 0, w) if nan_w.any() else w) / down_weight_factor * 1000).astype(np.intc)
+    return w_i, un_i, (pw * 100).astype(np.intc)
+
+
 def cut_general_graph(edges, edge_weights, unary_cost, pairwise_cost, n_iter=-1, algorithm='expansion', init_labels=None,
                       down_weight_factor=None):
     """ drop-in for ``gco.cut_general_graph`` (pyGCO) as the reference calls it (graph_cuts.py:735-744,
@@ -608,11 +627,7 @@ def cut_general_graph(edges, edge_weights, unary_cost, pairwise_cost, n_iter=-1,
     pw = np.asarray(pairwise_cost)
     is_float = any(a.dtype.kind == 'f' for a in (w, un, pw))
     if is_float:
-        if down_weight_factor is None:
-            down_weight_factor = max(np.abs(un).max(), (np.abs(w).max() if w.size else 0.) * pw.max()) + 1e-10
-        un_i = (un / down_weight_factor * 100000).astype(np.intc)
-        w_i = (w / down_weight_factor * 1000).astype(np.intc)
-        pw_i = (pw * 100).astype(np.intc)
+        w_i, un_i, pw_i = integerise_energies(w, un, pw, down_weight_factor)
     else:
         un_i, w_i, pw_i = un.astype(np.intc), w.astype(np.intc), pw.astype(np.intc)
     edges, w_i = _canonical_int_edges(edges, w_i)
