@@ -548,6 +548,32 @@ int isb_contingency_write(const void* y_true, int dtype_true, const void* y_pred
                           const long long* info, void* ws, size_t ws_bytes, int64_t* values_true, int64_t* values_pred, int64_t* counts,
                           isb_stream_t stream);
 
+/* k-means down-sampling of down_sample_dict_features_kmean (:1110-1134): the Lloyd runs of scikit-learn's
+ * KMeans(init='random', n_init=3, max_iter=5) and the sample nearest to each final centre.  X [n, D] f64 row-major, 1 <= k <= n;
+ * D <= 256, n <= 2^30 and k <= 4 194 240, else ISB_ERR_UNSUPPORTED.  ws: isb_kmeans_workspace_bytes(n, k, D) (0 out of range).
+ *
+ * isb_kmeans_lloyd continues one run of _kmeans_single_lloyd (unit weights) on the centred X from centres [k, D] (in / out),
+ * labels [n] i32 (in / out; -1 everywhere for a new run) and status [4] i32 (device, in / out; zeros for a new run):
+ *   status[0] 0 running, 1 strict convergence, 2 centre shift within tol, 3 stopped on an empty cluster, 4 max_iter sweeps done;
+ *   status[1] sweeps done; status[2] labels changed in the current sweep; status[3] empty clusters in the current sweep.
+ * A sweep labels every row by argmin_j |c_j|^2 - 2 x.c_j (FP64 tensor cores; lowest j on ties), writes the member sums [k, D] f64
+ * (members added in ascending row order) and counts [k] i32, and without an empty cluster sets c_j = sum_j * (1 / count_j), then
+ * stops strictly when no label changed or when the sum of squared centre shifts is <= tol.  A run that stops without strict
+ * convergence relabels the rows once more; every stopped run writes inertia [1] f64 = sum of (x - c_label)^2.  All of it is enqueued
+ * without a host read: the call enqueues `sweeps` sweeps (0 <= sweeps <= max_iter; max_iter - status[1] to finish the run, 0 to only
+ * relabel and sum the inertia of a run that has stopped), each of which does nothing once the run has stopped except its radix sort
+ * of the n (label, row) pairs.  A sweep with an empty cluster stops with status 3 and leaves labels, sums, counts and the centres it
+ * started from; the caller updates the centres, sets status (0 with status[1] + 1 sweeps to go on, or the code it stops with) and
+ * calls again.  Every call copies X into the workspace once (rows padded for the tensor-core tiles).  The member sums take one warp
+ * per cluster, so their time follows the largest cluster: with k = 1 one warp adds all n rows. */
+size_t isb_kmeans_workspace_bytes(int n, int k, int D);
+int isb_kmeans_lloyd(const double* X, int n, int D, int k, int max_iter, int sweeps, double tol, double* centres, int32_t* labels, int32_t* status,
+                     double* sums, int32_t* counts, double* inertia, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* nearest [k] i32: for every centre [k, D] the row of X of least squared distance sum_d (x_d - c_d)^2 (features added in order), the
+ * lowest row index among equal distances -- np.argmin(euclidean_distances(X, centres), axis=0) without the expansion's rounding */
+int isb_kmeans_nearest(const double* X, int n, int D, const double* centres, int k, int32_t* nearest, void* ws, size_t ws_bytes,
+                       isb_stream_t stream);
+
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);
 

@@ -137,6 +137,9 @@ SIGNATURES = {
     'isb_contingency_workspace_bytes': (_sz, [_i, _i]),
     'isb_contingency_count': (_i, [_vp, _i, _vp, _i, _ll, _vp, _i, _vp, _sz, C.POINTER(_ll), _vp]),
     'isb_contingency_write': (_i, [_vp, _i, _vp, _i, _ll, _vp, _i, C.POINTER(_ll), _vp, _sz, _vp, _vp, _vp, _vp]),
+    'isb_kmeans_workspace_bytes': (_sz, [_i, _i, _i]),
+    'isb_kmeans_lloyd': (_i, [_vp, _i, _i, _i, _i, _i, _d, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    'isb_kmeans_nearest': (_i, [_vp, _i, _i, _vp, _i, _vp, _vp, _sz, _vp]),
 }
 
 

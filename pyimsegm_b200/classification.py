@@ -1,5 +1,6 @@
 """
-The scoring half of the reference's ``imsegm/classification.py``: the metrics between annotations and segmentations.
+The reference's ``imsegm/classification.py`` without its classifier training: the metrics between annotations and segmentations,
+and the preparation of class-balanced training sets.
 
 Every number comes from one contingency table -- the pixels of every (annotation value, segmentation value) pair after the
 ``drop_labels`` mask -- counted on the device (``csrc/classification.cu``, one upload of the two maps and three passes over them).
@@ -28,16 +29,31 @@ Differences from the reference:
 - ``compute_stat_per_image`` runs the pairs one after the other on the device (the upload of a pair overlaps the counting of the
   previous one) and ignores ``nb_workers``; it shows no progress bar.
 
-Not provided: the training half of the module (the classifier zoo and its pipelines, parameter searches, cross-validation,
-feature selection, saving and loading classifiers, dataset balancing and down-sampling).  Those wrap scikit-learn estimators
-and have no pixel work to move to the device.  This is the one module of the package in which not every public name of the
-reference exists.
+The training sets: per-image superpixel features and labels into one class-balanced set (``compose_dict_label_features`` ..
+``convert_set_features_labels_2_dataset``).  ``balance_type='kmeans'`` runs scikit-learn's ``KMeans(init='random', n_init=3,
+max_iter=5)`` of every larger class on the device (``csrc/kmeans_sample.cu``); ``'random'`` and ``'unique'`` stay on the host with
+the reference's exact ``random`` / numpy semantics.  The k-means follows scikit-learn 1.9's ``fit``: the features centred on their
+column mean, ``tol = mean(var(X, axis=0)) * 1e-4``, the starting rows of the three runs drawn in order from numpy's global RNG (so a
+given ``np.random.seed`` gives scikit-learn's starts), Lloyd sweeps on the device with the host relocating empty clusters as
+``_relocate_empty_clusters_dense`` does, the best run by scikit-learn's rule, and its ``ConvergenceWarning``.  Then the row nearest
+to each centre.  The labels come from ``|c|^2 - 2 x.c`` in float64 as scikit-learn's, and the nearest rows from exact squared
+differences, so the selected rows can differ from scikit-learn's only where two distances agree to within rounding.  Features are
+clustered in float64 (scikit-learn clusters float32 features in float32), with at most 256 columns (``NotImplementedError``
+above).
+
+Not provided: the classifier zoo and its pipelines, parameter searches, cross-validation, feature selection, and saving and
+loading classifiers.  Those wrap scikit-learn estimators and have no heavy work to move to the device.  This is the one module of
+the package in which not every public name of the reference exists.
 """
+import collections
 import ctypes as C
 import logging
+import random
+import warnings
 
 import numpy as np
 from sklearn import metrics
+from sklearn.exceptions import ConvergenceWarning
 
 from . import _lib
 from .engine import get_engine
@@ -60,6 +76,11 @@ DICT_SCORING = {
     'precision': metrics.precision_score,
     'recall': metrics.recall_score,
 }
+
+#: decimal digits of the features before ``down_sample_dict_features_unique`` looks for equal rows
+ROUND_UNIQUE_FTS_DIGITS = 3
+# the k-means of down_sample_dict_features_kmean: KMeans(n_clusters=nb_samples, init='random', n_init=3, max_iter=5), tol 1e-4
+_KMEANS_N_INIT, _KMEANS_MAX_ITER, _KMEANS_TOL = 3, 5, 1e-4
 
 #: largest contingency table (cells)
 TABLE_MAX_CELLS = 1 << 28
@@ -541,3 +562,345 @@ def compute_metric_tpfp_tpfn(annot, segm, label_positive=None):
     """
     tp, _, fp, fn = compute_tp_tn_fp_fn(annot, segm, label_positive)
     return _ratio_tpfp_tpfn(tp, fp, fn)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# training sets: class-balanced features (k-means on the device)
+# ---------------------------------------------------------------------------------------------------------------------
+
+def _rows_array(blocks):
+    """the rows of the 2-D blocks stacked as ``np.array`` builds them from their ``tolist()``: floats as float64, integers as int64,
+    and ``np.array([])`` when there are no rows"""
+    blocks = [np.asarray(b) for b in blocks]
+    if sum(len(b) for b in blocks) == 0:
+        return np.array([])
+    rows = np.concatenate([b for b in blocks if len(b)])
+    if rows.dtype.kind == 'f':
+        return rows.astype(np.float64)
+    if rows.dtype.kind in 'iu' and (rows.dtype.kind == 'i' or rows.dtype.itemsize < 8):
+        return rows.astype(np.int64)
+    return np.array(rows.tolist())
+
+
+def shuffle_features_labels(features, labels):
+    """ features [n, D] and labels [n] permuted together by one ``np.random.shuffle`` of the row indices (reference
+    classification.py:1027-1051)
+
+    >>> np.random.seed(0)
+    >>> fts = np.random.random((5, 2))
+    >>> lbs = np.random.randint(0, 2, 5)
+    >>> fts_new, lbs_new = shuffle_features_labels(fts, lbs)
+    >>> np.array_equal(fts, fts_new)
+    False
+    >>> np.array_equal(lbs, lbs_new)
+    False
+    """
+    if len(features) != len(labels):
+        raise ValueError('features (%i) and labels (%i) should have equal length' % (len(features), len(labels)))
+    order = list(range(len(labels)))
+    np.random.shuffle(order)
+    return features[order, :], np.asarray(labels)[order]
+
+
+def convert_dict_label_features_2_vectors(dict_features):
+    """ {label: features [n_label, D]} -> (features [n, D] in the dict's order, list of the label of every row) (reference
+    classification.py:1054-1065)
+
+    >>> fts, lbs = convert_dict_label_features_2_vectors({1: np.ones((2, 3)), 0: np.zeros((1, 3))})
+    >>> fts.shape, lbs
+    ((3, 3), [1, 1, 0])
+    """
+    labels = []
+    for label, fts in dict_features.items():
+        labels.extend([label] * len(fts))
+    return _rows_array([dict_features[k] for k in dict_features]), labels
+
+
+def compose_dict_label_features(features, labels):
+    """ features [n, D] and labels [n] -> {label: its rows}, keys in the order of ``np.unique(labels)`` (reference
+    classification.py:1068-1080)
+
+    >>> d = compose_dict_label_features(np.arange(8).reshape(4, 2), np.array([1, 0, 1, 1]))
+    >>> sorted(d), d[0].tolist()
+    ([0, 1], [[2, 3]])
+    """
+    features = np.array(features)
+    dict_features = {}
+    for label in np.unique(labels):
+        dict_features[label] = features[labels == label, :]
+    return dict_features
+
+
+def down_sample_dict_features_random(dict_features, nb_samples):
+    """ at most ``nb_samples`` rows of every class: the first ``nb_samples`` of a ``random.shuffle`` (Python's global RNG) of its row
+    indices; smaller classes are copied (reference classification.py:1083-1107)
+
+    >>> np.random.seed(0)
+    >>> d_fts = {'a': np.random.random((100, 3))}
+    >>> d_fts = down_sample_dict_features_random(d_fts, 5)
+    >>> d_fts['a'].shape
+    (5, 3)
+    """
+    dict_features_new = {}
+    for label, features in dict_features.items():
+        if len(features) <= nb_samples:
+            dict_features_new[label] = features.copy()
+            continue
+        order = list(range(len(features)))
+        random.shuffle(order)
+        dict_features_new[label] = np.array(features)[order[:nb_samples], :]
+    return dict_features_new
+
+
+class _LloydRun(object):
+    """one Lloyd run: labels [n] int32, inertia, centres [k, D] (centred), sweeps"""
+
+    def __init__(self, labels, inertia, centres, n_iter):
+        self.labels, self.inertia, self.centres, self.n_iter = labels, inertia, centres, n_iter
+
+
+def _kmeans_seeds(n_samples, n_clusters):
+    """the starting rows of one run of KMeans(init='random') with unit weights, drawn from numpy's global RNG as
+    ``_init_centroids`` draws them"""
+    weight = np.ones(n_samples)
+    return np.random.choice(n_samples, size=n_clusters, replace=False, p=weight / weight.sum())
+
+
+def _relocate_empty_clusters(X, centres_old, sums, weights, labels):
+    """scikit-learn's _relocate_empty_clusters_dense (unit weights), in place on the member sums [k, D] and weights [k]: every empty
+    cluster takes one of the rows farthest from their centres, which leaves its cluster"""
+    empty = np.where(weights == 0)[0]
+    if len(empty) == 0:
+        return
+    dist = ((X - centres_old[labels]) ** 2).sum(axis=1)
+    far = np.argpartition(dist, -len(empty))[:-len(empty) - 1:-1]
+    if np.max(dist) == 0:                   # more clusters than distinct rows: nothing to move
+        return
+    for new_id, far_idx in zip(empty.tolist(), far.tolist()):
+        old_id = labels[far_idx]
+        sums[old_id] -= X[far_idx]
+        sums[new_id] = X[far_idx]
+        weights[new_id] = 1.
+        weights[old_id] -= 1.
+
+
+def _average_centres(sums, weights):
+    """scikit-learn's _average_centers: sum * (1 / weight); a cluster still empty takes the row of the heaviest cluster as it is at
+    that point of scikit-learn's in-place loop (averaged when the heaviest comes first, its sum otherwise)"""
+    heaviest = int(np.argmax(weights))
+    full = weights > 0
+    centres = sums.copy()
+    centres[full] = sums[full] * (1.0 / weights[full])[:, None]
+    empty = np.where(~full)[0]
+    centres[empty] = np.where((empty < heaviest)[:, None], sums[heaviest], centres[heaviest])
+    return centres
+
+
+def _same_clustering(labels1, labels2, n_clusters):
+    """scikit-learn's _is_same_clustering: every cluster of labels1 maps onto one cluster of labels2"""
+    mapping = np.full(n_clusters, -1, dtype=np.int64)
+    uq, first = np.unique(labels1, return_index=True)
+    mapping[uq] = labels2[first]
+    return bool(np.all(mapping[labels1] == labels2))
+
+
+def _lloyd(eng, d_x, X, centres, max_iter, tol):
+    """_kmeans_single_lloyd of scikit-learn from ``centres`` [k, D] on the centred rows X [n, D] (host) = d_x (device), unit
+    weights.  The sweeps run on the device; a sweep that leaves a cluster empty comes back here for the relocation."""
+    torch, lib, st = eng.torch, eng.lib, _lib.stream_ptr()
+    n, D = X.shape
+    k = len(centres)
+    d_c = eng.to_device(np.ascontiguousarray(centres, dtype=np.float64), 'km_centres')
+    labels = eng.buf('km_labels', n, torch.int32)
+    _lib.check(lib.isb_fill_i32(_lib.ptr(labels), n, -1, st))
+    status = eng.to_device(np.zeros(4, np.int32), 'km_status')
+    sums = eng.buf('km_sums', (k, D), torch.float64)
+    counts = eng.buf('km_counts', k, torch.int32)
+    inertia = eng.buf('km_inertia', 1, torch.float64)
+    ws_bytes = lib.isb_kmeans_workspace_bytes(n, k, D)
+    ws = eng.buf('km_ws', max(ws_bytes, 1), torch.uint8)
+    sweeps = max_iter
+    while True:
+        _lib.check(lib.isb_kmeans_lloyd(_lib.ptr(d_x), n, D, k, max_iter, sweeps, C.c_double(tol), _lib.ptr(d_c), _lib.ptr(labels), _lib.ptr(status),
+                                        _lib.ptr(sums), _lib.ptr(counts), _lib.ptr(inertia), _lib.ptr(ws), C.c_size_t(ws_bytes), st))
+        stat = eng.to_host(status).copy()
+        if stat[0] != 3:
+            break
+        # a cluster went empty: this sweep's update on the host, as lloyd_iter_chunked_dense does it
+        lab = eng.to_host(labels).copy()
+        c_old = eng.to_host(d_c).copy()
+        s = eng.to_host(sums).copy()
+        w = eng.to_host(counts).astype(np.float64)
+        _relocate_empty_clusters(X, c_old, s, w, lab)
+        c_new = _average_centres(s, w)
+        shift_tot = (np.sqrt(((c_new - c_old) ** 2).sum(axis=1)) ** 2).sum()
+        done = int(stat[1]) + 1
+        code = 1 if stat[2] == 0 else 2 if shift_tot <= tol else 4 if done >= max_iter else 0
+        d_c = eng.to_device(c_new, 'km_centres')
+        status = eng.to_device(np.array([code, done, 0, 0], np.int32), 'km_status')
+        sweeps = max_iter - done if code == 0 else 0
+    return _LloydRun(eng.to_host(labels).copy(), float(eng.to_host(inertia)[0]), eng.to_host(d_c).copy(), int(stat[1]))
+
+
+def _nearest_rows(eng, d_x, n, D, centres):
+    """for every centre the row of least exact squared distance, lowest row on ties (int64 [k])"""
+    torch, lib = eng.torch, eng.lib
+    k = len(centres)
+    d_c = eng.to_device(np.ascontiguousarray(centres, dtype=np.float64), 'km_centres')
+    nearest = eng.buf('km_nearest', k, torch.int32)
+    ws_bytes = lib.isb_kmeans_workspace_bytes(n, k, D)
+    ws = eng.buf('km_ws', max(ws_bytes, 1), torch.uint8)
+    _lib.check(lib.isb_kmeans_nearest(_lib.ptr(d_x), n, D, _lib.ptr(d_c), k, _lib.ptr(nearest), _lib.ptr(ws), C.c_size_t(ws_bytes),
+                                      _lib.stream_ptr()))
+    return eng.to_host(nearest).astype(np.int64)
+
+
+def _kmeans_sample(features, nb_samples, n_init=_KMEANS_N_INIT, max_iter=_KMEANS_MAX_ITER):
+    """np.argmin(KMeans(nb_samples, init='random', n_init, max_iter).fit_transform(features), axis=0) on the device:
+    (selected rows int64 [nb_samples], the runs in order, the best run)"""
+    X0 = np.asarray(features, dtype=np.float64)
+    if X0.ndim != 2:
+        raise ValueError('Expected 2D array, got %dD array instead' % X0.ndim)
+    if not np.all(np.isfinite(X0)):
+        raise ValueError('Input X contains NaN or infinity.')
+    n, D = X0.shape
+    if not 1 <= nb_samples <= n:
+        raise ValueError('n_samples=%d should be >= n_clusters=%d.' % (n, nb_samples))
+    tol = np.mean(np.var(X0, axis=0)) * _KMEANS_TOL
+    X_mean = X0.mean(axis=0)
+    X = X0 - X_mean
+    eng = get_engine()
+    d_x = eng.to_device(X, 'km_x')
+    runs, best = [], None
+    for _ in range(n_init):
+        run = _lloyd(eng, d_x, X, X[_kmeans_seeds(n, nb_samples)], max_iter, tol)
+        runs.append(run)
+        if best is None or (run.inertia < best.inertia and not _same_clustering(run.labels, best.labels, nb_samples)):
+            best = run
+    distinct = len(np.unique(best.labels))
+    if distinct < nb_samples:
+        warnings.warn('Number of distinct clusters ({}) found smaller than n_clusters ({}). Possibly due to duplicate points '
+                      'in X.'.format(distinct, nb_samples), ConvergenceWarning, stacklevel=3)
+    d_x0 = eng.to_device(X0, 'km_x')
+    return _nearest_rows(eng, d_x0, n, D, best.centres + X_mean), runs, best
+
+
+def down_sample_dict_features_kmean(dict_features, nb_samples):
+    """ ``nb_samples`` rows of every class: the rows nearest to the centres of KMeans(n_clusters=nb_samples, init='random',
+    n_init=3, max_iter=5) of its features, run on the device; the starts come from numpy's global RNG; smaller classes are copied
+    (reference classification.py:1110-1134)
+
+    >>> np.random.seed(0)
+    >>> d_fts = {'a': np.random.random((100, 3))}
+    >>> d_fts = down_sample_dict_features_kmean(d_fts, 5)  # doctest: +SKIP
+    >>> d_fts['a'].shape  # doctest: +SKIP
+    (5, 3)
+    """
+    dict_features_new = {}
+    for label, features in dict_features.items():
+        if len(features) <= nb_samples:
+            dict_features_new[label] = features.copy()
+            continue
+        selected, _, _ = _kmeans_sample(features, nb_samples)
+        dict_features_new[label] = features[selected, :]
+    return dict_features_new
+
+
+def unique_rows(data):
+    """ the distinct rows of a 2-D array, sorted lexicographically over the columns (numpy's structured-row ``np.unique``: rows
+    holding NaN never merge, -0.0 equals 0.0) (reference classification.py:1146-1156)
+
+    >>> unique_rows(np.array([[1, 2], [0, 5], [1, 2]]))
+    array([[0, 5],
+           [1, 2]])
+    """
+    data = np.array(data, order='C')
+    as_records = data.view(np.dtype([('f%d' % i, data.dtype) for i in range(data.shape[1])]))
+    return np.unique(as_records).view(data.dtype).reshape(-1, data.shape[1])
+
+
+def down_sample_dict_features_unique(dict_features):
+    """ the distinct rows of every class after rounding to ``ROUND_UNIQUE_FTS_DIGITS`` decimals (reference
+    classification.py:1159-1180)
+
+    >>> np.random.seed(0)
+    >>> d_fts = {'a': np.random.random((100, 3))}
+    >>> d_fts = down_sample_dict_features_unique(d_fts)
+    >>> d_fts['a'].shape
+    (100, 3)
+    """
+    dict_features_new = {}
+    for label in dict_features:
+        features = np.round(dict_features[label], ROUND_UNIQUE_FTS_DIGITS)
+        unique_fts = np.array(unique_rows(features))
+        if features.ndim != unique_fts.ndim:
+            raise ValueError('feature dim matching')
+        if features.shape[1] != unique_fts.shape[1]:
+            raise ValueError('features: %i <> %i' % (features.shape[1], unique_fts.shape[1]))
+        dict_features_new[label] = unique_fts
+    return dict_features_new
+
+
+def balance_dataset_by_(features, labels, balance_type='random', min_samples=None):
+    """ the same number of rows per class (reference classification.py:1183-1216): ``'random'``, ``'kmeans'`` (down to
+    ``min_samples``, default the smallest class) or ``'unique'`` (the distinct rounded rows); another name logs a warning and keeps
+    every row.  Returns (features [n, D], list of labels) grouped by class in the order of ``np.unique(labels)``.
+
+    >>> np.random.seed(0)
+    >>> fts, lbs = balance_dataset_by_(np.random.random((25, 3)), np.random.randint(0, 2, 25))
+    >>> fts.shape
+    (24, 3)
+    >>> lbs
+    [0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1]
+    """
+    logging.debug('balance dataset using "%s"', balance_type)
+    if not min_samples:
+        min_samples = min(collections.Counter(labels).values())
+    dict_features = compose_dict_label_features(features, labels)
+    kind = balance_type.lower()
+    if kind == 'random':
+        dict_features = down_sample_dict_features_random(dict_features, min_samples)
+    elif kind == 'kmeans':
+        dict_features = down_sample_dict_features_kmean(dict_features, min_samples)
+    elif kind == 'unique':
+        dict_features = down_sample_dict_features_unique(dict_features)
+    else:
+        logging.warning('not defined balancing method "%s"', balance_type)
+    return convert_dict_label_features_2_vectors(dict_features)
+
+
+def convert_set_features_labels_2_dataset(imgs_features, imgs_labels, drop_labels=None, balance_type=None):
+    """ the features and labels of every image (dicts by image name, taken in sorted name order) in one training set
+    (reference classification.py:1219-1262): rows whose label is in ``drop_labels`` left out, each image balanced by
+    ``balance_dataset_by_`` when ``balance_type`` is given.  Returns (features [n, D], labels int [n], rows per image).
+
+    >>> np.random.seed(0)
+    >>> d_fts = {'a': np.random.random((25, 3)),
+    ...          'b': np.random.random((30, 3)), }
+    >>> d_lbs = {'a': np.random.randint(0, 2, 25),
+    ...          'b': np.random.randint(0, 2, 30)}
+    >>> fts, lbs, sizes = convert_set_features_labels_2_dataset(d_fts, d_lbs)
+    >>> fts.shape
+    (55, 3)
+    >>> lbs.shape
+    (55,)
+    >>> sizes
+    [25, 30]
+    """
+    logging.debug('convert set of features and labels to single one')
+    if not all(k in imgs_labels for k in imgs_features):
+        raise ValueError('missing some items of %r' % imgs_labels.keys())
+    drop_labels = [] if drop_labels is None else drop_labels
+    blocks, labels_all, sizes = [], [], []
+    for name in sorted(imgs_features.keys()):
+        features = np.array(imgs_features[name])
+        labels = np.array(imgs_labels[name].astype(int))
+        for lb in drop_labels:
+            keep = labels != lb
+            features, labels = features[keep], labels[keep]
+        if balance_type is not None:
+            features, labels = balance_dataset_by_(features, labels, balance_type=balance_type)
+        blocks.append(features)
+        labels_all += np.asarray(labels).tolist()
+        sizes.append(len(labels))
+    return _rows_array(blocks), np.array(labels_all, dtype=int), sizes
