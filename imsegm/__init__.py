@@ -2,8 +2,9 @@
 Drop-in alias: ``import imsegm.pipelines`` (``superpixels``, ``descriptors``, ``graph_cuts``) resolves to the
 H100-native implementation in ``pyimsegm_b200`` for the SLIC -> features -> GraphCut hot path of Borda/pyImSegm and for the
 region growing (RG2SP) built on it, and for ``labeling``, ``ellipse_fitting``, ``annotation`` and ``classification``.  Of
-``classification`` the scoring (segmentations against annotations) and the training-set preparation (class balancing, k-means
-down-sampling on the device) are provided; the classifier training itself is not.
+``classification`` the scoring (segmentations against annotations), the training-set preparation (class balancing, k-means
+down-sampling on the device) and the classifier training (random forests and decision trees fitted on the device) are provided;
+cross-validation scoring and feature selection are not.
 """
 import sys
 

@@ -574,6 +574,33 @@ int isb_kmeans_lloyd(const double* X, int n, int D, int k, int max_iter, int swe
 int isb_kmeans_nearest(const double* X, int n, int D, const double* centres, int k, int32_t* nearest, void* ws, size_t ws_bytes,
                        isb_stream_t stream);
 
+/* exact-split Gini trees of scikit-learn's DecisionTreeClassifier / RandomForestClassifier fit (splitter 'best'), the classifier
+ * that create_classif_search_train_export (:656-759) trains; all T trees of a forest are built together, level by level.
+ *   x [n, D] f32 row-major (scikit-learn's trees cast X to float32), y [n] i32 class indices in [0, K), K <= 64;
+ *   counts [T, n] i32: the sample weight of every row in every tree (bootstrap counts, or ones); a row of count 0 is not in the tree;
+ *   seeds [T] u64 (device): the key of each tree's feature sampling.
+ *   max_features m in [1, D], min_samples_split >= 2, min_samples_leaf >= 1 (rows with a nonzero count), max_depth (-1: none),
+ *   min_impurity_decrease: the parameters as scikit-learn's fit resolves them.
+ * The split rules are scikit-learn 1.9's: Gini proxy improvement from the weighted class counts, positions where the next sorted value is
+ * above the previous + 1e-7f (float32) only, both sides >= min_samples_leaf rows, threshold x[p-1] / 2.0 + x[p] / 2.0 in f64, and the
+ * leaf tests of the depth-first builder.  Feature sampling differs from scikit-learn's sequential RNG: a node's candidates are the m
+ * non-constant features of least (h, feature), h = splitmix64(splitmix64(splitmix64(seed) ^ b) ^ feature) with b the node's
+ * breadth-first index in its tree (children of earlier parents first, left before right); equal proxies go to the lowest feature, then
+ * the lowest position.
+ * Outputs per tree t at [t * cap + node], nodes numbered in preorder (the depth-first builder's ids): left, right, feature (i32; -1, -1,
+ * -2 at a leaf), threshold (f64; -2.0 at a leaf), impurity (f64), n_node_samples (i32 rows), weighted_n_node_samples (f64),
+ * missing_go_to_left (u8: n_left > n_right at a split, 0 at a leaf), class_counts [.., K] i32 (weighted), node_count [T] i32 (device).
+ * cap >= 2 * nnz(counts[t]) - 1 for every t, else ISB_ERR_CAPACITY.  n_levels (host, optional): the levels built.
+ * Limits (ISB_ERR_UNSUPPORTED): D <= 2048, T * n * m < 2^31, a row count < 2^24, the total count of a tree < 2^26.
+ * The call synchronises the stream: it reads back a few integers per level to size the next launches.
+ * ws: isb_forest_fit_workspace_bytes(n, D, T, K, max_features) (0 out of range). */
+size_t isb_forest_fit_workspace_bytes(int n, int D, int T, int K, int max_features);
+int isb_forest_fit(const float* x, int n, int D, const int32_t* y, int K, const int32_t* counts, int T, const uint64_t* seeds, int max_features,
+                   int min_samples_split, int min_samples_leaf, int max_depth, double min_impurity_decrease, int cap, int32_t* left, int32_t* right,
+                   int32_t* feature, double* threshold, double* impurity, int32_t* n_node_samples, double* weighted_n_node_samples,
+                   uint8_t* missing_go_to_left, int32_t* class_counts, int32_t* node_count, int* n_levels /* host */, void* ws, size_t ws_bytes,
+                   isb_stream_t stream);
+
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);
 

@@ -41,19 +41,30 @@ differences, so the selected rows can differ from scikit-learn's only where two 
 clustered in float64 (scikit-learn clusters float32 features in float32), with at most 256 columns (``NotImplementedError``
 above).
 
-Not provided: the classifier zoo and its pipelines, parameter searches, cross-validation, feature selection, and saving and
-loading classifiers.  Those wrap scikit-learn estimators and have no heavy work to move to the device.  This is the one module of
-the package in which not every public name of the reference exists.
+The classifiers: the reference's zoo (``create_classifiers``), pipelines, parameter grids and distributions, searches, and saving and
+loading.  ``create_classif_search_train_export`` fits the final pipeline's StandardScaler and PCA on the host with scikit-learn, casts
+the transformed features to float32 and fits a ``'RandForest'`` or ``'DecTree'`` classifier on the device (``forest_fit.fit_tree_model``,
+``csrc/forest_fit.cu``): exact splits with scikit-learn 1.9's rules and its bootstrap draws, the features each node draws differing
+(see ``forest_fit``).  The other classifiers, parameters the device does not compute, and the parameter search itself
+(``GridSearchCV`` / ``RandomizedSearchCV``) stay on scikit-learn; after a search the refit of the best pipeline goes to the device.
+
+Not provided: cross-validation scoring and ROC (``eval_classif_cross_val_*``), ``feature_scoring_selection`` and
+``create_pipeline_neuron_net``.
 """
 import collections
 import ctypes as C
 import logging
+import os
+import pickle
 import random
 import warnings
 
 import numpy as np
-from sklearn import metrics
+from scipy.stats import randint as sp_randint
+from scipy.stats import uniform as sp_random
+from sklearn import decomposition, ensemble, linear_model, metrics, neighbors, pipeline, preprocessing, svm, tree
 from sklearn.exceptions import ConvergenceWarning
+from sklearn.model_selection import GridSearchCV, RandomizedSearchCV
 
 from . import _lib
 from .engine import get_engine
@@ -65,6 +76,16 @@ TEMPLATE_NAME_CLF = 'classifier_{}.pkl'
 DEFAULT_CLASSIF_NAME = 'RandForest'
 #: default (recommended) clustering for unsupervised segmentation
 DEFAULT_CLUSTERING = 'kMeans'
+#: file name of exported evaluation on feature quality
+NAME_CSV_FEATURES_SELECT = 'feature_selection.csv'
+#: exporting partial results about trained classifier
+NAME_CSV_CLASSIF_CV_SCORES = 'classif_{}_cross-val_scores-{}.csv'
+#: exporting partial results about trained classifier - Receiver Operating Characteristics
+NAME_CSV_CLASSIF_CV_ROC = 'classif_{}_cross-val_ROC-{}.csv'
+#: exporting partial results about trained classifier - Area Under Curve
+NAME_TXT_CLASSIF_CV_AUC = 'classif_{}_cross-val_AUC-{}.txt'
+#: default number of workers of a parameter search: half of the CPUs
+NB_WORKERS_SERACH = max(1, int((os.cpu_count() or 1) * 0.5))
 #: default types of computed metrics
 METRIC_AVERAGES = ('macro', 'weighted')
 #: default computed metrics
@@ -904,3 +925,320 @@ def convert_set_features_labels_2_dataset(imgs_features, imgs_labels, drop_label
         labels_all += np.asarray(labels).tolist()
         sizes.append(len(labels))
     return _rows_array(blocks), np.array(labels_all, dtype=int), sizes
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# classifiers: the reference's zoo, searches, training (trees and forests on the device), export
+# ---------------------------------------------------------------------------------------------------------------------
+
+def create_classifiers(nb_workers=-1):
+    """ every classifier of the reference with its default parameters (reference classification.py:86-124)
+
+    >>> classifs = create_classifiers()
+    >>> sorted(classifs)
+    ['AdaBoost', 'DecTree', 'GradBoost', 'KNN', 'LogistRegr', 'RandForest', 'SVM']
+    >>> sum([isinstance(create_clf_param_search_grid(k), dict) for k in classifs.keys()])
+    7
+    >>> sum([isinstance(create_clf_param_search_distrib(k), dict) for k in classifs.keys()])
+    7
+    """
+    return {
+        'RandForest': ensemble.RandomForestClassifier(n_estimators=20, min_samples_leaf=2, min_samples_split=3, n_jobs=nb_workers),
+        'GradBoost': ensemble.GradientBoostingClassifier(subsample=0.25, warm_start=False, max_depth=6, min_samples_leaf=6,
+                                                         n_estimators=200, min_samples_split=7),
+        'LogistRegr': linear_model.LogisticRegression(solver='sag', n_jobs=nb_workers),
+        'KNN': neighbors.KNeighborsClassifier(n_jobs=nb_workers),
+        'SVM': svm.SVC(kernel='rbf', probability=True, tol=2e-3, max_iter=5000),
+        'DecTree': tree.DecisionTreeClassifier(),
+        'AdaBoost': ensemble.AdaBoostClassifier(n_estimators=5),
+    }
+
+
+def create_clf_pipeline(name_classif=DEFAULT_CLASSIF_NAME, pca_coef=0.95):
+    """ StandardScaler, an optional PCA(pca_coef) and the named classifier (reference classification.py:127-143)
+
+    >>> create_clf_pipeline()  # doctest: +ELLIPSIS
+    Pipeline(...)
+    """
+    components = [('scaler', preprocessing.StandardScaler())]
+    if pca_coef is not None:
+        components += [('reduce_dim', decomposition.PCA(pca_coef))]
+    components += [('classif', create_classifiers()[name_classif])]
+    return pipeline.Pipeline(components)
+
+
+def create_clf_param_search_grid(name_classif=DEFAULT_CLASSIF_NAME):
+    """ parameter grid of a grid search (reference classification.py:146-208); {} and a warning for an unknown name
+
+    >>> create_clf_param_search_grid('RandForest') # doctest: +ELLIPSIS
+    {'classif__...': ...}
+    >>> dict_classif = create_classifiers()
+    >>> all(len(create_clf_param_search_grid(k)) > 0 for k in dict_classif)
+    True
+    >>> create_clf_param_search_grid('none')
+    {}
+    """
+
+    def _log_space(b, e, n):
+        return np.unique(np.logspace(b, e, n).astype(int)).tolist()
+
+    clf_params = {
+        'RandForest': {
+            'classif__n_estimators': _log_space(0, 2, 40),
+            'classif__min_samples_split': [2, 3, 5, 7, 9],
+            'classif__min_samples_leaf': [1, 2, 4, 6, 9],
+            'classif__criterion': ('gini', 'entropy'),
+        },
+        'KNN': {
+            'classif__n_neighbors': _log_space(0, 2, 20),
+            'classif__algorithm': ('ball_tree', 'kd_tree'),
+            'classif__weights': ('uniform', 'distance'),
+            'classif__leaf_size': _log_space(0, 1.5, 10),
+        },
+        'SVM': {
+            'classif__C': np.linspace(0.2, 1., 8).tolist(),
+            'classif__kernel': ('poly', 'rbf', 'sigmoid'),
+            'classif__degree': [1, 2, 4, 6, 9],
+        },
+        'DecTree': {
+            'classif__criterion': ('gini', 'entropy'),
+            'classif__min_samples_split': [2, 3, 5, 7, 9],
+            'classif__min_samples_leaf': range(1, 7, 2),
+        },
+        'GradBoost': {
+            'classif__n_estimators': _log_space(0, 2, 25),
+            'classif__max_depth': range(1, 7, 2),
+            'classif__min_samples_split': [2, 3, 5, 7, 9],
+            'classif__min_samples_leaf': range(1, 7, 2),
+        },
+        'LogistRegr': {
+            'classif__C': np.linspace(0., 1., 5).tolist(),
+            'classif__solver': ('lbfgs', 'sag'),
+        },
+        'AdaBoost': {
+            'classif__n_estimators': _log_space(0, 2, 20),
+        }
+    }
+    if name_classif not in clf_params:
+        clf_params[name_classif] = {}
+        logging.warning('not defined classifier name "%s"', name_classif)
+    return clf_params[name_classif]
+
+
+def create_clf_param_search_distrib(name_classif=DEFAULT_CLASSIF_NAME):
+    """ parameter distributions of a random search (reference classification.py:211-268); {} for an unknown name
+
+    >>> create_clf_param_search_distrib()  # doctest: +ELLIPSIS
+    {...}
+    >>> dict_classif = create_classifiers()
+    >>> all(len(create_clf_param_search_distrib(k)) > 0 for k in dict_classif)
+    True
+    >>> create_clf_param_search_distrib('none')
+    {}
+    """
+    clf_params = {
+        'RandForest': {
+            'classif__n_estimators': sp_randint(2, 25),
+            'classif__min_samples_split': sp_randint(2, 9),
+            'classif__min_samples_leaf': sp_randint(1, 7),
+        },
+        'KNN': {
+            'classif__n_neighbors': sp_randint(5, 25),
+            'classif__algorithm': ('ball_tree', 'kd_tree'),
+            'classif__weights': ('uniform', 'distance'),
+        },
+        'SVM': {
+            'classif__C': sp_random(0., 1.),
+            'classif__kernel': ('poly', 'rbf', 'sigmoid'),
+            'classif__degree': sp_randint(2, 9),
+        },
+        'DecTree': {
+            'classif__criterion': ('gini', 'entropy'),
+            'classif__min_samples_split': sp_randint(2, 9),
+            'classif__min_samples_leaf': sp_randint(1, 7),
+        },
+        'GradBoost': {
+            'classif__n_estimators': sp_randint(10, 200),
+            'classif__max_depth': sp_randint(1, 7),
+            'classif__min_samples_split': sp_randint(2, 9),
+            'classif__min_samples_leaf': sp_randint(1, 7),
+        },
+        'LogistRegr': {
+            'classif__C': sp_random(0., 1.),
+            'classif__solver': ('newton-cg', 'lbfgs', 'sag'),
+        },
+        'AdaBoost': {
+            'classif__n_estimators': sp_randint(2, 100),
+        }
+    }
+    return clf_params.get(name_classif, {})
+
+
+def search_params_cut_down_max_nb_iter(clf_parameters, nb_iter):
+    """ ``nb_iter`` capped at the number of combinations when every parameter is a list (reference classification.py:953-977)
+
+    >>> clf_params = create_clf_param_search_grid(DEFAULT_CLASSIF_NAME)
+    >>> search_params_cut_down_max_nb_iter(clf_params, 100)
+    100
+    >>> search_params_cut_down_max_nb_iter(clf_params, 1e6)
+    1450
+    """
+    counts = []
+    for k in clf_parameters:
+        vals = clf_parameters[k]
+        if hasattr(vals, '__iter__'):
+            counts.append(len(vals))
+        else:
+            return nb_iter
+    count = int(np.prod(counts))
+    if count < nb_iter:
+        nb_iter = count
+    return nb_iter
+
+
+def create_classif_search(name_clf, clf_pipeline, nb_labels, search_type='random', cross_val=10, eval_metric='f1', nb_iter=250,
+                          nb_workers=5):
+    """ scikit-learn's GridSearchCV (``search_type='grid'``) or RandomizedSearchCV of the pipeline, scored by ``eval_metric`` with
+    the weighted average for more than two labels (reference classification.py:980-1024)"""
+    score_weight = 'weighted' if nb_labels > 2 else 'binary'
+    scoring = metrics.make_scorer(DICT_SCORING[eval_metric.lower()], average=score_weight)
+    if search_type == 'grid':
+        clf_parameters = create_clf_param_search_grid(name_clf)
+        logging.info('init Grid search...')
+        return GridSearchCV(clf_pipeline, clf_parameters, scoring=scoring, cv=cross_val, n_jobs=nb_workers, verbose=1, refit=True)
+    clf_parameters = create_clf_param_search_distrib(name_clf)
+    nb_iter = search_params_cut_down_max_nb_iter(clf_parameters, nb_iter)
+    logging.info('init Randomized search...')
+    return RandomizedSearchCV(clf_pipeline, clf_parameters, scoring=scoring, cv=cross_val, n_jobs=nb_workers, n_iter=nb_iter, verbose=1,
+                              refit=True)
+
+
+def save_classifier(path_out, classif, clf_name, params, feature_names=None, label_names=None):
+    """ pickle {'params', 'name', 'clf_pipeline', 'features', 'label_names'} to ``path_out/classifier_<name>.pkl`` and return its path
+    (reference classification.py:547-586)
+
+    >>> import tempfile
+    >>> clf = create_classifiers()['RandForest']
+    >>> with tempfile.TemporaryDirectory() as tmp:
+    ...     p_clf = save_classifier(tmp, clf, 'TESTINNG', {})
+    ...     d_clf = load_classifier(p_clf)
+    >>> os.path.basename(p_clf)
+    'classifier_TESTINNG.pkl'
+    >>> sorted(d_clf.keys())
+    ['clf_pipeline', 'features', 'label_names', 'name', 'params']
+    >>> d_clf['clf_pipeline']  # doctest: +ELLIPSIS
+    RandomForestClassifier(...)
+    """
+    if not os.path.isdir(path_out):
+        raise FileNotFoundError('missing folder: %s' % path_out)
+    dict_classif = {
+        'params': params,
+        'name': clf_name,
+        'clf_pipeline': classif,
+        'features': feature_names,
+        'label_names': label_names,
+    }
+    path_clf = os.path.join(path_out, TEMPLATE_NAME_CLF.format(clf_name))
+    logging.info('export classif. of %s to "%s"', dict_classif, path_clf)
+    with open(path_clf, 'wb') as f:
+        pickle.dump(dict_classif, f)
+    return path_clf
+
+
+def load_classifier(path_classif):
+    """ the dictionary ``save_classifier`` wrote, or None when the file does not exist (reference classification.py:589-605)
+
+    >>> load_classifier('none.abc')
+    """
+    logging.info('import classifier from "%s"', path_classif)
+    if not os.path.isfile(path_classif):
+        logging.debug('classifier does not exist')
+        return None
+    with open(path_classif, 'rb') as f:
+        dict_clf = pickle.load(f)
+    logging.debug('load classifier: %r', dict_clf.keys())
+    return dict_clf
+
+
+def export_results_clf_search(path_out, clf_name, clf_search):
+    """ the search's ``cv_results_`` and best parameters as ``classif_<name>_search_params_{scores,best}.txt`` (reference
+    classification.py:608-632)"""
+    if not os.path.isdir(path_out):
+        raise FileNotFoundError('missing folder: %s' % path_out)
+
+    def _fn_path_out(s):
+        return os.path.join(path_out, 'classif_%s_%s.txt' % (clf_name, s))
+
+    with open(_fn_path_out('search_params_scores'), 'w') as fp:
+        results = 'no results'
+        if hasattr(clf_search, 'cv_results_'):
+            results = '\n'.join(['"%s": %r' % (k, clf_search.cv_results_[k]) for k in clf_search.cv_results_])
+        fp.write(results)
+    with open(_fn_path_out('search_params_best'), 'w') as fp:
+        params = clf_search.best_params_
+        rows = ['{:30s} {}'.format('"{}":'.format(k), params[k]) for k in params]
+        fp.write('\n'.join(rows))
+
+
+def _fit_pipeline(clf_pipeline, features, labels):
+    """``clf_pipeline.fit(features, labels)`` with a tree or forest as the final step fitted on the device: the transforms are fitted on
+    the host by scikit-learn, their output cast to float32 and the classifier fitted by ``forest_fit.fit_tree_model``.  Any other
+    classifier, or parameters the device does not compute, keep scikit-learn's fit."""
+    from sklearn.base import clone
+    from .forest_fit import _supported, fit_tree_model
+    steps = clf_pipeline.steps
+    name, final = steps[-1]
+    if type(clf_pipeline) is not pipeline.Pipeline or _supported(final) is None:
+        return clf_pipeline.fit(features, labels)
+    Xt = np.asarray(features)
+    for _, step in steps[:-1]:
+        if step is None or (isinstance(step, str) and step == 'passthrough'):
+            continue
+        Xt = step.fit_transform(Xt, labels)
+    fitted = fit_tree_model(clone(final), np.asarray(Xt, dtype=np.float32), labels)
+    if fitted is None:
+        fitted = clone(final).fit(Xt, labels)
+    clf_pipeline.steps[-1] = (name, fitted)
+    return clf_pipeline
+
+
+def create_classif_search_train_export(clf_name, features, labels, cross_val=10, nb_search_iter=100, search_type='random',
+                                       eval_metric='f1', nb_workers=NB_WORKERS_SERACH, path_out=None, params=None, pca_coef=0.98,
+                                       feature_names=None, label_names=None):
+    """ the pipeline ``create_clf_pipeline(clf_name, pca_coef)``, its parameters searched when ``nb_search_iter > 1`` or
+    ``search_type == 'grid'``, fitted on all features and exported to ``path_out`` when that is a directory (reference
+    classification.py:656-759).  Returns (fitted pipeline, path of the exported classifier or ``path_out``).  The final fit of a
+    ``'RandForest'`` / ``'DecTree'`` pipeline runs on the device (see the module's description).
+
+    >>> np.random.seed(0)
+    >>> lbs = np.random.randint(0, 3, 150)
+    >>> fts = np.random.random((150, 5)) + np.tile(lbs, (5, 1)).T
+    >>> _, _ = create_classif_search_train_export('LogistRegr', fts, lbs, nb_search_iter=0)
+    """
+    if not list(labels):
+        raise RuntimeError('some labels has to be given')
+    features = np.nan_to_num(features)
+    if len(features) != len(labels):
+        raise ValueError('features (%i) and labels (%i) should have equal length' % (len(features), len(labels)))
+    if not (features.ndim == 2 and features.shape[1] > 0):
+        raise ValueError('at least one feature is required')
+    logging.debug('training data: %r, labels (%i): %r', features.shape, len(labels), collections.Counter(labels))
+    logging.info('create Classifier: %s', clf_name)
+    clf_pipeline = create_clf_pipeline(clf_name, pca_coef)
+    if nb_search_iter > 1 or search_type == 'grid':
+        logging.debug('Performing param search...')
+        nb_labels = len(np.unique(labels))
+        clf_search = create_classif_search(clf_name, clf_pipeline, nb_labels=nb_labels, search_type=search_type, cross_val=cross_val,
+                                           eval_metric=eval_metric, nb_iter=nb_search_iter, nb_workers=nb_workers)
+        clf_search.fit(features, relabel_sequential(labels))
+        logging.info('Best score: %r', clf_search.best_score_)
+        clf_pipeline = clf_search.best_estimator_
+        logging.info('Best parameters set: \n %r', clf_pipeline.get_params())
+        if path_out is not None and os.path.isdir(path_out):
+            export_results_clf_search(path_out, clf_name, clf_search)
+    clf_pipeline = _fit_pipeline(clf_pipeline, features, labels)
+    if path_out is not None and os.path.isdir(path_out):
+        path_classif = save_classifier(path_out, clf_pipeline, clf_name, params, feature_names, label_names)
+    else:
+        path_classif = path_out
+    return clf_pipeline, path_classif
