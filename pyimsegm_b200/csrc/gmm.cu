@@ -361,7 +361,7 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
     __shared__ double s_logdet[KMAX];
     __shared__ double s_lower;
     __shared__ double s_cent[KMAX * DMAX];
-    __shared__ double s_tot[KMAX * (1 + DMAX)];
+    __shared__ double s_tot[KMAX * (1 + DMAX) + 1];   // k-means counts and sums, then the "a label changed" flag
     __shared__ int s_pick;
     const int N = n_dev ? min(*n_dev, N_in) : N_in;
     const int init = blockIdx.x / CL;
@@ -462,7 +462,7 @@ __global__ void __launch_bounds__(GT) k_gmm_fit(int N_in, const int* n_dev, int 
             changed = __syncthreads_or(changed);
             // new centres: count and coordinate sums of every cluster in ONE quantity-parallel pass over sample slices
             // (quantity q = (k, j): j == 0 the count, j >= 1 the sum of coordinate j-1); quantity Q carries the "changed" flag
-            const int Q = K * (1 + D);                 // <= 8 * 17 = 136 < GT
+            const int Q = K * (1 + D);                 // <= 8 * 17 = 136 < GT; s_tot holds Q + 1 values
             const int S = max(1, GT / (Q + 1));
             {
                 const int q = threadIdx.x % (Q + 1), sl = threadIdx.x / (Q + 1);

@@ -6,6 +6,7 @@ import pytest
 from sklearn import decomposition, mixture, preprocessing
 
 from conftest import synth_regions
+from oracle.mixture import shared_start_fit
 
 pytestmark = pytest.mark.gpu
 
@@ -25,19 +26,8 @@ def _blobs(D, K, seed, n=5000):
     return X, y, y0
 
 
-class _SharedStartBGM(mixture.BayesianGaussianMixture):
-    """BayesianGaussianMixture started from a given hard assignment (sklearn 1.9's _initialize_parameters signature)"""
-
-    def __init__(self, y0=None, **kw):
-        super().__init__(**kw)
-        self.y0 = y0
-
-    def _initialize_parameters(self, X, random_state, xp=None):
-        self._initialize(X, np.eye(self.n_components)[self.y0])
-
-
 def _ref_bgm(Z, K, y0, max_iter):
-    return _SharedStartBGM(y0=y0, n_components=K, covariance_type='full', n_init=1, max_iter=max_iter).fit(Z)
+    return shared_start_fit(Z, y0, K, 'BGM', max_iter)
 
 
 def _check_bgm(bgm, ref):
@@ -136,12 +126,7 @@ def test_scaler_pca_mixture_matches_sklearn_pipeline(kind, D, K):
         ref = _ref_bgm(P, K, y0, 99)
         _check_bgm(mm, ref)
     else:
-        resp = np.eye(K)[y0]
-        nk = resp.sum(0) + 10 * np.finfo(float).eps
-        means0 = resp.T @ P / nk[:, None]
-        covs0 = np.array([((resp[:, k, None] * (P - means0[k])).T @ (P - means0[k])) / nk[k] + 1e-6 * np.eye(P.shape[1]) for k in range(K)])
-        ref = mixture.GaussianMixture(K, covariance_type='full', max_iter=99, n_init=1, weights_init=nk / len(P), means_init=means0,
-                                      precisions_init=np.linalg.inv(covs0)).fit(P)
+        ref = shared_start_fit(P, y0, K, 'GMM', 99)
         assert mm.n_iter_ == ref.n_iter_ and mm.converged_ == ref.converged_
         np.testing.assert_allclose(mm.means_, ref.means_, rtol=1e-6, atol=1e-8)
         np.testing.assert_allclose(mm.lower_bound_, ref.lower_bound_, rtol=1e-8)

@@ -191,7 +191,8 @@ def test_pipeline_with_shared_model_equals_oracle(oracle):
 def test_device_gmm_matches_sklearn_from_shared_start():
     """estim_class_model (imsegm/graph_cuts.py:73-163): same EM as sklearn's GaussianMixture when both start from the
     same hard assignment; tolerance 1e-6 on parameters and probabilities (EM amplifies summation-order noise)"""
-    from sklearn import mixture, preprocessing
+    from sklearn import preprocessing
+    from oracle.mixture import shared_start_fit
     from pyimsegm_b200 import graph_cuts as gc
     rng = np.random.RandomState(3)
     K, D = 3, 3
@@ -207,12 +208,7 @@ def test_device_gmm_matches_sklearn_from_shared_start():
     np.testing.assert_allclose(scaler.mean_, Xs.mean_, rtol=1e-12)
     np.testing.assert_allclose(scaler.scale_, Xs.scale_, rtol=1e-12)
     Z = Xs.transform(X)
-    resp = np.eye(K)[y0]
-    nk = resp.sum(0) + 10 * np.finfo(float).eps
-    means0 = resp.T @ Z / nk[:, None]
-    covs0 = np.array([((resp[:, k, None] * (Z - means0[k])).T @ (Z - means0[k])) / nk[k] + 1e-6 * np.eye(D) for k in range(K)])
-    ref = mixture.GaussianMixture(K, covariance_type='full', max_iter=99, n_init=1, weights_init=nk / len(Z), means_init=means0,
-                                  precisions_init=np.linalg.inv(covs0)).fit(Z)
+    ref = shared_start_fit(Z, y0, K, 'GMM', max_iter=99)
     assert gmm.n_iter_ == ref.n_iter_ and gmm.converged_ == ref.converged_
     np.testing.assert_allclose(gmm.weights_, ref.weights_, rtol=1e-6)
     np.testing.assert_allclose(gmm.means_, ref.means_, rtol=1e-6, atol=1e-8)
@@ -231,7 +227,8 @@ def test_device_gmm_matches_sklearn_from_shared_start():
 def test_device_gmm_large_d_matches_sklearn_from_shared_start(D, K):
     """the large-D path of the device class model (batched FP64 GEMMs + Cholesky; colour + Leung-Malik features give
     D = 189): same EM as sklearn from the same hard start, tolerance 1e-6 as for the small path"""
-    from sklearn import mixture, preprocessing
+    from sklearn import preprocessing
+    from oracle.mixture import shared_start_fit
     from pyimsegm_b200 import graph_cuts as gc
     rng = np.random.RandomState(D)
     sizes = (700, 900, 600, 800)[:K]
@@ -245,12 +242,7 @@ def test_device_gmm_large_d_matches_sklearn_from_shared_start(D, K):
     model = gc.estim_class_model_device(X, K, use_scaler=True, max_iter=99, init_labels=y0)
     gmm = model.named_steps['model']
     Z = preprocessing.StandardScaler().fit(X).transform(X)
-    resp = np.eye(K)[y0]
-    nk = resp.sum(0) + 10 * np.finfo(float).eps
-    means0 = resp.T @ Z / nk[:, None]
-    covs0 = np.array([((resp[:, k, None] * (Z - means0[k])).T @ (Z - means0[k])) / nk[k] + 1e-6 * np.eye(D) for k in range(K)])
-    ref = mixture.GaussianMixture(K, covariance_type='full', max_iter=99, n_init=1, weights_init=nk / len(Z), means_init=means0,
-                                  precisions_init=np.linalg.inv(covs0)).fit(Z)
+    ref = shared_start_fit(Z, y0, K, 'GMM', max_iter=99)
     assert gmm.n_iter_ == ref.n_iter_ and gmm.converged_ == ref.converged_
     np.testing.assert_allclose(gmm.weights_, ref.weights_, rtol=1e-6)
     np.testing.assert_allclose(gmm.means_, ref.means_, rtol=1e-6, atol=1e-8)
