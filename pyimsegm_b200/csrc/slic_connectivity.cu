@@ -7,32 +7,55 @@
 // ("adjacent", 0 when none), otherwise it gets the next new label.
 //
 // Parallel decomposition with the same result:
-//   1. 4-connected component labelling by union-find; component id = its first pixel in raster order
-//      (row runs are linked without atomics, only run-to-run vertical links use atomicMin unions).
+//   1. 4-connected component labelling by union-find; component id = its first pixel in raster order.
+//      Each 32 x 64 tile is labelled in shared memory (its local roots are the first pixels of its local components, since
+//      local and global raster order agree inside a tile); only local roots take part in the global unions across the tile
+//      seams, and the size and box of a component are summed from its local roots.
 //   2. components >= max_size ("oversize", rare) are cut exactly as the truncated BFS would cut them: the
 //      pieces depend only on the component's own shape, so one thread replays the BFS per such component.
 //   3. a piece is "labelled before C" iff its first pixel precedes C's first pixel, so new labels of kept
-//      pieces are a raster-order prefix count of kept roots, and each small piece C replays its own BFS to
-//      find the last foreign neighbour pixel whose piece id is < C; chains small->small are followed to a
-//      kept piece (or to label 0 when the chain ends without one).
-// HBM traffic: a handful of 4 B/px passes over the label map and the scratch arrays.
+//      pieces are a raster-order prefix count of kept roots (a popcount over a bitmap of them), and each small piece C
+//      replays its own BFS to find the last foreign neighbour pixel whose piece id is < C; chains small->small are
+//      followed to a kept piece (or to label 0 when the chain ends without one).
+// HBM traffic: the label map read once, parent written once and read back once, out written once (16 B/px); everything else
+// is per local root or per piece.
 #include "common.cuh"
 
 namespace {
 
+constexpr int TH = 32, TW = 64, TPIX = TH * TW; // labelling tile
+constexpr int WIN = 4096;                        // small-piece window (box plus a one-pixel ring), pixels
+constexpr int RANK_WORDS = 1024;                 // kept-bitmap words per rank block (32768 pixels)
+
+// counters in ConnWs::ctr; k_small_adjacent reads its list length from [1] and its queue cursor from [2]
+enum { C_OVER = 0, C_FALLBACK = 1, C_QUEUE = 2, C_LROOTS = 3, C_WINDOW = 4, C_N = 8 };
+
 struct ConnWs {
-    int* comp;     // [HW] component id (root pixel index); ~id while an oversize split is being written
-    int* size;     // [HW] size, valid at roots
-    int* aux;      // [HW] at kept roots: new label; at small roots: adjacent piece id (-1 none)
-    int* queue;    // [HW] BFS queues
-    int* list;     // [HW] oversize list, later small-root list
-    int* row_cnt;  // [H + 1]
-    int* ctr;      // [8] counters: 0 n_oversize, 1 n_small, 2 queue cursor
-    int4* bbox;    // [n_oversize_max]
+    int* parent;    // [HW] pixel -> its tile-local root; local root -> global root after the root pass.  Flattened (pixel -> root)
+                    // when oversize components or fallback pieces exist: then ~piece start on oversize pixels, VISBIT from the fallback BFS
+    int* size;      // [HW] at local roots: their size, summed into the global root; at oversize piece starts: the piece size
+    int* ymax;      // [HW] box at local roots, summed the same way (a root's first row is its own row)
+    int* xmin;      // [HW]
+    int* xmax;      // [HW]
+    int* aux;       // [HW] at kept roots: new label; at small roots: -2-adjacent, or -1 when there is none
+    int* lroots;    // [HW] local roots; once classified, the BFS queues of the oversize split and of the fallback
+    int* window;    // [HW] small roots whose window fits WIN
+    int* fallback;  // [HW] the other small roots, and small pieces of oversize splits
+    int* over;      // [HW / 16 + 16] oversize roots (max_size >= 16)
+    int* ctr;       // [C_N] counters, then blk and kept: one zeroed range
+    int* blk;       // [n_rank_blocks] kept pieces per rank block
+    unsigned* kept; // [ceil(HW / 32)] kept-piece bitmap over first pixels
 };
 
-constexpr int VISBIT = 1 << 30; // 'visited by the small-piece BFS' flag kept inside comp[] (pixel indices stay below 2^30)
+constexpr int VISBIT = 1 << 30; // 'visited by the fallback BFS' flag kept inside parent[] (pixel indices stay below 2^30)
 __device__ __forceinline__ int dec(int c) { return (c < 0 ? ~c : c) & ~VISBIT; }
+
+// piece id of pixel p: through its local root (or, once flattened, its root) to the root, or the oversize piece it was cut into
+__device__ __forceinline__ int resolve(const int* parent, int p)
+{
+    const int a = parent[p];
+    return dec(a < 0 ? a : parent[a & ~VISBIT]);
+}
 
 __device__ __forceinline__ int find_root(const int* parent, int i)
 {
@@ -56,101 +79,215 @@ __device__ __forceinline__ void unite(int* parent, int a, int b)
     }
 }
 
-// one CTA per row: parent[p] = index of the start of p's run of equal labels
-__global__ void __launch_bounds__(256) k_row_runs(const int* __restrict__ lab, int H, int W, int* __restrict__ parent)
+__device__ __forceinline__ int sfind(const volatile int* par, int i)
 {
-    const int y = blockIdx.x;
-    const int* row = lab + (size_t)y * W;
-    int* prow = parent + (size_t)y * W;
-    __shared__ int s_warp[8];
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < W; base += 256) {
-        int x = base + threadIdx.x;
-        int v = -1; // start index if this pixel starts a run
-        if (x < W) v = (x == 0 || row[x - 1] != row[x]) ? x : -1;
-        // inclusive max-scan
+    while (true) {
+        int p = par[i];
+        if (p == i) return i;
+        i = p;
+    }
+}
+
+__device__ __forceinline__ void sunite(int* par, int a, int b)
+{
+    while (true) {
+        a = sfind(par, a);
+        b = sfind(par, b);
+        if (a == b) return;
+        if (a < b) { int t = a; a = b; b = t; }
+        int old = atomicMin(&par[a], b);
+        if (old == a) return;
+        a = old;
+    }
+}
+
+__device__ __forceinline__ void mark_kept(int r, unsigned* kept, int* blk)
+{
+    atomicOr(&kept[r >> 5], 1u << (r & 31));
+    atomicAdd(&blk[r / (32 * RANK_WORDS)], 1);
+}
+
+// one CTA per TH x TW tile: shared-memory union-find (smaller index wins, so a local root is the first pixel of its local
+// component), parent[p] = global index of p's local root, and at each local root its size and box; local roots are listed.
+__global__ void __launch_bounds__(256, 5) k_ccl_tile(const int* __restrict__ lab, int H, int W, int ntx, int* __restrict__ parent,
+                                                  int* __restrict__ size, int* __restrict__ ymax, int* __restrict__ xmin,
+                                                  int* __restrict__ xmax, int* __restrict__ lroots, int* ctr)
+{
+    constexpr int PT = TPIX / 256;
+    __shared__ int s_lab[TPIX]; // labels, then local sizes
+    __shared__ int s_par[TPIX];
+    __shared__ int s_ymax[TPIX], s_xmin[TPIX], s_xmax[TPIX];
+    __shared__ unsigned s_starts[TPIX / 32]; // run-start bits, two words per row
+    const int x0 = (blockIdx.x % ntx) * TW, y0 = (blockIdx.x / ntx) * TH;
+    const int tw = min(TW, W - x0), th = min(TH, H - y0);
+    const int lane = threadIdx.x & 31;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            int t = __shfl_up_sync(0xffffffffu, v, o);
-            if (lane >= o) v = max(v, t);
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k, ly = i / TW, lx = i % TW;
+        s_lab[i] = (ly < th && lx < tw) ? lab[(size_t)(y0 + ly) * W + x0 + lx] : 0;
+        s_ymax[i] = -1; s_xmin[i] = INT_MAX; s_xmax[i] = -1;
+    }
+    __syncthreads();
+    // every pixel starts at the first pixel of its row run (pixels outside the image are runs of their own), so the unions
+    // below only ever walk run starts
+#pragma unroll
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k, ly = i / TW, lx = i % TW;
+        const bool start = lx == 0 || lx >= tw || ly >= th || s_lab[i - 1] != s_lab[i];
+        const unsigned m = __ballot_sync(0xffffffffu, start);
+        if (lane == 0) s_starts[i / 32] = m;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k, ly = i / TW, lx = i % TW;
+        const unsigned long long row = ((unsigned long long)s_starts[2 * ly + 1] << 32) | s_starts[2 * ly];
+        s_par[i] = ly * TW + 63 - __clzll(row & (~0ull >> (63 - lx)));
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k, ly = i / TW, lx = i % TW;
+        if (ly == 0 || ly >= th || lx >= tw) continue;
+        const int l = s_lab[i];
+        if (s_lab[i - TW] != l) continue;
+        if (lx > 0 && s_lab[i - 1] == l && s_lab[i - TW - 1] == l) continue; // the left pixel makes the same link
+        sunite(s_par, i, i - TW);
+    }
+    __syncthreads();
+    // run starts find their roots (compressing in place: a new parent is the root, which every reader still finds above it),
+    // then every other pixel takes its run start's root
+#pragma unroll
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k;
+        if ((s_starts[i / 32] >> (i % 32)) & 1u) s_par[i] = sfind(s_par, i);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k;
+        if (!((s_starts[i / 32] >> (i % 32)) & 1u)) s_par[i] = s_par[s_par[i]];
+        s_lab[i] = 0;
+    }
+    __syncthreads();
+    // sizes and boxes, one row run at a time: its start adds the run into the root
+#pragma unroll
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k, ly = i / TW, lx = i % TW;
+        if (ly >= th || lx >= tw || !((s_starts[i / 32] >> (i % 32)) & 1u)) continue;
+        const unsigned long long row = ((unsigned long long)s_starts[2 * ly + 1] << 32) | s_starts[2 * ly];
+        const unsigned long long rest = lx == TW - 1 ? 0ull : row >> (lx + 1); // pixels past the tile's width are run starts
+        const int len = rest ? __ffsll((long long)rest) : TW - lx;
+        const int r = s_par[i];
+        atomicAdd(&s_lab[r], len);
+        atomicMax(&s_ymax[r], ly);
+        atomicMin(&s_xmin[r], lx);
+        atomicMax(&s_xmax[r], lx + len - 1);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < PT; ++k) {
+        const int i = threadIdx.x + 256 * k, ly = i / TW, lx = i % TW;
+        const bool valid = ly < th && lx < tw;
+        const int p = (y0 + ly) * W + x0 + lx;
+        const int r = s_par[i];
+        const bool is_root = valid && r == i;
+        if (valid) parent[p] = (y0 + r / TW) * W + x0 + r % TW;
+        if (is_root) {
+            size[p] = s_lab[i];
+            ymax[p] = y0 + s_ymax[i]; xmin[p] = x0 + s_xmin[i]; xmax[p] = x0 + s_xmax[i];
         }
-        if (lane == 31) s_warp[warp] = v;
-        __syncthreads();
-        int pre = s_carry;
-        for (int w = 0; w < warp; ++w) pre = max(pre, s_warp[w]);
-        v = max(v, pre);
-        if (x < W) prow[x] = y * W + v;
-        __syncthreads();
-        if (threadIdx.x == 255) s_carry = v;
-        __syncthreads();
+        const unsigned m = __ballot_sync(0xffffffffu, is_root);
+        int base = 0;
+        if (lane == 0 && m) base = atomicAdd(&ctr[C_LROOTS], __popc(m));
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (is_root) lroots[base + __popc(m & ((1u << lane) - 1u))] = p;
     }
 }
 
-__global__ void k_merge_vertical(const int* __restrict__ lab, int H, int W, int* parent)
+// one thread per pair of equal labels across a tile seam: global unions of local roots
+__global__ void k_ccl_seams(const int* __restrict__ lab, int H, int W, int nvs, int nhs, int* parent)
 {
-    size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= (size_t)H * W || p < (size_t)W) return;
-    int x = (int)(p % W);
-    int l = lab[p];
-    if (lab[p - W] != l) return;
-    // skip when the left neighbour already made the same link
-    if (x > 0 && lab[p - 1] == l && lab[p - W - 1] == l) return;
-    unite(parent, (int)p, (int)(p - W));
+    int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nvs + nhs) return;
+    int p, q;
+    if (t < nvs) { // vertical seams: (y, x - 1) | (y, x)
+        const int k = t / H, y = t - k * H, x = (k + 1) * TW;
+        p = y * W + x; q = p - 1;
+        const int l = lab[p];
+        if (lab[q] != l) return;
+        // inside a tile row the pair above, linked to this pair by both tiles, makes the same link
+        if (y % TH != 0 && lab[p - W] == l && lab[q - W] == l) return;
+    } else {       // horizontal seams: (y - 1, x) over (y, x)
+        t -= nvs;
+        const int k = t / W, x = t - k * W, y = (k + 1) * TH;
+        p = y * W + x; q = p - W;
+        const int l = lab[p];
+        if (lab[q] != l) return;
+        if (x % TW != 0 && lab[p - 1] == l && lab[q - 1] == l) return;
+    }
+    unite(parent, p, q);
 }
 
-__global__ void k_flatten_sizes(const int* __restrict__ lab, int H, int W, const int* __restrict__ parent, int* __restrict__ comp,
-                                int* size)
+// over the local roots: point each at its global root and add its size and box into it
+__global__ void k_ccl_roots(int* parent, int* size, int* ymax, int* xmin, int* xmax, const int* __restrict__ lroots,
+                            const int* __restrict__ ctr)
 {
-    size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= (size_t)H * W) return;
-    int x = (int)(p % W);
-    int rs = parent[p];                       // run start (or, for the run start itself, its tree parent)
-    int root = find_root(parent, rs);
-    comp[p] = root;
-    if (x == W - 1 || lab[p + 1] != lab[p]) {  // run end: add the run length once
-        // parent[p] is still the run start unless p starts the run itself (then it may point up the tree)
-        int xs = (x > 0 && lab[p - 1] == lab[p]) ? rs % W : x;
-        atomicAdd(&size[root], x - xs + 1);
+    const int n = ctr[C_LROOTS];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int lr = lroots[i];
+        const int g = find_root(parent, lr);
+        if (g == lr) continue;
+        parent[lr] = g;
+        atomicAdd(&size[g], size[lr]);
+        atomicMax(&ymax[g], ymax[lr]);
+        atomicMin(&xmin[g], xmin[lr]);
+        atomicMax(&xmax[g], xmax[lr]);
     }
 }
 
-__global__ void k_collect_oversize(int n, const int* __restrict__ comp, const int* __restrict__ size, int max_size, int* list,
-                                   int* ctr, int* aux)
+// over the global roots once sizes are final: oversize, kept (bitmap) or small (window or fallback list)
+__global__ void k_ccl_classify(int H, int W, int min_size, int max_size, const int* __restrict__ parent, const int* __restrict__ size,
+                               const int* __restrict__ ymax, const int* __restrict__ xmin, const int* __restrict__ xmax,
+                               const int* __restrict__ lroots, int* ctr, int* over, int* window, int* fallback, unsigned* kept, int* blk)
 {
-    int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    if (comp[p] == p && size[p] >= max_size) {
-        int slot = atomicAdd(&ctr[0], 1);
-        list[slot] = p;
-        aux[p] = slot;
+    const int n = ctr[C_LROOTS];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int g = lroots[i];
+        if (parent[g] != g) continue;
+        const int s = size[g];
+        if (s >= max_size) {
+            over[atomicAdd(&ctr[C_OVER], 1)] = g;
+        } else if (s >= min_size) {
+            mark_kept(g, kept, blk);
+        } else {
+            const int y = g / W;
+            const int wh = min(ymax[g] + 1, H - 1) - max(y - 1, 0) + 1;
+            const int ww = min(xmax[g] + 1, W - 1) - max(xmin[g] - 1, 0) + 1;
+            if (wh * ww <= WIN) window[atomicAdd(&ctr[C_WINDOW], 1)] = g;
+            else fallback[atomicAdd(&ctr[C_FALLBACK], 1)] = g;
+        }
     }
 }
 
-__global__ void k_oversize_bbox(int H, int W, const int* __restrict__ comp, const int* __restrict__ size, int max_size,
-                                const int* __restrict__ aux, const int* __restrict__ ctr, int4* bbox)
+// parent[p] = root of p in place (roots keep their value), for the oversize split and the fallback BFS, which read one hop;
+// a no-op when neither has work
+__global__ void k_ccl_flatten(int n, int* parent, const int* __restrict__ ctr)
 {
-    if (ctr[0] == 0) return;
-    size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= (size_t)H * W) return;
-    int r = comp[p];
-    if (size[r] < max_size) return;
-    int slot = aux[r];
-    int y = (int)(p / W), x = (int)(p % W);
-    atomicMin(&bbox[slot].x, y); atomicMax(&bbox[slot].y, y);
-    atomicMin(&bbox[slot].z, x); atomicMax(&bbox[slot].w, x);
+    if (ctr[C_OVER] == 0 && ctr[C_FALLBACK] == 0) return;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) parent[p] = parent[parent[p]];
 }
 
-// one thread per oversize component: replay the truncated BFS; assigned pixels get comp = ~piece_root
-__global__ void k_oversize_split(int H, int W, int* comp, int* size, int max_size, const int* __restrict__ list,
-                                 const int* __restrict__ ctr, const int4* __restrict__ bbox, int* queue)
+// one thread per oversize component: replay the truncated BFS over its box; assigned pixels get comp = ~piece_root, and each
+// piece is kept or listed for the fallback BFS
+__global__ void k_oversize_split(int H, int W, int* comp, int* size, const int* __restrict__ ymax, const int* __restrict__ xmin,
+                                 const int* __restrict__ xmax, int min_size, int max_size, const int* __restrict__ list, int* ctr,
+                                 int* fallback, unsigned* kept, int* blk, int* queue)
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= ctr[0]) return;
+    if (i >= ctr[C_OVER]) return;
     const int C = list[i];
-    const int4 bb = bbox[i];
+    const int4 bb = make_int4(C / W, ymax[C], xmin[C], xmax[C]);
     int* q = queue + (size_t)i * max_size;
     const int total = size[C];
     int assigned = 0;
@@ -180,85 +317,112 @@ __global__ void k_oversize_split(int H, int W, int* comp, int* size, int max_siz
             }
             size[start] = n;
             assigned += n;
+            if (n >= min_size) mark_kept(start, kept, blk);
+            else fallback[atomicAdd(&ctr[C_FALLBACK], 1)] = start;
         }
 }
 
-// rank of kept roots in raster order: per-row counts -> scan -> per-row assignment
-__global__ void __launch_bounds__(256) k_row_count_kept(int H, int W, const int* __restrict__ comp, const int* __restrict__ size,
-                                                        int min_size, int* row_cnt)
+// one CTA per RANK_WORDS words of the kept bitmap: a kept piece's label is the number of kept first pixels before it
+__global__ void __launch_bounds__(256) k_kept_ranks(int n_words, const unsigned* __restrict__ kept, const int* __restrict__ blk,
+                                                    int* aux, int* n_labels_out)
 {
-    const int y = blockIdx.x;
+    constexpr int WPT = RANK_WORDS / 256;
+    __shared__ int s_warp[8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int base = 0;
+    for (int j = threadIdx.x; j < (int)blockIdx.x; j += 256) base += blk[j];
+    unsigned bits[WPT];
     int c = 0;
-    for (int x = threadIdx.x; x < W; x += 256) {
-        int p = y * W + x;
-        c += (dec(comp[p]) == p && size[p] >= min_size) ? 1 : 0;
+#pragma unroll
+    for (int k = 0; k < WPT; ++k) {
+        const int w = blockIdx.x * RANK_WORDS + threadIdx.x * WPT + k;
+        bits[k] = w < n_words ? kept[w] : 0u;
+        c += __popc(bits[k]);
     }
-    __shared__ int s[256];
-    s[threadIdx.x] = c;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if (threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
-        __syncthreads();
+    // block sum of base, exclusive block scan of c
+    int incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+        base += __shfl_xor_sync(0xffffffffu, base, o);
     }
-    if (threadIdx.x == 0) row_cnt[y] = s[0];
-}
-
-__global__ void __launch_bounds__(1024) k_scan_rows(int H, int* row_cnt, int* n_labels_out)
-{
-    __shared__ int s_part[1024];
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
+    if (lane == 31) s_warp[warp] = incl;
+    __shared__ int s_base[8];
+    if (lane == 0) s_base[warp] = base;
     __syncthreads();
-    for (int base = 0; base < H; base += 1024) {
-        int i = base + threadIdx.x;
-        int v = i < H ? row_cnt[i] : 0;
-        s_part[threadIdx.x] = v;
-        __syncthreads();
-        for (int o = 1; o < 1024; o <<= 1) {
-            int t = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
-            __syncthreads();
-            s_part[threadIdx.x] += t;
-            __syncthreads();
-        }
-        int incl = s_part[threadIdx.x], carry = s_carry;
-        if (i < H) row_cnt[i] = carry + incl - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = carry + incl;
-        __syncthreads();
+    int off = 0, tot = 0;
+    base = 0;
+    for (int w = 0; w < 8; ++w) {
+        if (w < warp) off += s_warp[w];
+        tot += s_warp[w];
+        base += s_base[w];
+    }
+    int label = base + off + incl - c;
+#pragma unroll
+    for (int k = 0; k < WPT; ++k) {
+        const int w = blockIdx.x * RANK_WORDS + threadIdx.x * WPT + k;
+        for (unsigned b = bits[k]; b; b &= b - 1) aux[w * 32 + __ffs(b) - 1] = label++;
     }
     // when no component reaches min_size everything is merged into label 0: the map still holds one label
-    if (threadIdx.x == 0) { row_cnt[H] = s_carry; *n_labels_out = s_carry > 0 ? s_carry : 1; }
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *n_labels_out = base + tot > 0 ? base + tot : 1;
 }
 
-__global__ void __launch_bounds__(256) k_row_assign_labels(int H, int W, const int* __restrict__ comp, const int* __restrict__ size,
-                                                           int min_size, const int* __restrict__ row_cnt, int* aux, int* list, int* ctr)
+// one CTA per small piece whose box plus a one-pixel ring fits WIN pixels: the window's piece ids go to shared memory and one
+// thread replays the piece's BFS there, remembering the last foreign earlier-labelled neighbour piece.  A window piece is a
+// whole component below max_size, so its BFS is never truncated.
+__global__ void __launch_bounds__(256) k_small_window(int H, int W, const int* __restrict__ parent, const int* __restrict__ ymax,
+                                                      const int* __restrict__ xmin, const int* __restrict__ xmax,
+                                                      const int* __restrict__ list, const int* __restrict__ ctr, int* __restrict__ aux)
 {
-    const int y = blockIdx.x;
-    __shared__ int s_warp[8];
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) s_carry = row_cnt[y];
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < W; base += 256) {
-        int x = base + threadIdx.x;
-        int p = y * W + x;
-        bool root = x < W && dec(comp[p]) == p;
-        bool kept = root && size[p] >= min_size;
-        unsigned m = __ballot_sync(0xffffffffu, kept);
-        int pre = __popc(m & ((1u << lane) - 1u));
-        if (lane == 0) s_warp[warp] = __popc(m);
+    __shared__ int s_id[WIN];
+    __shared__ int s_q[WIN]; // queue entries (window row << 16) | window column
+    const int n_small = ctr[C_WINDOW];
+    for (int i = blockIdx.x; i < n_small; i += gridDim.x) {
+        const int C = list[i];
+        const int y = C / W, x = C - y * W;
+        const int wy0 = max(y - 1, 0), wx0 = max(xmin[C] - 1, 0);
+        const int wh = min(ymax[C] + 1, H - 1) - wy0 + 1, ww = min(xmax[C] + 1, W - 1) - wx0 + 1;
+        const int area = wh * ww;
+#pragma unroll 4
+        for (int j = threadIdx.x; j < area; j += 256) {
+            const int jy = j / ww;
+            s_id[j] = resolve(parent, (wy0 + jy) * W + wx0 + j - jy * ww);
+        }
         __syncthreads();
-        int off = s_carry;
-        for (int w = 0; w < warp; ++w) off += s_warp[w];
-        if (kept) aux[p] = off + pre;
-        else if (root) { aux[p] = -1; list[atomicAdd(&ctr[1], 1)] = p; }
-        __syncthreads();
-        if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < 8; ++w) t += s_warp[w]; s_carry += t; }
+        if (threadIdx.x == 0) {
+            int adjacent = -1;
+            const int cy0 = y - wy0, cx0 = x - wx0;
+            s_q[0] = (cy0 << 16) | cx0;
+            s_id[cy0 * ww + cx0] = INT_MAX; // visited: neither C nor below C
+            int n = 1;
+            for (int v = 0; v < n; ++v) {
+                const int cy = s_q[v] >> 16, cx = s_q[v] & 0xffff;
+                const int c = cy * ww + cx, gy = wy0 + cy, gx = wx0 + cx;
+                // the four neighbours in the original's order (+x, -x, +y, -y); an in-image neighbour lies inside the window
+                const bool ok4[4] = { gx + 1 < W, gx > 0, gy + 1 < H, gy > 0 };
+                const int nc4[4] = { c + 1, c - 1, c + ww, c - ww };
+                const int nq4[4] = { (cy << 16) | (cx + 1), (cy << 16) | (cx - 1), ((cy + 1) << 16) | cx, ((cy - 1) << 16) | cx };
+                int r4[4];
+#pragma unroll
+                for (int d = 0; d < 4; ++d) r4[d] = ok4[d] ? s_id[nc4[d]] : INT_MAX;
+#pragma unroll
+                for (int d = 0; d < 4; ++d) {
+                    if (r4[d] == C) { // the four neighbours of one pixel are distinct
+                        s_id[nc4[d]] = INT_MAX;
+                        s_q[n++] = nq4[d];
+                    } else if (r4[d] < C) {
+                        adjacent = r4[d];
+                    }
+                }
+            }
+            aux[C] = adjacent >= 0 ? -2 - adjacent : -1; // small roots store -2-adjacent (kept roots store label >= 0)
+        }
         __syncthreads();
     }
 }
 
-// one thread per small piece: replay its BFS, remember the last foreign earlier-labelled neighbour piece.
+// one thread per small piece the window does not take: replay its BFS, remember the last foreign earlier-labelled neighbour piece.
 // The kernel is a chain of dependent loads per piece (queue entry -> four neighbours), as long as the largest small piece: the queue of
 // a piece (fewer than min_size entries) lives in SHARED memory when it fits (SQ: 32 threads per CTA, entry j of lane l at q[32 j + l]),
 // which takes one of the two global round trips out of every BFS step.
@@ -308,34 +472,41 @@ __global__ void __launch_bounds__(SQ ? 32 : 256) k_small_adjacent(int H, int W, 
     }
 }
 
-__global__ void k_write_labels(int n, const int* __restrict__ comp, const int* __restrict__ size, int min_size,
-                               const int* __restrict__ aux, int* __restrict__ out)
+// WRITE_PX pixels per thread, a block width apart: their three dependent loads (parent, the local root's parent, aux) overlap
+constexpr int WRITE_PX = 4;
+__global__ void __launch_bounds__(256) k_ccl_write(int n, const int* __restrict__ parent, const int* __restrict__ aux,
+                                                   int* __restrict__ out)
 {
-    int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    int r = dec(comp[p]);
-    int a = aux[r];
-    // follow small -> adjacent chains (each hop goes to a piece with a smaller root index)
-    while (a < -1) { r = -2 - a; a = aux[r]; }
-    out[p] = a < 0 ? 0 : a;
+    const int p0 = blockIdx.x * 256 * WRITE_PX + threadIdx.x;
+    int r[WRITE_PX], a[WRITE_PX];
+#pragma unroll
+    for (int k = 0; k < WRITE_PX; ++k) r[k] = p0 + 256 * k < n ? parent[p0 + 256 * k] : 0;
+#pragma unroll
+    for (int k = 0; k < WRITE_PX; ++k) r[k] = dec(r[k] < 0 ? r[k] : parent[r[k] & ~VISBIT]);
+#pragma unroll
+    for (int k = 0; k < WRITE_PX; ++k) a[k] = aux[r[k]];
+#pragma unroll
+    for (int k = 0; k < WRITE_PX; ++k) {
+        // follow small -> adjacent chains (each hop goes to a piece with a smaller root index)
+        while (a[k] < -1) { r[k] = -2 - a[k]; a[k] = aux[r[k]]; }
+        if (p0 + 256 * k < n) out[p0 + 256 * k] = a[k] < 0 ? 0 : a[k];
+    }
 }
 
-static size_t carve(ConnWs& w, void* ws, size_t bytes, int H, int W)
+static size_t carve(ConnWs& w, void* ws, size_t bytes, int H, int W, int* n_zero)
 {
     WsCarver c(ws, bytes);
     size_t n = (size_t)H * W;
-    w.comp = c.take<int>(n); w.size = c.take<int>(n); w.aux = c.take<int>(n);
-    w.queue = c.take<int>(n); w.list = c.take<int>(n);
-    w.row_cnt = c.take<int>((size_t)H + 1);
-    w.ctr = c.take<int>(8);
-    w.bbox = c.take<int4>(n / 16 + 16);
+    w.parent = c.take<int>(n); w.size = c.take<int>(n);
+    w.ymax = c.take<int>(n); w.xmin = c.take<int>(n); w.xmax = c.take<int>(n);
+    w.aux = c.take<int>(n); w.lroots = c.take<int>(n); w.window = c.take<int>(n); w.fallback = c.take<int>(n);
+    w.over = c.take<int>(n / 16 + 16);
+    const size_t n_words = (n + 31) / 32, n_blk = (n_words + RANK_WORDS - 1) / RANK_WORDS;
+    w.ctr = c.take<int>(C_N + n_blk + n_words);
+    w.blk = w.ctr + C_N;
+    w.kept = (unsigned*)(w.blk + n_blk);
+    *n_zero = (int)(C_N + n_blk + n_words);
     return isb_align(c.off);
-}
-
-__global__ void k_init_bbox(int n, int4* bbox)
-{
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) bbox[i] = make_int4(INT_MAX, -1, INT_MAX, -1);
 }
 
 } // namespace
@@ -343,7 +514,8 @@ __global__ void k_init_bbox(int n, int4* bbox)
 extern "C" size_t isb_connectivity_workspace_bytes(int H, int W)
 {
     ConnWs w;
-    return carve(w, nullptr, 0, H, W);
+    int n_zero;
+    return carve(w, nullptr, 0, H, W, &n_zero);
 }
 
 extern "C" int isb_enforce_connectivity(const int32_t* labels, int H, int W, int min_size, int max_size, int32_t* out,
@@ -354,54 +526,52 @@ extern "C" int isb_enforce_connectivity(const int32_t* labels, int H, int W, int
     if (max_size < 1) max_size = 1;
     ISB_REQUIRE(max_size >= 16, "max_size < 16 is not supported on the device path (oversize table bound)");
     ConnWs w;
-    size_t need = carve(w, ws, ws_bytes, H, W);
+    int n_zero;
+    size_t need = carve(w, ws, ws_bytes, H, W, &n_zero);
     ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope prof(ISB_PROF_CONN, st);
     const int n = H * W;
-    const int nb = (n + 255) / 256;
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.size, 0, sizeof(int) * (size_t)n, st));
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.ctr, 0, sizeof(int) * 8, st));
-    k_row_runs<<<H, 256, 0, st>>>(labels, H, W, w.comp);
+    const int ntx = (W + TW - 1) / TW, nty = (H + TH - 1) / TH;
+    const int n_words = (n + 31) / 32, n_rank = (n_words + RANK_WORDS - 1) / RANK_WORDS;
+    int dev = 0, sms = 0;
+    ISB_CUDA_CHECK(cudaGetDevice(&dev));
+    ISB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    ISB_CUDA_CHECK(cudaMemsetAsync(w.ctr, 0, sizeof(int) * (size_t)n_zero, st));
+    k_ccl_tile<<<ntx * nty, 256, 0, st>>>(labels, H, W, ntx, w.parent, w.size, w.ymax, w.xmin, w.xmax, w.lroots, w.ctr);
     ISB_LAUNCH_CHECK();
-    k_merge_vertical<<<nb, 256, 0, st>>>(labels, H, W, w.comp);
-    ISB_LAUNCH_CHECK();
-    // comp doubles as the union-find parent array; flatten writes roots into aux first, then swap roles
-    k_flatten_sizes<<<nb, 256, 0, st>>>(labels, H, W, w.comp, w.aux, w.size);
-    ISB_LAUNCH_CHECK();
-    int* comp = w.aux;   // flattened component ids
-    int* aux = w.comp;   // parent array is dead now: reuse as aux
-    const int n_over_max = n / max_size + 1;
-    k_init_bbox<<<(n_over_max + 255) / 256, 256, 0, st>>>(n_over_max, w.bbox);
-    ISB_LAUNCH_CHECK();
-    k_collect_oversize<<<nb, 256, 0, st>>>(n, comp, w.size, max_size, w.list, w.ctr, aux);
-    ISB_LAUNCH_CHECK();
-    k_oversize_bbox<<<nb, 256, 0, st>>>(H, W, comp, w.size, max_size, aux, w.ctr, w.bbox);
-    ISB_LAUNCH_CHECK();
-    k_oversize_split<<<(n_over_max + 63) / 64, 64, 0, st>>>(H, W, comp, w.size, max_size, w.list, w.ctr, w.bbox, w.queue);
-    ISB_LAUNCH_CHECK();
-    k_row_count_kept<<<H, 256, 0, st>>>(H, W, comp, w.size, min_size, w.row_cnt);
-    ISB_LAUNCH_CHECK();
-    k_scan_rows<<<1, 1024, 0, st>>>(H, w.row_cnt, n_labels_out);
-    ISB_LAUNCH_CHECK();
-    k_row_assign_labels<<<H, 256, 0, st>>>(H, W, comp, w.size, min_size, w.row_cnt, aux, w.list, w.ctr);
-    ISB_LAUNCH_CHECK();
-    // the kernel reads the real count of small roots and strides over them
-    {
-        int dev = 0, sms = 0;
-        ISB_CUDA_CHECK(cudaGetDevice(&dev));
-        ISB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        if (min_size >= 1 && min_size <= 512) {
-            // a small piece has fewer than min_size pixels: its queue fits min_size entries of shared memory per thread
-            const size_t smem = sizeof(int) * 32 * (size_t)min_size;
-            ISB_CUDA_CHECK(cudaFuncSetAttribute(k_small_adjacent<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            k_small_adjacent<true><<<sms * 16, 32, smem, st>>>(H, W, comp, w.size, max_size, w.list, w.ctr, aux, w.queue);
-        } else {
-            k_small_adjacent<false><<<sms * 8, 256, 0, st>>>(H, W, comp, w.size, max_size, w.list, w.ctr, aux, w.queue);
-        }
+    const int nvs = (ntx - 1) * H, nhs = (nty - 1) * W;
+    if (nvs + nhs > 0) {
+        k_ccl_seams<<<(nvs + nhs + 255) / 256, 256, 0, st>>>(labels, H, W, nvs, nhs, w.parent);
         ISB_LAUNCH_CHECK();
     }
-    k_write_labels<<<nb, 256, 0, st>>>(n, comp, w.size, min_size, aux, out);
+    k_ccl_roots<<<sms * 4, 256, 0, st>>>(w.parent, w.size, w.ymax, w.xmin, w.xmax, w.lroots, w.ctr);
+    ISB_LAUNCH_CHECK();
+    k_ccl_classify<<<sms * 4, 256, 0, st>>>(H, W, min_size, max_size, w.parent, w.size, w.ymax, w.xmin, w.xmax, w.lroots, w.ctr,
+                                            w.over, w.window, w.fallback, w.kept, w.blk);
+    ISB_LAUNCH_CHECK();
+    k_ccl_flatten<<<sms * 8, 256, 0, st>>>(n, w.parent, w.ctr);
+    ISB_LAUNCH_CHECK();
+    // the local-root list is dead once classified: it becomes the BFS queue space
+    const int n_over_max = n / max_size + 1;
+    k_oversize_split<<<(n_over_max + 63) / 64, 64, 0, st>>>(H, W, w.parent, w.size, w.ymax, w.xmin, w.xmax, min_size, max_size, w.over,
+                                                            w.ctr, w.fallback, w.kept, w.blk, w.lroots);
+    ISB_LAUNCH_CHECK();
+    k_kept_ranks<<<n_rank, 256, 0, st>>>(n_words, w.kept, w.blk, w.aux, n_labels_out);
+    ISB_LAUNCH_CHECK();
+    k_small_window<<<sms * 6, 256, 0, st>>>(H, W, w.parent, w.ymax, w.xmin, w.xmax, w.window, w.ctr, w.aux);
+    ISB_LAUNCH_CHECK();
+    // the fallback reads the real count of its pieces and strides over them
+    if (min_size >= 1 && min_size <= 512) {
+        // a small piece has fewer than min_size pixels: its queue fits min_size entries of shared memory per thread
+        const size_t smem = sizeof(int) * 32 * (size_t)min_size;
+        ISB_CUDA_CHECK(cudaFuncSetAttribute(k_small_adjacent<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_small_adjacent<true><<<sms * 16, 32, smem, st>>>(H, W, w.parent, w.size, max_size, w.fallback, w.ctr, w.aux, w.lroots);
+    } else {
+        k_small_adjacent<false><<<sms * 8, 256, 0, st>>>(H, W, w.parent, w.size, max_size, w.fallback, w.ctr, w.aux, w.lroots);
+    }
+    ISB_LAUNCH_CHECK();
+    k_ccl_write<<<(n + 256 * WRITE_PX - 1) / (256 * WRITE_PX), 256, 0, st>>>(n, w.parent, w.aux, out);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }

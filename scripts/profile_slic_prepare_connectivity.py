@@ -15,9 +15,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-KERNELS = ('k_minmax', 'k_minmax_decode', 'k_blur_lab', 'k_row_runs', 'k_merge_vertical', 'k_flatten_sizes', 'k_init_bbox',
-           'k_collect_oversize', 'k_oversize_bbox', 'k_oversize_split', 'k_row_count_kept', 'k_scan_rows', 'k_row_assign_labels',
-           'k_small_adjacent', 'k_write_labels')
+KERNELS = ('k_minmax', 'k_minmax_decode', 'k_blur_lab', 'k_ccl_tile', 'k_ccl_seams', 'k_ccl_roots', 'k_ccl_classify',
+           'k_ccl_flatten', 'k_oversize_split', 'k_kept_ranks', 'k_small_window', 'k_small_adjacent', 'k_ccl_write')
 
 
 def kernel_key(name):
