@@ -30,6 +30,7 @@
 // the global workspace (L2 resident) -- the per-rank base pointers then simply point into global arrays.
 // This stage is latency/SMEM bound, not HBM bound: report time, not a roofline fraction (SURVEY.md section 8d).
 #include "common.cuh"
+#include "block_scan.cuh"
 #include <cooperative_groups.h>
 
 namespace cg = cooperative_groups;
@@ -67,35 +68,17 @@ struct GcArgs {
 
 __global__ void __launch_bounds__(NT) k_gc_build_csr(GcArgs a)
 {
-    __shared__ int s_scan[NT];
-    __shared__ int s_carry;
     const int N = a.n_nodes_dev ? min(*a.n_nodes_dev, a.N) : a.N;
     // an overflowed edge table (count > capacity) holds unspecified rows: cut nothing, the host sees the count and redoes the image
     const int E = a.n_edges_dev ? (*a.n_edges_dev > a.E_cap ? 0 : *a.n_edges_dev) : a.E_cap;
     for (int v = threadIdx.x; v < N; v += NT) a.fill[v] = 0;
     __syncthreads();
     for (int e = threadIdx.x; e < E; e += NT) { atomicAdd(&a.fill[a.edges[2 * e]], 1); atomicAdd(&a.fill[a.edges[2 * e + 1]], 1); }
-    if (threadIdx.x == 0) s_carry = 0;
     __syncthreads();
-    for (int base = 0; base < N; base += NT) {
-        int i = base + threadIdx.x;
-        int v = i < N ? __ldcg(&a.fill[i]) : 0;
-        s_scan[threadIdx.x] = v;
-        __syncthreads();
-        for (int o = 1; o < NT; o <<= 1) {
-            int t = threadIdx.x >= o ? s_scan[threadIdx.x - o] : 0;
-            __syncthreads();
-            s_scan[threadIdx.x] += t;
-            __syncthreads();
-        }
-        int incl = s_scan[threadIdx.x], carry = s_carry;
-        if (i < N) { a.off[i] = carry + incl - v; a.fill[i] = 0; }
-        __syncthreads();
-        if (threadIdx.x == NT - 1) s_carry = carry + incl;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) a.off[N] = s_carry;
-    __syncthreads();
+    // fill was written by the atomics above: read it past L1.  The scan's closing barrier orders the fill reset before the scatter.
+    const int A = cta_scan_chunks<NT, int>(N, [&](int i) { return __ldcg(&a.fill[i]); },
+                                           [&](int i, int off) { a.off[i] = off; a.fill[i] = 0; });
+    if (threadIdx.x == 0) a.off[N] = A;
     for (int e = threadIdx.x; e < E; e += NT) {
         int va = a.edges[2 * e], vb = a.edges[2 * e + 1];
         int pa = a.off[va] + atomicAdd(&a.fill[va], 1);

@@ -136,7 +136,7 @@ __global__ void __launch_bounds__(CPT_THREADS) k_ct_dense(int32_t* __restrict__ 
 {
     const long long beg = (long long)blockIdx.x * CPT_TILE + (long long)threadIdx.x * CPT_PER;
     int total;
-    long long o = tile_off[blockIdx.x] + block_exclusive_scan(thread_count(pres, beg, range), &total);
+    long long o = tile_off[blockIdx.x] + cta_exclusive_sum<CPT_THREADS>(thread_count(pres, beg, range), total);
     for (int k = 0; k < CPT_PER; ++k) {
         const long long i = beg + k;
         if (i < range && pres[i]) {

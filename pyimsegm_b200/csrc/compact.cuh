@@ -3,6 +3,7 @@
 // histogram of annotation.cu; each source keeps its own write kernel (what it writes per element differs).
 #pragma once
 #include "common.cuh"
+#include "block_scan.cuh"
 
 namespace {
 
@@ -21,60 +22,21 @@ __device__ __forceinline__ int thread_count(const T* __restrict__ v, long long b
     return c;
 }
 
-// exclusive prefix of v over the block; *total = block sum
-__device__ __forceinline__ int block_exclusive_scan(int v, int* total)
-{
-    __shared__ int warp_sum[CPT_THREADS / 32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    int inc = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-    }
-    if (lane == 31) warp_sum[wid] = inc;
-    __syncthreads();
-    if (wid == 0) {
-        int w = lane < CPT_THREADS / 32 ? warp_sum[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += u;
-        }
-        if (lane < CPT_THREADS / 32) warp_sum[lane] = w;   // inclusive over warps
-    }
-    __syncthreads();
-    const int before = wid ? warp_sum[wid - 1] : 0;
-    *total = warp_sum[CPT_THREADS / 32 - 1];
-    return before + inc - v;
-}
-
 template <typename T>
 __global__ void __launch_bounds__(CPT_THREADS) k_compact_count(const T* __restrict__ v, long long n, long long* __restrict__ tile_count)
 {
     const long long beg = (long long)blockIdx.x * CPT_TILE + (long long)threadIdx.x * CPT_PER;
     int total;
-    block_exclusive_scan(thread_count(v, beg, n), &total);
+    cta_exclusive_sum<CPT_THREADS>(thread_count(v, beg, n), total);
     if (threadIdx.x == 0) tile_count[blockIdx.x] = total;
 }
 
 // exclusive scan of the tile counts in one CTA (tiles are few: 16 384 for an 8192^2 map); total -> tile_off[n_tiles]
 __global__ void __launch_bounds__(1024) k_compact_scan(const long long* __restrict__ tile_count, int n_tiles, long long* __restrict__ tile_off)
 {
-    __shared__ long long part[1024];
-    const int per = (n_tiles + 1023) / 1024, t = threadIdx.x;
-    const int b0 = min(t * per, n_tiles), b1 = min(b0 + per, n_tiles);
-    long long s = 0;
-    for (int b = b0; b < b1; ++b) s += tile_count[b];
-    part[t] = s;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) {
-        const long long u = t >= o ? part[t - o] : 0;
-        __syncthreads();
-        part[t] += u;
-        __syncthreads();
-    }
-    long long run = t ? part[t - 1] : 0;
-    for (int b = b0; b < b1; ++b) { tile_off[b] = run; run += tile_count[b]; }
-    if (t == 1023) tile_off[n_tiles] = part[1023];
+    const long long total = cta_scan_chunks<1024, long long>(n_tiles, [&](int b) { return tile_count[b]; },
+                                                             [&](int b, long long off) { tile_off[b] = off; });
+    if (threadIdx.x == 0) tile_off[n_tiles] = total;
 }
 
 inline size_t compact_workspace_bytes(long long n)

@@ -10,6 +10,7 @@
 //   pyGCO cut_general_graph        float -> int conversion (see oracle/gc_oracle.cpp header)
 //   imsegm/pipelines.py:104,109    proba[slic], graph_labels[slic]
 #include "common.cuh"
+#include "block_scan.cuh"
 #include <cooperative_groups.h>
 namespace cg = cooperative_groups;
 
@@ -102,30 +103,11 @@ __global__ void k_centroid3d_fin(int nb, const unsigned long long* acc, double* 
 // exclusive scan of deg -> off (single CTA)
 __global__ void __launch_bounds__(1024) k_edge_offsets(int nb, AdjWs w, int cap, int* n_edges_out)
 {
-    __shared__ int s_part[1024];
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (int base = 0; base < nb; base += 1024) {
-        int i = base + threadIdx.x;
-        int v = i < nb ? w.deg[i] : 0;
-        s_part[threadIdx.x] = v;
-        __syncthreads();
-        for (int o = 1; o < 1024; o <<= 1) {
-            int t = threadIdx.x >= o ? s_part[threadIdx.x - o] : 0;
-            __syncthreads();
-            s_part[threadIdx.x] += t;
-            __syncthreads();
-        }
-        int incl = s_part[threadIdx.x], carry = s_carry;
-        if (i < nb) { w.off[i] = carry + incl - v; w.fill[i] = 0; }
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = carry + incl;
-        __syncthreads();
-    }
+    const int total = cta_scan_chunks<1024, int>(nb, [&](int i) { return w.deg[i]; },
+                                                 [&](int i, int off) { w.off[i] = off; w.fill[i] = 0; });
     if (threadIdx.x == 0) {
-        w.off[nb] = s_carry;
-        *n_edges_out = (w.ctr[1] || s_carry > cap) ? cap + 1 : s_carry;
+        w.off[nb] = total;
+        *n_edges_out = (w.ctr[1] || total > cap) ? cap + 1 : total;
     }
 }
 

@@ -294,7 +294,7 @@ __global__ void __launch_bounds__(CPT_THREADS) k_compact_write(const uint8_t* __
 {
     const long long beg = (long long)blockIdx.x * CPT_TILE + (long long)threadIdx.x * CPT_PER;
     int total;
-    long long o = tile_off[blockIdx.x] + block_exclusive_scan(thread_count(mask, beg, n), &total);
+    long long o = tile_off[blockIdx.x] + cta_exclusive_sum<CPT_THREADS>(thread_count(mask, beg, n), total);
     for (int k = 0; k < CPT_PER; ++k) {
         const long long i = beg + k;
         if (i < n && mask[i]) {

@@ -11,6 +11,7 @@
 // Ray features = grey erosion then grey dilation with a disc footprint, borders reflected (scipy.ndimage default mode).
 #include <float.h>
 #include "common.cuh"
+#include "block_scan.cuh"
 
 namespace {
 
@@ -27,34 +28,9 @@ __global__ void __launch_bounds__(256) k_med_count(const int* __restrict__ seg, 
 // exclusive scan counts[0..nb) -> start[0..nb], cursor = start (single CTA; nb is a superpixel count)
 __global__ void __launch_bounds__(1024) k_med_scan(const int* __restrict__ counts, int nb, int* __restrict__ start, int* __restrict__ cursor)
 {
-    __shared__ int s_w[32];
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    for (int base = 0; base < nb; base += 1024) {
-        const int i = base + threadIdx.x;
-        const int v = i < nb ? counts[i] : 0;
-        int incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-        if (lane == 31) s_w[wid] = incl;
-        __syncthreads();
-        if (wid == 0) {
-            const int t = s_w[lane];
-            int ti = t;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, ti, o); if (lane >= o) ti += u; }
-            s_w[lane] = ti - t;
-        }
-        __syncthreads();
-        const int excl = s_carry + s_w[wid] + incl - v;
-        if (i < nb) { start[i] = excl; cursor[i] = excl; }
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) start[nb] = s_carry;
+    const int total = cta_scan_chunks<1024, int>(nb, [&](int i) { return counts[i]; },
+                                                 [&](int i, int s) { start[i] = s; cursor[i] = s; });
+    if (threadIdx.x == 0) start[nb] = total;
 }
 
 __global__ void __launch_bounds__(256) k_med_scatter(const int* __restrict__ seg, size_t n, int nb, int* __restrict__ cursor, unsigned* __restrict__ order)

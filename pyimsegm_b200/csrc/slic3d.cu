@@ -16,6 +16,7 @@
 //    chains of small pieces are followed to a kept piece; new labels = raster-order rank of the kept pieces.
 // All distances in IEEE double without FMA, in the oracle's operation order.
 #include "common.cuh"
+#include "block_scan.cuh"
 #include <float.h>
 #include <limits.h>
 
@@ -321,35 +322,10 @@ __global__ void c3_piece_sizes(Cc3 c)
 // labels of the kept pieces: rank of their head voxel among the kept heads, in raster order (single CTA, chunked scan)
 __global__ void __launch_bounds__(1024) c3_rank(Cc3 c, int min_size)
 {
-    __shared__ int s_w[32];
-    __shared__ int s_carry, s_tot;
-    const int V = c.D * c.H * c.W;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (int base = 0; base < V; base += 1024) {
-        const int i = base + threadIdx.x;
-        const int f = (i < V && c.piece[i] == i && c.psize[i] >= min_size) ? 1 : 0;
-        int incl = f;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-        if (lane == 31) s_w[wid] = incl;
-        __syncthreads();
-        if (wid == 0) {
-            const int t = s_w[lane];
-            int ti = t;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, ti, o); if (lane >= o) ti += u; }
-            s_w[lane] = ti - t;
-            if (lane == 31) s_tot = ti;
-        }
-        __syncthreads();
-        if (f) c.newlab[i] = s_carry + s_w[wid] + incl - 1;
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry += s_tot;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) c.counters[2] = s_carry;
+    const auto kept_head = [&](int i) { return c.piece[i] == i && c.psize[i] >= min_size; };
+    const int total = cta_scan_chunks<1024, int>(c.D * c.H * c.W, [&](int i) { return kept_head(i) ? 1 : 0; },
+                                                 [&](int i, int rank) { if (kept_head(i)) c.newlab[i] = rank; });
+    if (threadIdx.x == 0) c.counters[2] = total;
 }
 
 // one thread per small piece: replay its BFS to find the LAST neighbour that belongs to an earlier piece

@@ -20,6 +20,7 @@
 // HBM traffic: the label map read once, parent written once and read back once, out written once (16 B/px); everything else
 // is per local root or per piece.
 #include "common.cuh"
+#include "block_scan.cuh"
 
 namespace {
 
@@ -327,10 +328,8 @@ __global__ void __launch_bounds__(256) k_kept_ranks(int n_words, const unsigned*
                                                     int* aux, int* n_labels_out)
 {
     constexpr int WPT = RANK_WORDS / 256;
-    __shared__ int s_warp[8];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int base = 0;
-    for (int j = threadIdx.x; j < (int)blockIdx.x; j += 256) base += blk[j];
+    int part = 0;
+    for (int j = threadIdx.x; j < (int)blockIdx.x; j += 256) part += blk[j];
     unsigned bits[WPT];
     int c = 0;
 #pragma unroll
@@ -339,26 +338,10 @@ __global__ void __launch_bounds__(256) k_kept_ranks(int n_words, const unsigned*
         bits[k] = w < n_words ? kept[w] : 0u;
         c += __popc(bits[k]);
     }
-    // block sum of base, exclusive block scan of c
-    int incl = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-        base += __shfl_xor_sync(0xffffffffu, base, o);
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __shared__ int s_base[8];
-    if (lane == 0) s_base[warp] = base;
-    __syncthreads();
-    int off = 0, tot = 0;
-    base = 0;
-    for (int w = 0; w < 8; ++w) {
-        if (w < warp) off += s_warp[w];
-        tot += s_warp[w];
-        base += s_base[w];
-    }
-    int label = base + off + incl - c;
+    // base = the kept first pixels of the rank blocks before this one, then the exclusive block scan of c
+    int base, tot;
+    cta_exclusive_sum<256>(part, base);
+    int label = base + cta_exclusive_sum<256>(c, tot);
 #pragma unroll
     for (int k = 0; k < WPT; ++k) {
         const int w = blockIdx.x * RANK_WORDS + threadIdx.x * WPT + k;
