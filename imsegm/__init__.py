@@ -3,8 +3,9 @@ Drop-in alias: ``import imsegm.pipelines`` (``superpixels``, ``descriptors``, ``
 H100-native implementation in ``pyimsegm_b200`` for the SLIC -> features -> GraphCut hot path of Borda/pyImSegm and for the
 region growing (RG2SP) built on it, and for ``labeling``, ``ellipse_fitting``, ``annotation`` and ``classification``.  Of
 ``classification`` the scoring (segmentations against annotations), the training-set preparation (class balancing, k-means
-down-sampling on the device) and the classifier training (random forests and decision trees fitted on the device) are provided;
-cross-validation scoring and feature selection are not.
+down-sampling on the device), the classifier training (random forests and decision trees fitted on the device) and the
+cross-validation (the fold generators, scores and mean ROC, every fold's forest built in one grouped device fit) are provided; feature
+selection is not.
 """
 import sys
 

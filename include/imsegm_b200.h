@@ -601,6 +601,28 @@ int isb_forest_fit(const float* x, int n, int D, const int32_t* y, int K, const 
                    uint8_t* missing_go_to_left, int32_t* class_counts, int32_t* node_count, int* n_levels /* host */, void* ws, size_t ws_bytes,
                    isb_stream_t stream);
 
+/* isb_forest_fit for trees of G groups in one call, level by level together: a group is one training set with its own transformed copy of
+ * the rows and its own resolved parameters (a cross-validation fold: its scaler / PCA, its max_features and leaf sizes).
+ *   x [G, n, Dmax] f32 (device): group g's rows, its features in columns [0, D[g]); columns at or beyond D[g] are never read;
+ *   D, max_features, min_samples_split, min_samples_leaf [G] i32 (host): per group, D[g] in [1, Dmax], max_features[g] in [1, D[g]],
+ *   min_samples_split[g] >= 2, min_samples_leaf[g] >= 1;
+ *   y [n] i32 class indices in [0, K) and K shared by every group (a class missing from a group's rows changes no Gini value);
+ *   counts [T, n] i32 (device), seeds [T] u64 (device) and tree_group [T] i32 (host, in [0, G)) per tree: a row outside the tree's
+ *   training set has count 0;
+ *   max_depth and min_impurity_decrease shared.
+ * Every tree is node for node the tree isb_forest_fit builds from its group's x [n, D[g]] and parameters alone.  Outputs, cap and n_levels
+ * (the levels of the deepest tree) as isb_forest_fit.  Argument errors (a group or tree index out of range, a parameter outside its range,
+ * D[g] > Dmax) return ISB_ERR_ARG before any device work.  Limits (ISB_ERR_UNSUPPORTED): those of isb_forest_fit with D = Dmax and
+ * m = max(max_features).
+ * ws: isb_forest_fit_groups_workspace_bytes(n, Dmax, G, T, K, max(max_features)) (0 out of range). */
+size_t isb_forest_fit_groups_workspace_bytes(int n, int Dmax, int G, int T, int K, int max_features_max);
+int isb_forest_fit_groups(const float* x, int n, int Dmax, int G, const int32_t* D /* host */, const int32_t* max_features /* host */,
+                          const int32_t* min_samples_split /* host */, const int32_t* min_samples_leaf /* host */, const int32_t* y, int K,
+                          const int32_t* counts, int T, const int32_t* tree_group /* host */, const uint64_t* seeds, int max_depth,
+                          double min_impurity_decrease, int cap, int32_t* left, int32_t* right, int32_t* feature, double* threshold,
+                          double* impurity, int32_t* n_node_samples, double* weighted_n_node_samples, uint8_t* missing_go_to_left,
+                          int32_t* class_counts, int32_t* node_count, int* n_levels /* host */, void* ws, size_t ws_bytes, isb_stream_t stream);
+
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);
 

@@ -48,8 +48,15 @@ the transformed features to float32 and fits a ``'RandForest'`` or ``'DecTree'``
 (see ``forest_fit``).  The other classifiers, parameters the device does not compute, and the parameter search itself
 (``GridSearchCV`` / ``RandomizedSearchCV``) stay on scikit-learn; after a search the refit of the best pipeline goes to the device.
 
-Not provided: cross-validation scoring and ROC (``eval_classif_cross_val_*``), ``feature_scoring_selection`` and
-``create_pipeline_neuron_net``.
+The cross-validation: the reference's fold generators (``HoldOut``, ``CrossValidate``, ``CrossValidateGroups``; pure host code), and
+``eval_classif_cross_val_scores`` / ``eval_classif_cross_val_roc`` with the reference's folds, relabelling, per-scoring error handling
+and files.  For a ``'RandForest'`` or ``'DecTree'`` classifier (alone or ending a Pipeline) the transforms are fitted fold by fold on
+the host and the forests of every (scoring, fold) pair are built in one grouped device fit (``forest_fit.TreeBatch``,
+``isb_forest_fit_groups``); each tree is the one ``fit_tree_model`` builds for that fold alone, the global RNG is consumed in
+scikit-learn's order, and the scores and ROC are scikit-learn's scorers and ``roc_curve`` on the fitted pipelines.  Other classifiers
+go through scikit-learn's ``cross_val_score``.
+
+Not provided: ``feature_scoring_selection`` and ``create_pipeline_neuron_net``.
 """
 import collections
 import ctypes as C
@@ -1242,3 +1249,345 @@ def create_classif_search_train_export(clf_name, features, labels, cross_val=10,
     else:
         path_classif = path_out
     return clf_pipeline, path_classif
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# cross-validation: the fold generators, scores and mean ROC (every fold's tree or forest in one grouped device fit)
+# ---------------------------------------------------------------------------------------------------------------------
+
+def _device_folds(classif):
+    """whether the folds of ``classif`` are fitted through forest_fit.TreeBatch: a supported tree / forest, or a Pipeline ending in one"""
+    from .forest_fit import _supported
+    final = classif.steps[-1][1] if type(classif) is pipeline.Pipeline else classif
+    return _supported(final) is not None
+
+
+def _fit_folds(classif, features, labels, fold_lists, catch=True):
+    """one fitted clone of ``classif`` per (train, test) of every list of ``fold_lists`` (None where its fit raised), as scikit-learn's
+    ``cross_val_score`` fits them one after the other: per fold the transforms of a Pipeline are fitted on the host by scikit-learn
+    (``fit_transform`` of the training rows, as ``Pipeline.fit``) and the final tree or forest is prepared, and every tree of every fold
+    is built in one grouped device fit.  ``fold_lists`` may be a generator: each list is split only after the folds before it are
+    prepared, so a splitter that draws from numpy's global RNG draws at scikit-learn's place.  ``catch=False`` raises the error of a
+    failing fit."""
+    from sklearn.base import clone
+    from .forest_fit import TreeBatch
+    X = np.asarray(features)
+    y = np.asarray(labels)
+    batch = TreeBatch(y)
+    out = []
+    for folds in fold_lists:
+        models = []
+        for train, _ in folds:
+            model = clone(classif)
+            train = np.asarray(train)
+            if train.dtype == bool:
+                train = np.nonzero(train)[0]
+            try:
+                if type(model) is pipeline.Pipeline:
+                    Xt = X[train]
+                    for _, step in model.steps[:-1]:
+                        if step is None or (isinstance(step, str) and step == 'passthrough'):
+                            continue
+                        Xt = step.fit_transform(Xt, y[train])
+                    batch.add(model.steps[-1][1], Xt, train)
+                else:
+                    batch.add(model, X[train], train)
+            except Exception:
+                if not catch:
+                    raise
+                logging.exception('fit of a cross-validation fold')
+                model = None
+            models.append(model)
+        out.append(models)
+    fitted = iter(batch.fit())
+    for models in out:
+        for j, model in enumerate(models):
+            if model is None:
+                continue
+            final = next(fitted)
+            if type(model) is pipeline.Pipeline:
+                model.steps[-1] = (model.steps[-1][0], final)
+            else:
+                models[j] = final
+    return out
+
+
+def _fold_scores(models, folds, scorer, features, labels):
+    """scikit-learn's ``cross_val_score`` of the fitted ``models`` (``error_score=nan``): NaN and a warning where a fit or a score
+    failed, ValueError when every fit failed"""
+    from sklearn.exceptions import FitFailedWarning
+    X = np.asarray(features)
+    y = np.asarray(labels)
+    if all(m is None for m in models):
+        raise ValueError('All the %d fits failed.' % len(models))
+    if any(m is None for m in models):
+        warnings.warn('%d fits failed out of a total of %d; their score is nan' % (sum(m is None for m in models), len(models)),
+                      FitFailedWarning)
+    scores = []
+    for model, (_, test) in zip(models, folds):
+        score = np.nan
+        if model is not None:
+            try:
+                score = scorer(model, X[test], y[test])
+            except Exception:
+                warnings.warn('Scoring failed. The score on this train-test partition for these parameters will be set to nan.',
+                              UserWarning)
+        scores.append(score)
+    return np.asarray(scores, dtype=np.float64)
+
+
+def eval_classif_cross_val_scores(clf_name, classif, features, labels, cross_val=10, path_out=None, scorings=METRIC_SCORING):
+    """ the cross-validation scores of ``classif`` for every scoring of ``scorings``, one row per fold (reference
+    classification.py:762-850), as a DataFrame, written to ``path_out`` as ``NAME_CSV_CLASSIF_CV_SCORES`` 'all-folds' and, with more
+    than one row, 'statistic' (``describe()``).
+
+    As the reference: the folds come from ``check_cv(cross_val, labels, classifier=True)`` -- an int gives ``StratifiedKFold``, an
+    iterable of (train, test) such as :class:`CrossValidateGroups` is used as it is -- the labels are renumbered with
+    ``relabel_sequential`` when there are two or fewer, each scoring refits every fold, a failing scoring leaves its column out, and a
+    failing fit or score gives NaN.  A ``'RandForest'`` / ``'DecTree'`` classifier, alone or at the end of a Pipeline, has the trees of
+    all (scoring, fold) pairs built in one grouped device fit (``forest_fit.TreeBatch``) with the transforms fitted fold by fold on the
+    host; every score is scikit-learn's scorer of the fitted pipeline on the held-out rows.  Other classifiers go through
+    scikit-learn's ``cross_val_score``.
+
+    >>> labels = np.array([0] * 150 + [1] * 100 + [2] * 50)
+    >>> data = np.tile(labels, (6, 1)).T.astype(float)
+    >>> data += 0.5 - np.random.random(data.shape)
+    >>> from sklearn.model_selection import StratifiedKFold
+    >>> cv = StratifiedKFold(n_splits=5, random_state=0, shuffle=True)
+    >>> df = eval_classif_cross_val_scores('KNN', create_classifiers()['KNN'], data, labels, cv)
+    >>> df.round(decimals=1).values.tolist()[0]
+    [1.0, 1.0, 1.0, 1.0]
+    """
+    import pandas as pd
+    from sklearn.model_selection import check_cv, cross_val_score
+    df_scoring = pd.DataFrame()
+    if _device_folds(classif):
+        prepared = []
+
+        def _folds_of_each_scoring():
+            lbs = labels
+            for scoring in scorings:
+                try:
+                    uq_labels = np.unique(lbs)
+                    if len(uq_labels) <= 2:
+                        lbs = relabel_sequential(lbs, uq_labels)
+                    scorer = metrics.check_scoring(classif, scoring=scoring)
+                    folds = list(check_cv(cross_val, lbs, classifier=True).split(features, lbs))
+                except Exception:
+                    logging.exception('model_selection.cross_val_score')
+                    continue
+                prepared.append((scoring, scorer, folds, lbs))
+                yield folds
+        try:    # the labels every scoring trains on: relabel_sequential is the same for each
+            labels_fit = relabel_sequential(labels, np.unique(labels)) if len(np.unique(labels)) <= 2 else labels
+        except Exception:
+            labels_fit = labels                         # every scoring fails on the same relabelling, nothing is fitted
+        fitted = _fit_folds(classif, features, np.asarray(labels_fit), _folds_of_each_scoring())
+        for (scoring, scorer, folds, lbs), models in zip(prepared, fitted):
+            try:
+                scores = _fold_scores(models, folds, scorer, features, lbs)
+                logging.info('Cross-Val score (%s = %f):\n %r', scoring, np.mean(scores), scores)
+                df_scoring[scoring] = scores
+            except Exception:
+                logging.exception('model_selection.cross_val_score')
+    else:
+        for scoring in scorings:
+            try:
+                uq_labels = np.unique(labels)
+                if len(uq_labels) <= 2:
+                    labels = relabel_sequential(labels, uq_labels)
+                scores = cross_val_score(classif, features, labels, cv=cross_val, scoring=scoring)
+                logging.info('Cross-Val score (%s = %f):\n %r', scoring, np.mean(scores), scores)
+                df_scoring[scoring] = scores
+            except Exception:
+                logging.exception('model_selection.cross_val_score')
+
+    if path_out is not None:
+        if not os.path.exists(path_out):
+            raise FileNotFoundError('missing: "%s"' % path_out)
+        df_scoring.to_csv(os.path.join(path_out, NAME_CSV_CLASSIF_CV_SCORES.format(clf_name, 'all-folds')))
+    if len(df_scoring) > 1:
+        df_stat = df_scoring.describe()
+        logging.info('cross_val scores: \n %r', df_stat)
+        if path_out is not None:
+            df_stat.to_csv(os.path.join(path_out, NAME_CSV_CLASSIF_CV_SCORES.format(clf_name, 'statistic')))
+    else:
+        logging.warning('no statistic collected')
+    return df_scoring
+
+
+def eval_classif_cross_val_roc(clf_name, classif, features, labels, cross_val, path_out=None, nb_steps=100):
+    """ the mean ROC curve over the folds of ``cross_val`` and every label (one-vs-rest), as a DataFrame of ``nb_steps`` (FP, TP)
+    rows, and its AUC (reference classification.py:853-950); written to ``path_out`` as ``NAME_CSV_CLASSIF_CV_ROC`` and
+    ``NAME_TXT_CLASSIF_CV_AUC`` ('mean').  As the reference: labels must be non-negative, ``cross_val`` is an iterable of (train, test)
+    or has ``split``, the i-th unique label is scored with ``predict_proba(...)[:, i]``, each fold's curve is closed by (0, 0) and
+    (1, 1) and interpolated (``np.interp``) at ``linspace(0, 1, nb_steps)``, and the mean curve starts at 0 and ends at 1.  The trees
+    of a ``'RandForest'`` / ``'DecTree'`` classifier (alone or ending a Pipeline) of every fold are built in one grouped device fit.
+
+    >>> np.random.seed(0)
+    >>> labels = np.array([0] * 150 + [1] * 100 + [3] * 50)
+    >>> data = np.tile(labels, (6, 1)).T.astype(float)
+    >>> data += np.random.random(data.shape)
+    >>> from sklearn.model_selection import StratifiedKFold
+    >>> cv = StratifiedKFold(n_splits=5, random_state=0, shuffle=True)
+    >>> fp_tp, auc = eval_classif_cross_val_roc('KNN', create_classifiers()['KNN'], data, labels, cv, nb_steps=11)
+    >>> fp_tp.shape, round(auc, 2)
+    ((11, 2), 0.94)
+    """
+    import pandas as pd
+    from sklearn.base import clone
+    uq_labels = np.unique(labels)
+    if np.any(uq_labels < 0):
+        raise ValueError('some labels are negative: %r' % uq_labels)
+    # one-vs-rest targets, column i for the i-th unique label
+    targets = (np.asarray(labels).reshape(-1, 1) == uq_labels.reshape(1, -1)).astype(np.float64)
+    folds = cross_val if hasattr(cross_val, '__iter__') else cross_val.split(features, labels)
+    if _device_folds(classif):
+        folds = list(folds)
+        fitted = _fit_folds(classif, features, labels, [folds], catch=False)[0]
+    else:
+        fitted = None
+    grid = np.linspace(0, 1, nb_steps)
+    tpr_sum, n_curves = np.zeros(nb_steps), 0
+    for k, (train, test) in enumerate(folds):
+        if fitted is None:
+            model = clone(classif).fit(np.copy(features[train], order='C'), np.copy(labels[train], order='C'))
+        else:
+            model = fitted[k]
+        proba = model.predict_proba(np.copy(features[test], order='C'))
+        for i in range(len(uq_labels)):
+            fpr, tpr, _ = metrics.roc_curve(targets[test, i], proba[:, i])
+            # the curve closed by (0, 0) and (1, 1), sampled on the grid; the sum is taken curve by curve
+            tpr_sum += np.interp(grid, [0.] + fpr.tolist() + [1.], [0.] + tpr.tolist() + [1.])
+            n_curves += 1
+    mean_tpr = tpr_sum / float(n_curves)
+    mean_tpr[0], mean_tpr[-1] = 0.0, 1.0
+    df_roc = pd.DataFrame(np.array([grid, mean_tpr]).T, columns=['FP', 'TP'])
+    auc = metrics.auc(grid, mean_tpr)
+    if path_out is not None:
+        if not os.path.exists(path_out):
+            raise FileNotFoundError('missing: "%s"' % path_out)
+        df_roc.to_csv(os.path.join(path_out, NAME_CSV_CLASSIF_CV_ROC.format(clf_name, 'mean')))
+        with open(os.path.join(path_out, NAME_TXT_CLASSIF_CV_AUC.format(clf_name, 'mean')), 'w') as fp:
+            fp.write(str(auc))
+    logging.debug('cross_val ROC: \n %r', df_roc)
+    return df_roc, auc
+
+
+class HoldOut(object):
+    """ one split: the first ``hold_out`` indices train, the rest test; with ``rand_seed`` (default 0; None or False: keep the order)
+    the indices are shuffled after ``np.random.seed(rand_seed)`` (reference classification.py:1401-1453)
+
+    >>> ho = HoldOut(10, 7, rand_seed=None)
+    >>> len(ho), list(ho)
+    (1, [([0, 1, 2, 3, 4, 5, 6], [7, 8, 9])])
+    >>> list(HoldOut(10, 7, rand_seed=0))
+    [([2, 8, 4, 9, 1, 6, 7], [3, 0, 5])]
+    """
+
+    def __init__(self, nb_samples, hold_out, rand_seed=0):
+        if nb_samples <= hold_out:
+            raise ValueError('total %i should be higher than hold Idx %i' % (nb_samples, hold_out))
+        self._total = nb_samples
+        self.hold_out = hold_out
+        self._indexes = list(range(nb_samples))
+        if rand_seed is not None and rand_seed is not False:
+            np.random.seed(rand_seed)
+            np.random.shuffle(self._indexes)
+
+    def __iter__(self):
+        yield self._indexes[:self.hold_out], self._indexes[self.hold_out:]
+
+    def __len__(self):
+        return 1
+
+
+class CrossValidate(object):
+    """ folds of ``nb_hold_out`` test samples (a count, or a fraction of ``nb_samples`` when below 1) walking over ``indexes`` (shuffled
+    after ``np.random.seed(rand_seed)`` when a seed is given), the rest training (reference classification.py:1456-1604).
+
+    - A fold that would start fewer than ``ignore_overflow`` samples (a count, or a fraction when below 1) before the end is dropped.
+    - A last fold that runs past the end by more than ``ignore_overflow`` takes its missing test samples from the first indices, and
+      trains on the samples between; by less, it is kept short.
+    - When more than half is held out, the folds are built for the complement and train and test are swapped ("reverse mode").
+
+    >>> cv = CrossValidate(7, 3, rand_seed=0)
+    >>> list(cv)  # doctest: +NORMALIZE_WHITESPACE
+    [([3, 0, 5, 4], [6, 2, 1]),
+     ([6, 2, 1, 4], [3, 0, 5]),
+     ([1, 3, 0, 5], [4, 6, 2])]
+    >>> len(CrossValidate(340, 0.33, ignore_overflow=0.0)), len(CrossValidate(340, 0.33, ignore_overflow=0.05))
+    (4, 3)
+    """
+
+    def __init__(self, nb_samples, nb_hold_out, rand_seed=None, ignore_overflow=0.01):
+        if nb_samples <= nb_hold_out:
+            raise ValueError('Number of holdout has to be smaller then total size.')
+        if nb_hold_out <= 0:
+            raise ValueError('Number of holdout has to be positive number.')
+        self._nb_samples = nb_samples
+        self._nb_hold_out = int(np.round(nb_samples * nb_hold_out)) if nb_hold_out < 1 else nb_hold_out
+        ignore_overflow = abs(ignore_overflow)
+        self._ignore_overflow = int(np.round(nb_samples * ignore_overflow)) if ignore_overflow < 1 else ignore_overflow
+        if self._nb_hold_out <= self._ignore_overflow:
+            raise ValueError('The tolerance of overflowing (%i) the split has to be larger than the number of hold out samples (%i).'
+                             % (self._ignore_overflow, self._nb_hold_out))
+        # more held out than kept: build the folds of the complement and swap train and test
+        self._revert = self._nb_hold_out > self._nb_samples / 2.
+        if self._revert:
+            self._nb_hold_out = self._nb_samples - self._nb_hold_out
+        self.indexes = list(range(self._nb_samples))
+        self._shuffle = rand_seed is not None and rand_seed is not False
+        if self._shuffle:
+            np.random.seed(rand_seed)
+            np.random.shuffle(self.indexes)
+        self.iter = 0
+
+    def _starts(self):
+        """the first position of every fold, without those starting within ``ignore_overflow`` of the end"""
+        return [i for i in range(0, self._nb_samples, self._nb_hold_out) if self._nb_samples - i >= self._ignore_overflow]
+
+    def __iter__(self):
+        for begin in self._starts():
+            end = begin + self._nb_hold_out
+            test = self.indexes[begin:end]
+            train = self.indexes[:begin] + self.indexes[end:]
+            over = end - self._nb_samples
+            if over > self._ignore_overflow:
+                # the last fold runs past the end: its test wraps onto the first indices, its training set is what lies between
+                test += self.indexes[:over]
+                train = self.indexes[over:begin]
+            if self._revert:
+                train, test = test, train
+            yield train, test
+
+    def __len__(self):
+        return len(self._starts())
+
+
+class CrossValidateGroups(CrossValidate):
+    """ :class:`CrossValidate` over groups of consecutive samples (``set_sizes``: the samples of each group, e.g. the superpixels of
+    each image): ``nb_hold_out`` counts groups, and a fold yields the sample indices of its groups in fold order (reference
+    classification.py:1607-1705).
+
+    >>> cv = CrossValidateGroups([2, 2, 1, 2, 1], 2, rand_seed=0)
+    >>> cv.set_indexes, cv.indexes
+    ([[0, 1], [2, 3], [4], [5, 6], [7]], [2, 0, 1, 3, 4])
+    >>> list(cv)  # doctest: +NORMALIZE_WHITESPACE
+    [([2, 3, 5, 6, 7], [4, 0, 1]),
+     ([4, 0, 1, 7], [2, 3, 5, 6]),
+     ([0, 1, 2, 3, 5, 6], [7, 4])]
+    """
+
+    def __init__(self, set_sizes, nb_hold_out, rand_seed=None, ignore_overflow=0.01):
+        super(CrossValidateGroups, self).__init__(len(set_sizes), nb_hold_out, rand_seed, ignore_overflow)
+        self._set_sizes = list(set_sizes)
+        ends = np.cumsum([0] + self._set_sizes).tolist()
+        self.set_indexes = [list(range(b, e)) for b, e in zip(ends[:-1], ends[1:])]
+
+    def _samples(self, groups):
+        return [i for g in groups for i in self.set_indexes[g]]
+
+    def __iter__(self):
+        for train, test in super(CrossValidateGroups, self).__iter__():
+            yield self._samples(train), self._samples(test)

@@ -1,6 +1,10 @@
 // forest_fit.cu -- exact-split Gini trees of scikit-learn's DecisionTreeClassifier / RandomForestClassifier (splitter 'best'),
 // every tree of a forest built together, level by level.
 //
+// The trees may belong to G groups (isb_forest_fit_groups): a group is one training set of its own -- its own float32 copy of the n rows
+// with D_g of the Dmax columns, its own max_features, min_samples_split and min_samples_leaf -- and every kernel that reads x or one of
+// those parameters looks them up through the node's tree and that tree's group.  isb_forest_fit is the one-group call.
+//
 // Rows are "entries": a (tree, row) pair with a nonzero count (the bootstrap count, or 1).  Each level holds the nodes created by
 // the level before (all trees together, in breadth-first order), and the active entries grouped by node.  Per level:
 //   k_ff_stats       class counts and weight of every node (integer atomics: the same integers in any order)
@@ -62,6 +66,17 @@ __device__ __forceinline__ float f32_unordered(unsigned o)
     return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
 }
 
+// the groups as the kernels read them: x [G, n, Dmax] and, per tree, its group; per group its columns and parameters
+struct FfGroups {
+    const float* x;
+    long long n;
+    int Dmax;
+    const int32_t* tree_group;                      // [T]
+    const int32_t *D, *m, *mss, *msl;               // [G] each
+    __device__ __forceinline__ int of_tree(int t) const { return tree_group[t]; }
+    __device__ __forceinline__ const float* rows(int q) const { return x + (size_t)q * n * Dmax; }
+};
+
 struct FfWs {
     // entries
     int32_t *e_row, *e_tree, *e_node;
@@ -85,12 +100,13 @@ struct FfWs {
     // per tree, and the values read back
     unsigned long long *t_seed, *t_w, *t_next;
     int32_t *t_nnz, *t_first, *t_nsplit;
+    int32_t* grp;                                   // tree_group [T], then D, m, mss, msl [G] each
     long long* info;                                // [0] error flags, [1] entries, [2] elements, [3] segments, [4] splits, [5] next entries
     void* tmp;
     size_t tmp_bytes, need;
 };
 
-FfWs carve(void* base, int n, int D, int T, int K, int m)
+FfWs carve(void* base, int n, int D, int T, int K, int m, int G)
 {
     // E entries; NN nodes of all trees; M elements of a level (each entry in one node, m candidates); S segments of a level: they are
     // numbered over the splittable nodes only, which hold >= 2 entries each, so at most E / 2 of them
@@ -117,6 +133,7 @@ FfWs carve(void* base, int n, int D, int T, int K, int m)
     w.s_sql = c.take<unsigned long long>(S); w.s_sqr = c.take<unsigned long long>(S); w.s_pos = c.take<int32_t>(S);
     w.t_seed = c.take<unsigned long long>(T); w.t_w = c.take<unsigned long long>(T); w.t_next = c.take<unsigned long long>(T);
     w.t_nnz = c.take<int32_t>(T); w.t_first = c.take<int32_t>(T); w.t_nsplit = c.take<int32_t>(T);
+    w.grp = c.take<int32_t>(T + 4ll * G);
     w.info = c.take<long long>(8);
     size_t a = 0, b = 0, s1 = 0, s2 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, a, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (const uint32_t*)nullptr,
@@ -219,8 +236,8 @@ __device__ __forceinline__ double gini_of(unsigned long long sq, double w)
 
 // impurity, and the leaf tests of the depth-first builder that come before node_split
 __global__ void k_ff_decide(int L0, int nl, int K, const int32_t* __restrict__ nd_cc, const int32_t* __restrict__ nd_rows,
-                            const unsigned long long* __restrict__ nd_w, const int32_t* __restrict__ nd_depth, int max_depth, int mss, int msl,
-                            double* __restrict__ nd_imp, int32_t* __restrict__ nd_split, int32_t* __restrict__ lv_rows)
+                            const unsigned long long* __restrict__ nd_w, const int32_t* __restrict__ nd_depth, const int32_t* __restrict__ nd_tree,
+                            int max_depth, FfGroups gr, double* __restrict__ nd_imp, int32_t* __restrict__ nd_split, int32_t* __restrict__ lv_rows)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i > nl) return;
@@ -234,6 +251,7 @@ __global__ void k_ff_decide(int L0, int nl, int K, const int32_t* __restrict__ n
     const double imp = gini_of(sq, (double)nd_w[g]);
     nd_imp[g] = imp;
     const int rows = nd_rows[g];
+    const int q = gr.of_tree(nd_tree[g]), mss = gr.mss[q], msl = gr.msl[q];
     const bool leaf = (max_depth >= 0 && nd_depth[g] >= max_depth) || rows < mss || rows < 2 * msl || imp <= FF_EPSILON;
     nd_split[g] = leaf ? 0 : 1;
     lv_rows[i] = rows;
@@ -242,18 +260,22 @@ __global__ void k_ff_decide(int L0, int nl, int K, const int32_t* __restrict__ n
 // non-constant bits: block (node, 32-feature word); lanes are features (coalesced rows of x), warps stride the node's rows
 constexpr int NC_WARPS = 4;
 __global__ void __launch_bounds__(NC_WARPS * 32)
-k_ff_nonconst(const float* __restrict__ x, int D, int L0, const int32_t* __restrict__ nd_split, const int32_t* __restrict__ lv_start,
+k_ff_nonconst(FfGroups gr, int L0, const int32_t* __restrict__ nd_split, const int32_t* __restrict__ nd_tree, const int32_t* __restrict__ lv_start,
               const uint32_t* __restrict__ g_idx, const int32_t* __restrict__ e_row, uint32_t* __restrict__ nc_bits, int W)
 {
     const int i = blockIdx.x, word = blockIdx.y;
     if (!nd_split[L0 + i]) return;
+    const int grp = gr.of_tree(nd_tree[L0 + i]), D = gr.D[grp];
+    if (word * 32 >= D) return;                         // words past the group's columns are never read
+    const float* x = gr.rows(grp);
+    const int Dmax = gr.Dmax;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int f = word * 32 + lane;
     const int b = lv_start[i], e = lv_start[i + 1];
     float lo = __int_as_float(0x7f800000), hi = -__int_as_float(0x7f800000);
     if (f < D) {
         for (int q = b + warp; q < e; q += NC_WARPS) {
-            const float v = x[(size_t)e_row[g_idx[q]] * D + f];
+            const float v = x[(size_t)e_row[g_idx[q]] * Dmax + f];
             lo = fminf(lo, v);
             hi = fmaxf(hi, v);
         }
@@ -276,7 +298,7 @@ k_ff_nonconst(const float* __restrict__ x, int D, int L0, const int32_t* __restr
 // candidate features of every splittable node, ascending feature index; lv_ncand = their number, lv_nelem = rows * candidates
 constexpr int CAND_THREADS = 128;
 __global__ void __launch_bounds__(CAND_THREADS)
-k_ff_candidates(int D, int W, int m, int L0, int nl, int32_t* __restrict__ nd_split, const int32_t* __restrict__ nd_tree,
+k_ff_candidates(FfGroups gr, int W, int L0, int nl, int32_t* __restrict__ nd_split, const int32_t* __restrict__ nd_tree,
                 const unsigned long long* __restrict__ nd_local, const unsigned long long* __restrict__ t_seed, const uint32_t* __restrict__ nc_bits,
                 const int32_t* __restrict__ nd_rows, int32_t* __restrict__ lv_ncand, long long* __restrict__ lv_nelem, int32_t* __restrict__ cand,
                 int cand_stride)
@@ -294,6 +316,7 @@ k_ff_candidates(int D, int W, int m, int L0, int nl, int32_t* __restrict__ nd_sp
     __shared__ unsigned long long s_hash[FF_DMAX];
     __shared__ unsigned char s_sel[FF_DMAX];
     __shared__ int s_count;
+    const int grp = gr.of_tree(nd_tree[g]), D = gr.D[grp], m = gr.m[grp];
     const uint32_t* bits = nc_bits + (size_t)i * W;
     const unsigned long long key = splitmix64(splitmix64(t_seed[nd_tree[g]]) ^ nd_local[g]);
     int mine = 0;
@@ -388,7 +411,7 @@ __device__ __forceinline__ int upper_index32(const int32_t* off, int n, int v)
 }
 
 // one (segment, ordered value) key per (candidate j, row) of every node; element layout = node, candidate, row
-__global__ void k_ff_fill(const float* __restrict__ x, int D, int L0, int nl, long long n_elem, const long long* __restrict__ lv_elemoff,
+__global__ void k_ff_fill(FfGroups gr, const int32_t* __restrict__ nd_tree, int L0, int nl, long long n_elem, const long long* __restrict__ lv_elemoff,
                           const int32_t* __restrict__ lv_segoff, const int32_t* __restrict__ lv_start, const int32_t* __restrict__ nd_rows,
                           const int32_t* __restrict__ cand, int cand_stride, const uint32_t* __restrict__ g_idx, const int32_t* __restrict__ e_row,
                           const uint32_t* __restrict__ e_pay, unsigned long long* __restrict__ k_in, uint32_t* __restrict__ p_in)
@@ -400,13 +423,14 @@ __global__ void k_ff_fill(const float* __restrict__ x, int D, int L0, int nl, lo
         const int j = (int)(r / rows), k = (int)(r % rows);
         const int e = (int)g_idx[lv_start[i] + k];
         const int f = cand[(size_t)i * cand_stride + j];
-        k_in[q] = ((unsigned long long)(lv_segoff[i] + j) << 32) | f32_ordered(x[(size_t)e_row[e] * D + f]);
+        const float* x = gr.rows(gr.of_tree(nd_tree[L0 + i]));
+        k_in[q] = ((unsigned long long)(lv_segoff[i] + j) << 32) | f32_ordered(x[(size_t)e_row[e] * gr.Dmax + f]);
         p_in[q] = e_pay[e];
     }
 }
 
 // one thread per segment: the allowed position of largest proxy improvement, the first one on ties (the strict > of node_split_best)
-__global__ void k_ff_scan(int L0, int nl, int n_seg, int K, int msl, const int32_t* __restrict__ lv_segoff, const long long* __restrict__ lv_elemoff,
+__global__ void k_ff_scan(int L0, int nl, int n_seg, int K, FfGroups gr, const int32_t* __restrict__ nd_tree, const int32_t* __restrict__ lv_segoff, const long long* __restrict__ lv_elemoff,
                           const int32_t* __restrict__ nd_rows, const int32_t* __restrict__ nd_cc, const unsigned long long* __restrict__ nd_w,
                           const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ pay, double* __restrict__ s_proxy,
                           int32_t* __restrict__ s_pos, double* __restrict__ s_thr, double* __restrict__ s_wl, unsigned long long* __restrict__ s_sql,
@@ -415,7 +439,7 @@ __global__ void k_ff_scan(int L0, int nl, int n_seg, int K, int msl, const int32
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_seg) return;
     const int i = upper_index32(lv_segoff, nl, s);
-    const int g = L0 + i, rows = nd_rows[g];
+    const int g = L0 + i, rows = nd_rows[g], msl = gr.msl[gr.of_tree(nd_tree[g])];
     const long long b = lv_elemoff[i] + (long long)(s - lv_segoff[i]) * rows;
     const int32_t* tot = nd_cc + (size_t)g * K;
     int left[FF_KMAX];
@@ -543,7 +567,7 @@ __global__ void k_ff_tree_advance(int T, unsigned long long* __restrict__ t_next
 }
 
 // each active entry to its child (x <= threshold goes left, as DecisionTreeClassifier.apply); entries of leaves leave the build
-__global__ void k_ff_route(const float* __restrict__ x, int D, int L1, int n_child, const uint32_t* __restrict__ g_idx, int n_active,
+__global__ void k_ff_route(FfGroups gr, const int32_t* __restrict__ nd_tree, int L1, int n_child, const uint32_t* __restrict__ g_idx, int n_active,
                            int32_t* __restrict__ e_node, const int32_t* __restrict__ e_row, const int32_t* __restrict__ nd_split,
                            const int32_t* __restrict__ nd_feature, const double* __restrict__ nd_thr, const int32_t* __restrict__ nd_left,
                            uint32_t* __restrict__ g_key, uint32_t* __restrict__ g_val)
@@ -554,7 +578,7 @@ __global__ void k_ff_route(const float* __restrict__ x, int D, int L1, int n_chi
     const int node = e_node[e];
     int child = -1;
     if (node >= 0 && nd_split[node]) {
-        const float v = x[(size_t)e_row[e] * D + nd_feature[node]];
+        const float v = gr.rows(gr.of_tree(nd_tree[node]))[(size_t)e_row[e] * gr.Dmax + nd_feature[node]];
         child = nd_left[node] + ((double)v <= nd_thr[node] ? 0 : 1);
     }
     e_node[e] = child;
@@ -632,31 +656,42 @@ int read_back(T* host, const T* dev, size_t n, cudaStream_t st)
     return ISB_OK;
 }
 
-} // namespace
-
-extern "C" size_t isb_forest_fit_workspace_bytes(int n, int D, int T, int K, int max_features)
+// the per-group parameters and the trees' groups (host arrays): ISB_ERR_ARG before any device work
+int check_groups(int Dmax, int G, const int32_t* D, const int32_t* m, const int32_t* mss, const int32_t* msl, int T, const int32_t* tree_group)
 {
-    if (check_sizes(n, D, T, K, max_features) != ISB_OK) return 0;
-    return carve(nullptr, n, D, T, K, max_features).need;
+    ISB_REQUIRE(G >= 1 && D && m && mss && msl && tree_group, "need G >= 1 and the per-group and per-tree arrays");
+    for (int q = 0; q < G; ++q) {
+        if (D[q] < 1 || D[q] > Dmax) { isb_set_error("group %d has %d features, not in [1, Dmax = %d]", q, D[q], Dmax); return ISB_ERR_ARG; }
+        if (m[q] < 1 || m[q] > D[q]) { isb_set_error("group %d: max_features %d not in [1, %d]", q, m[q], D[q]); return ISB_ERR_ARG; }
+        if (mss[q] < 2 || msl[q] < 1) { isb_set_error("group %d: min_samples_split %d < 2 or min_samples_leaf %d < 1", q, mss[q], msl[q]); return ISB_ERR_ARG; }
+    }
+    for (int t = 0; t < T; ++t)
+        if (tree_group[t] < 0 || tree_group[t] >= G) { isb_set_error("tree %d: group %d not in [0, %d)", t, tree_group[t], G); return ISB_ERR_ARG; }
+    return ISB_OK;
 }
 
-extern "C" int isb_forest_fit(const float* x, int n, int D, const int32_t* y, int K, const int32_t* counts, int T, const uint64_t* seeds,
-                              int max_features, int min_samples_split, int min_samples_leaf, int max_depth, double min_impurity_decrease, int cap,
-                              int32_t* left, int32_t* right, int32_t* feature, double* threshold, double* impurity, int32_t* n_node_samples,
-                              double* weighted_n_node_samples, uint8_t* missing_go_to_left, int32_t* class_counts, int32_t* node_count,
-                              int* n_levels, void* ws, size_t ws_bytes, isb_stream_t stream)
+int max_of(const int32_t* v, int n)
 {
-    if (int s = check_sizes(n, D, T, K, max_features)) return s;
-    ISB_REQUIRE(x && y && counts && seeds && left && right && feature && threshold && impurity && n_node_samples && weighted_n_node_samples &&
-                    missing_go_to_left && class_counts && node_count && ws, "null pointer");
-    ISB_REQUIRE(min_samples_split >= 2 && min_samples_leaf >= 1 && max_depth >= -1 && cap >= 1, "bad tree parameter");
-    ISB_REQUIRE(min_impurity_decrease == min_impurity_decrease, "min_impurity_decrease is NaN");
-    ISB_REQUIRE(ws_bytes >= isb_forest_fit_workspace_bytes(n, D, T, K, max_features), "workspace too small");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int m = max_features, W = (D + 31) / 32;
+    int r = v[0];
+    for (int i = 1; i < n; ++i) r = std::max(r, (int)v[i]);
+    return r;
+}
+
+// the level loop of both entry points, over validated arguments
+int fit_groups(const float* x, int n, int Dmax, int G, const int32_t* hD, const int32_t* hm, const int32_t* hmss, const int32_t* hmsl,
+               const int32_t* y, int K, const int32_t* counts, int T, const int32_t* htree_group, const uint64_t* seeds, int max_depth,
+               double min_impurity_decrease, int cap, int32_t* left, int32_t* right, int32_t* feature, double* threshold, double* impurity,
+               int32_t* n_node_samples, double* weighted_n_node_samples, uint8_t* missing_go_to_left, int32_t* class_counts,
+               int32_t* node_count, int* n_levels, void* ws, cudaStream_t st)
+{
+    const int mmax = max_of(hm, G), W = (Dmax + 31) / 32;
     const long long TN = (long long)T * n;
-    FfWs w = carve(ws, n, D, T, K, m);
-    const int cand_stride = m;
+    FfWs w = carve(ws, n, Dmax, T, K, mmax, G);
+    const int cand_stride = mmax;
+    std::vector<int32_t> grp(htree_group, htree_group + T);
+    for (const int32_t* a : {hD, hm, hmss, hmsl}) grp.insert(grp.end(), a, a + G);
+    ISB_CUDA_CHECK(cudaMemcpyAsync(w.grp, grp.data(), grp.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    const FfGroups gr{x, n, Dmax, w.grp, w.grp + T, w.grp + T + G, w.grp + T + 2 * G, w.grp + T + 3 * G};
 
     // entries, roots, per-tree totals
     ISB_CUDA_CHECK(cudaMemsetAsync(w.t_nnz, 0, T * sizeof(int32_t), st));
@@ -697,14 +732,14 @@ extern "C" int isb_forest_fit(const float* x, int n, int D, const int32_t* y, in
         ISB_LAUNCH_CHECK();
         k_ff_stats<<<blocks_of(n_active), TB, 0, st>>>(w.g_idx, n_active, w.e_node, w.e_pay, K, w.nd_cc, w.nd_rows, w.nd_w);
         ISB_LAUNCH_CHECK();
-        k_ff_decide<<<blocks_of(nl + 1), TB, 0, st>>>(L0, nl, K, w.nd_cc, w.nd_rows, w.nd_w, w.nd_depth, max_depth, min_samples_split,
-                                                      min_samples_leaf, w.nd_imp, w.nd_split, w.lv_rows);
+        k_ff_decide<<<blocks_of(nl + 1), TB, 0, st>>>(L0, nl, K, w.nd_cc, w.nd_rows, w.nd_w, w.nd_depth, w.nd_tree, max_depth, gr, w.nd_imp,
+                                                      w.nd_split, w.lv_rows);
         ISB_LAUNCH_CHECK();
         tb = w.tmp_bytes;
         ISB_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(w.tmp, tb, w.lv_rows, w.lv_start, nl + 1, st));
-        k_ff_nonconst<<<dim3(nl, W), NC_WARPS * 32, 0, st>>>(x, D, L0, w.nd_split, w.lv_start, w.g_idx, w.e_row, w.nc_bits, W);
+        k_ff_nonconst<<<dim3(nl, W), NC_WARPS * 32, 0, st>>>(gr, L0, w.nd_split, w.nd_tree, w.lv_start, w.g_idx, w.e_row, w.nc_bits, W);
         ISB_LAUNCH_CHECK();
-        k_ff_candidates<<<nl + 1, CAND_THREADS, 0, st>>>(D, W, m, L0, nl, w.nd_split, w.nd_tree, w.nd_local, w.t_seed, w.nc_bits, w.nd_rows,
+        k_ff_candidates<<<nl + 1, CAND_THREADS, 0, st>>>(gr, W, L0, nl, w.nd_split, w.nd_tree, w.nd_local, w.t_seed, w.nc_bits, w.nd_rows,
                                                           w.lv_ncand, w.lv_nelem, w.cand, cand_stride);
         ISB_LAUNCH_CHECK();
         tb = w.tmp_bytes;
@@ -718,13 +753,13 @@ extern "C" int isb_forest_fit(const float* x, int n, int D, const int32_t* y, in
         const int n_seg = (int)info[3];
         if (n_seg > 0) {
             k_ff_fill<<<(int)std::min<long long>(blocks_of(n_elem), 65535ll * 8), TB, 0, st>>>(
-                x, D, L0, nl, n_elem, w.lv_elemoff, w.lv_segoff, w.lv_start, w.nd_rows, w.cand, cand_stride, w.g_idx, w.e_row, w.e_pay, w.k_in, w.p_in);
+                gr, w.nd_tree, L0, nl, n_elem, w.lv_elemoff, w.lv_segoff, w.lv_start, w.nd_rows, w.cand, cand_stride, w.g_idx, w.e_row, w.e_pay, w.k_in, w.p_in);
             ISB_LAUNCH_CHECK();
             tb = w.tmp_bytes;
             ISB_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(w.tmp, tb, w.k_in, w.k_out, w.p_in, w.p_out, (int)n_elem, 0,
                                                            32 + bits_for((unsigned long long)n_seg), st));
             ISB_LAUNCH_CHECK();
-            k_ff_scan<<<blocks_of(n_seg, 128), 128, 0, st>>>(L0, nl, n_seg, K, min_samples_leaf, w.lv_segoff, w.lv_elemoff, w.nd_rows, w.nd_cc,
+            k_ff_scan<<<blocks_of(n_seg, 128), 128, 0, st>>>(L0, nl, n_seg, K, gr, w.nd_tree, w.lv_segoff, w.lv_elemoff, w.nd_rows, w.nd_cc,
                                                              w.nd_w, w.k_out, w.p_out, w.s_proxy, w.s_pos, w.s_thr, w.s_wl, w.s_sql, w.s_sqr);
             ISB_LAUNCH_CHECK();
         }
@@ -747,7 +782,7 @@ extern "C" int isb_forest_fit(const float* x, int n, int D, const int32_t* y, in
         ISB_LAUNCH_CHECK();
         if (n_split == 0) { L0 = L1; break; }
         const int n_child = 2 * n_split;
-        k_ff_route<<<blocks_of(n_active), TB, 0, st>>>(x, D, L1, n_child, w.g_idx, n_active, w.e_node, w.e_row, w.nd_split, w.nd_feature, w.nd_thr,
+        k_ff_route<<<blocks_of(n_active), TB, 0, st>>>(gr, w.nd_tree, L1, n_child, w.g_idx, n_active, w.e_node, w.e_row, w.nd_split, w.nd_feature, w.nd_thr,
                                                        w.nd_left, w.g_key, w.g_idx2);
         ISB_LAUNCH_CHECK();
         tb = w.tmp_bytes;
@@ -775,4 +810,57 @@ extern "C" int isb_forest_fit(const float* x, int n, int D, const int32_t* y, in
     ISB_LAUNCH_CHECK();
     if (n_levels) *n_levels = (int)level_begin.size();
     return ISB_OK;
+}
+
+} // namespace
+
+extern "C" size_t isb_forest_fit_workspace_bytes(int n, int D, int T, int K, int max_features)
+{
+    if (check_sizes(n, D, T, K, max_features) != ISB_OK) return 0;
+    return carve(nullptr, n, D, T, K, max_features, 1).need;
+}
+
+extern "C" int isb_forest_fit(const float* x, int n, int D, const int32_t* y, int K, const int32_t* counts, int T, const uint64_t* seeds,
+                              int max_features, int min_samples_split, int min_samples_leaf, int max_depth, double min_impurity_decrease, int cap,
+                              int32_t* left, int32_t* right, int32_t* feature, double* threshold, double* impurity, int32_t* n_node_samples,
+                              double* weighted_n_node_samples, uint8_t* missing_go_to_left, int32_t* class_counts, int32_t* node_count,
+                              int* n_levels, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    if (int s = check_sizes(n, D, T, K, max_features)) return s;
+    ISB_REQUIRE(x && y && counts && seeds && left && right && feature && threshold && impurity && n_node_samples && weighted_n_node_samples &&
+                    missing_go_to_left && class_counts && node_count && ws, "null pointer");
+    ISB_REQUIRE(min_samples_split >= 2 && min_samples_leaf >= 1 && max_depth >= -1 && cap >= 1, "bad tree parameter");
+    ISB_REQUIRE(min_impurity_decrease == min_impurity_decrease, "min_impurity_decrease is NaN");
+    ISB_REQUIRE(ws_bytes >= isb_forest_fit_workspace_bytes(n, D, T, K, max_features), "workspace too small");
+    const std::vector<int32_t> tree_group(T, 0);
+    return fit_groups(x, n, D, 1, &D, &max_features, &min_samples_split, &min_samples_leaf, y, K, counts, T, tree_group.data(), seeds,
+                      max_depth, min_impurity_decrease, cap, left, right, feature, threshold, impurity, n_node_samples, weighted_n_node_samples,
+                      missing_go_to_left, class_counts, node_count, n_levels, ws, (cudaStream_t)stream);
+}
+
+extern "C" size_t isb_forest_fit_groups_workspace_bytes(int n, int Dmax, int G, int T, int K, int max_features_max)
+{
+    if (G < 1 || check_sizes(n, Dmax, T, K, max_features_max) != ISB_OK) return 0;
+    return carve(nullptr, n, Dmax, T, K, max_features_max, G).need;
+}
+
+extern "C" int isb_forest_fit_groups(const float* x, int n, int Dmax, int G, const int32_t* D, const int32_t* max_features,
+                                     const int32_t* min_samples_split, const int32_t* min_samples_leaf, const int32_t* y, int K,
+                                     const int32_t* counts, int T, const int32_t* tree_group, const uint64_t* seeds, int max_depth,
+                                     double min_impurity_decrease, int cap, int32_t* left, int32_t* right, int32_t* feature, double* threshold,
+                                     double* impurity, int32_t* n_node_samples, double* weighted_n_node_samples, uint8_t* missing_go_to_left,
+                                     int32_t* class_counts, int32_t* node_count, int* n_levels, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    ISB_REQUIRE(n >= 1 && Dmax >= 1 && T >= 1 && K >= 1, "need n, Dmax, T, K >= 1");
+    if (int s = check_groups(Dmax, G, D, max_features, min_samples_split, min_samples_leaf, T, tree_group)) return s;
+    const int mmax = max_of(max_features, G);
+    if (int s = check_sizes(n, Dmax, T, K, mmax)) return s;
+    ISB_REQUIRE(x && y && counts && seeds && left && right && feature && threshold && impurity && n_node_samples && weighted_n_node_samples &&
+                    missing_go_to_left && class_counts && node_count && ws, "null pointer");
+    ISB_REQUIRE(max_depth >= -1 && cap >= 1, "bad tree parameter");
+    ISB_REQUIRE(min_impurity_decrease == min_impurity_decrease, "min_impurity_decrease is NaN");
+    ISB_REQUIRE(ws_bytes >= isb_forest_fit_groups_workspace_bytes(n, Dmax, G, T, K, mmax), "workspace too small");
+    return fit_groups(x, n, Dmax, G, D, max_features, min_samples_split, min_samples_leaf, y, K, counts, T, tree_group, seeds, max_depth,
+                      min_impurity_decrease, cap, left, right, feature, threshold, impurity, n_node_samples, weighted_n_node_samples,
+                      missing_go_to_left, class_counts, node_count, n_levels, ws, (cudaStream_t)stream);
 }
