@@ -4,8 +4,9 @@ H100-native implementation in ``pyimsegm_b200`` for the SLIC -> features -> Grap
 region growing (RG2SP) built on it, and for ``labeling``, ``ellipse_fitting``, ``annotation`` and ``classification``.  Of
 ``classification`` the scoring (segmentations against annotations), the training-set preparation (class balancing, k-means
 down-sampling on the device), the classifier training (random forests and decision trees fitted on the device) and the
-cross-validation (the fold generators, scores and mean ROC, every fold's forest built in one grouped device fit) are provided; feature
-selection is not.
+cross-validation (the fold generators, scores and mean ROC, every fold's forest built in one grouped device fit) and the feature
+scoring (the extra-trees importances fitted on the device, node for node scikit-learn's) are provided: every public name of the
+reference's module.
 """
 import sys
 

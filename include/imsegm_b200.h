@@ -623,6 +623,30 @@ int isb_forest_fit_groups(const float* x, int n, int Dmax, int G, const int32_t*
                           double* impurity, int32_t* n_node_samples, double* weighted_n_node_samples, uint8_t* missing_go_to_left,
                           int32_t* class_counts, int32_t* node_count, int* n_levels /* host */, void* ws, size_t ws_bytes, isb_stream_t stream);
 
+/* random-split Gini trees of scikit-learn's ExtraTreesClassifier fit, node for node the trees scikit-learn 1.9 builds (the forest of
+ * feature_scoring_selection); one CTA per tree replays the depth-first builder and every draw of its splitter.
+ *   x [n, D] f32 row-major, y [n] i32 class indices in [0, K), K <= 64, counts [T, n] i32: as isb_forest_fit;
+ *   rand_r_state [T] u32 (device): each tree's splitter state, RandomState(tree seed).randint(0, 2^31 - 1) (Splitter.init);
+ *   max_features, min_samples_split, min_samples_leaf, max_depth (-1: none), min_impurity_decrease: as isb_forest_fit;
+ *   small_rows: nodes of at most this many rows build their subtree on one warp from rows staged in shared memory (0: the default,
+ *   64; lowered until the staged rows fit 96 KiB).
+ * The rules are node_split_random's (_splitter.pyx) and DepthFirstTreeBuilder.build's (_tree.pyx): the Fisher-Yates feature draws
+ * rand_int(n_drawn_constants, f_i - n_found_constants) with the known / found / drawn constant bookkeeping, the features and
+ * constant_features arrays carried from node to node in depth-first order; a feature is constant when max <= min + 1e-7f (float32);
+ * threshold rand_uniform(min, max) in f64, min when it equals max; rows with (f64) x <= threshold go left; a candidate with fewer than
+ * min_samples_leaf rows on a side is rejected; the largest Gini proxy wins (the first on ties); missing_go_to_left = n_left > n_right;
+ * the builder's leaf tests; the left child is built first.  our_rand_r maps a state of 0 to 1.
+ * Outputs, their layout and cap: as isb_forest_fit.  Argument errors (including a negative count, a class outside [0, K) or a tree with
+ * no row) return ISB_ERR_ARG.  Limits (ISB_ERR_UNSUPPORTED): D <= 2048, K <= 64, T * n < 2^31, the total count of a tree < 2^26.
+ * The call synchronises the stream once, before the build, to check the counts.
+ * ws: isb_extra_trees_fit_workspace_bytes(n, D, T, K, max_features) (0 out of range), about 28 * T * n bytes. */
+size_t isb_extra_trees_fit_workspace_bytes(int n, int D, int T, int K, int max_features);
+int isb_extra_trees_fit(const float* x, int n, int D, const int32_t* y, int K, const int32_t* counts, int T, const uint32_t* rand_r_state,
+                        int max_features, int min_samples_split, int min_samples_leaf, int max_depth, double min_impurity_decrease,
+                        int small_rows, int cap, int32_t* left, int32_t* right, int32_t* feature, double* threshold, double* impurity,
+                        int32_t* n_node_samples, double* weighted_n_node_samples, uint8_t* missing_go_to_left, int32_t* class_counts,
+                        int32_t* node_count, void* ws, size_t ws_bytes, isb_stream_t stream);
+
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);
 

@@ -146,6 +146,9 @@ SIGNATURES = {
     'isb_forest_fit_groups_workspace_bytes': (_sz, [_i, _i, _i, _i, _i, _i]),
     'isb_forest_fit_groups': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _d, _i, _vp, _vp, _vp, _vp, _vp, _vp,
                                    _vp, _vp, _vp, _vp, C.POINTER(_i), _vp, _sz, _vp]),
+    'isb_extra_trees_fit_workspace_bytes': (_sz, [_i, _i, _i, _i, _i]),
+    'isb_extra_trees_fit': (_i, [_vp, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _d, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                 _vp, _vp, _sz, _vp]),
 }
 
 

@@ -1,6 +1,6 @@
 """
-The reference's ``imsegm/classification.py`` without its classifier training: the metrics between annotations and segmentations,
-and the preparation of class-balanced training sets.
+The reference's ``imsegm/classification.py``: the metrics between annotations and segmentations, the preparation of class-balanced
+training sets, the classifiers, their cross-validation and the feature scoring.
 
 Every number comes from one contingency table -- the pixels of every (annotation value, segmentation value) pair after the
 ``drop_labels`` mask -- counted on the device (``csrc/classification.cu``, one upload of the two maps and three passes over them).
@@ -56,7 +56,14 @@ the host and the forests of every (scoring, fold) pair are built in one grouped 
 scikit-learn's order, and the scores and ROC are scikit-learn's scorers and ``roc_curve`` on the fitted pipelines.  Other classifiers
 go through scikit-learn's ``cross_val_score``.
 
-Not provided: ``feature_scoring_selection`` and ``create_pipeline_neuron_net``.
+The feature scoring: ``feature_scoring_selection`` ranks the features by the importances of ``ExtraTreesClassifier(n_estimators=125,
+random_state=0)`` fitted on the device (``forest_fit.fit_extra_trees``, ``csrc/extra_trees_fit.cu``): one CTA per tree replays
+scikit-learn 1.9's depth-first build and every draw of its splitter, so the trees, importances and ranking are scikit-learn's bits.
+Features that are not finite as float32, or a table above the kernel's limits, are fitted by scikit-learn.  The F-test
+(``f_regression``), k-Best (``SelectKBest(f_classif)``) and variance (``VarianceThreshold``) scores are scikit-learn on the host,
+called as the reference calls them.  ``create_pipeline_neuron_net`` is the reference's unfitted BernoulliRBM + LogisticRegression
+pipeline.  Differences: the score table is built in one step (the reference's ``DataFrame.append`` is gone from pandas 2), and of
+more ``names`` than features the first D are used (the reference raises ``IndexError``).
 """
 import collections
 import ctypes as C
@@ -69,7 +76,7 @@ import warnings
 import numpy as np
 from scipy.stats import randint as sp_randint
 from scipy.stats import uniform as sp_random
-from sklearn import decomposition, ensemble, linear_model, metrics, neighbors, pipeline, preprocessing, svm, tree
+from sklearn import decomposition, ensemble, linear_model, metrics, neighbors, neural_network, pipeline, preprocessing, svm, tree
 from sklearn.exceptions import ConvergenceWarning
 from sklearn.model_selection import GridSearchCV, RandomizedSearchCV
 
@@ -1081,6 +1088,17 @@ def create_clf_param_search_distrib(name_classif=DEFAULT_CLASSIF_NAME):
     return clf_params.get(name_classif, {})
 
 
+def create_pipeline_neuron_net():
+    """ a BernoulliRBM feeding a LogisticRegression, unfitted (reference classification.py:271-283); fitted by scikit-learn
+
+    >>> create_pipeline_neuron_net()  # doctest: +ELLIPSIS
+    Pipeline(...)
+    """
+    logistic = linear_model.LogisticRegression()
+    rbm = neural_network.BernoulliRBM(learning_rate=0.05, n_components=35, n_iter=299, verbose=False)
+    return pipeline.Pipeline(steps=[('rbm', rbm), ('logistic', logistic)])
+
+
 def search_params_cut_down_max_nb_iter(clf_parameters, nb_iter):
     """ ``nb_iter`` capped at the number of combinations when every parameter is a list (reference classification.py:953-977)
 
@@ -1185,6 +1203,71 @@ def export_results_clf_search(path_out, clf_name, clf_search):
         params = clf_search.best_params_
         rows = ['{:30s} {}'.format('"{}":'.format(k), params[k]) for k in params]
         fp.write('\n'.join(rows))
+
+
+def feature_scoring_selection(features, labels, names=None, path_out=''):
+    """ score every feature and rank them by the importances of ``ExtraTreesClassifier(n_estimators=125, random_state=0)`` (reference
+    classification.py:474-544); the forest is fitted on the device (``forest_fit.fit_extra_trees``), node for node scikit-learn's
+
+    :param ndarray features: np.array<nb_samples, nb_features>
+    :param ndarray labels: np.array<nb_samples, 1>
+    :param list(str) names: the feature names ('1' .. 'D' when None or shorter than the features)
+    :param str path_out: a directory to write ``NAME_CSV_FEATURES_SELECT`` into, when it exists
+    :return tuple(list(int),DF): indices of decreasing importance, DataFrame of the scores
+
+    >>> from sklearn.datasets import make_classification
+    >>> features, labels = make_classification(
+    ...     n_samples=250, n_features=5, n_informative=3, n_redundant=0, n_repeated=0,
+    ...     n_classes=2, random_state=0, shuffle=False)
+    >>> indices, df_scoring = feature_scoring_selection(features, labels)  # doctest: +ELLIPSIS
+    >>> indices
+    array([1, 0, 2, 3, 4]...)
+    >>> df_scoring.sort_index(axis=1)  # doctest: +NORMALIZE_WHITESPACE +ELLIPSIS
+             ExtTree    F-test    k-Best variance
+    feature
+    1        0.24...   0.75...   0.75...  2.49...
+    2        0.33...  58.94...  58.94...  1.85...
+    3        0.22...   2.24...   2.24...  1.54...
+    4        0.10...   4.02...   4.02...  0.96...
+    5        0.09...   0.02...   0.02...  1.01...
+    >>> features[:, 2] = 1
+    >>> path_out = 'test_fts-select'
+    >>> os.mkdir(path_out)
+    >>> indices, df_scoring = feature_scoring_selection(features.tolist(), labels.tolist(), path_out=path_out)
+    >>> indices  # doctest: +ELLIPSIS
+    array([1, 0, 3, 4, 2]...)
+    >>> import shutil
+    >>> shutil.rmtree(path_out, ignore_errors=True)
+    """
+    import pandas as pd
+    from sklearn import feature_selection
+    from .forest_fit import fit_extra_trees
+    logging.info('Feature selection for %s', names)
+    features = np.array(features) if not isinstance(features, np.ndarray) else features
+    labels = np.array(labels) if not isinstance(labels, np.ndarray) else labels
+    logging.debug('Features: %r and labels: %r', features.shape, labels.shape)
+    forest = fit_extra_trees(ensemble.ExtraTreesClassifier(n_estimators=125, random_state=0), features, labels)
+    if forest is None:
+        forest = ensemble.ExtraTreesClassifier(n_estimators=125, random_state=0).fit(features, labels)
+    f_test, _ = feature_selection.f_regression(features, labels)
+    k_best = feature_selection.SelectKBest(feature_selection.f_classif, k='all')
+    k_best.fit(features, labels)
+    variances = feature_selection.VarianceThreshold().fit(features, labels)
+    imp = collections.OrderedDict([('ExtTree', forest.feature_importances_), ('k-Best', k_best.scores_),
+                                   ('variance', variances.variances_), ('F-test', f_test)])
+    indices = np.argsort(forest.feature_importances_)[::-1]
+    nb_features = features.shape[1]
+    if names is None or len(names) < nb_features:
+        names = [str(i) for i in range(1, nb_features + 1)]
+    names = list(names)[:nb_features]
+    df_scoring = pd.DataFrame({k: [v[i] for i in range(nb_features)] for k, v in imp.items()},
+                              index=pd.Index(names, name='feature'))
+    logging.debug(df_scoring)
+    if os.path.exists(path_out):
+        path_csv = os.path.join(path_out, NAME_CSV_FEATURES_SELECT)
+        logging.debug('export Feature scoting to "%s"', path_csv)
+        df_scoring.to_csv(path_csv)
+    return indices, df_scoring
 
 
 def _fit_pipeline(clf_pipeline, features, labels):

@@ -25,6 +25,7 @@
 // -fmad=false, so nothing is contracted into an FMA: the impurities, proxies, improvements and thresholds are the same bits as the
 // oracle's (oracle/forest.py).  Class counts are integers below 2^26 per tree, so every sum of squared counts is exact in float64.
 #include "common.cuh"
+#include "tree_split.cuh"
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -32,12 +33,7 @@
 
 namespace {
 
-constexpr int FF_KMAX = 64;                  // classes (isb_forest_predict_proba's limit)
-constexpr int FF_DMAX = 2048;                // feature columns
-constexpr long long FF_WMAX = 1ll << 26;     // total count of a tree: squared class counts stay below 2^52
 constexpr int FF_CMAX = (1 << 24) - 1;       // count of one row (24 bits of the sort payload)
-constexpr float FEATURE_THRESHOLD = 1e-7f;   // _partitioner.pxd: a float32 constant, added in float32
-constexpr double FF_EPSILON = 2.220446049250313e-16;  // np.finfo('double').eps of _tree.pyx
 constexpr int TB = 256;
 
 inline int bits_for(unsigned long long v)   // bits to hold 0..v
@@ -227,11 +223,6 @@ __global__ void k_ff_stats(const uint32_t* __restrict__ g_idx, int n_active, con
     atomicAdd(nd_cc + (size_t)node * K + (pay & 0xff), (int)(pay >> 8));
     atomicAdd(nd_rows + node, 1);
     atomicAdd(nd_w + node, (unsigned long long)(pay >> 8));
-}
-
-__device__ __forceinline__ double gini_of(unsigned long long sq, double w)
-{
-    return 1.0 - (double)sq / (w * w);                 // Gini.node_impurity / children_impurity
 }
 
 // impurity, and the leaf tests of the depth-first builder that come before node_split
@@ -469,7 +460,7 @@ __global__ void k_ff_scan(int L0, int nl, int n_seg, int K, FfGroups gr, const i
         if (nxt <= __fadd_rn(prev, FEATURE_THRESHOLD)) continue;       // _partitioner.next_p skips ties
         if (p < msl || rows - p < msl) continue;
         const double dwl = (double)wl, dwr = (double)(wtot - wl);
-        const double proxy = -dwr * gini_of(sqr, dwr) - dwl * gini_of(sql, dwl);
+        const double proxy = gini_proxy(sql, dwl, sqr, dwr);
         if (proxy > best) {
             best = proxy;
             bpos = p;
@@ -511,8 +502,7 @@ __global__ void k_ff_choose(int L0, int nl, const int32_t* __restrict__ lv_ncand
     const int s = s0 + bj;
     const double wn = (double)nd_w[g], wl = s_wl[s], wr = wn - wl;
     const double il = gini_of(s_sql[s], wl), ir = gini_of(s_sqr[s], wr);
-    // Criterion.impurity_improvement
-    const double improvement = (wn / (double)t_w[nd_tree[g]]) * (nd_imp[g] - (wr / wn * ir) - (wl / wn * il));
+    const double improvement = impurity_improvement(wn, (double)t_w[nd_tree[g]], nd_imp[g], wl, il, ir);
     if (improvement + FF_EPSILON < min_impurity_decrease) { nd_split[g] = 0; return; }
     const int n_left = s_pos[s];
     nd_feature[g] = cand[(size_t)i * cand_stride + bj];

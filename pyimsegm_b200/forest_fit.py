@@ -18,6 +18,11 @@ node, except that equal improvements go to the lowest feature index where scikit
 cross-validation), in one device call (``isb_forest_fit_groups``): every tree of every forest is built level by level together, and
 each tree is node for node the tree :func:`fit_tree_model` builds for that estimator alone.  The seeds and bootstrap rows are drawn
 estimator by estimator in list order, so numpy's global RNG is consumed as scikit-learn's sequential fits consume it.
+
+:func:`fit_extra_trees` fits an ``ExtraTreesClassifier`` (``isb_extra_trees_fit``, csrc/extra_trees_fit.cu) with scikit-learn's own
+draws: each tree's splitter state is ``RandomState(tree seed).randint(0, 2^31 - 1)`` as ``Splitter.init`` draws it, and one CTA per
+tree replays the depth-first build and every draw of ``node_split_random``, so the trees are scikit-learn's node for node and
+``feature_importances_`` / ``predict_proba`` are its bits.  :func:`fit_tree_model` and the grouped fits do not take extra trees.
 """
 import collections
 import ctypes as C
@@ -173,13 +178,13 @@ def _within_limits(T, n, D, m):
     return D <= MAX_FEATURES and 2 * E < 2 ** 31 and E * m < 2 ** 31 and E < 2 ** 30
 
 
-def _prepare(estimator, X, y, n_rows=None):
+def _prepare(estimator, X, y, n_rows=None, admit=_supported):
     """the parameters of ``estimator`` resolved against (X, y) and its seeds and bootstrap counts drawn from ``random_state`` as
     scikit-learn draws them, or None -- before any draw -- when the device does not compute the fit.  ``n_rows``: the rows of the
-    device call the forest will be part of (its limits are checked at that size)"""
-    from sklearn.ensemble import RandomForestClassifier
+    device call the forest will be part of (its limits are checked at that size); ``admit``: the estimator's parameters, or None"""
+    from sklearn.ensemble import ExtraTreesClassifier, RandomForestClassifier
     from sklearn.utils import check_random_state
-    p = _supported(estimator)
+    p = admit(estimator)
     if p is None:
         return None
     X = np.asarray(X)
@@ -202,7 +207,7 @@ def _prepare(estimator, X, y, n_rows=None):
     max_features, mss, msl, max_depth = _resolve(p, n, D)
     if not 1 <= max_features <= D:
         return None
-    forest = type(estimator) is RandomForestClassifier
+    forest = type(estimator) in (RandomForestClassifier, ExtraTreesClassifier)
     T = int(p['n_estimators']) if forest else 1
     if n_rows is not None and not _within_limits(T, n_rows, D, max_features):
         return None
@@ -442,3 +447,113 @@ def fit_tree_models(estimators, features, labels, train_rows=None):
         rows = np.arange(batch.n) if rows is None else np.asarray(rows, dtype=np.int64).ravel()
         batch.add(est, X[rows], rows)
     return batch.fit()
+
+
+# ---- extra trees (isb_extra_trees_fit, csrc/extra_trees_fit.cu) ----
+
+#: the share of the free device memory one isb_extra_trees_fit call may take; a larger forest goes in consecutive calls of whole trees
+EXTRA_MEMORY_SHARE = 0.8
+_RAND_R_MAX = 2 ** 31 - 1
+
+
+def _supported_extra(est):
+    """the parameters of an ExtraTreesClassifier that isb_extra_trees_fit computes, or None"""
+    from sklearn.ensemble import ExtraTreesClassifier
+    if type(est) is not ExtraTreesClassifier:
+        return None
+    p = est.get_params(deep=False)
+    if p.get('criterion') != 'gini' or p.get('class_weight') is not None or p.get('max_leaf_nodes') is not None:
+        return None
+    if p.get('ccp_alpha', 0.0) > 0 or p.get('min_weight_fraction_leaf', 0.0) > 0 or p.get('monotonic_cst') is not None:
+        return None
+    if p.get('max_samples') is not None or p.get('oob_score') or p.get('warm_start'):
+        return None
+    return p
+
+
+def _rand_r_states(seeds):
+    """each tree's splitter state: Splitter.init draws ``randint(0, RAND_R_MAX)`` from the tree's RandomState(seed), the first draw
+    from it (DecisionTreeClassifier._fit hands the RandomState to the splitter untouched)"""
+    return np.array([np.random.RandomState(int(s)).randint(0, _RAND_R_MAX) for s in seeds], dtype=np.uint32)
+
+
+def _extra_chunks(T, n, K, ws_per_tree, budget):
+    """consecutive ranges [t0, t1) of the trees, each one isb_extra_trees_fit call within ``budget`` bytes of device memory"""
+    cap = 2 * n - 1
+    per_tree = ws_per_tree + 4 * n + 4 + cap * (4 * 4 + 8 * 3 + 1 + 4 * K)
+    step = max(1, min(T, int(budget // per_tree)))
+    return [(t0, min(T, t0 + step)) for t0 in range(0, T, step)]
+
+
+def _fit_arrays_extra(X, y, K, counts, states, max_features, min_samples_split, min_samples_leaf, max_depth, min_impurity_decrease,
+                      budget=None, small_rows=0):
+    """every extra tree on the device: X [n, D] float32, y [n] class indices, counts [T, n], states [T] u32 -> list of per-tree dicts
+    of preorder node arrays as :func:`_fit_arrays` returns them.  A forest above ``budget`` bytes (default: EXTRA_MEMORY_SHARE of the
+    free device memory) is built in consecutive calls of whole trees"""
+    import torch
+    from .engine import get_engine
+    eng = get_engine()
+    lib, st = eng.lib, _lib.stream_ptr()
+    n, D = X.shape
+    T = len(counts)
+    ws1 = lib.isb_extra_trees_fit_workspace_bytes(n, D, 1, K, max_features)
+    if ws1 == 0:
+        raise NotImplementedError('imsegm_b200: extra trees over %d rows x %d features, %d classes, are above the limits of '
+                                  'isb_extra_trees_fit' % (n, D, K))
+    if budget is None:
+        free, _ = torch.cuda.mem_get_info(eng.device)
+        budget = EXTRA_MEMORY_SHARE * (free + torch.cuda.memory_reserved(eng.device) - torch.cuda.memory_allocated(eng.device))
+    d_x = eng.to_device(np.ascontiguousarray(X, dtype=np.float32), 'et_x')
+    d_y = eng.to_device(np.ascontiguousarray(y, dtype=np.int32), 'et_y')
+    names = ('left', 'right', 'feature', 'threshold', 'impurity', 'n_node_samples', 'weighted_n_node_samples', 'missing_go_to_left',
+             'class_counts')
+    i32, f64, dev = torch.int32, torch.float64, eng.device
+    kinds = {'threshold': f64, 'impurity': f64, 'weighted_n_node_samples': f64, 'missing_go_to_left': torch.uint8}
+    trees = []
+    for t0, t1 in _extra_chunks(T, n, K, ws1, budget):
+        Tc = t1 - t0
+        cnt = np.ascontiguousarray(counts[t0:t1], dtype=np.int32)
+        cap = 2 * int((cnt > 0).sum(axis=1).max()) - 1
+        ws_bytes = lib.isb_extra_trees_fit_workspace_bytes(n, D, Tc, K, max_features)
+        if ws_bytes == 0:
+            raise NotImplementedError('imsegm_b200: %d extra trees over %d rows are above the limits of isb_extra_trees_fit' % (Tc, n))
+        d_c = eng.to_device(cnt, 'et_counts')
+        d_s = eng.to_device(np.ascontiguousarray(states[t0:t1], dtype=np.uint32).view(np.int32), 'et_states')
+        out = {k: torch.empty((Tc, cap, K) if k == 'class_counts' else (Tc, cap), dtype=kinds.get(k, i32), device=dev) for k in names}
+        node_count = torch.empty(Tc, dtype=i32, device=dev)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        _lib.check(lib.isb_extra_trees_fit(_lib.ptr(d_x), n, D, _lib.ptr(d_y), K, _lib.ptr(d_c), Tc, _lib.ptr(d_s), max_features,
+                                           min_samples_split, min_samples_leaf, max_depth, C.c_double(min_impurity_decrease),
+                                           small_rows, cap, *[_lib.ptr(out[k]) for k in names], _lib.ptr(node_count), _lib.ptr(ws),
+                                           C.c_size_t(ws_bytes), st))
+        del ws
+        nodes = eng.to_host(node_count).astype(np.int64)
+        width = int(nodes.max())
+        host = {k: eng.to_host(out[k][:, :width].contiguous()) for k in names}
+        del out
+        for t in range(Tc):
+            nn = int(nodes[t])
+            tree = {k: host[k][t, :nn].copy() for k in names}
+            tree['node_count'] = nn
+            trees.append(tree)
+    return trees
+
+
+def fit_extra_trees(estimator, X, y):
+    """``estimator.fit(X, y)`` on the device for an unfitted ExtraTreesClassifier: returns the estimator, fitted -- the trees are
+    scikit-learn's node for node, so ``feature_importances_`` and ``predict_proba`` are its bits -- or None when one of its parameters is
+    outside what the device computes (criterion other than 'gini', class_weight, max_leaf_nodes, ccp_alpha > 0, min_weight_fraction_leaf
+    > 0, max_samples, oob_score, warm_start, monotonic_cst), when X is not finite as float32, y has several outputs or more than 64
+    classes, or the size is above the kernel's limits.  The seeds, bootstrap rows and splitter states are drawn from ``random_state`` as
+    scikit-learn draws them (``random_state=None`` draws from numpy's global RNG)."""
+    prep = _prepare(estimator, X, y, admit=_supported_extra)
+    if prep is None:
+        return None
+    if prep.T * prep.n >= 2 ** 31:
+        return None
+    try:
+        trees = _fit_arrays_extra(prep.X, prep.y, prep.K, prep.counts, _rand_r_states(prep.seeds), prep.max_features, prep.mss, prep.msl,
+                                  prep.max_depth, prep.mid)
+    except NotImplementedError:
+        return None
+    return _assemble(prep, trees)
