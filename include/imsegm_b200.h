@@ -139,7 +139,8 @@ size_t isb_slic3d_kmeans_workspace_bytes(int D, int H, int W, int n_seeds);
 int isb_slic3d_kmeans(const double* vol_scaled, int D, int H, int W, const double* seeds_zyx, int n_seeds, int step_z, int step_y,
                       int step_x, double step, const double* spacing_host, int max_iter, int32_t* labels, void* ws, size_t ws_bytes,
                       isb_stream_t stream);
-/* _enforce_label_connectivity_cython on a volume (6 neighbours in the order x+1, x-1, y+1, y-1, z+1, z-1) */
+/* _enforce_label_connectivity_cython on a volume (6 neighbours in the order x+1, x-1, y+1, y-1, z+1, z-1).  The workspace
+ * grows with D*H*W only; max_size does not change it. */
 size_t isb_connectivity3d_workspace_bytes(int D, int H, int W, int max_size);
 int isb_enforce_connectivity3d(const int32_t* labels, int D, int H, int W, int min_size, int max_size, int32_t* out,
                                int32_t* n_labels_out, void* ws, size_t ws_bytes, isb_stream_t stream);

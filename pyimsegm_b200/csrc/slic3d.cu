@@ -200,9 +200,10 @@ struct Cc3 {
     int* assigned;  // [V] split replay: voxel already in a piece / BFS replay of small pieces: voxel already queued
     int* adj;       // [V] at the head of a small piece: the piece it merges into (-1: label 0)
     int* newlab;    // [V] at the head of a kept piece: its label
-    int* queue;     // [2 V + max_size]
+    int* queue;     // [V] BFS queues: max_size entries per component >= max_size in the split (#big * max_size <= V), then
+                    //     psize entries per small piece in their replay (sum of psize <= V); the split is done when the replay starts
     int* big;       // [V] roots of the components >= max_size
-    int* counters;  // [0] #big, [1] queue cursor, [2] number of kept pieces
+    int* counters;  // [0] #big, [1] queue cursor of the small-piece replay, [2] number of kept pieces
     int D, H, W;
 };
 
@@ -227,9 +228,9 @@ __global__ void c3_init(Cc3 c)
 {
     const size_t V = (size_t)c.D * c.H * c.W;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < 3) c.counters[i] = 0;         // before the bound check: a volume of one or two voxels still clears all three
     if (i >= V) return;
     c.parent[i] = (int)i; c.size[i] = 0; c.psize[i] = 0; c.assigned[i] = 0; c.adj[i] = -1; c.newlab[i] = -1;
-    if (i < 3) c.counters[i] = 0;
 }
 
 __global__ void c3_union(Cc3 c, const int* __restrict__ seg)
@@ -284,13 +285,13 @@ __global__ void c3_split(Cc3 c, int max_size)
     if (t >= c.counters[0]) return;
     const int root = c.big[t];
     const int V = c.D * c.H * c.W;
+    int* q = c.queue + (size_t)t * max_size;   // the component's own queue, reused by each of its pieces
     int remaining = c.size[root];
     int scan = root;
     while (remaining > 0) {
         while (scan < V && !(c.parent[scan] == root && c.assigned[scan] == 0)) ++scan;
         if (scan >= V) break;
         const int head = scan;
-        int* q = c.queue + atomicAdd(&c.counters[1], max_size);
         c.assigned[head] = 1; c.piece[head] = head; q[0] = head;
         int size = 1, visited = 0;
         while (visited < size && size < max_size) {
@@ -363,14 +364,14 @@ __global__ void c3_write(Cc3 c, int min_size, int* __restrict__ out, int* __rest
     out[i] = h >= 0 ? c.newlab[h] : 0;                         // no earlier neighbour at all: the original's default label 0
 }
 
-static size_t carve_cc3(Cc3& c, void* ws, size_t bytes, int D, int H, int W, int max_size)
+static size_t carve_cc3(Cc3& c, void* ws, size_t bytes, int D, int H, int W)
 {
     WsCarver w(ws, bytes);
     const size_t V = (size_t)D * H * W;
     c.D = D; c.H = H; c.W = W;
     c.parent = w.take<int>(V); c.size = w.take<int>(V); c.piece = w.take<int>(V); c.psize = w.take<int>(V);
     c.assigned = w.take<int>(V); c.adj = w.take<int>(V); c.newlab = w.take<int>(V);
-    c.queue = w.take<int>(3 * V + (size_t)max_size + 64);
+    c.queue = w.take<int>(V);
     c.big = w.take<int>(V);
     c.counters = w.take<int>(4);
     return isb_align(w.off);
@@ -445,7 +446,8 @@ extern "C" int isb_slic3d_kmeans(const double* vol_scaled, int D, int H, int W, 
 extern "C" size_t isb_connectivity3d_workspace_bytes(int D, int H, int W, int max_size)
 {
     Cc3 c;
-    return carve_cc3(c, nullptr, 0, D, H, W, max_size);
+    (void)max_size;                       // the queues fit in V entries whatever max_size is
+    return carve_cc3(c, nullptr, 0, D, H, W);
 }
 
 extern "C" int isb_enforce_connectivity3d(const int32_t* labels, int D, int H, int W, int min_size, int max_size, int32_t* out,
@@ -456,7 +458,7 @@ extern "C" int isb_enforce_connectivity3d(const int32_t* labels, int D, int H, i
     ISB_REQUIRE((size_t)D * H * W < (size_t)INT_MAX / 4, "volume too large");
     if (max_size < 1) max_size = 1;
     Cc3 c;
-    const size_t need = carve_cc3(c, ws, ws_bytes, D, H, W, max_size);
+    const size_t need = carve_cc3(c, ws, ws_bytes, D, H, W);
     ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t V = (size_t)D * H * W;
