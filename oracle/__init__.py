@@ -30,11 +30,19 @@ def build(force=False):
     stale = (not os.path.isfile(so)) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if force or stale:
         subprocess.check_call(['make', '-C', _HERE, 'liboracle.so'], stdout=subprocess.DEVNULL)
-    ref_dir = os.path.join(_HERE, '_ref')
-    has_ref = os.path.isdir(ref_dir) and any(f.startswith('features_cython') for f in os.listdir(ref_dir))
+    has_ref = _ref_module_path(False) is not None and _ref_module_path(True) is not None
     ref_tree = os.environ.get('IMSEGM_REFERENCE')
     if ref_tree and os.path.isdir(ref_tree) and (force or not has_ref):
         subprocess.call(['make', '-C', _HERE, 'ref', 'REF=' + os.path.abspath(ref_tree)], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+
+
+def _ref_module_path(strict):
+    ref_dir = os.path.join(_HERE, '_ref', 'strict') if strict else os.path.join(_HERE, '_ref')
+    if os.path.isdir(ref_dir):
+        for f in sorted(os.listdir(ref_dir)):
+            if f.startswith('features_cython') and f.endswith('.so'):
+                return os.path.join(ref_dir, f)
+    return None
 
 
 def lib():
@@ -53,19 +61,22 @@ def lib():
     return _LIB
 
 
-def ref_features_cython():
-    """the reference's own Cython module compiled unchanged (oracle/_ref), or None when it was not built"""
+_REF_MODULES = {}
+
+
+def ref_features_cython(strict=False):
+    """the reference's own Cython module compiled unchanged, or None when it was not built: with setup.py's flags
+    (-O3 -ffast-math -march=native, oracle/_ref) or, ``strict``, IEEE-strict with the oracle's CFLAGS (oracle/_ref/strict)"""
     import importlib.util
-    ref_dir = os.path.join(_HERE, '_ref')
-    if not os.path.isdir(ref_dir):
-        return None
-    for f in os.listdir(ref_dir):
-        if f.startswith('features_cython') and f.endswith('.so'):
-            spec = importlib.util.spec_from_file_location('features_cython', os.path.join(ref_dir, f))
-            mod = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(mod)
-            return mod
-    return None
+    if strict not in _REF_MODULES:
+        path = _ref_module_path(strict)
+        if path is None:
+            return None
+        spec = importlib.util.spec_from_file_location('features_cython', path)
+        mod = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(mod)
+        _REF_MODULES[strict] = mod
+    return _REF_MODULES[strict]
 
 
 def _p(a, t):
@@ -430,9 +441,10 @@ def label_hist2d(segm_select, struc_elem, nb_labels):
 
 
 def ray_angles(angle_step):
-    """(sin, cos) as float32 exactly like features_cython.pyx:247-268 forms them"""
-    angles = np.arange(0, 360, angle_step, dtype=np.float32)
-    rads = [float(np.float32(np.deg2rad(a))) for a in angles]          # `rad` is a C float in the reference
+    """(sin, cos) as float32 exactly like features_cython.pyx:247-268 forms them: `angle_step` is a C float; each float32
+    angle is boxed to a Python float, so np.deg2rad runs in float64, and the result is stored to the C float `rad`"""
+    angles = np.arange(0, 360, float(np.float32(angle_step)), dtype=np.float32)
+    rads = [float(np.float32(np.deg2rad(float(a)))) for a in angles]
     return (np.array([np.sin(r) for r in rads], dtype=np.float32), np.array([np.cos(r) for r in rads], dtype=np.float32))
 
 
@@ -440,8 +452,10 @@ def ray_features2d(seg_binary, position, angle_step=5., edge=1):
     seg = np.ascontiguousarray(seg_binary, dtype=np.int8)
     s, c = ray_angles(float(angle_step))
     out = np.empty(len(s), dtype=np.float32)
-    lib().oracle_ray_features2d(_p(seg, C.c_int8), seg.shape[0], seg.shape[1], int(position[0]), int(position[1]),
-                                _p(s, C.c_float), _p(c, C.c_float), len(s), int(edge), _p(out, C.c_float))
+    rc = lib().oracle_ray_features2d(_p(seg, C.c_int8), seg.shape[0], seg.shape[1], int(position[0]), int(position[1]),
+                                     _p(s, C.c_float), _p(c, C.c_float), len(s), int(edge), _p(out, C.c_float))
+    if rc != 0:
+        raise IndexError('position %r is out of bounds for a mask of shape %r' % (tuple(position), seg.shape))
     return out
 
 

@@ -92,13 +92,17 @@ int oracle_label_hist2d(const int16_t* segm, const int16_t* selem, int H, int W,
     return 0;
 }
 
-/* features_cython.pyx:239.  seg: H*W int8 (0/1), pos = (row, col), angles[n] in degrees (f32), edge = 1 ('up') or -1 ('down').
- * sin/cos of the angle are supplied by the caller (the reference takes them from numpy in double, then stores to float). */
+/* features_cython.pyx:239.  seg: H*W int8 (0/1), pos = (row, col) in [-H, H) x [-W, W), edge = 1 ('up') or -1 ('down').
+ * sin/cos of the angle are supplied by the caller (the reference takes them from numpy in double, then stores to float).
+ * The reference indexes its memoryview with wraparound, so a negative start reads row H + pr / column W + pc, while the
+ * march itself starts from (pr, pc).  Its round() is Python's builtin on a non-negative value: half to even, i.e. rintf. */
 int oracle_ray_features2d(const int8_t* seg, int H, int W, int pr, int pc, const float* sin_a, const float* cos_a, int n_ang, int edge,
                           float* ray_dist)
 {
+    if (pr < -H || pr >= H || pc < -W || pc >= W) return -1;
+    const int8_t start = seg[(long)(pr < 0 ? pr + H : pr) * W + (pc < 0 ? pc + W : pc)];
     for (int i = 0; i < n_ang; ++i) ray_dist[i] = -1.0f;
-    if (seg[(long)pr * W + pc] && edge == 1) {
+    if (start && edge == 1) {
         for (int i = 0; i < n_ang; ++i) ray_dist[i] = 0.0f;
         return 0;
     }
@@ -108,11 +112,11 @@ int oracle_ray_features2d(const int8_t* seg, int H, int W, int pr, int pc, const
         float g0 = sin_a[i], g1 = cos_a[i];
         float gmax = fmaxf(fabsf(g0), fabsf(g1));
         g0 /= gmax; g1 /= gmax;
-        int8_t last = seg[(long)pr * W + pc];
+        int8_t last = start;
         for (int s = 0; s < diag; ++s) {
             pos0 += g0; pos1 += g1;
-            if (pos0 < 0 || roundf(pos0) >= H || pos1 < 0 || roundf(pos1) >= W) break;
-            int8_t actual = seg[(long)((int)roundf(pos0)) * W + (int)roundf(pos1)];
+            if (pos0 < 0 || rintf(pos0) >= H || pos1 < 0 || rintf(pos1) >= W) break;
+            int8_t actual = seg[(long)((int)rintf(pos0)) * W + (int)rintf(pos1)];
             if ((edge == 1 && actual) || (edge == -1 && last && !actual)) {
                 float dx = pos0 - (float)pr, dy = pos1 - (float)pc;
                 /* the products and the sum are C floats, np.sqrt then works on the Python float (double), the store rounds to f32 */

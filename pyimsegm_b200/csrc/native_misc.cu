@@ -74,7 +74,9 @@ __global__ void k_label_hist(const short* __restrict__ segm, const short* __rest
     if (l >= 0 && l < nb_labels && selem[i] == 1) atomicAdd(&hist[l], 1u);
 }
 
-// one thread per (position, angle)
+// one thread per (position, angle).  Positions lie in [-H, H) x [-W, W) (checked by the caller): like the reference's
+// wraparound memoryview, a negative start reads pixel (H + pr, W + pc) while the march starts from (pr, pc).  The reference
+// rounds the marching position with Python's round(), half to even, which is rintf on these non-negative values.
 __global__ void k_ray_features(const signed char* __restrict__ seg, int H, int W, const int* __restrict__ pos, int n_pos, const float* __restrict__ sin_a,
                                const float* __restrict__ cos_a, int n_ang, int edge, float* __restrict__ out)
 {
@@ -82,7 +84,7 @@ __global__ void k_ray_features(const signed char* __restrict__ seg, int H, int W
     if (t >= n_pos * n_ang) return;
     const int p = t / n_ang, i = t - p * n_ang;
     const int pr = pos[2 * p], pc = pos[2 * p + 1];
-    const signed char start = seg[(size_t)pr * W + pc];
+    const signed char start = seg[(size_t)(pr < 0 ? pr + H : pr) * W + (pc < 0 ? pc + W : pc)];
     if (start && edge == 1) { out[t] = 0.0f; return; } // the position sits inside the border label
     float dist = -1.0f;
     const int diag = (int)sqrt((double)W * W + (double)H * H);
@@ -93,8 +95,8 @@ __global__ void k_ray_features(const signed char* __restrict__ seg, int H, int W
     signed char last = start;
     for (int s = 0; s < diag; ++s) {
         pos0 = __fadd_rn(pos0, g0); pos1 = __fadd_rn(pos1, g1);
-        if (pos0 < 0 || roundf(pos0) >= H || pos1 < 0 || roundf(pos1) >= W) break;
-        const signed char actual = seg[(size_t)((int)roundf(pos0)) * W + (int)roundf(pos1)];
+        if (pos0 < 0 || rintf(pos0) >= H || pos1 < 0 || rintf(pos1) >= W) break;
+        const signed char actual = seg[(size_t)((int)rintf(pos0)) * W + (int)rintf(pos1)];
         if ((edge == 1 && actual) || (edge == -1 && last && !actual)) {
             const float dx = __fsub_rn(pos0, (float)pr), dy = __fsub_rn(pos1, (float)pc);
             dist = (float)sqrt((double)__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)));

@@ -223,15 +223,19 @@ def cython_label_hist_seg2d(segm_select, struc_elem, nb_labels):
 
 
 def ray_angle_tables(angle_step):
-    """(sin, cos) float32 tables of the ray directions exactly as features_cython.pyx:247-268 forms them"""
-    angles = np.arange(0, 360, angle_step, dtype=np.float32)
-    rads = [float(np.float32(np.deg2rad(a))) for a in angles]
+    """(sin, cos) float32 tables of the ray directions exactly as features_cython.pyx:247-268 forms them: the step is a C
+    float, each float32 angle goes to np.deg2rad as a Python float (so the radians are computed in float64) and is stored to
+    a float32 ``rad``, whose sine and cosine are again taken in float64 and stored to float32"""
+    angles = np.arange(0, 360, float(np.float32(angle_step)), dtype=np.float32)
+    rads = [float(np.float32(np.deg2rad(float(a)))) for a in angles]
     return np.array([np.sin(r) for r in rads], dtype=np.float32), np.array([np.cos(r) for r in rads], dtype=np.float32)
 
 
 def cython_ray_features_seg2d(seg_binary, position, angle_step=5., edge='up'):
     """ Ray features: distance from ``position`` to the first boundary along rays every ``angle_step`` degrees
     (reference descriptors.py:1628-1660).  ``position`` may also be an [n, 2] array: all positions run in one launch.
+    As in the reference, a position in ``[-H, H) x [-W, W)`` is accepted and a negative coordinate starts the ray from the
+    wrapped pixel; any other position raises ``IndexError``.
 
     :return ndarray: ray distances, float32 [n_angles] (or [n, n_angles])
     """
@@ -239,7 +243,15 @@ def cython_ray_features_seg2d(seg_binary, position, angle_step=5., edge='up'):
     from . import _lib
     edge_int = {'down': -1, 'up': 1}[edge]
     seg = np.array(seg_binary, dtype=np.int8)
+    if seg.ndim != 2:
+        raise ValueError('the mask of the Ray features has to be 2-D, got shape %r' % (seg.shape, ))
     pos = np.atleast_2d(np.array(position, dtype=np.int32))
+    if pos.ndim != 2 or pos.shape[1] != 2:
+        raise ValueError('positions have to be (row, col) pairs, got shape %r' % (np.shape(position), ))
+    lo, hi = -np.array(seg.shape), np.array(seg.shape)
+    out_of_range = np.any((pos < lo) | (pos >= hi), axis=1)
+    if out_of_range.any():
+        raise IndexError('position %r is out of bounds for a mask of shape %r' % (tuple(pos[np.argmax(out_of_range)]), seg.shape))
     sin_a, cos_a = ray_angle_tables(float(angle_step))
     eng = get_engine()
     d_seg, d_pos = eng.to_device(seg, 'ray_seg'), eng.to_device(pos, 'ray_pos')

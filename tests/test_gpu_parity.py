@@ -321,9 +321,12 @@ def test_config1_reference_cpu_case(oracle):
 def test_remaining_native_functions(oracle):
     """gray 3-D statistics, label histogram and ray features of imsegm/features_cython.pyx (:144-282): doctest goldens of
     imsegm/descriptors.py:470-478, :1479-1485, :1641-1653, the oracle, and the reference module compiled unchanged.
-    Ray distances: 1e-5 relative against the compiled reference (it is built with -ffast-math, its last float ulp is
-    compiler dependent); exact against the oracle and against the integer goldens."""
+    Ray distances: bit-exact against the oracle, against the integer goldens and, where it was built, against the reference
+    module compiled IEEE-strict (oracle/_ref/strict); 1e-5 relative against the stored outputs of the module built with the
+    reference's own -O3 -ffast-math -march=native, whose last float ulp depends on the compiler."""
     from pyimsegm_b200 import descriptors as ds
+    from test_ray_features_host import ref_trace, strict_module
+    strict = strict_module()
     image = np.zeros((2, 3, 8))
     image[0, :, 2:6] = 1
     image[1, :, 3:7] = 3
@@ -357,6 +360,8 @@ def test_remaining_native_functions(oracle):
         got = ds.cython_ray_features_seg2d(noise, pos, 7.5, edge)
         for p, g, ref in zip(pos, got, gold['ray_noise_' + edge]):
             assert np.array_equal(g, oracle.ray_features2d(noise, p, 7.5, e))
+            if strict is not None:
+                assert np.array_equal(g, ref_trace(strict, noise, p, 7.5, e))
             np.testing.assert_allclose(g, ref, rtol=1e-5)
 
 
