@@ -256,6 +256,27 @@ int isb_disc_label_hist(const int32_t* segm, const double* proba, int H, int W, 
                         const int32_t* diameters, int n_diam, const uint8_t* selem, int mh, int mw, int nb_labels, double* hist,
                         double* sizes, isb_stream_t stream);
 
+/* The disc label counts of isb_disc_label_hist for a label map, from run-length rows (center_detection.cu): the map is encoded as
+ * the start column and label of every maximal run of each row (one CTA scan per row, in ws), then one CTA per position counts every
+ * diameter, each disc row dy as the clipped lengths of the runs under [col - w, col + w], w = floor(sqrt(d^2 - dy^2)) in integers.
+ * Same arguments, counts and output layout as isb_disc_label_hist's label-map case (values outside [0, nb_labels) are skipped but
+ * count in the size; the disc is clipped to the image; nb_labels <= 4096).  ws: isb_label_runs_workspace_bytes(H, W), 8 H W bytes
+ * and some -- sized by the image, not by the label count. */
+size_t isb_label_runs_workspace_bytes(int H, int W);
+int isb_ring_label_hist(const int32_t* segm, int H, int W, const int32_t* positions, int n_pos, const int32_t* diameters, int n_diam,
+                        int nb_labels, double* hist, double* sizes, void* ws, size_t ws_bytes, isb_stream_t stream);
+
+/* sklearn.cluster.DBSCAN(eps, min_samples).fit(points).labels_ for n float64 points [n, 2] (Euclidean): neighbours are the points
+ * with dx * dx + dy * dy <= eps * eps (scikit-learn's KD-tree test), the point itself included; core points have at least
+ * min_samples neighbours; clusters are numbered by their smallest core index; a non-core point takes the smallest cluster among its
+ * core neighbours, else -1.  labels out [n] i32; centres (optional) out [n, 2] f64, rows [0, n_clusters) = the mean of each
+ * cluster's points summed in index order (np.mean(points[labels == c], axis=0)); n_clusters: host int.  The call synchronises
+ * the stream.  Non-finite points or eps <= 0 return ISB_ERR_ARG; any finite points and eps are clustered (cells of side about eps,
+ * coarser when the points span more than 2^29 of them).  n may be 0.  ws: isb_dbscan_workspace_bytes(n), about 80 n bytes. */
+size_t isb_dbscan_workspace_bytes(int n);
+int isb_dbscan(const double* points, int n, double eps, int min_samples, int32_t* labels, double* centres, int* n_clusters, void* ws,
+               size_t ws_bytes, isb_stream_t stream);
+
 /* computeRayFeaturesBinary2d (features_cython.pyx:239) for n_pos positions at once: out [n_pos, n_ang] f32, -1 where the ray
  * leaves the image, 0 where the position lies inside the border label (edge 'up').  sin_a / cos_a: the f32 sines and cosines
  * of the ray angles as the reference forms them (np.deg2rad of the f32 angle, stored to float).  edge: 1 'up', -1 'down'. */

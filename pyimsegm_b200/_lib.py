@@ -102,6 +102,10 @@ SIGNATURES = {
     'isb_filter_response_2d': (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp]),
     'isb_gaussian_filter_2d': (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp]),
     'isb_disc_label_hist': (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    'isb_label_runs_workspace_bytes': (_sz, [_i, _i]),
+    'isb_ring_label_hist': (_i, [_vp, _i, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    'isb_dbscan_workspace_bytes': (_sz, [_i]),
+    'isb_dbscan': (_i, [_vp, _i, _d, _i, _vp, _vp, C.POINTER(_i), _vp, _sz, _vp]),
     'isb_region_label_hist': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     'isb_gather': (_i, [_vp, _ll, _vp, _vp, _i, _vp, _vp, _vp]),
     'isb_segment_median_workspace_bytes': (_sz, [_ll, _i]),

@@ -507,10 +507,15 @@ def adjust_bounding_box_crop(image_size, bbox_size, position):
     return tuple(int(v) for v in im_begin), tuple(int(v) for v in im_end), tuple(int(v) for v in bb_begin), tuple(int(v) for v in bb_end)
 
 
+#: discs over a label map are counted from run-length rows (``isb_ring_label_hist``); False sends them through
+#: ``isb_disc_label_hist``'s pixel walk instead, which scripts/bench_center_detection.py times against it
+RUN_LENGTH_DISCS = True
+
+
 def _device_label_hists(segm, positions, nb_labels, diameters=None, struc_elem=None):
     """label histograms under discs (``diameters``) or one explicit structuring element about every position, one launch
-    (``isb_disc_label_hist``).  ``segm`` is [H, W] labels or [H, W, K] per-label maps.
-    Returns (hist [n_pos, n_elems, nb_labels], sizes [n_pos, n_elems])."""
+    (``isb_ring_label_hist`` for discs over a label map, ``isb_disc_label_hist`` otherwise).  ``segm`` is [H, W] labels or
+    [H, W, K] per-label maps.  Returns (hist [n_pos, n_elems, nb_labels], sizes [n_pos, n_elems])."""
     import ctypes as C
     from . import _lib
     segm = np.asarray(segm)
@@ -541,6 +546,12 @@ def _device_label_hists(segm, positions, nb_labels, diameters=None, struc_elem=N
         n_el = len(diam)
     hist = eng.buf('hist_out64', (len(pos), n_el, int(nb_labels)), torch.float64)
     sizes = eng.buf('hist_sizes', (len(pos), n_el), torch.float64)
+    if d_seg is not None and d_diam is not None and RUN_LENGTH_DISCS:
+        ws_bytes = eng.lib.isb_label_runs_workspace_bytes(H, W)
+        ws = eng.buf('hist_runs_ws', (ws_bytes, ), torch.uint8)
+        _lib.check(eng.lib.isb_ring_label_hist(_lib.ptr(d_seg), H, W, _lib.ptr(d_pos), len(pos), _lib.ptr(d_diam), n_el, int(nb_labels),
+                                               _lib.ptr(hist), _lib.ptr(sizes), _lib.ptr(ws), ws_bytes, _lib.stream_ptr()))
+        return eng.to_host(hist).copy(), eng.to_host(sizes).copy()
     _lib.check(eng.lib.isb_disc_label_hist(_lib.ptr(d_seg), _lib.ptr(d_proba), H, W, _lib.ptr(d_pos), len(pos), _lib.ptr(d_diam), n_el,
                                            _lib.ptr(d_sel), mh, mw, int(nb_labels), _lib.ptr(hist), _lib.ptr(sizes), _lib.stream_ptr()))
     return eng.to_host(hist).copy(), eng.to_host(sizes).copy()
