@@ -76,7 +76,9 @@ __host__ __device__ void conic_params(const double v[3], const double P[3][3], d
     const double width = sqrt(2.0 * num / den1);
     const double height = sqrt(2.0 * num / den2);
     double phi = 0.5 * atan((2.0 * b) / (a - c));
-    if (a > c) phi += 0.5 * 3.141592653589793;
+    // a == c puts atan's axis at +-pi/4 on the larger eigenvalue of [[a, b], [b, c]], as a > c does, while width comes from the
+    // smaller one for either sign of the eigenvector: turn it by pi / 2 there too (skimage's a > c leaves theta on the other axis)
+    if (a >= c) phi += 0.5 * 3.141592653589793;
     out[0] = nan_to_num(x0); out[1] = nan_to_num(y0); out[2] = nan_to_num(width); out[3] = nan_to_num(height); out[4] = nan_to_num(phi);
 }
 
@@ -139,6 +141,98 @@ __host__ __device__ bool eigvec3(const double M[3][3], double lam, double v[3])
     return true;
 }
 
+// x <- (M - lam I)^{-1} x by LU with partial pivoting; a pivot smaller than tiny is taken as tiny, since inverse iteration solves
+// with a shift that is an eigenvalue to rounding
+__host__ __device__ void shifted_solve(const double M[3][3], double lam, double tiny, double x[3])
+{
+    double A[3][3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) A[i][j] = M[i][j] - (i == j ? lam : 0.0);
+    for (int k = 0; k < 3; ++k) {
+        int piv = k;
+        for (int i = k + 1; i < 3; ++i)
+            if (fabs(A[i][k]) > fabs(A[piv][k])) piv = i;
+        if (piv != k) {
+            for (int j = 0; j < 3; ++j) { const double t = A[k][j]; A[k][j] = A[piv][j]; A[piv][j] = t; }
+            const double t = x[k]; x[k] = x[piv]; x[piv] = t;
+        }
+        if (fabs(A[k][k]) < tiny) A[k][k] = A[k][k] < 0.0 ? -tiny : tiny;
+        for (int i = k + 1; i < 3; ++i) {
+            const double l = A[i][k] / A[k][k];
+            for (int j = k + 1; j < 3; ++j) A[i][j] = A[i][j] - l * A[k][j];
+            x[i] = x[i] - l * x[k];
+        }
+    }
+    for (int i = 2; i >= 0; --i) {
+        double t = x[i];
+        for (int j = i + 1; j < 3; ++j) t = t - A[i][j] * x[j];
+        x[i] = t / A[i][i];
+    }
+}
+
+// unit eigenvector of M for the eigenvalue nearest lam: three steps of inverse iteration on M itself from the start vector v.  The
+// residual of the result is a rounding of |M|, whatever digits the characteristic polynomial lost on lam (LAPACK's eigenvectors
+// have the same backward error); false when a step does not give a finite nonzero vector
+__host__ __device__ bool inverse_iteration(const double M[3][3], double lam, double tiny, double v[3])
+{
+    for (int it = 0; it < 3; ++it) {
+        double x[3] = {v[0], v[1], v[2]};
+        shifted_solve(M, lam, tiny, x);
+        const double nn = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
+        if (!(nn > 0.0) || !isfinite(nn)) return false;
+        for (int i = 0; i < 3; ++i) v[i] = x[i] / nn;
+    }
+    return true;
+}
+
+// the three eigenvectors of M (unit, one per row of V), from eigenvalues that need only be near: the cubic's root of smallest
+// magnitude, its eigenvector by inverse iteration, then the other two eigenvalues from the 2 x 2 block that remains after a
+// Householder reflection takes that eigenvector to e1; returns how many eigenvectors it found
+__host__ __device__ int eig3_vectors(const double M[3][3], double V[3][3])
+{
+    double nrm = 0.0;
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) nrm += M[i][j] * M[i][j];
+    nrm = sqrt(nrm);
+    if (!(nrm > 0.0) || !isfinite(nrm)) return 0;
+    const double tiny = 2.220446049250313e-16 * nrm;
+    double lam[3];
+    const int nr = eig3_real(M, lam);
+    double l0 = lam[0];
+    for (int k = 1; k < nr; ++k)
+        if (fabs(lam[k]) < fabs(l0)) l0 = lam[k];
+    double v[3] = {1.0, 1.0, 1.0};
+    if (!eigvec3(M, l0, v)) { v[0] = 1.0; v[1] = 1.0; v[2] = 1.0; }
+    if (!inverse_iteration(M, l0, tiny, v)) return 0;
+    // B = H M H with H = I - 2 u u^T / u^T u, H v = -+e1: its lower-right 2 x 2 block holds the other two eigenvalues
+    double u[3] = {v[0] + (v[0] >= 0.0 ? 1.0 : -1.0), v[1], v[2]};
+    const double uu = u[0] * u[0] + u[1] * u[1] + u[2] * u[2];
+    double H[3][3], T[3][3], B[3][3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) H[i][j] = (i == j ? 1.0 : 0.0) - 2.0 * u[i] * u[j] / uu;
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) T[i][j] = M[i][0] * H[0][j] + M[i][1] * H[1][j] + M[i][2] * H[2][j];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) B[i][j] = H[i][0] * T[0][j] + H[i][1] * T[1][j] + H[i][2] * T[2][j];
+    const double p = B[1][1], q = B[1][2], r = B[2][1], s = B[2][2];
+    const double half = 0.5 * (p + s), hd = 0.5 * (p - s);
+    // the pencil of the direct fit has real eigenvalues: a discriminant that rounding pushed below zero is a double root
+    const double sq = sqrt(fmax(hd * hd + q * r, 0.0));
+    const double la = half + (half >= 0.0 ? sq : -sq);
+    const double lb = la != 0.0 ? (p * s - q * r) / la : half - (half >= 0.0 ? sq : -sq);
+    for (int i = 0; i < 3; ++i) V[0][i] = v[i];
+    int n = 1;
+    const double others[2] = {la, lb};
+    for (int k = 0; k < 2; ++k) {
+        double w[3] = {1.0, 1.0, 1.0};
+        if (!eigvec3(M, others[k], w)) { w[0] = 1.0; w[1] = 1.0; w[2] = 1.0; }
+        if (!inverse_iteration(M, others[k], tiny, w)) continue;
+        for (int i = 0; i < 3; ++i) V[n][i] = w[i];
+        ++n;
+    }
+    return n;
+}
+
 // direct (Halir-Flusser) fit from the 21 scatter sums; S1 = D1^T D1, S2 = D1^T D2, S3 = D2^T D2 with D1 = [x^2, xy, y^2], D2 = [x, y, 1]
 __host__ __device__ Fit fit_from_scatter(const double S1[3][3], const double S2[3][3], const double S3[3][3])
 {
@@ -155,11 +249,11 @@ __host__ __device__ Fit fit_from_scatter(const double S1[3][3], const double S2[
     for (int j = 0; j < 3; ++j) { M[0][j] = 0.5 * R[2][j]; M[1][j] = -R[1][j]; M[2][j] = 0.5 * R[0][j]; }
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) P[i][j] = -iS3[i][0] * S2[j][0] + -iS3[i][1] * S2[j][1] + -iS3[i][2] * S2[j][2];
-    double lam[3], v[3], a1[3];
-    const int n = eig3_real(M, lam);
+    double V[3][3], a1[3];
+    const int n = eig3_vectors(M, V);
     int admissible = 0;
     for (int k = 0; k < n; ++k) {
-        if (!eigvec3(M, lam[k], v)) continue;
+        const double* v = V[k];
         if (4.0 * (v[0] * v[2]) - v[1] * v[1] > 0) {
             ++admissible;
             a1[0] = v[0]; a1[1] = v[1]; a1[2] = v[2];
@@ -231,11 +325,24 @@ __global__ void __launch_bounds__(ETHREADS) k_ellipse_trials(
         if (tid < 5) s_p[tid] = params_in[5 * (size_t)t + tid];
         if (tid == 0) s_status = 1;
     } else if (tid < 32) {
-        // 21 scatter sums: lane-strided over the samples in their drawn order, then a fixed butterfly
+        // 21 scatter sums: lane-strided over the samples in their drawn order, then a fixed butterfly.  The samples are taken
+        // about their mean: about the origin the sums of x^4 lose the ellipse's digits to its distance from there (8 000 px out,
+        // numpy's fit of the same samples misses some ellipses), about the mean they keep them
+        double ox = 0.0, oy = 0.0;
+        for (int s = samp_off[t] + tid; s < samp_off[t + 1]; s += 32) {
+            ox += cp[2 * (size_t)samp_idx[s]];
+            oy += cp[2 * (size_t)samp_idx[s] + 1];
+        }
+        for (int o = 16; o > 0; o >>= 1) {
+            ox += __shfl_xor_sync(0xffffffffu, ox, o);
+            oy += __shfl_xor_sync(0xffffffffu, oy, o);
+        }
+        const int n_smp = samp_off[t + 1] - samp_off[t];
+        if (n_smp > 0) { ox = ox / n_smp; oy = oy / n_smp; }
         double acc[21];
         for (int k = 0; k < 21; ++k) acc[k] = 0.0;
         for (int s = samp_off[t] + tid; s < samp_off[t + 1]; s += 32) {
-            const double x = cp[2 * (size_t)samp_idx[s]], y = cp[2 * (size_t)samp_idx[s] + 1];
+            const double x = cp[2 * (size_t)samp_idx[s]] - ox, y = cp[2 * (size_t)samp_idx[s] + 1] - oy;
             const double d1[3] = {x * x, x * y, y * y}, d2[3] = {x, y, 1.0};
             int k = 0;
             for (int i = 0; i < 3; ++i)
@@ -259,6 +366,7 @@ __global__ void __launch_bounds__(ETHREADS) k_ellipse_trials(
             const Fit f = fit_from_scatter(S1, S2, S3);
             s_status = f.status;
             for (int i = 0; i < 5; ++i) s_p[i] = f.p[i];
+            if (f.status == 1) { s_p[0] = f.p[0] + ox; s_p[1] = f.p[1] + oy; }
         }
     }
     __syncthreads();
