@@ -19,13 +19,14 @@ namespace {
 // ------------------------------------------------------------------ adjacency ------------------------------------------------------
 
 struct AdjWs {
-    unsigned long long* table; // [slots] keys (b << 32 | a), empty = ~0
+    unsigned long long* table; // [slots] keys (b << 32 | a), empty = 0 (b > a >= 0, so no key is 0)
+    int* ctr;                  // [4] 0: unique edges, 1: overflow flag
     int* deg;                  // [nb]    number of edges whose larger endpoint is b
     int* off;                  // [nb+1]
     int* fill;                 // [nb]
     int* tmp_a;                // [cap]
-    int* ctr;                  // [4] 0: unique edges, 1: overflow flag
     int slots;
+    size_t zeroed;             // bytes from `table` through `deg`: cleared by one memset before the scan
 };
 
 __device__ __forceinline__ unsigned hash64(unsigned long long k)
@@ -34,18 +35,21 @@ __device__ __forceinline__ unsigned hash64(unsigned long long k)
     return (unsigned)k;
 }
 
-__device__ void edge_insert(const AdjWs& w, int l0, int l1)
+__device__ __forceinline__ unsigned long long edge_key(int l0, int l1)
 {
-    int a = min(l0, l1), b = max(l0, l1);
-    unsigned long long key = ((unsigned long long)(unsigned)b << 32) | (unsigned)a;
+    return ((unsigned long long)(unsigned)max(l0, l1) << 32) | (unsigned)min(l0, l1);
+}
+
+__device__ void table_insert(const AdjWs& w, unsigned long long key)
+{
     unsigned mask = (unsigned)w.slots - 1u;
     unsigned h = hash64(key) & mask;
     for (int probe = 0; probe < w.slots; ++probe) {
         unsigned long long cur = w.table[h];
         if (cur == key) return;
-        if (cur == ~0ull) {
-            unsigned long long old = atomicCAS(&w.table[h], ~0ull, key);
-            if (old == ~0ull) { atomicAdd(&w.deg[b], 1); atomicAdd(&w.ctr[0], 1); return; }
+        if (cur == 0) {
+            unsigned long long old = atomicCAS(&w.table[h], 0ull, key);
+            if (old == 0) { atomicAdd(&w.deg[key >> 32], 1); atomicAdd(&w.ctr[0], 1); return; }
             if (old == key) return;
         }
         h = (h + 1) & mask;
@@ -53,33 +57,79 @@ __device__ void edge_insert(const AdjWs& w, int l0, int l1)
     atomicExch(&w.ctr[1], 1); // table full
 }
 
+// A CTA's pixels meet a few dozen label pairs, each many times: the CTA collects its pairs in a shared-memory set and inserts each
+// into the global table once.  A pair that finds no free slot within CTA_PROBES goes to the global table directly.
+constexpr int CTA_SLOTS = 512, CTA_PROBES = 32;
+
+__device__ void cta_set_clear(unsigned long long* s)
+{
+    for (int i = threadIdx.x; i < CTA_SLOTS; i += blockDim.x) s[i] = 0;
+    __syncthreads();
+}
+
+__device__ void cta_set_insert(unsigned long long* s, const AdjWs& w, unsigned long long key)
+{
+    unsigned h = hash64(key) & (CTA_SLOTS - 1);
+    for (int probe = 0; probe < CTA_PROBES; ++probe) {
+        unsigned long long cur = s[h];
+        if (cur == key) return;
+        if (cur == 0) {
+            cur = atomicCAS(&s[h], 0ull, key);
+            if (cur == 0 || cur == key) return;
+        }
+        h = (h + 1) & (CTA_SLOTS - 1);
+    }
+    table_insert(w, key);
+}
+
+__device__ void cta_set_flush(const unsigned long long* s, const AdjWs& w)
+{
+    __syncthreads();
+    for (int i = threadIdx.x; i < CTA_SLOTS; i += blockDim.x)
+        if (s[i]) table_insert(w, s[i]);
+}
+
+// a CTA takes a tile of ETW columns x ETH rows, a thread one column of ETR rows: the thread skips a pair it has just inserted (a
+// boundary across its rows gives the same horizontal pair row after row), the set the rest
+constexpr int ETW = 64, ETR = 4, ETH = ETR * (256 / ETW);
+
 __global__ void __launch_bounds__(256) k_edge_scan(const int* __restrict__ seg, int H, int W, AdjWs w)
 {
-    size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= (size_t)H * W) return;
-    int y = (int)(p / W), x = (int)(p % W);
-    int l = seg[p];
-    if (x + 1 < W) {
-        int r = seg[p + 1];
-        // skip when the pixel above saw the same pair
-        if (r != l && !(y > 0 && seg[p - W] == l && seg[p - W + 1] == r)) edge_insert(w, l, r);
+    __shared__ unsigned long long s_set[CTA_SLOTS];
+    cta_set_clear(s_set);
+    const int x = blockIdx.x * ETW + (int)(threadIdx.x % ETW);
+    const int y0 = blockIdx.y * ETH + (int)(threadIdx.x / ETW) * ETR, y1 = min(y0 + ETR, H);
+    if (x < W && y0 < H) {
+        unsigned long long last = 0;
+        int l = seg[(size_t)y0 * W + x];
+        for (int y = y0; y < y1; ++y) {
+            const size_t p = (size_t)y * W + x;
+            const int d = y + 1 < H ? seg[p + W] : l;
+            if (x + 1 < W) {
+                const int r = seg[p + 1];
+                if (r != l && edge_key(l, r) != last) { last = edge_key(l, r); cta_set_insert(s_set, w, last); }
+            }
+            if (d != l && edge_key(l, d) != last) { last = edge_key(l, d); cta_set_insert(s_set, w, last); }
+            l = d;
+        }
     }
-    if (y + 1 < H) {
-        int d = seg[p + W];
-        if (d != l && !(x > 0 && seg[p - 1] == l && seg[p + W - 1] == d)) edge_insert(w, l, d);
-    }
+    cta_set_flush(s_set, w);
 }
 
 // the same for a volume: 6-connectivity = the pairs with the x+1, y+1 and z+1 neighbour (reference superpixels.py:145-154)
 __global__ void __launch_bounds__(256) k_edge_scan3d(const int* __restrict__ seg, int D, int H, int W, AdjWs w)
 {
-    size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= (size_t)D * H * W) return;
-    const int x = (int)(p % W), y = (int)((p / W) % H), z = (int)(p / ((size_t)H * W));
-    const int l = seg[p];
-    if (x + 1 < W) { const int r = seg[p + 1]; if (r != l) edge_insert(w, l, r); }
-    if (y + 1 < H) { const int d = seg[p + W]; if (d != l) edge_insert(w, l, d); }
-    if (z + 1 < D) { const int b = seg[p + (size_t)H * W]; if (b != l) edge_insert(w, l, b); }
+    __shared__ unsigned long long s_set[CTA_SLOTS];
+    cta_set_clear(s_set);
+    const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < (size_t)D * H * W) {
+        const int x = (int)(p % W), y = (int)((p / W) % H), z = (int)(p / ((size_t)H * W));
+        const int l = seg[p];
+        if (x + 1 < W) { const int r = seg[p + 1]; if (r != l) cta_set_insert(s_set, w, edge_key(l, r)); }
+        if (y + 1 < H) { const int d = seg[p + W]; if (d != l) cta_set_insert(s_set, w, edge_key(l, d)); }
+        if (z + 1 < D) { const int b = seg[p + (size_t)H * W]; if (b != l) cta_set_insert(s_set, w, edge_key(l, b)); }
+    }
+    cta_set_flush(s_set, w);
 }
 
 // centroids (z, y, x) of the labels of a volume, (-1, -1, -1) for absent labels (superpixels.py:205-242 for 3-D input)
@@ -116,7 +166,7 @@ __global__ void k_edge_fill(AdjWs w, int cap)
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= w.slots) return;
     unsigned long long key = w.table[i];
-    if (key == ~0ull) return;
+    if (key == 0) return;
     int b = (int)(key >> 32), a = (int)(key & 0xffffffffu);
     int pos = w.off[b] + atomicAdd(&w.fill[b], 1);
     if (pos < cap) w.tmp_a[pos] = a;
@@ -144,11 +194,12 @@ static size_t carve_adj(AdjWs& w, void* ws, size_t bytes, int nb, int cap)
     WsCarver c(ws, bytes);
     w.slots = pow2_at_least(2LL * cap);
     w.table = c.take<unsigned long long>((size_t)w.slots);
+    w.ctr = c.take<int>(4);
     w.deg = c.take<int>(nb);
+    w.zeroed = c.off;
     w.off = c.take<int>((size_t)nb + 1);
     w.fill = c.take<int>(nb);
     w.tmp_a = c.take<int>(cap);
-    w.ctr = c.take<int>(4);
     return isb_align(c.off);
 }
 
@@ -276,17 +327,50 @@ __global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024) k_gc_energie
 
 // ------------------------------------------------------------------ gathers --------------------------------------------------------
 
-__global__ void __launch_bounds__(256) k_gather(const int* __restrict__ seg, long long n, const int* __restrict__ lut_i,
+constexpr int GV = 4, GW = 32 * GV; // pixels per thread and per warp of k_gather
+
+// n_vec: the pixels covered by whole warps of GW when every pointer is 16-byte aligned (0 otherwise); the rest goes pixel by pixel.
+// A warp's GW pixels are read and written as 16-byte pieces by consecutive lanes, so every store instruction covers 512 contiguous
+// bytes: a lane loads four labels and stores four classes; segm_soft's GW * K values are stored in order as pairs, each lane
+// looking up the labels of its pair in shared memory.
+__global__ void __launch_bounds__(256) k_gather(const int* __restrict__ seg, long long n, long long n_vec, const int* __restrict__ lut_i,
                                                 const double* __restrict__ lut_p, int K, int* __restrict__ out_i, double* __restrict__ out_p)
 {
-    long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    int l = seg[p];
-    if (out_i) out_i[p] = lut_i[l];
-    if (out_p) {
-        const double* src = lut_p + (size_t)l * K;
-        double* dst = out_p + (size_t)p * K;
-        for (int k = 0; k < K; ++k) dst[k] = src[k];
+    __shared__ int s_lab[256 * GV];
+    const long long p0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * GV;
+    if (p0 >= n) return;
+    if (p0 < n_vec) {
+        const int4 l = *reinterpret_cast<const int4*>(seg + p0);
+        if (out_i) *reinterpret_cast<int4*>(out_i + p0) = make_int4(__ldg(lut_i + l.x), __ldg(lut_i + l.y), __ldg(lut_i + l.z), __ldg(lut_i + l.w));
+        if (out_p) {
+            const int lane = threadIdx.x & 31;
+            *reinterpret_cast<int4*>(s_lab + threadIdx.x * GV) = l;
+            __syncwarp();
+            const int* lab = s_lab + (threadIdx.x - lane) * GV;
+            double2* dst = reinterpret_cast<double2*>(out_p + (p0 - lane * GV) * K);
+            // pair i holds values 2i and 2i + 1 of the warp; value e is channel e % K of pixel e / K.  i steps by 32, e by 64.
+            int q = 2 * lane / K, k = 2 * lane % K;
+            const int dq = 64 / K, dk = 64 % K;
+#pragma unroll 2
+            for (int i = lane; i < GW * K / 2; i += 32) {
+                const double v0 = __ldg(lut_p + (size_t)lab[q] * K + k);
+                const int q1 = k + 1 == K ? q + 1 : q, k1 = k + 1 == K ? 0 : k + 1;
+                const double v1 = __ldg(lut_p + (size_t)lab[q1] * K + k1);
+                dst[i] = make_double2(v0, v1);
+                q += dq; k += dk;
+                if (k >= K) { k -= K; ++q; }
+            }
+        }
+        return;
+    }
+    for (long long p = p0; p < min(p0 + GV, n); ++p) {
+        const int l = seg[p];
+        if (out_i) out_i[p] = lut_i[l];
+        if (out_p) {
+            const double* src = lut_p + (size_t)l * K;
+            double* dst = out_p + (size_t)p * K;
+            for (int k = 0; k < K; ++k) dst[k] = src[k];
+        }
     }
 }
 
@@ -303,16 +387,14 @@ extern "C" int isb_adjacency_edges(const int32_t* seg, int H, int W, int nb, int
 {
     ISB_REQUIRE(seg && edges && n_edges_out && ws, "null pointer");
     ISB_REQUIRE(H > 0 && W > 0 && nb > 0 && cap > 0, "bad sizes");
+    ISB_REQUIRE((H + ETH - 1) / ETH <= 65535, "label map taller than the scan grid (1 048 560 rows)");
     AdjWs w;
     size_t need = carve_adj(w, ws, ws_bytes, nb, cap);
     ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope prof(ISB_PROF_ADJ, st);
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.table, 0xFF, sizeof(unsigned long long) * (size_t)w.slots, st));
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.deg, 0, sizeof(int) * (size_t)nb, st));
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.ctr, 0, sizeof(int) * 4, st));
-    size_t n = (size_t)H * W;
-    k_edge_scan<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg, H, W, w);
+    ISB_CUDA_CHECK(cudaMemsetAsync(w.table, 0, w.zeroed, st));
+    k_edge_scan<<<dim3((W + ETW - 1) / ETW, (H + ETH - 1) / ETH), 256, 0, st>>>(seg, H, W, w);
     ISB_LAUNCH_CHECK();
     k_edge_offsets<<<1, 1024, 0, st>>>(nb, w, cap, n_edges_out);
     ISB_LAUNCH_CHECK();
@@ -333,9 +415,7 @@ extern "C" int isb_adjacency_edges_3d(const int32_t* seg, int D, int H, int W, i
     ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope prof(ISB_PROF_ADJ, st);
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.table, 0xFF, sizeof(unsigned long long) * (size_t)w.slots, st));
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.deg, 0, sizeof(int) * (size_t)nb, st));
-    ISB_CUDA_CHECK(cudaMemsetAsync(w.ctr, 0, sizeof(int) * 4, st));
+    ISB_CUDA_CHECK(cudaMemsetAsync(w.table, 0, w.zeroed, st));
     size_t n = (size_t)D * H * W;
     k_edge_scan3d<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seg, D, H, W, w);
     ISB_LAUNCH_CHECK();
@@ -422,7 +502,10 @@ extern "C" int isb_gather(const int32_t* seg, long long npx, const int32_t* lut_
     ISB_REQUIRE(seg && npx > 0, "bad arguments");
     ISB_REQUIRE((!out_i || lut_i) && (!out_p || (lut_p && K > 0)), "LUT missing for a requested output");
     ProfScope prof(ISB_PROF_GATHER, (cudaStream_t)stream);
-    k_gather<<<(unsigned)((npx + 255) / 256), 256, 0, (cudaStream_t)stream>>>(seg, npx, lut_i, lut_p, K, out_i, out_p);
+    const bool aligned = (((uintptr_t)seg | (uintptr_t)out_i | (uintptr_t)out_p) & 15) == 0;
+    const long long groups = (npx + GV - 1) / GV;
+    k_gather<<<(unsigned)((groups + 255) / 256), 256, 0, (cudaStream_t)stream>>>(seg, npx, aligned ? npx / GW * GW : 0, lut_i, lut_p, K,
+                                                                                out_i, out_p);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }

@@ -9,7 +9,8 @@
 // products are formed in f32 exactly as the Cython code does (float val; val * val), accumulation is f64.
 //
 // Mapping: a thread owns one image column inside a strip of SROWS rows, so warp loads are coalesced along x and
-// label runs along y (~ one superpixel height) are accumulated in registers; one flush of atomics per run.
+// label runs along y (~ one superpixel height) are accumulated in registers; the runs that end in the same row on neighbouring
+// lanes with the same label are summed across the warp, and one lane flushes them with one set of atomics.
 // Algorithmic HBM bytes: pass 1 = image bytes + 4 B/px labels, pass 2 the same.
 #include "common.cuh"
 
@@ -26,42 +27,83 @@ struct StatWs {
 
 __device__ __forceinline__ float clean(float v) { return isnan(v) ? 0.0f : v; } // np.nan_to_num (descriptors.py:824)
 
+// Runs that end in the same row on neighbouring lanes of a warp with the same label (a boundary across the columns, or the end of the
+// strip) are summed across those lanes before one lane flushes them.  A segment is a maximal group of consecutive flushing lanes with
+// one key; every lane of the warp calls this.  Returns the lane one past the segment that starts at or spans this lane (use it with
+// seg_sum); *head tells whether this lane is the segment's first, the one that holds its sum.
+__device__ __forceinline__ int run_segment_end(bool flush, int key, bool* head)
+{
+    const int lane = threadIdx.x & 31;
+    const unsigned fl = __ballot_sync(0xffffffffu, flush);
+    const int prev = __shfl_up_sync(0xffffffffu, key, 1);
+    *head = flush && !(lane > 0 && ((fl >> (lane - 1)) & 1) && prev == key);
+    const unsigned starts = __ballot_sync(0xffffffffu, !flush || *head) & ~((2u << lane) - 1u); // segment starts above this lane
+    return starts ? __ffs(starts) - 1 : 32;
+}
+
+// after log2(32) steps lane i holds the sum of lanes [i, end): each step adds the partial of lane i + o when that lane is in the segment
+template <typename T> __device__ __forceinline__ T seg_sum(T v, int end)
+{
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const T u = __shfl_down_sync(0xffffffffu, v, o);
+        if (lane + o < end) v += u;
+    }
+    return v;
+}
+
+// Every lane of a warp walks the y loop to its end (the shuffles of the flush need all 32), lanes beyond W with no label.  The next
+// row's label and pixel are loaded before the current row's flush, so two rows of loads are in flight per thread.
 __global__ void __launch_bounds__(256) k_stats_pass1(const void* __restrict__ img, int dtype, const int* __restrict__ seg, int H, int W,
                                                      int y_off, StatWs ws)
 {
     const int x = blockIdx.x * 256 + threadIdx.x;
-    if (x >= W) return;
+    const bool live = x < W;
     const int y0 = blockIdx.y * SROWS, y1 = min(y0 + SROWS, H);
     int cur = -1;
     double s0 = 0, s1 = 0, s2 = 0, e0 = 0, e1 = 0, e2 = 0;
-    long long cnt = 0, sy = 0;
+    int cnt = 0;
+    long long sy = 0;
+    int nl = -1;
+    float n0 = 0, n1 = 0, n2 = 0;
+    auto load = [&](int y) {
+        nl = -1;
+        if (live && y < y1) {
+            const size_t p = (size_t)y * W + x;
+            nl = seg[p];
+            if (img) { n0 = clean(load_as_f32(img, dtype, 3 * p)); n1 = clean(load_as_f32(img, dtype, 3 * p + 1)); n2 = clean(load_as_f32(img, dtype, 3 * p + 2)); }
+        }
+    };
+    load(y0);
     for (int y = y0; y <= y1; ++y) {
-        int l = -1;
-        float v0 = 0, v1 = 0, v2 = 0;
-        if (y < y1) {
-            size_t p = (size_t)y * W + x;
-            l = seg[p];
-            if (img) {
-                v0 = clean(load_as_f32(img, dtype, 3 * p));
-                v1 = clean(load_as_f32(img, dtype, 3 * p + 1));
-                v2 = clean(load_as_f32(img, dtype, 3 * p + 2));
+        const int l = nl;
+        const float v0 = n0, v1 = n1, v2 = n2;
+        load(y + 1);
+        const bool flush = cur >= 0 && l != cur;
+        if (__any_sync(0xffffffffu, flush)) {
+            bool head;
+            const int end = run_segment_end(flush, cur, &head);
+            const double t0 = seg_sum(s0, end), t1 = seg_sum(s1, end), t2 = seg_sum(s2, end);
+            const double u0 = seg_sum(e0, end), u1 = seg_sum(e1, end), u2 = seg_sum(e2, end);
+            const int tc = seg_sum(cnt, end);
+            const long long ty = seg_sum(sy, end), tx = seg_sum((long long)cnt * x, end);
+            if (head) {
+                double* a = ws.acc + 6 * (size_t)cur;
+                atomicAdd(a, t0); atomicAdd(a + 1, t1); atomicAdd(a + 2, t2);
+                atomicAdd(a + 3, u0); atomicAdd(a + 4, u1); atomicAdd(a + 5, u2);
+                unsigned long long* ia = (unsigned long long*)(ws.iacc + 3 * (size_t)cur);
+                atomicAdd(ia, (unsigned long long)tc);
+                atomicAdd(ia + 1, (unsigned long long)ty);
+                atomicAdd(ia + 2, (unsigned long long)tx);
             }
         }
         if (l != cur) {
-            if (cur >= 0) {
-                double* a = ws.acc + 6 * (size_t)cur;
-                atomicAdd(a, s0); atomicAdd(a + 1, s1); atomicAdd(a + 2, s2);
-                atomicAdd(a + 3, e0); atomicAdd(a + 4, e1); atomicAdd(a + 5, e2);
-                unsigned long long* ia = (unsigned long long*)(ws.iacc + 3 * (size_t)cur);
-                atomicAdd(ia, (unsigned long long)cnt);
-                atomicAdd(ia + 1, (unsigned long long)sy);
-                atomicAdd(ia + 2, (unsigned long long)(cnt * x));
-            }
             cur = l;
             s0 = s1 = s2 = e0 = e1 = e2 = 0;
             cnt = 0; sy = 0;
         }
-        if (y < y1) {
+        if (l >= 0) {
             s0 += (double)v0; s1 += (double)v1; s2 += (double)v2;
             e0 += (double)__fmul_rn(v0, v0); e1 += (double)__fmul_rn(v1, v1); e2 += (double)__fmul_rn(v2, v2);
             cnt += 1; sy += y + y_off;
@@ -81,32 +123,48 @@ __global__ void k_stats_means(int nb, StatWs ws)
     }
 }
 
+// the same walk as pass 1 over the squared deviations from the f32 mean
 __global__ void __launch_bounds__(256) k_stats_pass2(const void* __restrict__ img, int dtype, const int* __restrict__ seg, int H, int W,
                                                      StatWs ws)
 {
     const int x = blockIdx.x * 256 + threadIdx.x;
-    if (x >= W) return;
+    const bool live = x < W;
     const int y0 = blockIdx.y * SROWS, y1 = min(y0 + SROWS, H);
     int cur = -1;
     double a0 = 0, a1 = 0, a2 = 0;
     float m0 = 0, m1 = 0, m2 = 0;
+    int nl = -1;
+    float n0 = 0, n1 = 0, n2 = 0;
+    auto load = [&](int y) {
+        nl = -1;
+        if (live && y < y1) {
+            const size_t p = (size_t)y * W + x;
+            nl = seg[p];
+            n0 = clean(load_as_f32(img, dtype, 3 * p)); n1 = clean(load_as_f32(img, dtype, 3 * p + 1)); n2 = clean(load_as_f32(img, dtype, 3 * p + 2));
+        }
+    };
+    load(y0);
     for (int y = y0; y <= y1; ++y) {
-        int l = -1;
-        size_t p = (size_t)y * W + x;
-        if (y < y1) l = seg[p];
-        if (l != cur) {
-            if (cur >= 0) {
+        const int l = nl;
+        const float v0 = n0, v1 = n1, v2 = n2;
+        load(y + 1);
+        const bool flush = cur >= 0 && l != cur;
+        if (__any_sync(0xffffffffu, flush)) {
+            bool head;
+            const int end = run_segment_end(flush, cur, &head);
+            const double t0 = seg_sum(a0, end), t1 = seg_sum(a1, end), t2 = seg_sum(a2, end);
+            if (head) {
                 double* a = ws.var + 3 * (size_t)cur;
-                atomicAdd(a, a0); atomicAdd(a + 1, a1); atomicAdd(a + 2, a2);
+                atomicAdd(a, t0); atomicAdd(a + 1, t1); atomicAdd(a + 2, t2);
             }
+        }
+        if (l != cur) {
             cur = l;
             a0 = a1 = a2 = 0;
             if (l >= 0) { m0 = ws.meanf[3 * (size_t)l]; m1 = ws.meanf[3 * (size_t)l + 1]; m2 = ws.meanf[3 * (size_t)l + 2]; }
         }
-        if (y < y1) {
-            float d0 = __fsub_rn(clean(load_as_f32(img, dtype, 3 * p)), m0);
-            float d1 = __fsub_rn(clean(load_as_f32(img, dtype, 3 * p + 1)), m1);
-            float d2 = __fsub_rn(clean(load_as_f32(img, dtype, 3 * p + 2)), m2);
+        if (l >= 0) {
+            const float d0 = __fsub_rn(v0, m0), d1 = __fsub_rn(v1, m1), d2 = __fsub_rn(v2, m2);
             a0 += (double)__fmul_rn(d0, d0); a1 += (double)__fmul_rn(d1, d1); a2 += (double)__fmul_rn(d2, d2);
         }
     }
