@@ -304,10 +304,11 @@ int isb_centroids_3d(const int32_t* seg, int D, int H, int W, int nb, double* ce
 
 /* compute_unary_cost (imsegm/graph_cuts.py:523-540), compute_edge_weights / compute_edge_model / compute_spatial_dist
  * (:574-657, :383-439, :303-336), create_pairwise_matrix_uniform (:442-456), and pyGCO's float->int conversion.
- *   proba [N,K] f64, edges [E,2] i32 (n_edges read from device n_edges_dev when non-null, else E), centres [N,2] f64
+ *   proba [N,K] f64, edges [E,2] i32 (n_edges read from device n_edges_dev when non-null, else E), centres [N,2] or [N,3] f64
  *   metric : 0 = constant 1, 1 = lT (max_k dp^2), 2 = l1, 3 = l2   -> w = exp(-d / (2 std(d)^2))
- *   spatial: 1 = divide by the relative centroid distance (the reference does so for edge_type 'model' and
- *            'spatial' exactly, not for 'model_l1' / 'model_l2', graph_cuts.py:646)
+ *   spatial: 0 = off; 1 (or 2) = divide by the relative centroid distance over centres (y, x) [N,2] of a label map, 3 = the same
+ *            over centres (z, y, x) [N,3] of a label volume (isb_centroids_3d).  The reference does so for edge_type 'model' and
+ *            'spatial' exactly, not for 'model_l1' / 'model_l2' (graph_cuts.py:646)
  *   out: unary [N,K] f64, edge_w [E] f64, and the integerised (unary_i [N,K], edge_wi [E], smooth_i [K,K]) i32 */
 int isb_gc_energies(const double* proba, int N, const int32_t* n_nodes_dev /* optional device N */, int K, const int32_t* edges, int E,
                     const int32_t* n_edges_dev,
@@ -353,6 +354,11 @@ int isb_mixture_fit_predict(int kind, const double* feat, int N, int D, int ld, 
  *   descending, sign-flipped) | explained_variance_[D] | explained_variance_ratio_[D] | singular_values_[D] | mean_ components_^T [D] |
  *   n_components | noise_variance | n_samples | ok;  n_components_out: optional device int32.  The transform is isb_class_transform
  *   with these tables.  D <= 232 (else ISB_ERR_UNSUPPORTED), N >= 2. */
+/* sklearn StandardScaler().fit_transform of feat [N, ld] f64 (first D columns; the real row count from the optional device n_dev), bit
+ * for bit: the mean and the corrected two-pass variance in numpy's summation order (row after row for D > 1, pairwise for D == 1),
+ * _is_constant_feature's scale 1.  The mixture fit's scaler kernel in its exact mode.  params_out [2 D]: mean_ | scale_;
+ * out [N, D] = (x - mean_) / scale_ (rows past the real count untouched). */
+int isb_standard_scaler(const double* feat, int N, int D, int ld, const int32_t* n_dev, double* params_out, double* out, isb_stream_t stream);
 size_t isb_pca_workspace_bytes(int N, int D);
 int isb_pca_params_len(int D);
 int isb_pca_fit(const double* feat, int N, int D, int ld, const int32_t* n_dev, int use_scaler, double coef, int n_components,

@@ -669,8 +669,66 @@ __global__ void __launch_bounds__(256, 2) k_dgemm_batched(const double* __restri
     }
 }
 
+// one column of StandardScaler's sums in numpy's order: what = 0 sums x, 1 sums x - T, 2 sums (x - T)^2, each term rounded on its own.
+// np.sum(X, axis=0) adds the rows one after the other when X has several columns; a single column is a contiguous reduction, which
+// numpy sums pairwise (blocks of at most 128 in eight interleaved partials, split in halves rounded down to a multiple of 8 above).
+__device__ __forceinline__ double np_term(const double* col, int ld, long long i, double T, int what)
+{
+    const double x = col[(size_t)i * ld];
+    if (what == 0) return x;
+    const double t = __dsub_rn(x, T);
+    return what == 1 ? t : __dmul_rn(t, t);
+}
+
+__device__ double np_block_sum(const double* col, int ld, long long lo, long long n, double T, int what)
+{
+    if (n < 8) {
+        double r = -0.0;
+        for (long long i = 0; i < n; ++i) r = __dadd_rn(r, np_term(col, ld, lo + i, T, what));
+        return r;
+    }
+    double r[8];
+    for (int j = 0; j < 8; ++j) r[j] = np_term(col, ld, lo + j, T, what);
+    long long i = 8;
+    for (; i < n - (n % 8); i += 8)
+        for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], np_term(col, ld, lo + i + j, T, what));
+    double res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])), __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
+    for (; i < n; ++i) res = __dadd_rn(res, np_term(col, ld, lo + i, T, what));
+    return res;
+}
+
+__device__ double np_column_sum(const double* col, int ld, long long N, bool pairwise, double T, int what)
+{
+    if (!pairwise) {
+        double s = np_term(col, ld, 0, T, what);
+        for (long long i = 1; i < N; ++i) s = __dadd_rn(s, np_term(col, ld, i, T, what));
+        return s;
+    }
+    // the recursion of numpy's pairwise_sum, walked with an explicit stack: stage 0 = descend left, 1 = descend right, 2 = add
+    constexpr int DEPTH = 32;     // > log2(2^31 / 128) + 1 levels
+    long long s_lo[DEPTH], s_n[DEPTH];
+    double s_left[DEPTH];
+    int s_stage[DEPTH];
+    int top = 0;
+    s_lo[0] = 0; s_n[0] = N; s_stage[0] = 0;
+    double ret = 0.0;
+    while (top >= 0) {
+        const long long lo = s_lo[top], n = s_n[top];
+        if (n <= 128) { ret = np_block_sum(col, ld, lo, n, T, what); --top; continue; }
+        long long n2 = n / 2;
+        n2 -= n2 % 8;
+        if (s_stage[top] == 0) { s_stage[top] = 1; ++top; s_lo[top] = lo; s_n[top] = n2; s_stage[top] = 0; }
+        else if (s_stage[top] == 1) { s_left[top] = ret; s_stage[top] = 2; ++top; s_lo[top] = lo + n2; s_n[top] = n - n2; s_stage[top] = 0; }
+        else { ret = __dadd_rn(s_left[top], ret); --top; }
+    }
+    return ret;
+}
+
 // StandardScaler for many features: one CTA per 32 features, warps over the samples, lanes over the features; per-warp partials
-// are added in warp order (k_gmm_scale walks the features one by one -- fine for D <= 16, 2.4 ms at D = 189)
+// are added in warp order (k_gmm_scale walks the features one by one -- fine for D <= 16, 2.4 ms at D = 189).
+// EXACT: the statistics of scikit-learn's StandardScaler.fit bit for bit (_incremental_mean_and_var's corrected two-pass variance
+// with numpy's summation order, _is_constant_feature), one lane per feature; the transform below is then StandardScaler.transform.
+template <bool EXACT>
 __global__ void __launch_bounds__(1024) k_big_scale(const double* __restrict__ feat, int N_in, const int* n_dev, int D, int ld, int use_scaler,
                                                    GmmWs w)
 {
@@ -679,6 +737,33 @@ __global__ void __launch_bounds__(1024) k_big_scale(const double* __restrict__ f
     const int N = n_dev ? min(*n_dev, N_in) : N_in;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int d = blockIdx.x * 32 + lane;
+    if (EXACT) {
+        if (wid == 0) {
+            double mu = 0.0, sc = 1.0;
+            if (d < D && N > 0) {
+                const double* col = feat + d;
+                const double n = (double)N;
+                const double s = np_column_sum(col, ld, N, D == 1, 0.0, 0);
+                mu = __ddiv_rn(__dadd_rn(0.0, s), n);
+                const double T = __ddiv_rn(s, n);
+                const double corr = np_column_sum(col, ld, N, D == 1, T, 1);
+                const double sq = np_column_sum(col, ld, N, D == 1, T, 2);
+                const double var = __ddiv_rn(__dsub_rn(sq, __ddiv_rn(__dmul_rn(corr, corr), n)), n);
+                const double ne = __dmul_rn(n, DBL_EPSILON), nme = __dmul_rn(__dmul_rn(n, mu), DBL_EPSILON);
+                const double ub = __dadd_rn(__dmul_rn(ne, var), __dmul_rn(nme, nme));
+                sc = var <= ub ? 1.0 : sqrt(var);
+                if (!use_scaler) { mu = 0.0; sc = 1.0; }
+                w.scale[d] = mu; w.scale[D + d] = sc;
+            }
+            s_mean[lane] = mu; s_scale[lane] = sc;
+        }
+        __syncthreads();
+        if (d < D) {
+            const double mu = s_mean[lane], sc = s_scale[lane];
+            for (int n = wid; n < N; n += 32) w.xs[(size_t)n * D + d] = __ddiv_rn(__dsub_rn(feat[(size_t)n * ld + d], mu), sc);
+        }
+        return;
+    }
     double a = 0;
     if (d < D) for (int n = wid; n < N; n += 32) a += feat[(size_t)n * ld + d];
     s_acc[wid][lane] = a;
@@ -1411,7 +1496,7 @@ static int mixture_fit_predict(const double* feat, int N, int D, int ld, const i
     ProfScope prof(ISB_PROF_GMM, st);
     if (D > DMAX) {
         int best = -1;
-        k_big_scale<<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
+        k_big_scale<false><<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
         ISB_LAUNCH_CHECK();
         if (KIND == MIX_BGM) {
             k_bgm_prior<<<D * (D + 1) / 2, GT, 0, st>>>(N, n_dev, D, w);
@@ -1791,13 +1876,27 @@ extern "C" int isb_pca_fit(const double* feat, int N, int D, int ld, const int32
     ProfScope prof(ISB_PROF_GMM, st);
     GmmWs w = {};
     w.xs = p.xs; w.scale = p.scale;
-    k_big_scale<<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
+    k_big_scale<false><<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, use_scaler, w);
     ISB_LAUNCH_CHECK();
     const BatchStride bs = { 0, 0, 0, 0, 0, 0, (size_t)D * D };
     k_dgemm_batched<true, false><<<dim3((D + TN - 1) / TN, (D + TM - 1) / TM, KS), 256, 0, st>>>(
         p.xs, D, p.xs, D, p.gram, D, bs, D, D, N, n_dev, 0, nullptr, 1, 1, KS, 0, FuseW());
     ISB_LAUNCH_CHECK();
     k_pca_eig<<<1, PT, 0, st>>>(N, n_dev, D, coef, n_components, p, params_out, n_components_out);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_standard_scaler(const double* feat, int N, int D, int ld, const int32_t* n_dev, double* params_out, double* out,
+                                   isb_stream_t stream)
+{
+    ISB_REQUIRE(feat && params_out && out, "null pointer");
+    ISB_REQUIRE(N > 0 && D > 0 && ld >= D, "bad sizes");
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfScope prof(ISB_PROF_GMM, st);
+    GmmWs w = {};
+    w.xs = out; w.scale = params_out;
+    k_big_scale<true><<<(D + 31) / 32, 1024, 0, st>>>(feat, N, n_dev, D, ld, 1, w);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }

@@ -3,7 +3,7 @@
 // Replaces (reference Python, no native code):
 //   imsegm/superpixels.py:115-177  make_graph_segm_connect_grid2d_conn4 / get_segment_diffs_2d_conn4 /
 //                                  make_graph_segment_connect_edges   (per-pixel dict loop + np.unique)
-//   imsegm/graph_cuts.py:303-336   compute_spatial_dist
+//   imsegm/graph_cuts.py:303-336   compute_spatial_dist (centres (y, x) of a label map, (z, y, x) of a label volume)
 //   imsegm/graph_cuts.py:383-439   compute_edge_model
 //   imsegm/graph_cuts.py:523-540   compute_unary_cost
 //   imsegm/graph_cuts.py:574-657   compute_edge_weights (clamp to [1e-3, 1e3])
@@ -287,7 +287,13 @@ __global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024) k_gc_energie
         }
         edge_w[e] = dist;
         dsum += dist;
-        if (spatial) {
+        if (spatial == 3) {   // np.einsum('ij,ij->i', diff, diff) over (z, y, x), left to right
+            const double cz = centres[3 * a] - centres[3 * b], cy = centres[3 * a + 1] - centres[3 * b + 1];
+            const double cx = centres[3 * a + 2] - centres[3 * b + 2];
+            const double s = sqrt(cz * cz + cy * cy + cx * cx);
+            sp[e] = s;
+            ssum += s;
+        } else if (spatial) {
             double cy = centres[2 * a] - centres[2 * b], cx = centres[2 * a + 1] - centres[2 * b + 1];
             double s = sqrt(cy * cy + cx * cx);
             sp[e] = s;
@@ -453,6 +459,7 @@ extern "C" int isb_gc_energies(const double* proba, int N, const int32_t* n_node
     ISB_REQUIRE(proba && edges && pairwise && unary && edge_w && unary_i && edge_wi && smooth_i && ws, "null pointer");
     ISB_REQUIRE(N > 0 && K > 0 && E >= 0, "bad sizes");
     ISB_REQUIRE(metric >= 0 && metric <= 3, "metric must be 0..3");
+    ISB_REQUIRE(spatial >= 0 && spatial <= 3, "spatial must be 0 (off), 1 or 2 (centres [N, 2]) or 3 (centres [N, 3])");
     ISB_REQUIRE(!spatial || centres, "centres are required for spatially normalised edge weights");
     ISB_REQUIRE(ws_bytes >= isb_gc_energies_workspace_bytes(N, K, E), "workspace too small");
     ProfScope prof(ISB_PROF_ENERGY, (cudaStream_t)stream);

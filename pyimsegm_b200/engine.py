@@ -349,6 +349,39 @@ class Engine(object):
                                       _lib.stream_ptr()))
         return edges, n_edges, cap, centres
 
+    def gray_table(self, d_vol, d_seg, nb, flags):
+        """the statistics ``flags`` (in :data:`~.descriptors.NAMES_FEATURE_FLAGS` order, any of mean / std / energy / median) of a
+        gray volume [D,H,W] over its label volume, one column each, as compute_image3d_gray_statistic lays them out: feat [nb, len(flags)]
+        f64 (cached buffer; NaN voxels count as 0, NaN and -0 results are written as +0)"""
+        torch, lib = self.torch, self.lib
+        D, H, W = (int(v) for v in d_vol.shape)
+        code = _lib.dtype_code(d_vol.dtype)
+        st = _lib.stream_ptr()
+        feat = self.buf('feat3d', (nb, len(flags)), torch.float64)
+        native = [f for f in flags if f in FLAG_BITS]
+        if native:
+            wsb = lib.isb_gray_stats_workspace_bytes(int(nb))
+            ws = self.buf('ws_gray', (wsb,), torch.uint8)
+            self._ck(lib.isb_gray_stats(_lib.ptr(d_vol), code, _lib.ptr(d_seg), C.c_longlong(D * H * W), int(nb), flag_bits(native)[0],
+                                        _lib.ptr(feat), len(flags), 0, _lib.ptr(ws), C.c_size_t(wsb), st))
+        if 'median' in flags:
+            wsb = lib.isb_segment_median_workspace_bytes(C.c_longlong(D * H * W), int(nb))
+            ws = self.buf('ws_median', (wsb,), torch.uint8)
+            self._ck(lib.isb_segment_median_2d(_lib.ptr(d_vol), code, _lib.ptr(d_seg), D * H, W, 1, int(nb), _lib.ptr(feat), len(flags),
+                                               list(flags).index('median'), _lib.ptr(ws), C.c_size_t(wsb), st))
+        return feat
+
+    def standard_scaler(self, d_feat, d_n=None):
+        """sklearn StandardScaler().fit_transform of device features [N, D] bit for bit (isb_standard_scaler; the real row count
+        from the device ``d_n``): returns (scaled [N, D], mean_ | scale_ [2 D]) device tensors"""
+        torch = self.torch
+        N, D = int(d_feat.shape[0]), int(d_feat.shape[1])
+        out = self.buf('feat_scaled', (N, D), torch.float64)
+        params = self.buf('scaler_params', (2 * D, ), torch.float64)
+        self._ck(self.lib.isb_standard_scaler(_lib.ptr(d_feat), N, D, int(d_feat.stride(0)), _lib.ptr(d_n), _lib.ptr(params), _lib.ptr(out),
+                                              _lib.stream_ptr()))
+        return out, params
+
     def slic_label_bound(self, H, W, n_segments, min_size_factor=0.5):
         """upper bound on the number of labels after connectivity enforcement (each kept label has >= min_size px)"""
         min_size = max(1, int(min_size_factor * (H * W / n_segments)))
@@ -438,7 +471,11 @@ class Engine(object):
         return edges, n_edges, cap
 
     def gc_energies(self, d_proba, d_edges, E, d_n_edges, d_centres, edge_mode, edge_cost, pairwise, d_n_nodes=None):
+        """isb_gc_energies; centres [N, 3] (z, y, x) of a label volume take its 3-D spatial mode, centres [N, 2] the 2-D one"""
         torch, lib = self.torch, self.lib
+        spatial = int(edge_mode[1])
+        if spatial and d_centres is not None and d_centres.dim() == 2 and int(d_centres.shape[1]) == 3:
+            spatial = 3
         N, K = int(d_proba.shape[0]), int(d_proba.shape[1])
         d_pw = self.const_device(np.ascontiguousarray(pairwise, dtype=np.float64), 'pairwise')
         unary = self.buf('unary', (N, K), torch.float64)
@@ -449,7 +486,7 @@ class Engine(object):
         wsb = lib.isb_gc_energies_workspace_bytes(N, K, int(E))
         ws = self.buf('ws_energy', (wsb,), torch.uint8)
         self._ck(lib.isb_gc_energies(_lib.ptr(d_proba), N, _lib.ptr(d_n_nodes), K, _lib.ptr(d_edges), int(E), _lib.ptr(d_n_edges), _lib.ptr(d_centres),
-                                     int(edge_mode[0]), int(edge_mode[1]), C.c_double(edge_cost), _lib.ptr(d_pw), _lib.ptr(unary), _lib.ptr(edge_w),
+                                     int(edge_mode[0]), spatial, C.c_double(edge_cost), _lib.ptr(d_pw), _lib.ptr(unary), _lib.ptr(edge_w),
                                      _lib.ptr(unary_i), _lib.ptr(edge_wi), _lib.ptr(smooth_i), _lib.ptr(ws), C.c_size_t(wsb),
                                      _lib.stream_ptr()))
         return unary, edge_w, unary_i, edge_wi, smooth_i
@@ -564,15 +601,15 @@ class Engine(object):
         return proba
 
     def gather(self, d_seg, lut_i=None, lut_p=None, out_i=None):
-        """``lut_i[d_seg]`` (into ``out_i`` when given, a contiguous [H,W] int32 tensor) and ``lut_p[d_seg]`` of a contiguous label map
-        [H,W] (device, one launch): returns (segm or None, segm_soft or None)"""
+        """``lut_i[d_seg]`` (into ``out_i`` when given, a contiguous int32 tensor of the label map's shape) and ``lut_p[d_seg]`` of a
+        contiguous label map [H,W] or label volume [D,H,W] (device, one launch): returns (segm or None, segm_soft [..., K] or None)"""
         torch, lib = self.torch, self.lib
-        H, W = int(d_seg.shape[0]), int(d_seg.shape[1])
+        shape = tuple(int(v) for v in d_seg.shape)
         if lut_i is not None and out_i is None:
-            out_i = self.buf('segm', (H, W), torch.int32)
+            out_i = self.buf('segm', shape, torch.int32)
         K = int(lut_p.shape[1]) if lut_p is not None else 0
-        out_p = self.buf('segm_soft', (H, W, K), torch.float64) if lut_p is not None else None
-        self._ck(lib.isb_gather(_lib.ptr(d_seg), C.c_longlong(H * W), _lib.ptr(lut_i), _lib.ptr(lut_p), K, _lib.ptr(out_i),
+        out_p = self.buf('segm_soft', shape + (K, ), torch.float64) if lut_p is not None else None
+        self._ck(lib.isb_gather(_lib.ptr(d_seg), C.c_longlong(int(np.prod(shape))), _lib.ptr(lut_i), _lib.ptr(lut_p), K, _lib.ptr(out_i),
                                 _lib.ptr(out_p), _lib.stream_ptr()))
         return out_i, out_p
 

@@ -13,6 +13,9 @@ The image goes to the device once; label map, features, class model, graph, ener
 host synchronises ONCE, when the results are downloaded.  A caller-fitted mixture or tree model is compiled to device tables
 (:mod:`.class_models`) and evaluated there too; any other model, or a self-fitted one the device GMM does not cover, costs one
 round trip: features [N, D] down, probabilities [N, K] up.
+
+Gray volumes have the same resident form: :func:`segment_resident_volume` (a device volume in, device results out) and
+:func:`segment_volumes_batch` (host volumes over CUDA streams) run ``pipe_gray3d_slic_features_model_graphcut``'s stages on the device.
 """
 import logging
 
@@ -437,6 +440,170 @@ def pipe_gray3d_slic_features_model_graphcut(image, nb_classes, dict_features, s
     proba = model.predict_proba(features)
     graph_labels = segment_graph_cut_general(slic, proba, image, features, gc_regul)
     return graph_labels[slic]
+
+
+#: statistics of a gray volume that the resident volume path computes on the device (compute_image3d_gray_statistic's columns)
+RESIDENT_VOLUME_FLAGS = ('mean', 'std', 'energy', 'median')
+
+
+def _volume_flags(dict_features):
+    """the statistic columns of the resident volume feature table, in compute_selected_features_gray3d's order (the union of the
+    ``color*`` groups' flags), or None when the dictionary needs the stage path (``tLM*`` groups, ``meanGrad``)"""
+    from .descriptors import NAMES_FEATURE_FLAGS
+    if not dict_features or not all(k.startswith('color') for k in dict_features):
+        return None
+    flags = set(f for v in dict_features.values() for f in v)
+    if not flags or not flags <= set(RESIDENT_VOLUME_FLAGS):
+        return None
+    return [f for f in NAMES_FEATURE_FLAGS if f in flags]
+
+
+def _compiled_volume_model(model, n_features):
+    """the device form of a caller-fitted model for a volume feature table of ``n_features`` columns, or None (host predict_proba)"""
+    from . import graph_cuts
+    if not graph_cuts.USE_DEVICE_PREDICT:
+        return None
+    cm = compile_model(model)
+    return cm if cm is not None and cm.n_features_in == n_features else None
+
+
+def _volume_model(model, n_features):
+    """``model`` as _run_resident_volume takes it: a resident fit tuple and a CompiledModel stay as they are, a fitted model (or its
+    bound ``predict_proba``) is compiled when class_models supports it, anything else is called as proba_fn(features)"""
+    if isinstance(model, (tuple, CompiledModel)):
+        return model
+    fitted = model.__self__ if getattr(model, '__name__', None) == 'predict_proba' and hasattr(model, '__self__') else model
+    return _compiled_volume_model(fitted, n_features) or (model if callable(model) else model.predict_proba)
+
+
+def _run_resident_volume(eng, d_vol, model, dict_features, spacing, sp_size, sp_regul, gc_regul, gc_edge_type='model'):
+    """pipe_gray3d_slic_features_model_graphcut's hot path on the device: 3-D SLIC, the gray statistics into a device table,
+    norm_features (StandardScaler, bit for bit), the class model, the 6-connected supervoxel graph, its energies with the (z, y, x)
+    centroids, alpha-expansion and the two gathers.  ``model``: ('fit', nb_classes, use_scaler, max_iter[, kind, n_init, pca_coef])
+    (:func:`_fit_model`) or a :class:`~.class_models.CompiledModel` -> nothing syncs with the host; a callable proba_fn(features) ->
+    one round trip (the standardised features down, the probabilities up).  ``d_vol``: a gray volume [D, H, W] on the device or on
+    the host (uploaded).  Returns (d_segm int32 [D, H, W], d_soft f64 [D, H, W, K], check): ``check`` is None or (d_n_edges, edge_cap)
+    still to be verified by the caller (:func:`~.engine.edges_fit`)."""
+    from . import graph_cuts
+    from .superpixels import slic3d_params
+    flags = _volume_flags(dict_features)
+    if flags is None:
+        raise ValueError('the resident volume path computes the statistics %r of "color" groups, got %r'
+                         % (RESIDENT_VOLUME_FLAGS, dict_features))
+    if sp_regul <= 0.:
+        raise ValueError('slic. regularisation must be positive')
+    if not hasattr(d_vol, 'is_cuda'):
+        d_vol = eng.to_device(_supported_dtype(np.asarray(d_vol)), 'volume')
+    if d_vol.dim() != 3:
+        raise ValueError('expected a gray volume [D, H, W], got shape %r' % (tuple(d_vol.shape), ))
+    shape = tuple(int(v) for v in d_vol.shape)
+    n_seg, compact = slic3d_params(shape, sp_size, sp_regul, spacing)
+    if n_seg < 1 or compact < 1:
+        raise ValueError('superpixel size %r / compactness do not fit the volume %r' % (sp_size, shape))
+    d_seg, d_n = eng.slic3d(d_vol, n_seg, compact, spacing, sigma=1.0)
+    nb = eng.slic_label_bound(int(np.prod(shape)), 1, n_seg)
+    d_feat = eng.gray_table(d_vol, d_seg, nb, flags)
+    d_x, _ = eng.standard_scaler(d_feat, d_n)
+    if isinstance(model, CompiledModel):
+        d_proba = eng.class_model_predict(d_x, model, d_n=d_n)
+    elif isinstance(model, tuple):
+        nb_classes, use_scaler, max_iter, kind, n_init, pca_coef = _fit_spec(model)
+        d_proba = graph_cuts.device_fit_predict(eng, d_x, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef, d_n=d_n)[0]
+    else:
+        n = int(eng.to_host(d_n)[0])
+        proba = np.ascontiguousarray(model(eng.to_host(d_x[:n]).copy()), dtype=np.float64)
+        d_proba = eng.to_device(np.concatenate([proba, np.zeros((nb - n, proba.shape[1]))]), 'proba')
+    if (not isinstance(gc_regul, (list, np.ndarray))) and gc_regul <= 0:
+        proba = eng.to_host(d_proba[:int(eng.to_host(d_n)[0])])
+        return eng.gather(d_seg, _argmin_labels_device(eng, proba), d_proba) + (None, )
+    K = int(d_proba.shape[1])
+    cap = edge_capacity(nb, ndim=3)
+    d_edges, d_n_edges, _, d_centres = eng.graph3d(d_seg, nb, cap)
+    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, cap, d_n_edges, d_centres, graph_cuts._edge_mode(gc_edge_type), 1.0,
+                                                       graph_cuts.compute_pairwise_cost(gc_regul, (nb, K)), d_n_nodes=d_n)
+    d_labels, _, _ = eng.alpha_expansion(nb, K, cap, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, -1, d_n_nodes=d_n)
+    d_segm, d_soft = eng.gather(d_seg, d_labels, d_proba)
+    return d_segm, d_soft, (d_n_edges, cap)
+
+
+def segment_resident_volume(d_vol, model, dict_features, spacing=(12, 1, 1), sp_size=15, sp_regul=0.2, gc_regul=0.1):
+    """ pipe_gray3d_slic_features_model_graphcut with the gray volume ALREADY on the device (a cuda tensor [D, H, W]) and the
+    results left there: returns (segm int32 [D, H, W], segm_soft float64 [D, H, W, K]) device tensors.  ``model`` is a fitted model
+    (or its bound ``predict_proba``) -- evaluated on the device when :func:`~.class_models.compile_model` supports it --, a callable
+    proba_fn(features), or ('fit', nb_classes, use_scaler, max_iter) (:func:`_fit_model`) for the class model fitted on the GPU.  The
+    model sees the standardised features, as in the reference.  ``dict_features``: ``color`` groups of mean / std / energy / median.
+    The indices in ``segm`` are not mapped through the model's ``classes_``.
+    A volume's supervoxel graph has no planar bound on its edges, so the call reads the edge count back (4 bytes) once the cut is
+    enqueued and redoes the volume with a larger table when it overflowed; nothing else synchronises with the host. """
+    eng = get_engine()
+    flags = _volume_flags(dict_features)
+    model = _volume_model(model, len(flags) if flags else 0)
+    while True:
+        d_segm, d_soft, check = _run_resident_volume(eng, d_vol, model, dict_features, spacing, sp_size, sp_regul, gc_regul)
+        if check is None or edges_fit(eng.to_host(check[0])[0], check[1]):
+            return d_segm, d_soft
+
+
+def _segment_volume_stages(volume, proba_fn, dict_features, spacing, sp_size, sp_regul, gc_regul):
+    """the volume pipeline through the numpy-facing stage functions (any feature dictionary): (segm [D, H, W], segm_soft [D, H, W, K])"""
+    from .descriptors import compute_selected_features_gray3d, norm_features
+    from .superpixels import segment_slic_img3d_gray
+    volume = np.asarray(volume)
+    slic = segment_slic_img3d_gray(volume, sp_size=sp_size, relative_compact=sp_regul, space=spacing)
+    features, _ = compute_selected_features_gray3d(volume, slic, dict_features)
+    features[np.isnan(features)] = 0
+    features, _ = norm_features(features)
+    proba = proba_fn(features)
+    graph_labels = segment_graph_cut_general(slic, proba, volume, features, gc_regul)
+    return graph_labels[slic].astype(np.int32), proba[slic]
+
+
+def segment_volumes_batch(list_volumes, nb_classes=None, model_pipeline=None, dict_features=FTS_SET_SIMPLE, spacing=(12, 1, 1),
+                          sp_size=15, sp_regul=0.2, gc_regul=0.1, use_scaler=True, nb_streams=3, max_in_flight=6):
+    """ pipe_gray3d_slic_features_model_graphcut over a LIST of gray volumes: consecutive volumes alternate over ``nb_streams`` CUDA
+    streams with their own buffers, so the upload of volume i+1 and the download of volume i-1 overlap the kernels of volume i (as
+    :func:`segment_images_batch` does for colour images).  Dictionaries with ``tLM*`` groups or ``meanGrad`` go through the stage
+    functions, one volume after the other.
+
+    :param int nb_classes: fit the class model per volume on the GPU (the reference's ``estim_class_model(features, nb_classes)``), or
+    :param model_pipeline: a fitted model used for every volume; its ``classes_`` relabel the result
+    :return list(tuple(ndarray,ndarray)): (segm int32 [D, H, W], segm_soft [D, H, W, K]) per volume, in input order
+    """
+    if (nb_classes is None) == (model_pipeline is None):
+        raise ValueError('give either nb_classes (per-volume GMM) or model_pipeline')
+    flags = _volume_flags(dict_features)
+    if model_pipeline is None:
+        if flags is None or not device_gmm_applicable(len(flags), nb_classes):
+            def proba_fn(features):
+                return estim_class_model(features, nb_classes, use_scaler=use_scaler).predict_proba(features)
+            return [_segment_volume_stages(v, proba_fn, dict_features, spacing, sp_size, sp_regul, gc_regul) for v in list_volumes]
+        model = _fit_model(nb_classes, use_scaler)
+    else:
+        model = _volume_model(model_pipeline, len(flags)) if flags is not None else model_pipeline.predict_proba
+    classes = getattr(model_pipeline, 'classes_', None)
+
+    def relabel(segm):
+        return segm if classes is None else np.asarray(classes)[segm]
+
+    if flags is None:
+        return [(relabel(segm), soft) for segm, soft in
+                (_segment_volume_stages(v, model, dict_features, spacing, sp_size, sp_regul, gc_regul) for v in list_volumes)]
+
+    def launch(eng, volume):
+        d_segm, d_soft, check = _run_resident_volume(eng, volume, model, dict_features, spacing, sp_size, sp_regul, gc_regul)
+        return eng.download((d_segm, d_soft) + ((check[0], ) if check is not None else ())) + (check, )
+
+    def finish(idx, hosts, check):
+        if check is not None and not edges_fit(hosts[2][0], check[1]):
+            # the edge table overflowed: redo this volume on the caller's stream with the grown table
+            d_segm, d_soft = segment_resident_volume(get_engine().to_device(_supported_dtype(np.asarray(list_volumes[idx])), 'volume'),
+                                                     model, dict_features, spacing, sp_size, sp_regul, gc_regul)
+            (segm, soft), done = get_engine().download((d_segm, d_soft))
+            done.synchronize()
+            return relabel(segm.numpy()), soft.numpy()
+        return relabel(hosts[0].numpy()), hosts[1].numpy()
+
+    return _over_streams(list_volumes, nb_streams, max_in_flight, launch, finish)
 
 
 def segment_resident(d_image, model, dict_features, sp_size=30, sp_regul=0.2, gc_regul=1., gc_edge_type='model'):

@@ -43,6 +43,14 @@ def slic_params(shape_hw, sp_size, relative_compact):
     return int(nb_pixels / (sp_size ** 2)), (sp_size * relative_compact) ** 1.5
 
 
+def slic3d_params(shape, sp_size, relative_compact, space):
+    """native 3-D SLIC parameters (n_segments, compactness) of a volume from the reference's (size, regularisation, spacing)
+    (superpixels.py:97-101)"""
+    nb_pixels = np.prod(shape)
+    size = np.prod(sp_size / np.asarray(space, dtype=np.float32) * min(space))
+    return int(nb_pixels / size), int((size * relative_compact) ** 1.5)
+
+
 def segment_slic_img2d(img, sp_size=50, relative_compact=0.1, slico=False):
     """ SLIC superpixels of a 2-D colour (or gray) image, computed on the GPU
 
@@ -79,10 +87,7 @@ def segment_slic_img3d_gray(im, sp_size=50, relative_compact=0.1, space=IMAGE_SP
     im = np.asarray(im)
     if im.ndim != 3:
         raise ValueError('expected a gray volume [D, H, W], got shape %r' % (im.shape, ))
-    nb_pixels = np.prod(im.shape)
-    size = np.prod(sp_size / np.asarray(space, dtype=np.float32) * min(space))
-    n_seg = int(nb_pixels / size)
-    compact = int((size * relative_compact) ** 1.5)
+    n_seg, compact = slic3d_params(im.shape, sp_size, relative_compact, space)
     logging.debug('SLIC 3d gray: NB=%i compact=%f spacing=%r volume %r', n_seg, compact, space, im.shape)
     if n_seg < 1 or compact < 1:
         raise ValueError('superpixel size %r / compactness do not fit the volume %r' % (sp_size, im.shape))
