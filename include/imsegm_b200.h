@@ -52,20 +52,21 @@ int isb_profile_collect(double* ms_out /* host */, long long* count_out /* host 
  *     slic(img f64[H,W,3] in [0,1], n_segments, compactness, sigma=1, enforce_connectivity=True, slic_zero)
  * ------------------------------------------------------------------------------------------------------------------ */
 
-/* min-max rescale to [0,1] (imsegm/superpixels.py:53-54), gaussian pre-blur (scipy.ndimage semantics: symmetric
+/* min-max rescale to [0,1] (imsegm/superpixels.py:53-54; in float32 for an ISB_F32 image, as numpy computes it, in f64
+ * otherwise), gaussian pre-blur (scipy.ndimage semantics: symmetric
  * 1-D correlate, mode reflect, depth(len 1) -> rows -> cols), rgb2lab, multiply by ratio = 1/compactness.
  *   img        : [H,W,C] interleaved, C in {1,3} (gray is replicated, superpixels.py:50-51), dtype = isb_dtype
  *   w_half     : HOST pointer, radius+1 doubles, w_half[0] = centre tap (radius <= 8; radius 0 = no blur)
  *   lab_planar : out, [3,H,W] f64
- *   minmax_out : out, 4 doubles (device) -- [0] min and [1] max of the raw image ([2..3] scratch); max == min makes
- *                the result NaN
+ *   minmax_out : out, 4 doubles (device) -- [0] min and [1] max of the raw image ([2..3] scratch); max == min, or a NaN
+ *                sample (both extrema are then NaN), makes the result NaN
  *   rescale    : 1 = apply the reference wrapper's min-max rescale when (min != 0 or max != 1); 0 = never;
  *                2 = as 1 with the extrema the caller left in minmax_out[0..1] (row-band mode: the extrema of the whole
  *                image, merged by a collective from isb_image_minmax of every band) */
 int isb_slic_prepare(const void* img, int dtype, int H, int W, int C, const double* w_half, int radius, double ratio,
                      int rescale, double* lab_planar, double* minmax_out /* room for 4 doubles */, isb_stream_t stream);
 
-/* minimum and maximum of n samples (NaN ignored) -> minmax_out[0..1]; [2..3] scratch */
+/* minimum and maximum of n samples -> minmax_out[0..1]; [2..3] scratch.  numpy's rule: when any sample is NaN, both are NaN */
 int isb_image_minmax(const void* img, int dtype, long long n, double* minmax_out /* room for 4 doubles */, isb_stream_t stream);
 
 size_t isb_slic_kmeans_workspace_bytes(int H, int W, int n_seeds, int step_y, int step_x);
@@ -678,7 +679,8 @@ int isb_extra_trees_fit(const float* x, int n, int D, const int32_t* y, int K, c
 /* dst[0..n) = value (initial labeling of isb_alpha_expansion and similar small fills) */
 int isb_fill_i32(int32_t* dst, long long n, int32_t value, isb_stream_t stream);
 
-/* dst[i] = dst[i] (op) src[i] over n 8-byte words; op 0 int64 sum, 1 int64 max, 2 f64 min, 3 f64 max, 4 f64 sum.  What a
+/* dst[i] = dst[i] (op) src[i] over n 8-byte words; op 0 int64 sum, 1 int64 max, 2 f64 min, 3 f64 max (both NaN when either
+ * side is NaN), 4 f64 sum.  What a
  * collective does between GPUs in row-band mode, for several bands held by one GPU. */
 int isb_combine(void* dst, const void* src, long long n, int op, isb_stream_t stream);
 

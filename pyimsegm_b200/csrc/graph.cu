@@ -490,8 +490,11 @@ __global__ void k_combine(void* dst, const void* src, long long n, int op)
     if (i >= n) return;
     if (op == 0) ((long long*)dst)[i] += ((const long long*)src)[i];
     else if (op == 1) { long long a = ((long long*)dst)[i], b = ((const long long*)src)[i]; ((long long*)dst)[i] = a > b ? a : b; }
-    else if (op == 2) ((double*)dst)[i] = fmin(((double*)dst)[i], ((const double*)src)[i]);
-    else if (op == 3) ((double*)dst)[i] = fmax(((double*)dst)[i], ((const double*)src)[i]);
+    else if (op == 2 || op == 3) {
+        // numpy's minimum / maximum: NaN on either side gives NaN (fmin / fmax would drop it)
+        const double a = ((double*)dst)[i], b = ((const double*)src)[i];
+        ((double*)dst)[i] = (a != a || b != b) ? a + b : (op == 2 ? fmin(a, b) : fmax(a, b));
+    }
     else ((double*)dst)[i] = ((double*)dst)[i] + ((const double*)src)[i];
 }
 

@@ -290,7 +290,10 @@ __global__ void __launch_bounds__(ATHREADS, 5) k_assign(const __grid_constant__ 
                 {
                     // lower bound of this candidate's distance for ALL of the thread's pixels, in float.  Spatial term: the centre is
                     // at least |cx - x| away in x and |cy - ymid| - (AROWS-1)/2 in y; 2e-3 px absorbs the float conversion of
-                    // coordinates up to 16k, the factor 0.998 the rounding of the few float operations.  Colour term: each channel
+                    // the centre for coordinates below 2^16 (half an ulp is 2^-9 px there), the factor 0.998 the rounding of the few
+                    // float operations.  Past 2^16 the conversion moves a centre by up to 2^-8 px (2^-7 past 2^17), more than the
+                    // slack, so the bound is proven only for sides below 65 536 px; on taller or wider images no input has been
+                    // found where it rejects a candidate that wins or ties (tests/test_gpu_slic_edges.py).  Colour term: each channel
                     // is at least the gap between the pixels' box and the centre; the box, the centre and every operation round
                     // towards a smaller result, so the term is at most the exact sum of squares, and the factor 0.998 leaves room
                     // for the rounding of the double chain (the double distance is at least the exact one times 1 - 2^-50).

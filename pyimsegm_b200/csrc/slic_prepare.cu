@@ -1,4 +1,6 @@
 // slic_prepare.cu -- SLIC pre-pass: min/max -> rescale -> gaussian blur -> rgb2lab -> * 1/compactness -> planar f64.
+// The rescale runs in the image's own precision as numpy does it (float32 for a float32 image, float64 otherwise); the
+// blur and everything after it run in f64 for every input type.
 //
 // Replaces (reference call stack, SURVEY.md section 3.1):
 //   imsegm/superpixels.py:53-54   img = (img - img.min()) / float(img.max() - img.min())
@@ -89,18 +91,23 @@ __device__ __forceinline__ void rgb2lab_px(double r, double g, double b, double&
     B = dmul(200.0, dsub(f[1], f[2]));
 }
 
+// numpy's min / max: a NaN sample makes the result NaN (fmin / fmax would skip it).  A NaN is sticky in both reductions: it wins
+// every comparison it takes part in.
+__device__ __forceinline__ double nan_min(double a, double b) { return (a < b || a != a) ? a : b; }
+__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
+
 __global__ void k_minmax(const void* img, int dtype, size_t n, unsigned long long* mm)
 {
     double lo = 1.0 / 0.0, hi = -1.0 / 0.0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         double v = load_as_f64(img, dtype, i);
-        lo = fmin(lo, v);
-        hi = fmax(hi, v);
+        lo = nan_min(lo, v);
+        hi = nan_max(hi, v);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-        lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
-        hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+        lo = nan_min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+        hi = nan_max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
     }
     __shared__ double slo[32], shi[32];
     int w = threadIdx.x >> 5, l = threadIdx.x & 31;
@@ -112,10 +119,13 @@ __global__ void k_minmax(const void* img, int dtype, size_t n, unsigned long lon
         hi = l < nw ? shi[l] : -1.0 / 0.0;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
-            lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
-            hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+            lo = nan_min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+            hi = nan_max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
         }
         if (l == 0) {
+            // in the ordered map a NaN with the sign bit set is below -inf and one without it above +inf, so the atomics keep it
+            if (lo != lo) lo = __longlong_as_double((long long)0xFFF8000000000000ull);
+            if (hi != hi) hi = __longlong_as_double(0x7FF8000000000000ll);
             atomicMin(&mm[0], f64_ordered(lo));
             atomicMax(&mm[1], f64_ordered(hi));
         }
@@ -124,8 +134,10 @@ __global__ void k_minmax(const void* img, int dtype, size_t n, unsigned long lon
 
 __global__ void k_minmax_decode(const unsigned long long* mm, double* out)
 {
-    out[0] = f64_unordered(mm[0]);
-    out[1] = f64_unordered(mm[1]);
+    const double lo = f64_unordered(mm[0]), hi = f64_unordered(mm[1]);
+    const double nan = __longlong_as_double(0x7FF8000000000000ll);
+    out[0] = lo != lo ? nan : lo;
+    out[1] = hi != hi ? nan : hi;
 }
 
 // k_blur_lab: one CTA = TX output columns x SH output rows, walked down in chunks of K rows.
@@ -159,6 +171,10 @@ __global__ void __launch_bounds__(NT, 2) k_blur_lab(const void* __restrict__ img
     const double mn = minmax[0], mx = minmax[1];
     const bool do_rescale = rescale && (mn != 0.0 || mx != 1.0);
     const double span = dsub(mx, mn);
+    // a float32 image is rescaled in float32, as numpy does (img - img.min()) / float(img.max() - img.min()) for it; the
+    // extrema are float32 values, so they convert back exactly
+    const bool rescale_f32 = dtype == ISB_F32;
+    const float mnf = (float)mn, spanf = __fsub_rn((float)mx, mnf);
     const size_t HW = (size_t)H * W;
 
     for (int ix = threadIdx.x; ix < IW; ix += NT) s_gx[ix] = reflect_index(x0 + ix - R, W);
@@ -166,7 +182,7 @@ __global__ void __launch_bounds__(NT, 2) k_blur_lab(const void* __restrict__ img
 
     // rescale, then the depth axis of skimage's [1,H,W,3] array: all its taps reflect onto the same sample
     auto prep = [&](double v) {
-        if (do_rescale) v = ddiv(dsub(v, mn), span);
+        if (do_rescale) v = rescale_f32 ? (double)__fdiv_rn(__fsub_rn((float)v, mnf), spanf) : ddiv(dsub(v, mn), span);
         if (R > 0) {
             double t = dmul(v, gw.w[0]);
 #pragma unroll

@@ -37,6 +37,26 @@ def _supported_dtype(img):
     return img.astype(np.float64)
 
 
+def _slic_input(img):
+    """(image the device reads, whether the device rescales it) for segment_slic_img2d
+
+    The reference wrapper rescales ``(img - img.min()) / float(img.max() - img.min())`` in numpy (superpixels.py:53-54), i.e. in
+    the image's own dtype.  The device does the same for uint8, uint16, float32 and float64 images.  A boolean image goes up as
+    uint8: it is already in [0, 1] whenever numpy can rescale it (numpy refuses to subtract booleans, so a constant boolean image,
+    which the reference rejects, gives one NaN-coloured segment here).  Every other dtype -- float16, where numpy rescales in
+    float16, and the integer types, where ``img - img.min()`` wraps when the range overflows the type -- is rescaled on the host by
+    the reference's own expression and uploaded as float64 that the device leaves as it is.
+    """
+    if img.dtype in (np.uint8, np.uint16, np.float32, np.float64):
+        return img, True
+    if img.dtype == bool:
+        return img.astype(np.uint8), True
+    lo, hi = img.min(), img.max()
+    if lo != 0. or hi != 1.:
+        img = (img - lo) / float(hi - lo)
+    return img.astype(np.float64), False
+
+
 def slic_params(shape_hw, sp_size, relative_compact):
     """native SLIC parameters from the reference's (size, regularisation) pair (superpixels.py:57-58)"""
     nb_pixels = int(np.prod(shape_hw))
@@ -60,14 +80,14 @@ def segment_slic_img2d(img, sp_size=50, relative_compact=0.1, slico=False):
     :param bool slico: parameter-free SLICO / ASLIC variant (skimage's slic_zero)
     :return ndarray: segmentation [H, W], labels 0..N-1
     """
-    img = _supported_dtype(_as_rgb_like(img))
+    img, rescale = _slic_input(_as_rgb_like(img))
     eng = get_engine()
     n_seg, compact = slic_params(img.shape[:2], sp_size, relative_compact)
     logging.debug('SLIC 2d: NB=%i compact=%f image %r', n_seg, compact, img.shape)
     if n_seg < 1:
         raise ValueError('superpixel size %r is larger than the image %r' % (sp_size, img.shape))
     d_img = eng.to_device(img, 'image')
-    labels, _ = eng.slic(d_img, n_seg, compact, sigma=1.0, enforce_connectivity=True, slic_zero=slico)
+    labels, _ = eng.slic(d_img, n_seg, compact, sigma=1.0, enforce_connectivity=True, slic_zero=slico, rescale=rescale)
     return eng.to_host(labels).astype(np.int64)
 
 

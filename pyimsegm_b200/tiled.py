@@ -166,9 +166,14 @@ def slic_tiled(image, n_segments, compactness, sigma=1.0, max_iter=10, slic_zero
             if i > 0:
                 _combine(lib, mm.data_ptr(), mm_b.data_ptr(), 1, OP_MIN_F64)
                 _combine(lib, mm.data_ptr() + 8, mm_b.data_ptr() + 8, 1, OP_MAX_F64)
-    if rescale:
+    if rescale and comm.world > 1:
+        # a NaN sample makes both extrema NaN (numpy's rule, kept by isb_image_minmax and isb_combine); the collectives' min and
+        # max need not keep a NaN, so a flag carries it across the GPUs
+        has_nan = torch.isnan(mm[0:1]).to(torch.float64)
         comm.all_reduce(mm[0:1], 'min')
         comm.all_reduce(mm[1:2], 'max')
+        comm.all_reduce(has_nan, 'max')
+        mm[0:2].masked_fill_(has_nan > 0, float('nan'))
 
     # 2) blur + rgb2lab of every raw slab, band descriptors
     descs, keep = [], []

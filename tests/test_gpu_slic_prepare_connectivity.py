@@ -44,15 +44,17 @@ def _device_lab(img, sigma, ratio, rescale, minmax=None):
 
 
 def _oracle_lab(oracle, img, sigma, ratio, minmax):
-    x = img.astype(np.float64)
+    """the reference wrapper's rescale in numpy, in the image's own dtype (float32 stays float32), then f64"""
+    x = img
     if x.ndim == 2:
         x = x[..., None]
     if x.shape[2] == 1:
         x = np.repeat(x, 3, axis=2)
     if minmax is not None:
-        mn, mx = minmax
+        mn, mx = (x.dtype.type(v) for v in minmax)
         if mn != 0.0 or mx != 1.0:
-            x = (x - mn) / (mx - mn)
+            x = (x - mn) / float(mx - mn)
+    x = x.astype(np.float64)
     if sigma > 0:
         x = oracle.gaussian_blur(x, sigma)
     return oracle.rgb2lab_scaled(x, ratio)
@@ -87,7 +89,8 @@ def _check_lab(oracle, img, sigma, rescale=1, minmax=None, ratio=0.37):
 @pytest.mark.parametrize('sigma', [0, 0.5, 1, 2])
 @pytest.mark.parametrize('dtype', [np.uint8, np.uint16, np.float32, np.float64])
 @pytest.mark.parametrize('gray', [False, True])
-def test_lab_planes_bit_exact(oracle, sigma, dtype, gray):
+def test_lab_planes_bit_exact_numpy_rescale(oracle, sigma, dtype, gray):
+    """the reference's min-max rescale as numpy computes it, in the image's own dtype (float32 in float32), then f64"""
     # 75 x 150: W not a multiple of 32 or of the 128-column tile, H not a multiple of the 64-row strip or the 8-row chunk
     shape = (75, 150) if gray else (75, 150, 3)
     _check_lab(oracle, _image(shape, dtype, seed=int(sigma * 10) + 3 * gray), sigma)
