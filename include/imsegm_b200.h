@@ -140,6 +140,41 @@ size_t isb_slic3d_kmeans_workspace_bytes(int D, int H, int W, int n_seeds);
 int isb_slic3d_kmeans(const double* vol_scaled, int D, int H, int W, const double* seeds_zyx, int n_seeds, int step_z, int step_y,
                       int step_x, double step, const double* spacing_host, int max_iter, int32_t* labels, void* ws, size_t ws_bytes,
                       isb_stream_t stream);
+
+/* Slab form of the 3-D sweeps: one volume cut into z-slabs, one (or a few) per GPU, as isb_slic_band_* cuts an image into row
+ * bands.  isb_slic3d_prepare_slab blurs slices [z_off, z_off + S) of a volume of depth D (z reflects at the volume's borders, not
+ * the slab's); the slices within r_z of either end of an interior slab are not exact, so a caller hands it its k-means slab +-
+ * r_z slices (clipped to the volume) and keeps the k-means slab.  The cluster state is replicated in every slab's workspace and
+ * lives in the coordinates of the whole volume; a slab assigns every voxel of its k-means slab -- its owned slices + halo, clipped
+ * -- from every alive cluster whose +-2*step window meets it, and sums the clusters whose centre slice it owns (all their members
+ * are inside the slab; a cluster with a member beyond +-halo slices of its centre -- a voxel that no window reached kept its old
+ * label -- is counted in xchg[5 n_seeds] and the caller must then redo the sweeps on the whole volume).  Per sweep:
+ *     isb_slic3d_slab_assign -> isb_slic3d_slab_update(xchg) -> [sum xchg as int64 over the slabs] -> isb_slic3d_slab_import(xchg)
+ * xchg is [5*n_seeds + 1] int64: per cluster the bit patterns of (cz, cy, cx, cv) and an alive flag (1), all zero in every slab
+ * but the owner's and zero for a cluster that died, so the integer sum is an exact merge.  There is no SLICO in 3-D, hence no
+ * finalize step.  The labels of the k-means slab are bit-identical to isb_slic3d_kmeans on the whole volume.
+ * Workspace: isb_slic3d_kmeans_workspace_bytes(slab_slices, height, width, n_seeds). */
+int isb_slic3d_prepare_slab(const void* vol, int dtype, int S, int H, int W, int z_off, int D, const double* w_z, int r_z,
+                            const double* w_y, int r_y, const double* w_x, int r_x, double ratio, double* tmp, double* out,
+                            isb_stream_t stream);
+typedef struct isb_slic3d_slab {
+    int32_t depth, height, width;   /* the whole volume */
+    int32_t z_off, slab_slices;     /* voxel memory held by this slab: slices [z_off, z_off + slab_slices) (its k-means slab) */
+    int32_t own_lo, own_hi;         /* global slices whose clusters this slab sums; the slabs' [own_lo, own_hi) partition the volume */
+    int32_t halo;                   /* >= 2*step_z; the slab covers [own_lo - halo, own_hi + halo) clipped to the volume */
+    int32_t n_seeds, step_z, step_y, step_x;
+    double step;
+    double spacing[3];              /* (z, y, x) weights of the spatial distance */
+    const double* vol_slab;         /* [slab_slices, height, width] prepared (blurred, * 1/compactness) voxels */
+    const double* seeds_zyx;        /* [n_seeds, 3] seeds of the whole volume */
+    int32_t* labels_slab;           /* [slab_slices, height, width] */
+    void* ws; size_t ws_bytes;
+} isb_slic3d_slab_t;
+int isb_slic3d_slab_begin(const isb_slic3d_slab_t* slab, isb_stream_t stream);
+int isb_slic3d_slab_assign(const isb_slic3d_slab_t* slab, isb_stream_t stream);
+int isb_slic3d_slab_update(const isb_slic3d_slab_t* slab, int64_t* xchg, isb_stream_t stream);
+int isb_slic3d_slab_import(const isb_slic3d_slab_t* slab, const int64_t* xchg, isb_stream_t stream);
+
 /* _enforce_label_connectivity_cython on a volume (6 neighbours in the order x+1, x-1, y+1, y-1, z+1, z-1).  The workspace
  * grows with D*H*W only; max_size does not change it. */
 size_t isb_connectivity3d_workspace_bytes(int D, int H, int W, int max_size);
@@ -178,6 +213,15 @@ int isb_segment_stats_finish(int nb, int flags, const double* acc, const double*
 size_t isb_gray_stats_workspace_bytes(int nb);
 int isb_gray_stats(const void* img, int dtype, const int32_t* seg, long long n, int nb, int flags, double* feat, int ld, int col0,
                    void* ws, size_t ws_bytes, isb_stream_t stream);
+/* The same statistics with caller-owned accumulators, so that z-slabs of one volume can be merged by a collective between the
+ * calls (isb_gray_stats runs exactly these three steps): acc [nb,2] f64 (sum, sum of squares), cnt [nb] i64, var [nb] f64
+ * (squared deviations from the f32 mean).  accumulate / deviation ADD into acc+cnt / var (the caller zeroes them). */
+int isb_gray_stats_accumulate(const void* img, int dtype, const int32_t* seg, long long n, int nb, double* acc, int64_t* cnt,
+                              isb_stream_t stream);
+int isb_gray_stats_deviation(const void* img, int dtype, const int32_t* seg, long long n, int nb, const double* acc, const int64_t* cnt,
+                             float* meanf_scratch /* [nb] */, double* var, isb_stream_t stream);
+int isb_gray_stats_finish(int nb, int flags, const double* acc, const double* var, const int64_t* cnt, double* feat, int ld, int col0,
+                          isb_stream_t stream);
 
 /* computeLabelHistogram2d (features_cython.pyx:222): hist[l] = #{p : segm_select[p] == l >= 0 and struc_elem[p] == 1} */
 int isb_label_hist_2d(const int16_t* segm_select, const int16_t* struc_elem, int H, int W, int nb_labels, uint32_t* hist,

@@ -28,7 +28,17 @@ class SlicBand(C.Structure):
                 ('labels_slab', C.c_void_p), ('ws', C.c_void_p), ('ws_bytes', C.c_size_t)]
 
 
+class Slic3dSlab(C.Structure):
+    """isb_slic3d_slab_t of include/imsegm_b200.h"""
+    _fields_ = [('depth', C.c_int32), ('height', C.c_int32), ('width', C.c_int32), ('z_off', C.c_int32), ('slab_slices', C.c_int32),
+                ('own_lo', C.c_int32), ('own_hi', C.c_int32), ('halo', C.c_int32),
+                ('n_seeds', C.c_int32), ('step_z', C.c_int32), ('step_y', C.c_int32), ('step_x', C.c_int32),
+                ('step', C.c_double), ('spacing', C.c_double * 3), ('vol_slab', C.c_void_p), ('seeds_zyx', C.c_void_p),
+                ('labels_slab', C.c_void_p), ('ws', C.c_void_p), ('ws_bytes', C.c_size_t)]
+
+
 _bp = C.POINTER(SlicBand)
+_sp = C.POINTER(Slic3dSlab)
 
 #: every symbol declared in include/imsegm_b200.h: name -> (restype, argtypes)
 SIGNATURES = {
@@ -55,6 +65,11 @@ SIGNATURES = {
     'isb_slic_set_tile_cap': (_i, [_i]),
     'isb_slic_full_scan_tiles': (_ll, []),
     'isb_slic3d_prepare': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _d, _vp, _vp, _vp]),
+    'isb_slic3d_prepare_slab': (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _d, _vp, _vp, _vp]),
+    'isb_slic3d_slab_begin': (_i, [_sp, _vp]),
+    'isb_slic3d_slab_assign': (_i, [_sp, _vp]),
+    'isb_slic3d_slab_update': (_i, [_sp, _vp, _vp]),
+    'isb_slic3d_slab_import': (_i, [_sp, _vp, _vp]),
     'isb_slic3d_kmeans_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'isb_slic3d_kmeans': (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _d, C.POINTER(_d), _i, _vp, _vp, _sz, _vp]),
     'isb_connectivity3d_workspace_bytes': (_sz, [_i, _i, _i, _i]),
@@ -98,6 +113,9 @@ SIGNATURES = {
     'isb_combine': (_i, [_vp, _vp, _ll, _i, _vp]),
     'isb_gray_stats_workspace_bytes': (_sz, [_i]),
     'isb_gray_stats': (_i, [_vp, _i, _vp, _ll, _i, _i, _vp, _i, _i, _vp, _sz, _vp]),
+    'isb_gray_stats_accumulate': (_i, [_vp, _i, _vp, _ll, _i, _vp, _vp, _vp]),
+    'isb_gray_stats_deviation': (_i, [_vp, _i, _vp, _ll, _i, _vp, _vp, _vp, _vp, _vp]),
+    'isb_gray_stats_finish': (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     'isb_label_hist_2d': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     'isb_ray_features_2d': (_i, [_vp, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp]),
     'isb_filter_response_2d': (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp]),

@@ -12,9 +12,9 @@ constexpr int GSTRIP = 16;
 
 __device__ __forceinline__ float clean(float v) { return isnan(v) ? 0.0f : v; }
 
-// pass 0: sum, sum of squares (f32 product), count.  pass 1: sum (v - mean_f32)^2.
+// pass 0: sum, sum of squares (f32 product) -> acc [nb][2], count -> cnt.  pass 1: sum (v - mean_f32)^2 -> acc [nb] (the variance sums).
 __global__ void __launch_bounds__(256) k_gray_stats(const void* __restrict__ img, int dtype, const int* __restrict__ seg, long long n, int pass,
-                                                    double* acc /* [nb][3]: sum, sumsq, var */, long long* cnt, const float* meanf)
+                                                    double* acc, long long* cnt, const float* meanf)
 {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long beg = t * GSTRIP, end = min(beg + GSTRIP, n);
@@ -27,8 +27,8 @@ __global__ void __launch_bounds__(256) k_gray_stats(const void* __restrict__ img
         const int l = i < end ? seg[i] : -1;
         if (l != cur) {
             if (cur >= 0) {
-                if (pass == 0) { atomicAdd(&acc[3 * (size_t)cur], s); atomicAdd(&acc[3 * (size_t)cur + 1], e); atomicAdd((unsigned long long*)&cnt[cur], (unsigned long long)c); }
-                else atomicAdd(&acc[3 * (size_t)cur + 2], s);
+                if (pass == 0) { atomicAdd(&acc[2 * (size_t)cur], s); atomicAdd(&acc[2 * (size_t)cur + 1], e); atomicAdd((unsigned long long*)&cnt[cur], (unsigned long long)c); }
+                else atomicAdd(&acc[cur], s);
             }
             cur = l; s = 0; e = 0; c = 0;
             if (pass == 1 && l >= 0) m = meanf[l];
@@ -45,12 +45,12 @@ __global__ void k_gray_means(int nb, const double* acc, const long long* cnt, fl
 {
     int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= nb) return;
-    double m = acc[3 * (size_t)k];
+    double m = acc[2 * (size_t)k];
     if (cnt[k] > 0) m = m / (double)cnt[k];
     meanf[k] = (float)m;
 }
 
-__global__ void k_gray_finalize(int nb, int flags, const double* acc, const long long* cnt, double* feat, int ld, int col0)
+__global__ void k_gray_finalize(int nb, int flags, const double* acc, const double* var, const long long* cnt, double* feat, int ld, int col0)
 {
     int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= nb) return;
@@ -59,7 +59,7 @@ __global__ void k_gray_finalize(int nb, int flags, const double* acc, const long
     double* row = feat + (size_t)k * ld;
     for (int st = 0; st < 3; ++st) {
         if (!(flags & (1 << st))) continue;
-        double v = acc[3 * (size_t)k + (st == 0 ? 0 : (st == 1 ? 2 : 1))];
+        double v = st == 0 ? acc[2 * (size_t)k] : (st == 1 ? var[k] : acc[2 * (size_t)k + 1]);
         if (c > 0) v = v / (double)c;
         if (st == 1) v = sqrt(v);
         row[col++] = isnan(v) ? 0.0 : (v == 0.0 ? 0.0 : v);
@@ -142,32 +142,82 @@ extern "C" int isb_region_label_hist(const int32_t* slic, const int32_t* annot, 
     return ISB_OK;
 }
 
-extern "C" size_t isb_gray_stats_workspace_bytes(int nb) { return isb_align(sizeof(double) * 3 * (size_t)nb) + isb_align(sizeof(long long) * (size_t)nb) + isb_align(sizeof(float) * (size_t)nb) + 1024; }
+namespace {
+
+struct GrayWs {
+    double* acc;      // [nb][2] sum, sum of squares
+    long long* cnt;   // [nb]
+    float* meanf;     // [nb]
+    double* var;      // [nb]
+};
+
+static size_t carve_gray(GrayWs& w, void* ws, size_t bytes, int nb)
+{
+    WsCarver c(ws, bytes);
+    w.acc = c.take<double>(2 * (size_t)nb);
+    w.cnt = c.take<long long>(nb);
+    w.meanf = c.take<float>(nb);
+    w.var = c.take<double>(nb);
+    return isb_align(c.off);
+}
+
+static unsigned gray_blocks(long long n) { return (unsigned)(((n + GSTRIP - 1) / GSTRIP + 255) / 256); }
+
+} // namespace
+
+extern "C" size_t isb_gray_stats_workspace_bytes(int nb)
+{
+    GrayWs w;
+    return carve_gray(w, nullptr, 0, nb);
+}
+
+extern "C" int isb_gray_stats_accumulate(const void* img, int dtype, const int32_t* seg, long long n, int nb, double* acc, int64_t* cnt,
+                                         isb_stream_t stream)
+{
+    ISB_REQUIRE(img && seg && acc && cnt, "null pointer");
+    ISB_REQUIRE(n > 0 && nb > 0 && dtype >= ISB_U8 && dtype <= ISB_F64, "bad arguments");
+    k_gray_stats<<<gray_blocks(n), 256, 0, (cudaStream_t)stream>>>(img, dtype, seg, n, 0, acc, (long long*)cnt, nullptr);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_gray_stats_deviation(const void* img, int dtype, const int32_t* seg, long long n, int nb, const double* acc,
+                                        const int64_t* cnt, float* meanf_scratch, double* var, isb_stream_t stream)
+{
+    ISB_REQUIRE(img && seg && acc && cnt && meanf_scratch && var, "null pointer");
+    ISB_REQUIRE(n > 0 && nb > 0 && dtype >= ISB_U8 && dtype <= ISB_F64, "bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    k_gray_means<<<(nb + 255) / 256, 256, 0, st>>>(nb, acc, (const long long*)cnt, meanf_scratch);
+    ISB_LAUNCH_CHECK();
+    k_gray_stats<<<gray_blocks(n), 256, 0, st>>>(img, dtype, seg, n, 1, var, nullptr, meanf_scratch);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_gray_stats_finish(int nb, int flags, const double* acc, const double* var, const int64_t* cnt, double* feat, int ld,
+                                     int col0, isb_stream_t stream)
+{
+    ISB_REQUIRE(acc && cnt && feat && (var || !(flags & 2)), "null pointer");
+    ISB_REQUIRE(nb > 0, "bad sizes");
+    k_gray_finalize<<<(nb + 255) / 256, 256, 0, (cudaStream_t)stream>>>(nb, flags, acc, var, (const long long*)cnt, feat, ld, col0);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
 
 extern "C" int isb_gray_stats(const void* img, int dtype, const int32_t* seg, long long n, int nb, int flags, double* feat, int ld, int col0,
                               void* ws, size_t ws_bytes, isb_stream_t stream)
 {
     ISB_REQUIRE(img && seg && feat && ws, "null pointer");
     ISB_REQUIRE(n > 0 && nb > 0 && dtype >= ISB_U8 && dtype <= ISB_F64, "bad arguments");
-    ISB_REQUIRE(ws_bytes >= isb_gray_stats_workspace_bytes(nb), "workspace too small");
-    WsCarver c(ws, ws_bytes);
-    double* acc = c.take<double>(3 * (size_t)nb);
-    long long* cnt = c.take<long long>(nb);
-    float* meanf = c.take<float>(nb);
+    GrayWs w;
+    const size_t need = carve_gray(w, ws, ws_bytes, nb);
+    ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    ISB_CUDA_CHECK(cudaMemsetAsync(ws, 0, isb_align(c.off), st));
-    const unsigned blocks = (unsigned)(((n + GSTRIP - 1) / GSTRIP + 255) / 256);
-    k_gray_stats<<<blocks, 256, 0, st>>>(img, dtype, seg, n, 0, acc, cnt, meanf);
-    ISB_LAUNCH_CHECK();
-    if (flags & 2) {
-        k_gray_means<<<(nb + 255) / 256, 256, 0, st>>>(nb, acc, cnt, meanf);
-        ISB_LAUNCH_CHECK();
-        k_gray_stats<<<blocks, 256, 0, st>>>(img, dtype, seg, n, 1, acc, cnt, meanf);
-        ISB_LAUNCH_CHECK();
-    }
-    k_gray_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, flags, acc, cnt, feat, ld, col0);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
+    ISB_CUDA_CHECK(cudaMemsetAsync(ws, 0, need, st));
+    if (int rc = isb_gray_stats_accumulate(img, dtype, seg, n, nb, w.acc, (int64_t*)w.cnt, stream)) return rc;
+    if (flags & 2)
+        if (int rc = isb_gray_stats_deviation(img, dtype, seg, n, nb, w.acc, (const int64_t*)w.cnt, w.meanf, w.var, stream)) return rc;
+    return isb_gray_stats_finish(nb, flags, w.acc, w.var, (const int64_t*)w.cnt, feat, ld, col0, stream);
 }
 
 extern "C" int isb_label_hist_2d(const int16_t* segm_select, const int16_t* struc_elem, int H, int W, int nb_labels, uint32_t* hist,

@@ -14,6 +14,9 @@
 //  * connectivity: union-find components (root = first raster voxel), components >= max_size cut by replaying the truncated BFS
 //    (one thread per such component), pieces < min_size replay their own BFS to find the last earlier-labelled neighbour piece,
 //    chains of small pieces are followed to a kept piece; new labels = raster-order rank of the kept pieces.
+//  * slab mode (isb_slic3d_slab_*): the same sweeps over one z-slab of a volume per GPU; the scan clips each window to the slab's
+//    slices, the owner of a cluster's centre slice writes its sums to an int64 exchange record (k3_update), k3_import takes the
+//    records merged over the slabs.
 // All distances in IEEE double without FMA, in the oracle's operation order.
 #include "common.cuh"
 #include "block_scan.cuh"
@@ -33,18 +36,22 @@ __global__ void k3_load(const void* __restrict__ vol, int dtype, size_t n, doubl
     out[i] = v;
 }
 
-__global__ void k3_blur_axis(const double* __restrict__ in, double* __restrict__ out, int D, int H, int W, int axis,
+// the array holds slices [z_off, z_off + S) of a volume of depth D: z reflects at the volume's borders, so a slice whose window
+// of +- r_z slices lies inside the array (clipped to the volume) gets the value the whole volume gives it
+__global__ void k3_blur_axis(const double* __restrict__ in, double* __restrict__ out, int S, int H, int W, int z_off, int D, int axis,
                              const double* __restrict__ w, int r)
 {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (size_t)D * H * W) return;
-    const int x = (int)(i % W), y = (int)((i / W) % H), z = (int)(i / ((size_t)H * W));
+    if (i >= (size_t)S * H * W) return;
+    const int x = (int)(i % W), y = (int)((i / W) % H), z = (int)(i / ((size_t)H * W)) + z_off;
     const int c = axis == 0 ? z : (axis == 1 ? y : x), n = axis == 0 ? D : (axis == 1 ? H : W);
     const long st = axis == 0 ? (long)H * W : (axis == 1 ? W : 1);
+    // the slices within r_z of a slab's ends read past the array: those are clamped to it, and their values are not used
+    const int lo = axis == 0 ? z_off : 0, hi = axis == 0 ? z_off + S - 1 : n - 1;
     double t = __dmul_rn(in[i], w[0]);
     for (int j = r; j >= 1; --j) {
-        const double a = in[i + (long)(reflect_index(c - j, n) - c) * st];
-        const double b = in[i + (long)(reflect_index(c + j, n) - c) * st];
+        const double a = in[i + (long)(min(max(reflect_index(c - j, n), lo), hi) - c) * st];
+        const double b = in[i + (long)(min(max(reflect_index(c + j, n), lo), hi) - c) * st];
         t = __dadd_rn(t, __dmul_rn(__dadd_rn(a, b), w[j]));
     }
     out[i] = t;
@@ -63,6 +70,8 @@ struct Km3 {
     unsigned long long* dist;                          // [V] bit pattern of the current minimum
     int* lab_new;                                      // [V]
     int n, D, H, W, step_z, step_y, step_x;
+    int z_off, Dg;                                     // voxel memory: slices [z_off, z_off + D) of a volume of depth Dg
+    int own_lo, own_hi, halo;                          // slab mode (xchg != null in k3_update): the owned slices and the halo
     double sz, sy, sx, sw;
 };
 
@@ -100,9 +109,11 @@ __global__ void __launch_bounds__(256) k3_scan(Km3 s, const double* __restrict__
     if (!s.alive[k]) return;
     const double cz = s.cz[k], cy = s.cy[k], cx = s.cx[k], cv = s.cv[k];
     int z0, z1, y0, y1, x0, x1;
-    window3(cz, s.step_z, s.D, z0, z1);
+    window3(cz, s.step_z, s.Dg, z0, z1);
     window3(cy, s.step_y, s.H, y0, y1);
     window3(cx, s.step_x, s.W, x0, x1);
+    z0 = max(z0, s.z_off); z1 = min(z1, s.z_off + s.D);      // the slices this slab holds (all of them for a whole volume)
+    if (z1 <= z0) return;
     const int wy = y1 - y0, wx = x1 - x0;
     const long total = (long)(z1 - z0) * wy * wx;
     for (long i = threadIdx.x; i < total; i += blockDim.x) {
@@ -111,7 +122,7 @@ __global__ void __launch_bounds__(256) k3_scan(Km3 s, const double* __restrict__
         const double ty = __dmul_rn(s.sy, __dsub_rn(cy, (double)y));
         const double tx = __dmul_rn(s.sx, __dsub_rn(cx, (double)x));
         double dc = __dmul_rn(__dadd_rn(__dadd_rn(__dmul_rn(tz, tz), __dmul_rn(ty, ty)), __dmul_rn(tx, tx)), s.sw);
-        const size_t p = ((size_t)z * s.H + y) * s.W + x;
+        const size_t p = ((size_t)(z - s.z_off) * s.H + y) * s.W + x;
         const double d0 = __dsub_rn(vol[p], cv);
         dc = __dadd_rn(dc, __dmul_rn(d0, d0));
         const unsigned long long bits = (unsigned long long)__double_as_longlong(dc);
@@ -128,27 +139,39 @@ __global__ void k3_commit(Km3 s, int* __restrict__ labels)
     if (i >= V) return;
     int l = s.lab_new[i];
     if (l != INT_MAX) labels[i] = l; else l = labels[i];
-    const int x = (int)(i % s.W), y = (int)((i / s.W) % s.H), z = (int)(i / ((size_t)s.H * s.W));
+    const int x = (int)(i % s.W), y = (int)((i / s.W) % s.H), z = (int)(i / ((size_t)s.H * s.W)) + s.z_off;
     int* b = s.bb + 6 * (size_t)l;
     atomicMin(&b[0], z); atomicMax(&b[1], z); atomicMin(&b[2], y); atomicMax(&b[3], y); atomicMin(&b[4], x); atomicMax(&b[5], x);
 }
 
-// centroid sums: one warp per cluster over the box of its members, in raster order
-__global__ void __launch_bounds__(256) k3_update(Km3 s, const double* __restrict__ vol, const int* __restrict__ labels)
+// centroid sums: one warp per cluster over the box of its members, in raster order.
+// Slab mode (xchg != null): the cluster is summed by the slab that owns the slice of the centre the assignment used; every member
+// the assignment gave it lies within 2*step_z slices of that centre, i.e. inside the owner's k-means slab.  A member box that
+// reaches beyond +- halo slices (a voxel no window reached kept the label of a cluster centred further away) is counted in
+// xchg[5n]: the owner's sums would miss it.  The owner writes the record xchg[5k..5k+4] = bits(cz, cy, cx, cv), 1 (alive); every
+// other slab, and the owner of a cluster that lost its last voxel, leaves zeros, so an integer sum over the slabs is an exact merge.
+__global__ void __launch_bounds__(256) k3_update(Km3 s, const double* __restrict__ vol, const int* __restrict__ labels,
+                                                 long long* __restrict__ xchg)
 {
     __shared__ double buf[8][32];
     const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
     const int k = blockIdx.x * 8 + wl;
-    if (k >= s.n || !s.alive[k]) return;
+    if (k >= s.n) return;
     const int* b = s.bb + 6 * (size_t)k;
     const int z0 = b[0], z1 = b[1], y0 = b[2], y1 = b[3], x0 = b[4], x1 = b[5];
+    if (xchg) {
+        const int cr = s.alive[k] ? (int)s.cz[k] : 0;   // slice of the centre the assignment used
+        if (lane == 0 && z1 >= z0 && (!s.alive[k] || z0 < cr - s.halo || z1 > cr + s.halo))
+            atomicAdd((unsigned long long*)&xchg[5 * (size_t)s.n], 1ull);
+        if (!s.alive[k] || cr < s.own_lo || cr >= s.own_hi) return;
+    } else if (!s.alive[k]) return;
     double acc = 0.0;
     long long cnt = 0, sumz = 0, sumy = 0, sumx = 0;
     for (int z = z0; z <= z1; ++z)
         for (int y = y0; y <= y1; ++y)
             for (int xb = x0; xb <= x1; xb += 32) {
                 const int x = xb + lane;
-                const size_t p = ((size_t)z * s.H + y) * s.W + x;
+                const size_t p = ((size_t)(z - s.z_off) * s.H + y) * s.W + x;
                 const bool m = x <= x1 && labels[p] == k;
                 const unsigned mask = __ballot_sync(0xffffffffu, m);
                 if (!mask) continue;
@@ -164,10 +187,27 @@ __global__ void __launch_bounds__(256) k3_update(Km3 s, const double* __restrict
     if (lane == 0) {
         if (cnt > 0) {
             const double dn = (double)cnt;
-            s.cz[k] = __ddiv_rn((double)sumz, dn); s.cy[k] = __ddiv_rn((double)sumy, dn); s.cx[k] = __ddiv_rn((double)sumx, dn);
-            s.cv[k] = __ddiv_rn(acc, dn);
-        } else s.alive[k] = 0;   // no voxel: dead for good
+            const double cz = __ddiv_rn((double)sumz, dn), cy = __ddiv_rn((double)sumy, dn), cx = __ddiv_rn((double)sumx, dn);
+            const double cv = __ddiv_rn(acc, dn);
+            if (xchg) {
+                long long* r = xchg + 5 * (size_t)k;
+                r[0] = __double_as_longlong(cz); r[1] = __double_as_longlong(cy); r[2] = __double_as_longlong(cx);
+                r[3] = __double_as_longlong(cv); r[4] = 1;
+            } else { s.cz[k] = cz; s.cy[k] = cy; s.cx[k] = cx; s.cv[k] = cv; }
+        } else if (!xchg) s.alive[k] = 0;   // no voxel: dead for good
     }
+}
+
+// slab mode: take the merged exchange records (see k3_update) as the replicated cluster state
+__global__ void k3_import(Km3 s, const long long* __restrict__ xchg)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= s.n) return;
+    const long long* r = xchg + 5 * (size_t)k;
+    if (r[4] == 1) {
+        s.cz[k] = __longlong_as_double(r[0]); s.cy[k] = __longlong_as_double(r[1]); s.cx[k] = __longlong_as_double(r[2]);
+        s.cv[k] = __longlong_as_double(r[3]);
+    } else s.alive[k] = 0;   // its owner found no voxel, or it was dead already (an alive cluster has exactly one owner)
 }
 
 __global__ void k3_fill(int* p, size_t n, int v)
@@ -379,27 +419,35 @@ static size_t carve_cc3(Cc3& c, void* ws, size_t bytes, int D, int H, int W)
 
 } // namespace
 
-extern "C" int isb_slic3d_prepare(const void* vol, int dtype, int D, int H, int W, const double* w_z, int r_z, const double* w_y, int r_y,
-                                  const double* w_x, int r_x, double ratio, double* tmp, double* out, isb_stream_t stream)
+extern "C" int isb_slic3d_prepare_slab(const void* vol, int dtype, int S, int H, int W, int z_off, int D, const double* w_z, int r_z,
+                                       const double* w_y, int r_y, const double* w_x, int r_x, double ratio, double* tmp, double* out,
+                                       isb_stream_t stream)
 {
     ISB_REQUIRE(vol && w_z && w_y && w_x && tmp && out, "null pointer");
-    ISB_REQUIRE(D > 0 && H > 0 && W > 0 && r_z >= 0 && r_y >= 0 && r_x >= 0, "bad sizes");
+    ISB_REQUIRE(S > 0 && H > 0 && W > 0 && r_z >= 0 && r_y >= 0 && r_x >= 0, "bad sizes");
+    ISB_REQUIRE(z_off >= 0 && z_off + S <= D, "slab outside the volume");
     ISB_REQUIRE(dtype >= ISB_U8 && dtype <= ISB_F64, "bad dtype");
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t n = (size_t)D * H * W;
+    const size_t n = (size_t)S * H * W;
     const unsigned blocks = (unsigned)((n + 255) / 256);
     k3_load<<<blocks, 256, 0, st>>>(vol, dtype, n, out);
     ISB_LAUNCH_CHECK();
-    k3_blur_axis<<<blocks, 256, 0, st>>>(out, tmp, D, H, W, 0, w_z, r_z);
+    k3_blur_axis<<<blocks, 256, 0, st>>>(out, tmp, S, H, W, z_off, D, 0, w_z, r_z);
     ISB_LAUNCH_CHECK();
-    k3_blur_axis<<<blocks, 256, 0, st>>>(tmp, out, D, H, W, 1, w_y, r_y);
+    k3_blur_axis<<<blocks, 256, 0, st>>>(tmp, out, S, H, W, z_off, D, 1, w_y, r_y);
     ISB_LAUNCH_CHECK();
-    k3_blur_axis<<<blocks, 256, 0, st>>>(out, tmp, D, H, W, 2, w_x, r_x);
+    k3_blur_axis<<<blocks, 256, 0, st>>>(out, tmp, S, H, W, z_off, D, 2, w_x, r_x);
     ISB_LAUNCH_CHECK();
     // image * ratio is its own rounding step (np.ascontiguousarray(image * ratio))
     k3_scale<<<blocks, 256, 0, st>>>(tmp, out, n, ratio);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
+}
+
+extern "C" int isb_slic3d_prepare(const void* vol, int dtype, int D, int H, int W, const double* w_z, int r_z, const double* w_y, int r_y,
+                                  const double* w_x, int r_x, double ratio, double* tmp, double* out, isb_stream_t stream)
+{
+    return isb_slic3d_prepare_slab(vol, dtype, D, H, W, 0, D, w_z, r_z, w_y, r_y, w_x, r_x, ratio, tmp, out, stream);
 }
 
 extern "C" size_t isb_slic3d_kmeans_workspace_bytes(int D, int H, int W, int n_seeds)
@@ -419,6 +467,7 @@ extern "C" int isb_slic3d_kmeans(const double* vol_scaled, int D, int H, int W, 
     const size_t need = carve_km3(s, ws, ws_bytes, D, H, W, n_seeds);
     ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     s.n = n_seeds; s.D = D; s.H = H; s.W = W; s.step_z = step_z; s.step_y = step_y; s.step_x = step_x;
+    s.z_off = 0; s.Dg = D; s.own_lo = 0; s.own_hi = D; s.halo = D;
     s.sz = spacing_host[0]; s.sy = spacing_host[1]; s.sx = spacing_host[2]; s.sw = 1.0 / (step * step);
     cudaStream_t st = (cudaStream_t)stream;
     const size_t V = (size_t)D * H * W;
@@ -437,9 +486,91 @@ extern "C" int isb_slic3d_kmeans(const double* vol_scaled, int D, int H, int W, 
         ISB_LAUNCH_CHECK();
         k3_commit<<<vblocks, 256, 0, st>>>(s, labels);
         ISB_LAUNCH_CHECK();
-        k3_update<<<(n_seeds + 7) / 8, 256, 0, st>>>(s, vol_scaled, labels);
+        k3_update<<<(n_seeds + 7) / 8, 256, 0, st>>>(s, vol_scaled, labels, nullptr);
         ISB_LAUNCH_CHECK();
     }
+    return ISB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Slab mode: the same sweeps with one z-slab of the volume per GPU.  The cluster state is replicated; what crosses the GPUs
+// each sweep is the exchange buffer of k3_update (summed as int64 by the caller's collective).
+// ---------------------------------------------------------------------------------------------------------------------
+namespace {
+
+static int slab_state(const isb_slic3d_slab_t* b, Km3& s)
+{
+    ISB_REQUIRE(b && b->vol_slab && b->seeds_zyx && b->labels_slab && b->ws, "null pointer");
+    ISB_REQUIRE(b->depth > 0 && b->height > 0 && b->width > 0 && b->slab_slices > 0 && b->n_seeds > 0 && b->step_z > 0 && b->step_y > 0 &&
+                b->step_x > 0 && b->step > 0, "bad sizes");
+    ISB_REQUIRE((size_t)b->depth * b->height * b->width < (size_t)INT_MAX, "volume too large");
+    ISB_REQUIRE(b->z_off >= 0 && b->z_off + b->slab_slices <= b->depth, "slab outside the volume");
+    ISB_REQUIRE(b->own_lo >= b->z_off && b->own_hi <= b->z_off + b->slab_slices && b->own_lo < b->own_hi, "owned slices outside the slab");
+    ISB_REQUIRE(b->halo >= 2 * b->step_z, "halo must be at least 2 * step_z slices");
+    ISB_REQUIRE(b->z_off <= (b->own_lo - b->halo > 0 ? b->own_lo - b->halo : 0), "slab does not cover the halo below the owned slices");
+    ISB_REQUIRE(b->z_off + b->slab_slices >= (b->own_hi + b->halo < b->depth ? b->own_hi + b->halo : b->depth),
+                "slab does not cover the halo above the owned slices");
+    const size_t need = carve_km3(s, b->ws, b->ws_bytes, b->slab_slices, b->height, b->width, b->n_seeds);
+    ISB_REQUIRE(need <= b->ws_bytes, "workspace too small");
+    s.n = b->n_seeds; s.D = b->slab_slices; s.H = b->height; s.W = b->width;
+    s.step_z = b->step_z; s.step_y = b->step_y; s.step_x = b->step_x;
+    s.z_off = b->z_off; s.Dg = b->depth; s.own_lo = b->own_lo; s.own_hi = b->own_hi; s.halo = b->halo;
+    s.sz = b->spacing[0]; s.sy = b->spacing[1]; s.sx = b->spacing[2]; s.sw = 1.0 / (b->step * b->step);
+    return ISB_OK;
+}
+
+} // namespace
+
+extern "C" int isb_slic3d_slab_begin(const isb_slic3d_slab_t* b, isb_stream_t stream)
+{
+    Km3 s;
+    if (int rc = slab_state(b, s)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t V = (size_t)s.D * s.H * s.W;
+    k3_fill<<<(unsigned)((V + 255) / 256), 256, 0, st>>>(b->labels_slab, V, 0);
+    ISB_LAUNCH_CHECK();
+    k3_seed<<<(s.n + 255) / 256, 256, 0, st>>>(s, b->seeds_zyx);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_slic3d_slab_assign(const isb_slic3d_slab_t* b, isb_stream_t stream)
+{
+    Km3 s;
+    if (int rc = slab_state(b, s)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t V = (size_t)s.D * s.H * s.W;
+    const size_t m = V > (size_t)s.n ? V : (size_t)s.n;
+    k3_clear<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(s);
+    ISB_LAUNCH_CHECK();
+    k3_scan<0><<<s.n, 256, 0, st>>>(s, b->vol_slab);
+    ISB_LAUNCH_CHECK();
+    k3_scan<1><<<s.n, 256, 0, st>>>(s, b->vol_slab);
+    ISB_LAUNCH_CHECK();
+    k3_commit<<<(unsigned)((V + 255) / 256), 256, 0, st>>>(s, b->labels_slab);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_slic3d_slab_update(const isb_slic3d_slab_t* b, int64_t* xchg, isb_stream_t stream)
+{
+    Km3 s;
+    if (int rc = slab_state(b, s)) return rc;
+    ISB_REQUIRE(xchg, "null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    ISB_CUDA_CHECK(cudaMemsetAsync(xchg, 0, sizeof(int64_t) * (5 * (size_t)s.n + 1), st));
+    k3_update<<<(s.n + 7) / 8, 256, 0, st>>>(s, b->vol_slab, b->labels_slab, (long long*)xchg);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_slic3d_slab_import(const isb_slic3d_slab_t* b, const int64_t* xchg, isb_stream_t stream)
+{
+    Km3 s;
+    if (int rc = slab_state(b, s)) return rc;
+    ISB_REQUIRE(xchg, "null pointer");
+    k3_import<<<(s.n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(s, (const long long*)xchg);
+    ISB_LAUNCH_CHECK();
     return ISB_OK;
 }
 

@@ -323,13 +323,20 @@ class Engine(object):
                                        _lib.ptr(km), _lib.ptr(ws), C.c_size_t(wsb), st))
         if not enforce_connectivity:
             return km, None
+        return self.enforce_connectivity3d(km, n_segments, min_size_factor, max_size_factor)
+
+    def enforce_connectivity3d(self, d_km, n_segments, min_size_factor=0.5, max_size_factor=3):
+        """connectivity pass over a k-means label volume [D,H,W] (device): returns (labels int32 [D,H,W], n_labels device int32[1])"""
+        torch, lib = self.torch, self.lib
+        D, H, W = (int(v) for v in d_km.shape)
+        st = _lib.stream_ptr()
         segment_size = D * H * W / n_segments
         min_size, max_size = int(min_size_factor * segment_size), int(max_size_factor * segment_size)
         cwsb = lib.isb_connectivity3d_workspace_bytes(D, H, W, max(max_size, 1))
         cws = self.buf('ws_conn3d', (cwsb,), torch.uint8)
         out = self.buf('labels3d', (D, H, W), torch.int32)
         n_labels = self.buf('n_labels', (1,), torch.int32)
-        self._ck(lib.isb_enforce_connectivity3d(_lib.ptr(km), D, H, W, min_size, max_size, _lib.ptr(out), _lib.ptr(n_labels), _lib.ptr(cws),
+        self._ck(lib.isb_enforce_connectivity3d(_lib.ptr(d_km), D, H, W, min_size, max_size, _lib.ptr(out), _lib.ptr(n_labels), _lib.ptr(cws),
                                                 C.c_size_t(cwsb), st))
         return out, n_labels
 

@@ -449,15 +449,19 @@ def _device_energies(eng, segments, proba, edge_type, edge_cost, pairwise):
     return d_edges, E, eng.gc_energies(d_proba, d_edges, E, None, centres, mode, float(edge_cost), pairwise)
 
 
-def device_graphcut(eng, res, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, edge_cap):
-    """graph-cut tail of the device pipelines over the label map ``res.d_seg`` and its centroids ``res.d_centres``: adjacency,
-    energies, alpha-expansion (all asynchronous).  ``nb`` may be an upper bound of the label count when ``d_n_nodes`` (device
-    scalar) carries the real one.  Returns (class per label [nb] device, n_edges device int32[1]); the result only holds when the
-    table of ``edge_cap`` rows took every edge, see :func:`~.engine.edges_fit`"""
+def device_graphcut(eng, d_seg, d_centres, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, edge_cap):
+    """graph-cut tail of the device pipelines over the label map ``d_seg`` and its centroids ``d_centres``: adjacency,
+    energies, alpha-expansion (all asynchronous).  A label volume [D, H, W] takes its 6-connected graph and its (z, y, x) centroids
+    from :meth:`~.engine.Engine.graph3d` instead (pass ``d_centres`` None).  ``nb`` may be an upper bound of the label count
+    when ``d_n_nodes`` (device scalar) carries the real one.  Returns (class per label [nb] device, n_edges device int32[1]); the
+    result only holds when the table of ``edge_cap`` rows took every edge, see :func:`~.engine.edges_fit`"""
     K = int(d_proba.shape[1])
     pairwise = compute_pairwise_cost(gc_regul, (nb, K))
-    d_edges, d_n_edges, _ = eng.adjacency(res.d_seg, nb, edge_cap)
-    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, edge_cap, d_n_edges, res.d_centres, _edge_mode(gc_edge_type), 1.0,
+    if d_seg.dim() == 3:
+        d_edges, d_n_edges, _, d_centres = eng.graph3d(d_seg, nb, edge_cap)
+    else:
+        d_edges, d_n_edges, _ = eng.adjacency(d_seg, nb, edge_cap)
+    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, edge_cap, d_n_edges, d_centres, _edge_mode(gc_edge_type), 1.0,
                                                        pairwise, d_n_nodes=d_n_nodes)
     d_labels, _, _ = eng.alpha_expansion(nb, K, edge_cap, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, -1, d_n_nodes=d_n_nodes)
     return d_labels, d_n_edges

@@ -223,7 +223,7 @@ def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul,
     soft = eng.early_soft(res.d_seg, d_proba) if early_soft else None
 
     def second_half():
-        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, cap)
+        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res.d_seg, res.d_centres, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, cap)
         return eng.gather(res.d_seg, d_labels, None if early_soft else d_proba) + (d_n_edges, )
 
     key2 = ('cut', id(eng), res.d_seg.data_ptr(), d_proba.data_ptr(), res.d_centres.data_ptr(), res.shape, res.nb_bound,
@@ -516,12 +516,8 @@ def _run_resident_volume(eng, d_vol, model, dict_features, spacing, sp_size, sp_
     if (not isinstance(gc_regul, (list, np.ndarray))) and gc_regul <= 0:
         proba = eng.to_host(d_proba[:int(eng.to_host(d_n)[0])])
         return eng.gather(d_seg, _argmin_labels_device(eng, proba), d_proba) + (None, )
-    K = int(d_proba.shape[1])
     cap = edge_capacity(nb, ndim=3)
-    d_edges, d_n_edges, _, d_centres = eng.graph3d(d_seg, nb, cap)
-    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, cap, d_n_edges, d_centres, graph_cuts._edge_mode(gc_edge_type), 1.0,
-                                                       graph_cuts.compute_pairwise_cost(gc_regul, (nb, K)), d_n_nodes=d_n)
-    d_labels, _, _ = eng.alpha_expansion(nb, K, cap, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, -1, d_n_nodes=d_n)
+    d_labels, d_n_edges = graph_cuts.device_graphcut(eng, d_seg, None, nb, d_proba, gc_regul, gc_edge_type, d_n, cap)
     d_segm, d_soft = eng.gather(d_seg, d_labels, d_proba)
     return d_segm, d_soft, (d_n_edges, cap)
 

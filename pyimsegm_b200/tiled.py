@@ -26,6 +26,23 @@ takes the gradient of the owned rows +- 1 and keeps the owned rows; the Leung-Ma
 band order between the two halves of the battery step.  Models: :func:`pipe_color2d_slic_features_model_graphcut_tiled` fits any
 device ``estim_model`` / ``pca_coef`` on the replicated feature table, :func:`segment_color2d_slic_features_model_graphcut_tiled`
 applies a caller-fitted one (on the device when ``class_models.compile_model`` takes it, on every rank's host otherwise).
+
+Slab mode: ONE gray volume cut into z-slabs the same way (:func:`slab_plan` is :func:`plan_bands` along z), for
+:func:`pipe_gray3d_slic_features_model_graphcut_tiled` and :func:`segment_gray3d_slic_features_model_graphcut_tiled`:
+
+* slab ``i`` owns slices [own_lo, own_hi); its k-means slab is the owned slices +- ``2 step_z + 1`` (every member the assignment
+  gives a cluster lies within ``2 step_z`` slices of its centre), its raw slab the k-means slab +- the z-blur radius; the blur
+  reflects z at the volume's borders, not the slab's.  A cluster is owned by the slab whose owned slices hold its centre's z at
+  the start of the sweep.
+* per sweep the slabs exchange ``5 n + 1`` int64 words (``isb_slic3d_slab_*``): per cluster the bit patterns of (cz, cy, cx, cv)
+  and an alive flag, zero in every slab but the owner's, then the orphan counter; the integer sum is an exact merge.  A voxel no
+  window reaches, with a label whose centre is beyond the halo, makes every rank redo the sweeps on the whole volume.
+* replicated: every rank gets the whole k-means label volume (slab broadcasts) and runs the 3-D connectivity, the statistics'
+  finish, the scaler, the class model and the cut on the whole supervoxel graph.  Mean / std / energy are accumulated over the
+  owned slices and all-reduced between the calls; a median is refused.
+* memory per rank: its raw slabs (dtype + two f64 copies), 16 bytes per k-means-slab voxel, and about 44 bytes per voxel of the
+  WHOLE volume (label volume, connectivity workspace and output): slabs share out the voxel-sized blur and sweeps but do not raise
+  the largest volume one GPU can take; the connectivity's int voxel indices cap a volume below 2^31 / 4 voxels.
 """
 import ctypes as C
 import logging
@@ -33,7 +50,7 @@ import logging
 import numpy as np
 
 from . import _lib
-from .engine import edge_capacity, edges_fit, flag_bits, gaussian_half_kernel, get_engine, slic_seed_grid
+from .engine import edge_capacity, edges_fit, flag_bits, gaussian_half_kernel, get_engine, slic_seed_grid, slic_seed_grid3d
 
 OP_SUM_I64, OP_MAX_I64, OP_MIN_F64, OP_MAX_F64, OP_SUM_F64 = 0, 1, 2, 3, 4
 
@@ -554,13 +571,14 @@ def _prepare_image(image, layout, sp_size, sp_regul):
 
 
 def _banded_segment(eng, shape, comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm):
-    """the tail both banded pipelines share: ``front(force_whole)`` -> (res, d_proba) runs the banded SLIC (``defer_check``), the
-    feature table and the class probabilities; then the soft segmentation of the owned rows, the graph cut on the replicated
-    superpixel graph, the LUT gather of the owned rows and one download.  Orphan pixels beyond the halo redo the front on the whole
-    image, an edge table that was too small redoes the cut.  Returns (segm, segm_soft or None, (row_lo, row_hi)) on the host."""
+    """the tail the banded pipelines share, for an image [H, W] cut into row bands or a volume [D, H, W] cut into z-slabs:
+    ``front(force_whole)`` -> (res, d_proba) runs the banded SLIC (``defer_check``), the feature table and the class probabilities;
+    then the soft segmentation of the owned rows (slices), the graph cut on the replicated superpixel graph (4-connected in 2-D,
+    6-connected in 3-D: :func:`~.graph_cuts.device_graphcut`), the LUT gather of the owned rows and one download.  Orphan pixels
+    beyond the halo redo the front on the whole image, an edge table that was too small redoes the cut.  Returns (segm,
+    segm_soft or None, (lo, hi)) on the host, the rows (slices) [lo, hi) of this rank."""
     from . import graph_cuts
     torch = eng.torch
-    H, W = shape
     force_whole, redo_front = False, True
     while True:
         if redo_front:
@@ -568,10 +586,11 @@ def _banded_segment(eng, shape, comm, bands_per_rank, front, gc_regul, gc_edge_t
             redo_front = False
         lo, hi = res.bands[res.local[0]].own_lo, res.bands[res.local[-1]].own_hi
         soft = eng.early_soft(res.d_seg[lo:hi], d_proba) if want_soft else None
-        cap = edge_capacity(res.nb_bound)
-        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res, res.nb_bound, d_proba, gc_regul, gc_edge_type, res.d_n_labels, cap)
+        cap = edge_capacity(res.nb_bound, ndim=len(shape))
+        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res.d_seg, res.d_centres, res.nb_bound, d_proba, gc_regul, gc_edge_type,
+                                                         res.d_n_labels, cap)
         # 5) LUT gather of the owned rows
-        d_full = eng.buf('segm', (H, W), torch.int32) if gather_segm else None
+        d_full = eng.buf('segm', tuple(shape), torch.int32) if gather_segm else None
         d_segm, _ = eng.gather(res.d_seg[lo:hi], d_labels, out_i=d_full[lo:hi] if gather_segm else None)
         if gather_segm and comm.world > 1:
             for r in range(comm.world):
@@ -665,6 +684,251 @@ def segment_color2d_slic_features_model_graphcut_tiled(image, model_pipeline, di
         return res, eng.to_device(padded, 'proba')
 
     segm, soft, rows = _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm)
+    if classes is not None:
+        segm = np.asarray(classes)[segm]
+    return segm, soft, rows
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# z-slab mode: ONE gray volume cut into slabs of slices, one slab (or a few) per GPU
+# ---------------------------------------------------------------------------------------------------------------------
+
+def slab_plan(shape, n_segments, spacing, n_slabs, sigma=1.0):
+    """the z-slabs of the 3-D SLIC of a volume ``shape`` = (D, H, W): (:func:`plan_bands` along z with a halo of ``2 step_z + 1``
+    slices and the z-blur's radius, seeds (z, y, x), steps (z, y, x), the half kernels (weights, radius) of the z, y, x blurs)"""
+    halves = [gaussian_half_kernel(s) for s in np.array([sigma, sigma, sigma], dtype=np.float64) / np.asarray(spacing, dtype=np.float64)]
+    seeds, steps = slic_seed_grid3d(tuple(shape), n_segments)
+    return plan_bands(shape[0], n_slabs, 2 * steps[0] + 1, halves[0][1]), seeds, steps, halves
+
+
+def slic3d_tiled(volume, n_segments, compactness, spacing, sigma=1.0, max_iter=10, comm=None, bands_per_rank=1, eng=None,
+                 min_size_factor=0.5, max_size_factor=3, enforce_connectivity=True, defer_check=False, force_whole=False):
+    """ 3-D SLIC of one host gray volume over the z-slabs of ``comm`` (every rank passes the same volume; it uploads only the raw
+    slices of its slabs).  The slabs are :func:`plan_bands` along z: owned slices, k-means slab = owned +- ``2 step_z + 1``, raw
+    slab = k-means slab +- the z-blur radius.  Per sweep the slabs exchange 5 int64 words per cluster (``isb_slic3d_slab_*``).
+
+    :param ndarray volume: [D, H, W] host array, dtype uint8 / uint16 / float32 / float64
+    :return TiledSuperpixels: ``d_seg`` = the whole label volume on this GPU (identical on every rank), ``d_raw[i]`` = the raw slices
+        ``bands[local[i]].raw_lo:raw_hi`` still on the device for the statistics
+    :param bool defer_check: do not synchronise to read the orphan counter ``res.d_err``; the caller reads it with its own
+        results and calls again with ``force_whole=True`` when it is not zero
+    :param bool force_whole: skip the banded sweeps, every rank runs them on the whole volume (the fallback)
+    """
+    eng = eng or get_engine()
+    torch, lib = eng.torch, eng.lib
+    comm = comm or default_comm()
+    volume = np.asarray(volume)
+    D, H, W = (int(v) for v in volume.shape)
+    code = _lib.dtype_code(volume.dtype)
+    st = _lib.stream_ptr()
+    spacing = np.ascontiguousarray(spacing, dtype=np.float64)
+    bands, seeds, (tz, ty, tx), halves = slab_plan((D, H, W), n_segments, spacing, comm.world * int(bands_per_rank), sigma)
+    d_w = [eng.const_device(w, 'slic3d_w%d' % axis) for axis, (w, _) in enumerate(halves)]
+    n_seeds = len(seeds)
+    halo = 2 * tz + 1
+    local = list(range(comm.rank * bands_per_rank, (comm.rank + 1) * bands_per_rank))
+    owner = lambda b: b // bands_per_rank  # noqa: E731
+
+    res = TiledSuperpixels()
+    res.shape, res.bands, res.local = (D, H, W), bands, local
+    res.d_raw = [eng.to_device(volume[bands[b].raw_lo:bands[b].raw_hi], 'ts%d_raw' % i) for i, b in enumerate(local)]
+    d_seeds = eng.const_device(seeds, 'seeds3d')
+    xchg = [eng.buf('ts%d_xchg' % i, (5 * n_seeds + 1,), torch.int64) for i in range(len(local))]
+    err = eng.buf('ts_err', (1,), torch.int64)
+    err.zero_()
+
+    # 1) blur of every raw slab, slab descriptors
+    descs, keep = [], []
+    for i, b in enumerate([] if force_whole else local):
+        bd = bands[b]
+        S, slab = bd.raw_hi - bd.raw_lo, bd.km_hi - bd.km_lo
+        tmp = eng.buf('ts_tmp', (S, H, W), torch.float64)
+        prep = eng.buf('ts%d_vol' % i, (S, H, W), torch.float64)
+        _lib.check(lib.isb_slic3d_prepare_slab(_lib.ptr(res.d_raw[i]), code, S, H, W, bd.raw_lo, D, _lib.ptr(d_w[0]), halves[0][1],
+                                               _lib.ptr(d_w[1]), halves[1][1], _lib.ptr(d_w[2]), halves[2][1], C.c_double(1.0 / compactness),
+                                               _lib.ptr(tmp), _lib.ptr(prep), st))
+        labels = eng.buf('ts%d_labels' % i, (slab, H, W), torch.int32)
+        wsb = lib.isb_slic3d_kmeans_workspace_bytes(slab, H, W, n_seeds)
+        ws = eng.buf('ts%d_ws' % i, (wsb,), torch.uint8)
+        d = _lib.Slic3dSlab(depth=D, height=H, width=W, z_off=bd.km_lo, slab_slices=slab, own_lo=bd.own_lo, own_hi=bd.own_hi, halo=halo,
+                            n_seeds=n_seeds, step_z=tz, step_y=ty, step_x=tx, step=float(max(tz, ty, tx)), spacing=(C.c_double * 3)(*spacing),
+                            vol_slab=prep.data_ptr() + (bd.km_lo - bd.raw_lo) * H * W * 8, seeds_zyx=d_seeds.data_ptr(),
+                            labels_slab=labels.data_ptr(), ws=ws.data_ptr(), ws_bytes=wsb)
+        descs.append(d)
+        keep.append((prep, labels, ws))
+        _lib.check(lib.isb_slic3d_slab_begin(C.byref(d), st))
+
+    # 2) the sweeps: assign, sum the owned clusters, merge, take the merged centres
+    for _ in range(0 if force_whole else int(max_iter)):
+        for i, d in enumerate(descs):
+            _lib.check(lib.isb_slic3d_slab_assign(C.byref(d), st))
+            _lib.check(lib.isb_slic3d_slab_update(C.byref(d), _lib.ptr(xchg[i]), st))
+            if i > 0:
+                _combine(lib, xchg[0].data_ptr(), xchg[i].data_ptr(), 5 * n_seeds + 1, OP_SUM_I64)
+        comm.all_reduce(xchg[0], 'sum')
+        _combine(lib, err.data_ptr(), xchg[0].data_ptr() + 8 * 5 * n_seeds, 1, OP_SUM_I64)
+        for d in descs:
+            _lib.check(lib.isb_slic3d_slab_import(C.byref(d), _lib.ptr(xchg[0]), st))
+
+    # 3) the whole k-means label volume on every GPU
+    full = eng.buf('ts_full', (D, H, W), torch.int32)
+    res.d_err = err
+    if not force_whole:
+        for i, b in enumerate(local):
+            bd = bands[b]
+            full[bd.own_lo:bd.own_hi].copy_(keep[i][1][bd.own_lo - bd.km_lo:bd.own_hi - bd.km_lo])
+        if comm.world > 1:
+            for bd in bands:
+                comm.broadcast(full[bd.own_lo:bd.own_hi], owner(bd.index))
+    if force_whole or (not defer_check and int(eng.to_host(err)[0]) != 0):
+        # some voxel kept the label of a cluster centred beyond the halo (no window covers it): the slab sums are not trustworthy,
+        # every rank redoes the sweeps on the whole volume on its own GPU
+        logging.warning('slic3d_tiled: orphan voxels beyond the halo, redoing the sweeps on the whole volume on every GPU')
+        res.fell_back = True
+        km, _ = eng.slic3d(eng.to_device(volume, 'volume'), n_segments, compactness, spacing, sigma=sigma, max_iter=max_iter,
+                           enforce_connectivity=False)
+        full.copy_(km)
+    if not enforce_connectivity:
+        res.d_seg = full
+        return res
+    res.d_seg, res.d_n_labels = eng.enforce_connectivity3d(full, n_segments, min_size_factor, max_size_factor)
+    res.nb_bound = eng.slic_label_bound(D * H * W, 1, n_segments, min_size_factor)
+    return res
+
+
+def gray_stats_tiled(res, volume_dtype, flags, comm=None, eng=None):
+    """statistics ``flags`` (of mean / std / energy, in that order) of the slab-cut volume over ``res.d_seg``, one column each, as
+    :meth:`~.engine.Engine.gray_table` lays them out: every slab accumulates its owned slices, the accumulators are summed over the
+    GPUs between the calls, every GPU finishes the same [nb, len(flags)] table"""
+    eng = eng or get_engine()
+    torch, lib = eng.torch, eng.lib
+    comm = comm or default_comm()
+    D, H, W = res.shape
+    code, itemsize = _lib.dtype_code(np.dtype(volume_dtype)), np.dtype(volume_dtype).itemsize
+    nb = int(res.nb_bound)
+    st = _lib.stream_ptr()
+    bits, _ = flag_bits(flags)
+    acc = eng.buf('ts_gacc', (nb, 2), torch.float64)
+    cnt = eng.buf('ts_gcnt', (nb,), torch.int64)
+    acc.zero_()
+    cnt.zero_()
+
+    def slices(i):
+        bd = res.bands[res.local[i]]
+        n = (bd.own_hi - bd.own_lo) * H * W
+        return (C.c_void_p(res.d_raw[i].data_ptr() + (bd.own_lo - bd.raw_lo) * H * W * itemsize),
+                C.c_void_p(res.d_seg.data_ptr() + bd.own_lo * H * W * 4), C.c_longlong(n))
+
+    for i in range(len(res.local)):
+        img, seg, n = slices(i)
+        _lib.check(lib.isb_gray_stats_accumulate(img, code, seg, n, nb, _lib.ptr(acc), _lib.ptr(cnt), st))
+    comm.all_reduce(acc, 'sum')
+    comm.all_reduce(cnt, 'sum')
+    var = None
+    if bits & 2:
+        var = eng.buf('ts_gvar', (nb,), torch.float64)
+        meanf = eng.buf('ts_gmeanf', (nb,), torch.float32)
+        var.zero_()
+        for i in range(len(res.local)):
+            img, seg, n = slices(i)
+            _lib.check(lib.isb_gray_stats_deviation(img, code, seg, n, nb, _lib.ptr(acc), _lib.ptr(cnt), _lib.ptr(meanf), _lib.ptr(var), st))
+        comm.all_reduce(var, 'sum')
+    feat = eng.buf('feat3d', (nb, len(flags)), torch.float64)
+    _lib.check(lib.isb_gray_stats_finish(nb, bits, _lib.ptr(acc), _lib.ptr(var), _lib.ptr(cnt), _lib.ptr(feat), len(flags), 0, st))
+    res.d_feat = feat
+    return feat
+
+
+def _admit_volume(dict_features):
+    """the statistic columns of a feature dictionary the slab path takes (``color`` groups' mean / std / energy, in
+    compute_selected_features_gray3d's order); NotImplementedError for any other, before any device work"""
+    from .pipelines import _volume_flags
+    flags = _volume_flags(dict_features)
+    if flags is None or 'median' in flags:
+        raise NotImplementedError('the slab path computes mean / std / energy of "color" groups of a gray volume; a median does not '
+                                  'decompose over slabs, texture and meanGrad have no volume form (got %r)' % (dict_features, ))
+    return flags
+
+
+def _prepare_volume(volume, sp_size, sp_regul, spacing, n_slabs):
+    """(host volume in a device dtype, n_segments, compactness) with the volume pipelines' argument errors"""
+    from .superpixels import _supported_dtype, slic3d_params
+    if sp_regul <= 0.:
+        raise ValueError('slic. regularisation must be positive')
+    volume = np.asarray(volume)
+    if volume.ndim != 3:
+        raise ValueError('expected a gray volume [D, H, W], got shape %r' % (volume.shape, ))
+    plan_bands(volume.shape[0], n_slabs, 1, 0)          # ValueError: more slabs than slices
+    n_seg, compact = slic3d_params(volume.shape, sp_size, sp_regul, spacing)
+    if n_seg < 1 or compact < 1:
+        raise ValueError('superpixel size %r / compactness do not fit the volume %r' % (sp_size, volume.shape))
+    return _supported_dtype(volume), n_seg, compact
+
+
+def _volume_front(eng, volume, n_seg, compact, spacing, flags, comm, bands_per_rank, force_whole):
+    """slab SLIC, the statistics table and norm_features (the device StandardScaler): (res, standardised features [nb, len(flags)])"""
+    res = slic3d_tiled(volume, n_seg, compact, spacing, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
+                       force_whole=force_whole)
+    feat = gray_stats_tiled(res, volume.dtype, flags, comm=comm, eng=eng)
+    return res, eng.standard_scaler(feat, res.d_n_labels)[0]
+
+
+def pipe_gray3d_slic_features_model_graphcut_tiled(volume, nb_classes, dict_features, spacing=(12, 1, 1), sp_size=15, sp_regul=0.2,
+                                                   gc_regul=0.1, use_scaler=True, max_iter=99, comm=None, bands_per_rank=1, want_soft=True,
+                                                   gather_segm=False):
+    """ ``pipe_gray3d_slic_features_model_graphcut`` (reference pipelines.py:382-431) for one gray volume cut into z-slabs over the
+    GPUs of ``comm``.  Every rank passes the same host volume and gets the slices it owns.  The features are mean / std / energy of
+    ``color`` groups (not median); the class model (GaussianMixture, ``sqrt(max_iter)`` restarts) is fitted on the GPU on the
+    replicated, standardised feature table, as :func:`~.pipelines.segment_resident_volume` does.
+
+    :return tuple: (segm [slices, H, W] int32, segm_soft [slices, H, W, K] float64 or None, (z_lo, z_hi)); with ``gather_segm``
+        ``segm`` is the whole [D, H, W] volume on every rank (``segm_soft`` stays sliced: it is 8*K bytes per voxel)
+    """
+    from . import graph_cuts
+    flags = _admit_volume(dict_features)
+    if not graph_cuts.device_gmm_applicable(len(flags), nb_classes):
+        raise NotImplementedError('the slab path fits the class model on the GPU, which does not take %d classes' % nb_classes)
+    kind, n_init, n_iter = graph_cuts.class_model_spec('GMM', nb_classes, max_iter)
+    comm = comm or default_comm()
+    volume, n_seg, compact = _prepare_volume(volume, sp_size, sp_regul, spacing, comm.world * int(bands_per_rank))
+    eng = get_engine()
+
+    def front(force_whole):
+        res, d_x = _volume_front(eng, volume, n_seg, compact, spacing, flags, comm, bands_per_rank, force_whole)
+        return res, graph_cuts.device_fit_predict(eng, d_x, int(nb_classes), use_scaler, kind, n_init, n_iter, None, d_n=res.d_n_labels)[0]
+
+    return _banded_segment(eng, volume.shape, comm, bands_per_rank, front, gc_regul, 'model', want_soft, gather_segm)
+
+
+def segment_gray3d_slic_features_model_graphcut_tiled(volume, model_pipeline, dict_features, spacing=(12, 1, 1), sp_size=15, sp_regul=0.2,
+                                                      gc_regul=0.1, comm=None, bands_per_rank=1, want_soft=True, gather_segm=False):
+    """ the volume pipeline with a caller-fitted model (fitted on standardised supervoxel features, as the reference's
+    pipe_gray3d_slic_features_model_graphcut feeds its model) for one gray volume cut into z-slabs over the GPUs of ``comm``.  A
+    model that ``class_models.compile_model`` takes is evaluated on the device on every rank; any other model's ``predict_proba``
+    runs on the host of every rank, on the same replicated table.  The labels are mapped through the model's ``classes_``.
+
+    :return tuple: (segm [slices, H, W], segm_soft [slices, H, W, K] float64 or None, (z_lo, z_hi)) as
+        :func:`pipe_gray3d_slic_features_model_graphcut_tiled`
+    """
+    from .pipelines import _compiled_volume_model
+    flags = _admit_volume(dict_features)
+    comm = comm or default_comm()
+    volume, n_seg, compact = _prepare_volume(volume, sp_size, sp_regul, spacing, comm.world * int(bands_per_rank))
+    classes = getattr(model_pipeline, 'classes_', None)
+    eng = get_engine()
+    compiled = _compiled_volume_model(model_pipeline, len(flags))
+
+    def front(force_whole):
+        res, d_x = _volume_front(eng, volume, n_seg, compact, spacing, flags, comm, bands_per_rank, force_whole)
+        if compiled is not None:
+            return res, eng.class_model_predict(d_x, compiled, d_n=res.d_n_labels)
+        nb = int(eng.to_host(res.d_n_labels)[0])
+        proba = np.asarray(model_pipeline.predict_proba(eng.to_host(d_x[:nb]).copy()), dtype=np.float64)
+        padded = np.zeros((int(res.nb_bound), proba.shape[1]))      # the rows of the label bound, as a device model gives
+        padded[:nb] = proba
+        return res, eng.to_device(padded, 'proba')
+
+    segm, soft, rows = _banded_segment(eng, volume.shape, comm, bands_per_rank, front, gc_regul, 'model', want_soft, gather_segm)
     if classes is not None:
         segm = np.asarray(classes)[segm]
     return segm, soft, rows
