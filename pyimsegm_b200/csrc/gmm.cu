@@ -1543,8 +1543,9 @@ static int mixture_fit_predict(const double* feat, int N, int D, int ld, const i
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// PCA fit: sklearn.decomposition.PCA with the covariance_eigh solver (the one it picks for N >= 10 D, D <= 1000 -- every superpixel
-// feature table), restated on the device:  C = (X^T X - n mu mu^T) / (n - 1) on the scaled features, symmetric eigensolver, descending
+// PCA fit: sklearn.decomposition.PCA with the covariance_eigh solver (the one its 'auto' picks for N >= 10 D, D <= 1000; with fewer
+// samples it picks the exact 'full' SVD, which this equals up to rounding), restated on the device:  C = (X^T X - n mu mu^T) / (n - 1)
+// on the scaled features, symmetric eigensolver, descending
 // order, negative eigenvalues clipped to 0, svd_flip(u_based_decision=False) on the rows of components_, explained variance ratio,
 // component count from the ratio (float pca_coef) or as given, noise variance.
 // X^T X is the split-K Gram GEMM of the mixture M-step; the eigensolver is Householder tridiagonalisation + implicit QL (the rotations
@@ -1676,16 +1677,23 @@ __global__ void __launch_bounds__(PT) k_pca_eig(int N_in, const int* n_dev, int 
         }
         __syncthreads();
     }
-    // implicit QL with shifts on (d, e): thread 0 finds the rotations of a sweep, every thread applies them to its row of Z
+    // implicit QL with shifts on (d, e): thread 0 finds the rotations of a sweep, every thread applies them to its row of Z.
+    // An off-diagonal splits the matrix when it is negligible next to its two diagonal entries or, as in EISPACK's tql2, below
+    // eps |T| (deflating it moves an eigenvalue by at most that): the relative test alone never accepts the rounding-level entries
+    // of the null space when samples are far fewer than features, and the sweeps there ran out of iterations
     {
         int l = 0, iter = 0;
-        if (tid == 0) { s_fail = 0; }
+        double anorm = 0.0;
+        if (tid == 0) { s_fail = 0; for (int i = 0; i < n; ++i) anorm = fmax(anorm, fabs(s_d[i]) + fabs(s_e[i])); }
         while (true) {
             if (tid == 0) {
                 s_nrot = 0; s_done = 0;
                 while (l < n) {
                     int mm = l;
-                    for (; mm < n - 1; ++mm) { const double dd = fabs(s_d[mm]) + fabs(s_d[mm + 1]); if (fabs(s_e[mm]) + dd == dd) break; }
+                    for (; mm < n - 1; ++mm) {
+                        const double dd = fabs(s_d[mm]) + fabs(s_d[mm + 1]);
+                        if (fabs(s_e[mm]) + dd == dd || fabs(s_e[mm]) <= DBL_EPSILON * anorm) break;
+                    }
                     if (mm == l) { ++l; iter = 0; continue; }
                     if (iter++ == 60) { s_fail = 1; ++l; iter = 0; continue; }
                     double g = (s_d[l + 1] - s_d[l]) / (2.0 * s_e[l]);
@@ -1771,8 +1779,11 @@ __global__ void __launch_bounds__(PT) k_pca_eig(int N_in, const int* n_dev, int 
             nc += 1;
         }
         nc = max(1, min(nc, n));
+        // sklearn averages explained_variance_[nc:], which has min(N, D) entries: the eigenvalues past N - 1 (zero up to rounding
+        // when samples are fewer than features) are not part of it
+        const int r = min(n, N);
         double noise = 0.0;
-        if (nc < min(n, N)) { for (int i = nc; i < n; ++i) noise += o_ev[i]; noise /= (n - nc); }
+        if (nc < r) { for (int i = nc; i < r; ++i) noise += o_ev[i]; noise /= (r - nc); }
         o_tail[0] = nc; o_tail[1] = noise; o_tail[2] = N; o_tail[3] = s_fail ? 0.0 : 1.0;
         if (n_comp_out) *n_comp_out = nc;
     }

@@ -246,9 +246,20 @@ def device_fit_predict(eng, d_feat, nb_classes, use_scaler, kind, n_init, max_it
     return proba, params, d_pca, dims
 
 
+def _check_pca_count(pca_coef, nb_samples, nb_features):
+    """ the ValueError of the reference's ``PCA(pca_coef)`` (scikit-learn's ``PCA._fit_full``) for a component count above
+    min(n_samples, n_features), raised before any device work; the message names the solver scikit-learn's 'auto' picks """
+    N, D = int(nb_samples), int(nb_features)
+    if isinstance(pca_coef, (int, np.integer)) and not isinstance(pca_coef, (bool, np.bool_)) and pca_coef > min(N, D):
+        solver = 'covariance_eigh' if D <= 1000 and N >= 10 * D else 'full'
+        raise ValueError('n_components=%d must be between 0 and min(n_samples, n_features)=%d with svd_solver=%r'
+                         % (pca_coef, min(N, D), solver))
+
+
 def fit_class_model_device(features, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef=None, init_labels=None, seed=None):
     """ the class model of a :func:`class_model_spec` triple fitted on the GPU: the same kind of object as :func:`estim_class_model` """
     features = np.ascontiguousarray(features, dtype=np.float64)
+    _check_pca_count(pca_coef, features.shape[0], features.shape[1])
     eng = get_engine()
     d_feat = eng.to_device(features, 'feat_in')
     if init_labels is not None:

@@ -107,3 +107,19 @@ def test_fit_entries_reject_bad_arguments_without_a_gpu():
     assert lib.isb_pca_fit(*args) == _lib.ISB_ERR_UNSUPPORTED and 'D <=' in err()
     assert lib.isb_pca_params_len(189) == 189 * 189 + 7 * 189 + 4
     assert lib.isb_pca_workspace_bytes(5000, 189) >= 8 * (5000 * 189 + 11 * 189 * 189)
+
+
+@pytest.mark.parametrize('N,D,k', [(30, 40, 31), (30, 40, 40), (400, 40, 41), (100, 40, 41), (2, 189, 3)])
+def test_component_count_above_min_n_d_is_sklearns_error(N, D, k):
+    """an integer pca_coef above min(N, D) raises the ValueError of the reference's PCA(pca_coef), message included, in the device
+    fit's entry before any device work (so also on a machine without a GPU)"""
+    from sklearn import decomposition
+    from pyimsegm_b200 import graph_cuts as gc
+    X = np.random.RandomState(N + D).normal(size=(N, D))
+    with pytest.raises(ValueError) as ref:
+        decomposition.PCA(k).fit(X)
+    with pytest.raises(ValueError) as dev:
+        gc.fit_class_model_device(X, 2, True, 'GMM', 1, 10, k)
+    assert str(dev.value) == str(ref.value)
+    gc._check_pca_count(min(N, D), N, D)
+    gc._check_pca_count(0.95, N, D)

@@ -3,7 +3,9 @@ the edges of its kernels: the thread-block cluster size of the single-kernel pat
 <= 4096, <= 16384 and above), the feature widths around DMAX = 16, the 32-feature scaler blocks, the 96-wide GEMM tiles and DBIG = 232,
 the class counts 1, 2 and KMAX = 8, the sample counts of the large-D E-step (8 per CTA), GEMM rows (96) and split-K Gram ranges,
 a device-side sample count below the buffer height, the device's own k-means++ start (bit for bit), the choice among restarts, failed
-restarts and degenerate inputs.
+restarts and degenerate inputs.  Every case but the failed restarts runs for both kinds, GaussianMixture and
+BayesianGaussianMixture (BGM: digamma terms, Dirichlet-process weights, the priors, the ELBO as convergence and restart criterion);
+the BGM's covariance prior keeps every covariance positive definite, so a BGM restart cannot fail.
 
 Tolerances are those of the other shared-start tests: scaler rtol 1e-12; weights, means and covariances rtol 1e-6, atol 1e-8; lower
 bound rtol 1e-8; n_iter_ and converged_ exact; predict_proba rtol 1e-5, atol 1e-9."""
@@ -16,6 +18,14 @@ from sklearn import preprocessing
 from oracle import mixture as om
 
 pytestmark = pytest.mark.gpu
+
+
+def _with_bgm(cases, bgm_cases=None):
+    """parameters (kind, *case): the GaussianMixture cases under the ids they had before the kind was a parameter, then the
+    BayesianGaussianMixture cases (by default the same) with ids prefixed 'BGM-'"""
+    name = lambda c: '-'.join(map(str, c))  # noqa: E731
+    return ([pytest.param('GMM', *c, id=name(c)) for c in cases]
+            + [pytest.param('BGM', *c, id='BGM-' + name(c)) for c in (cases if bgm_cases is None else bgm_cases)])
 
 
 def _blobs(D, K, n, seed, inform=0.6):
@@ -106,17 +116,16 @@ def test_cluster_sizes_match_sklearn(kind, D, N):
 # ---- feature widths and class counts --------------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize('kind,D', [('GMM', d) for d in (1, 2, 15, 16, 17, 32, 33, 95, 96, 97, 192, 193, 232)]
-                         + [('BGM', d) for d in (1, 17, 232)])
+                         + [('BGM', d) for d in (1, 2, 15, 16, 17, 33, 96, 97, 193, 232)])
 def test_dimensions_match_sklearn(kind, D):
     X, _, y0 = _blobs(D, 3, 3000 if D <= 33 else 1500, seed=3 * D + 1)
     _compare(X, y0, 3, kind)
 
 
-@pytest.mark.parametrize('K', [1, 2, 8])
-@pytest.mark.parametrize('D', [9, 189])
-def test_class_counts_match_sklearn(D, K):
+@pytest.mark.parametrize('kind,D,K', _with_bgm([(D, K) for D in (9, 189) for K in (1, 2, 8)]))
+def test_class_counts_match_sklearn(kind, D, K):
     X, _, y0 = _blobs(D, K, 3000 if D <= 16 else 1500, seed=D + 11 * K)
-    _compare(X, y0, K, max_iter=99 if D <= 16 else 15)
+    _compare(X, y0, K, kind, max_iter=99 if D <= 16 else 15)
 
 
 def test_unsupported_sizes_are_refused_and_fit_on_the_host(monkeypatch):
@@ -155,8 +164,9 @@ def test_large_d_sample_counts_match_sklearn(N):
 
 # ---- a device-side sample count below the buffer height --------------------------------------------------------------------------
 
-@pytest.mark.parametrize('D,N_in,n_dev', [(3, 4000, 3000), (3, 20000, 700), (3, 20000, 21), (40, 4000, 3000), (40, 20000, 700)])
-def test_rows_past_n_dev_are_not_samples(D, N_in, n_dev):
+@pytest.mark.parametrize('kind,D,N_in,n_dev', _with_bgm([(3, 4000, 3000), (3, 20000, 700), (3, 20000, 21), (40, 4000, 3000),
+                                                        (40, 20000, 700)]))
+def test_rows_past_n_dev_are_not_samples(kind, D, N_in, n_dev):
     """the buffer holds N_in rows, the device count n_dev; the rows past it are NaN.  The fit must be the one of the first n_dev
     rows; when the cluster size does not change (same CL bucket, or the large-D path, whose launches follow n_dev) bit for bit"""
     X, _, y0 = _blobs(D, 3, n_dev, seed=n_dev + D)
@@ -166,11 +176,11 @@ def test_rows_past_n_dev_are_not_samples(D, N_in, n_dev):
     y0p[:n_dev] = y0
     cl = lambda n: 1 if n <= 1024 else 2 if n <= 4096 else 4 if n <= 16384 else 8  # noqa: E731
     same = D > 16 or cl(N_in) == cl(n_dev)
-    proba, params = _fit(Xp, 3, init=y0p, n_dev=n_dev)
+    proba, params = _fit(Xp, 3, kind, init=y0p, n_dev=n_dev)
     assert np.isfinite(proba).all()
     Z = preprocessing.StandardScaler().fit_transform(X)
-    _check(params, proba, X, om.shared_start_fit(Z, y0, 3), 3)
-    proba1, params1 = _fit(X, 3, init=y0)
+    _check(params, proba, X, om.shared_start_fit(Z, y0, 3, kind), 3, kind)
+    proba1, params1 = _fit(X, 3, kind, init=y0)
     if same:
         assert np.array_equal(params, params1) and np.array_equal(proba, proba1)
     # the device's own start, 9 restarts: equal to the oracle's k-means++ labels of the first n_dev rows handed in as init_labels
@@ -178,11 +188,11 @@ def test_rows_past_n_dev_are_not_samples(D, N_in, n_dev):
     assert min(least.values()) > 1e-9, least
     Yp = np.zeros((9, N_in), np.int32)
     Yp[:, :n_dev] = Y
-    proba2, params2 = _fit(Xp, 3, n_init=9, n_dev=n_dev)
-    proba3, params3 = _fit(Xp, 3, init=Yp, n_dev=n_dev)
+    proba2, params2 = _fit(Xp, 3, kind, n_init=9, n_dev=n_dev)
+    proba3, params3 = _fit(Xp, 3, kind, init=Yp, n_dev=n_dev)
     assert np.array_equal(params2, params3) and np.array_equal(proba2, proba3)
     if same:
-        assert np.array_equal(params2, _fit(X, 3, n_init=9)[1])
+        assert np.array_equal(params2, _fit(X, 3, kind, n_init=9)[1])
 
 
 # ---- the device's k-means++ / Lloyd start, exactly -------------------------------------------------------------------------------
@@ -196,11 +206,12 @@ def _overlapping(D, K, n, seed):
 
 
 @pytest.mark.parametrize('seed', [0, 1, 7])
-@pytest.mark.parametrize('D,N,K', [(3, 500, 3), (3, 3000, 3), (3, 20000, 3), (40, 500, 3), (40, 3000, 3), (16, 3000, 8)])
-def test_device_kmeanspp_start_is_the_oracle_start(D, N, K, seed):
+@pytest.mark.parametrize('kind,D,N,K', _with_bgm([(3, 500, 3), (3, 3000, 3), (3, 20000, 3), (40, 500, 3), (40, 3000, 3), (16, 3000, 8)]))
+def test_device_kmeanspp_start_is_the_oracle_start(kind, D, N, K, seed):
     """9 restarts from the device's own start against the same fit from the oracle's restatement of that start: the EM from equal
     labels is one deterministic kernel, so the two parameter vectors are equal bit for bit exactly when every restart drew the
-    same centres and ended Lloyd with the same labels.  (16, 3000, 8) is the widest Lloyd exchange of the single kernel."""
+    same centres and ended Lloyd with the same labels.  (16, 3000, 8) is the widest Lloyd exchange of the single kernel.  The
+    'BGM' variant of estim_class_model runs its 9 restarts from the same start."""
     X = _overlapping(D, K, N, seed=100 + N + D)
     Z = preprocessing.StandardScaler().fit_transform(X)
     Y, least = om.kmeanspp_starts(Z, K, seed, 9)
@@ -208,19 +219,18 @@ def test_device_kmeanspp_start_is_the_oracle_start(D, N, K, seed):
     # drawn for the wrong restart changes the exported vector, whose last slot is the winner's index)
     assert min(least.values()) > 1e-9, least
     assert len({r.tobytes() for r in Y}) == 9
-    proba, params = _fit(X, K, n_init=9, seed=seed)
-    proba_o, params_o = _fit(X, K, init=Y, seed=seed)
+    proba, params = _fit(X, K, kind, n_init=9, seed=seed)
+    proba_o, params_o = _fit(X, K, kind, init=Y, seed=seed)
     assert np.array_equal(params, params_o), 'exported restart %d (oracle start: %d)' % (_best_index(params, D, K), _best_index(params_o, D, K))
     assert np.array_equal(proba, proba_o)
 
 
 # ---- the choice among restarts, failed restarts ----------------------------------------------------------------------------------
 
-@pytest.mark.parametrize('case', ['quality', 'tie'])
-@pytest.mark.parametrize('D', [3, 40])
-def test_restart_choice_is_sklearns(D, case):
-    """four EM iterations from starts of different quality: the device exports the restart with the largest lower bound, the first
-    one on a tie (sklearn's strict >), with that restart's n_iter_, converged_ and lower bound"""
+@pytest.mark.parametrize('kind,D,case', _with_bgm([(D, case) for D in (3, 40) for case in ('quality', 'tie')]))
+def test_restart_choice_is_sklearns(kind, D, case):
+    """four EM iterations from starts of different quality: the device exports the restart with the largest lower bound (the
+    ELBO for the BGM), the first one on a tie (sklearn's strict >), with that restart's n_iter_, converged_ and lower bound"""
     X, y, _ = _blobs(D, 3, 2000, seed=D + 5)
     rng = np.random.RandomState(D)
     start = lambda f: np.where(rng.rand(len(y)) < f, y, rng.randint(0, 3, len(y))).astype(np.int32)  # noqa: E731
@@ -228,13 +238,13 @@ def test_restart_choice_is_sklearns(D, case):
     if case == 'tie':
         Y0[2] = Y0[1]
     Z = preprocessing.StandardScaler().fit_transform(X)
-    best, ref, lowers = om.shared_start_best(Z, Y0, 3, max_iter=4)
+    best, ref, lowers = om.shared_start_best(Z, Y0, 3, kind, max_iter=4)
     runner_up = max(lb for i, lb in enumerate(lowers) if i != best and lb != lowers[best])
     assert lowers[best] - runner_up > 1e-6 * abs(lowers[best]), lowers
     assert best == 1
-    proba, params = _fit(X, 3, init=Y0, max_iter=4)
+    proba, params = _fit(X, 3, kind, init=Y0, max_iter=4)
     assert _best_index(params, D, 3) == best
-    _check(params, proba, X, ref, 3)
+    _check(params, proba, X, ref, 3, kind)
 
 
 def _failing_start(D, seed):
@@ -276,32 +286,32 @@ def test_every_restart_failed(D):
 
 # ---- degenerate inputs ------------------------------------------------------------------------------------------------------------
 
-@pytest.mark.parametrize('case', ['empty_component', 'constant_columns', 'no_scaler', 'one_iteration'])
-@pytest.mark.parametrize('D', [5, 40])
-def test_degenerate_inputs_match_sklearn(D, case):
+@pytest.mark.parametrize('kind,D,case', _with_bgm([(D, case) for D in (5, 40)
+                                                   for case in ('empty_component', 'constant_columns', 'no_scaler', 'one_iteration')]))
+def test_degenerate_inputs_match_sklearn(kind, D, case):
     X, y, y0 = _blobs(D, 3, 2500, seed=D + len(case))
     Z = preprocessing.StandardScaler().fit_transform(X)
     if case == 'empty_component':
         y0 = np.where(y0 == 2, 1, y0).astype(np.int32)             # component 2 has no member: nk = 10 eps, covariance reg_covar I
-        _compare(X, y0, 3)
+        _compare(X, y0, 3, kind)                                   # (for the BGM: the covariance prior)
     elif case == 'constant_columns':
         X[:, 1], X[:, 3] = 0.1, 2.5                                # scale 1, the centred column rounding noise (0.1) or exactly 0
-        proba, params = _fit(X, 3, init=y0)
+        proba, params = _fit(X, 3, kind, init=y0)
         assert params[D + 1] == 1.0 and params[D + 3] == 1.0
         Z = preprocessing.StandardScaler().fit_transform(X)
-        _check(params, proba, X, om.shared_start_fit(Z, y0, 3), 3)
+        _check(params, proba, X, om.shared_start_fit(Z, y0, 3, kind), 3, kind)
     elif case == 'no_scaler':
-        proba, params = _fit(X, 3, init=y0, use_scaler=False)
-        _check(params, proba, X, om.shared_start_fit(X, y0, 3), 3, use_scaler=False)
+        proba, params = _fit(X, 3, kind, init=y0, use_scaler=False)
+        _check(params, proba, X, om.shared_start_fit(X, y0, 3, kind), 3, kind, use_scaler=False)
     else:
         # the 'kmeans' variant's shape: 9 restarts, one iteration each, never converged
         rng = np.random.RandomState(D)
         Y0 = np.stack([np.where(rng.rand(len(y)) < f, y, rng.randint(0, 3, len(y))) for f in np.linspace(0.1, 0.5, 9)]).astype(np.int32)
-        best, ref, lowers = om.shared_start_best(Z, Y0, 3, max_iter=1)
+        best, ref, lowers = om.shared_start_best(Z, Y0, 3, kind, max_iter=1)
         assert sorted(lowers)[-1] - sorted(lowers)[-2] > 1e-6 * abs(lowers[best]), lowers
-        proba, params = _fit(X, 3, init=Y0, max_iter=1)
+        proba, params = _fit(X, 3, kind, init=Y0, max_iter=1)
         assert _best_index(params, D, 3) == best
-        _check(params, proba, X, ref, 3)
+        _check(params, proba, X, ref, 3, kind)
         assert ref.n_iter_ == 1 and not ref.converged_
 
 
