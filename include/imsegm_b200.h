@@ -350,7 +350,9 @@ int isb_centroids_3d(const int32_t* seg, int D, int H, int W, int nb, double* ce
 /* compute_unary_cost (imsegm/graph_cuts.py:523-540), compute_edge_weights / compute_edge_model / compute_spatial_dist
  * (:574-657, :383-439, :303-336), create_pairwise_matrix_uniform (:442-456), and pyGCO's float->int conversion.
  *   proba [N,K] f64, edges [E,2] i32 (n_edges read from device n_edges_dev when non-null, else E), centres [N,2] or [N,3] f64
- *   metric : 0 = constant 1, 1 = lT (max_k dp^2), 2 = l1, 3 = l2   -> w = exp(-d / (2 std(d)^2))
+ *   metric : 0 = constant 1, 1 = lT (max_k dp^2), 2 = l1, 3 = l2   -> w = exp(-d / (2 std(d)^2));
+ *            4 = edge_w already holds the clamped weights (isb_gc_vector_edge_weights): only edge_cost and the integerisation
+ *            are applied (spatial must be 0)
  *   spatial: 0 = off; 1 (or 2) = divide by the relative centroid distance over centres (y, x) [N,2] of a label map, 3 = the same
  *            over centres (z, y, x) [N,3] of a label volume (isb_centroids_3d).  The reference does so for edge_type 'model' and
  *            'spatial' exactly, not for 'model_l1' / 'model_l2' (graph_cuts.py:646)
@@ -361,6 +363,20 @@ int isb_gc_energies(const double* proba, int N, const int32_t* n_nodes_dev /* op
                     double* unary, double* edge_w, int32_t* unary_i, int32_t* edge_wi, int32_t* smooth_i, void* ws,
                     size_t ws_bytes, isb_stream_t stream);
 size_t isb_gc_energies_workspace_bytes(int N, int K, int E);
+
+/* the 'color' and 'features' edge weights of compute_edge_weights (imsegm/graph_cuts.py:621-657) over a device edge table:
+ *   vec [nb, ld] f64 (first D columns): the per-label vectors, edges [cap, 2] i32 with the count in the optional device n_edges_dev
+ *   (an overflowed table, count > cap, reads no edge), centres [nb, 2] (y, x) f64
+ *   metric 2: d = L1 distance of the endpoints' vectors ('color'), 3: L2 distance ('features')
+ *   edge_w [cap] f64 out: w = exp(-(d / (2 std(d)^2))) with numpy's population std over the real edges (two deterministic passes,
+ *   no host read; std 0 gives numpy's NaN / inf), divided by the relative centroid distance of 'spatial', clamped to [1e-3, 1e3]
+ *   by comparisons (NaN stays NaN).  isb_gc_energies with metric 4 then integerises edge_w in place.
+ *   ws: isb_gc_energies_workspace_bytes(nb, 1, cap) */
+int isb_gc_vector_edge_weights(const double* vec, int nb, int D, int ld, const int32_t* edges, int cap, const int32_t* n_edges_dev,
+                               const double* centres, int metric, double* edge_w, void* ws, size_t ws_bytes, isb_stream_t stream);
+/* np.array(img, dtype=float) of n samples, divided by 255 when minmax[1] (device; isb_image_minmax's maximum) > 1: the image
+ * compute_edge_weights takes the 'color' means of.  A NaN maximum compares false and leaves the image unscaled, as np.max does. */
+int isb_image_unit_scale(const void* img, int dtype, long long n, const double* minmax, double* out, isb_stream_t stream);
 
 /* gco.cut_general_graph(..., algorithm='expansion', n_iter) on integer energies (imsegm/graph_cuts.py:735-744).
  * One CTA cluster per graph; push-relabel max-flow; a site keeps its label iff it can reach the sink in the

@@ -85,6 +85,8 @@ SIGNATURES = {
     'isb_gc_energies_workspace_bytes': (_sz, [_i, _i, _i]),
     'isb_standard_scaler': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'isb_gc_energies': (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _d, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    'isb_gc_vector_edge_weights': (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _sz, _vp]),
+    'isb_image_unit_scale': (_i, [_vp, _i, _ll, _vp, _vp, _vp]),
     'isb_alpha_expansion_workspace_bytes': (_sz, [_i, _i, _i]),
     'isb_alpha_expansion': (_i, [_i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     'isb_mixture_fit_workspace_bytes': (_sz, [_i, _i, _i, _i, _i]),

@@ -6,7 +6,8 @@
 //   imsegm/graph_cuts.py:303-336   compute_spatial_dist (centres (y, x) of a label map, (z, y, x) of a label volume)
 //   imsegm/graph_cuts.py:383-439   compute_edge_model
 //   imsegm/graph_cuts.py:523-540   compute_unary_cost
-//   imsegm/graph_cuts.py:574-657   compute_edge_weights (clamp to [1e-3, 1e3])
+//   imsegm/graph_cuts.py:574-657   compute_edge_weights (clamp to [1e-3, 1e3]; 'color' / 'features' vectors compared by
+//                                  isb_gc_vector_edge_weights, the 'color' image scaled by isb_image_unit_scale)
 //   pyGCO cut_general_graph        float -> int conversion (see oracle/gc_oracle.cpp header)
 //   imsegm/pipelines.py:104,109    proba[slic], graph_labels[slic]
 #include "common.cuh"
@@ -230,6 +231,9 @@ __device__ double block_max(double v, double* s_red)
 }
 
 constexpr int ECL = 8;   // CTAs of the energy kernel's thread-block cluster
+// The cluster kernels below declare __launch_bounds__(1024, 1): with the thread bound alone, nvcc 12.9 gives k_gc_energies 32 registers
+// and 56 bytes of spills; with one CTA per SM stated it takes 64 registers and spills nothing.  1024 threads
+// at 64 registers fill an SM's register file, so such a CTA runs alone on its SM either way.
 
 // the four global quantities of the energy construction (largest unary, mean / deviation of the edge distances, largest weight) are
 // reduced over the cluster through distributed shared memory: partials added / compared in rank order, the same value in every CTA
@@ -245,38 +249,21 @@ __device__ double cluster_reduce(double v, bool is_max, double* s_red, double* s
     return tot;
 }
 
-// one cluster of ECL CTAs per graph.  vfeat [N, D]: the per-vertex vectors the edge metric compares (proba for 'model').
-__global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024) k_gc_energies(const double* __restrict__ proba, int N_in, const int* n_nodes_dev, int K, const int* __restrict__ edges, int E_in,
-                                                      const int* n_edges_dev, const double* __restrict__ centres,
-                                                      const double* __restrict__ vfeat, int D, int metric, int spatial,
-                                                      double edge_cost, const double* __restrict__ pairwise, double* unary,
-                                                      double* edge_w, int* unary_i, int* edge_wi, int* smooth_i, double* sp)
+// the clamped weight of every edge (reference graph_cuts.py:574-657) into edge_w [E], run by every thread of the cluster: the distance
+// of the two endpoints' rows of vfeat [., ld] by `metric` (0 none, 1 lT, 2 l1, 3 l2), w = exp(-d / (2 std(d)^2)) with numpy's
+// population std (mean first, then the mean of the squared deviations, each reduced over the cluster), divided by the relative
+// centroid distance when `spatial` is set, clamped to [1e-3, 1e3] by comparisons that leave a NaN weight NaN.  sp [E]: scratch.
+__device__ __forceinline__ void cluster_edge_weights(const int* __restrict__ edges, int E, const double* __restrict__ centres, const double* __restrict__ vfeat,
+                                     int D, int ld, int metric, int spatial, double* edge_w, double* sp, double* s_red, double* s_x, int tid,
+                                     int nth)
 {
-    __shared__ double s_red[32];
-    __shared__ double s_x;
-    const int tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;   // the cluster is the whole grid
-    // an overflowed edge table (count > capacity) holds unspecified rows: no edge is read, the host redoes the image
-    const int E = n_edges_dev ? (*n_edges_dev > E_in ? 0 : *n_edges_dev) : E_in;
-    const int N = n_nodes_dev ? min(*n_nodes_dev, N_in) : N_in;
-    // unary = |-log(clip(p, 0.01, 0.99))|
-    double umax = 0.0;
-    for (int i = tid; i < N * K; i += nth) {
-        double p = proba[i];
-        if (p < 0.01) p = 0.01;
-        if (p > 1.0 - 0.01) p = 1.0 - 0.01;
-        double u = fabs(-log(p));
-        unary[i] = u;
-        umax = fmax(umax, fabs(u));
-    }
-    umax = cluster_reduce(umax, true, s_red, &s_x);
-    // edge distances
     double dsum = 0.0, ssum = 0.0;
     for (int e = tid; e < E; e += nth) {
         int a = edges[2 * e], b = edges[2 * e + 1];
         double dist = 0.0;
         if (metric != 0) {
-            const double* va = vfeat + (size_t)a * D;
-            const double* vb = vfeat + (size_t)b * D;
+            const double* va = vfeat + (size_t)a * ld;
+            const double* vb = vfeat + (size_t)b * ld;
             for (int k = 0; k < D; ++k) {
                 double df = va[k] - vb[k];
                 if (metric == 1) dist = fmax(dist, df * df);        // lT: max_k (dp)^2
@@ -300,22 +287,59 @@ __global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024) k_gc_energie
             ssum += s;
         }
     }
-    dsum = cluster_reduce(dsum, false, s_red, &s_x);
-    ssum = cluster_reduce(ssum, false, s_red, &s_x);
+    dsum = cluster_reduce(dsum, false, s_red, s_x);
+    ssum = cluster_reduce(ssum, false, s_red, s_x);
     const double dmean = E > 0 ? dsum / E : 0.0, smean = E > 0 ? ssum / E : 1.0;
     double vsum = 0.0;
     if (metric != 0)
         for (int e = tid; e < E; e += nth) { double t = edge_w[e] - dmean; vsum += t * t; }
-    vsum = cluster_reduce(vsum, false, s_red, &s_x);
+    vsum = cluster_reduce(vsum, false, s_red, s_x);
     const double sd = sqrt(E > 0 ? vsum / E : 0.0);
     const double denom = 2.0 * (sd * sd);
-    double wmax = 0.0;
     for (int e = tid; e < E; e += nth) {
         double wv = metric != 0 ? exp(-edge_w[e] / denom) : 1.0;
         if (spatial) wv = wv / (sp[e] / smean);
         if (wv < 1e-3) wv = 1e-3;
         if (wv > 1e3) wv = 1e3;
-        wv *= edge_cost;
+        edge_w[e] = wv;
+    }
+}
+
+// an overflowed edge table (count > capacity) holds unspecified rows: no edge is read, the host redoes the image
+__device__ __forceinline__ int edge_count(const int* n_edges_dev, int E_in)
+{
+    return n_edges_dev ? (*n_edges_dev > E_in ? 0 : *n_edges_dev) : E_in;
+}
+
+constexpr int METRIC_GIVEN = 4;   // edge_w already holds the clamped weights (isb_gc_vector_edge_weights)
+
+// one cluster of ECL CTAs per graph.  vfeat [N, D]: the per-vertex vectors the edge metric compares (proba for 'model').
+__global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024, 1) k_gc_energies(const double* __restrict__ proba, int N_in, const int* n_nodes_dev, int K, const int* __restrict__ edges, int E_in,
+                                                      const int* n_edges_dev, const double* __restrict__ centres,
+                                                      const double* __restrict__ vfeat, int D, int metric, int spatial,
+                                                      double edge_cost, const double* __restrict__ pairwise, double* unary,
+                                                      double* edge_w, int* unary_i, int* edge_wi, int* smooth_i, double* sp)
+{
+    __shared__ double s_red[32];
+    __shared__ double s_x;
+    const int tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;   // the cluster is the whole grid
+    const int E = edge_count(n_edges_dev, E_in);
+    const int N = n_nodes_dev ? min(*n_nodes_dev, N_in) : N_in;
+    // unary = |-log(clip(p, 0.01, 0.99))|
+    double umax = 0.0;
+    for (int i = tid; i < N * K; i += nth) {
+        double p = proba[i];
+        if (p < 0.01) p = 0.01;
+        if (p > 1.0 - 0.01) p = 1.0 - 0.01;
+        double u = fabs(-log(p));
+        unary[i] = u;
+        umax = fmax(umax, fabs(u));
+    }
+    umax = cluster_reduce(umax, true, s_red, &s_x);
+    if (metric != METRIC_GIVEN) cluster_edge_weights(edges, E, centres, vfeat, D, D, metric, spatial, edge_w, sp, s_red, &s_x, tid, nth);
+    double wmax = 0.0;
+    for (int e = tid; e < E; e += nth) {
+        const double wv = edge_w[e] * edge_cost;
         edge_w[e] = wv;
         wmax = fmax(wmax, fabs(wv));
     }
@@ -329,6 +353,19 @@ __global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024) k_gc_energie
     // edge_w as in the reference, fmax above kept it out of wmax, and its capacity is 0 (graph_cuts.integerise_energies on the host)
     for (int e = tid; e < E; e += nth) { const double wv = edge_w[e]; edge_wi[e] = isnan(wv) ? 0 : (int)((wv / dwf) * 1000.0); }
     for (int i = tid; i < K * K; i += nth) smooth_i[i] = (int)(pairwise[i] * 100.0);
+}
+
+// the 'color' / 'features' weights of compute_edge_weights over one graph (the energy kernel's cluster, without the energies)
+__global__ void __cluster_dims__(ECL, 1, 1) __launch_bounds__(1024, 1) k_vector_edge_weights(const double* __restrict__ vec, int D, int ld,
+                                                                                          const int* __restrict__ edges, int E_in,
+                                                                                          const int* n_edges_dev,
+                                                                                          const double* __restrict__ centres, int metric,
+                                                                                          double* edge_w, double* sp)
+{
+    __shared__ double s_red[32];
+    __shared__ double s_x;
+    const int tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
+    cluster_edge_weights(edges, edge_count(n_edges_dev, E_in), centres, vec, D, ld, metric, 1, edge_w, sp, s_red, &s_x, tid, nth);
 }
 
 // ------------------------------------------------------------------ gathers --------------------------------------------------------
@@ -458,13 +495,47 @@ extern "C" int isb_gc_energies(const double* proba, int N, const int32_t* n_node
 {
     ISB_REQUIRE(proba && edges && pairwise && unary && edge_w && unary_i && edge_wi && smooth_i && ws, "null pointer");
     ISB_REQUIRE(N > 0 && K > 0 && E >= 0, "bad sizes");
-    ISB_REQUIRE(metric >= 0 && metric <= 3, "metric must be 0..3");
+    ISB_REQUIRE(metric >= 0 && metric <= METRIC_GIVEN, "metric must be 0..4");
+    ISB_REQUIRE(metric != METRIC_GIVEN || !spatial, "given edge weights (metric 4) are already spatially normalised: spatial must be 0");
     ISB_REQUIRE(spatial >= 0 && spatial <= 3, "spatial must be 0 (off), 1 or 2 (centres [N, 2]) or 3 (centres [N, 3])");
     ISB_REQUIRE(!spatial || centres, "centres are required for spatially normalised edge weights");
     ISB_REQUIRE(ws_bytes >= isb_gc_energies_workspace_bytes(N, K, E), "workspace too small");
     ProfScope prof(ISB_PROF_ENERGY, (cudaStream_t)stream);
     k_gc_energies<<<ECL, 1024, 0, (cudaStream_t)stream>>>(proba, N, n_nodes_dev, K, edges, E, n_edges_dev, centres, proba, K, metric, spatial, edge_cost,
                                                          pairwise, unary, edge_w, unary_i, edge_wi, smooth_i, (double*)ws);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+extern "C" int isb_gc_vector_edge_weights(const double* vec, int nb, int D, int ld, const int32_t* edges, int cap, const int32_t* n_edges_dev,
+                                          const double* centres, int metric, double* edge_w, void* ws, size_t ws_bytes, isb_stream_t stream)
+{
+    ISB_REQUIRE(vec && edges && centres && edge_w && ws, "null pointer");
+    ISB_REQUIRE(nb > 0 && D > 0 && cap > 0, "bad sizes");
+    ISB_REQUIRE(ld >= D, "ld must be >= D");
+    ISB_REQUIRE(metric == 2 || metric == 3, "metric must be 2 (l1, 'color') or 3 (l2, 'features')");
+    ISB_REQUIRE(ws_bytes >= isb_gc_energies_workspace_bytes(nb, 1, cap), "workspace too small");
+    ProfScope prof(ISB_PROF_ENERGY, (cudaStream_t)stream);
+    k_vector_edge_weights<<<ECL, 1024, 0, (cudaStream_t)stream>>>(vec, D, ld, edges, cap, n_edges_dev, centres, metric, edge_w, (double*)ws);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+// np.array(image, dtype=float), divided by 255 when max(image) > 1 (compute_edge_weights' 'color' vectors): max from minmax[1] on the
+// device, so a NaN maximum (numpy's np.max of an image with a NaN) compares false and leaves the image unscaled
+__global__ void k_unit_scale(const void* img, int dtype, long long n, const double* minmax, double* out)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double v = load_as_f64(img, dtype, (size_t)i);
+    out[i] = minmax[1] > 1.0 ? v / 255.0 : v;
+}
+
+extern "C" int isb_image_unit_scale(const void* img, int dtype, long long n, const double* minmax, double* out, isb_stream_t stream)
+{
+    ISB_REQUIRE(img && minmax && out && n > 0, "bad arguments");
+    ISB_REQUIRE(dtype >= ISB_U8 && dtype <= ISB_F64, "bad dtype");
+    k_unit_scale<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(img, dtype, n, minmax, out);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }

@@ -16,6 +16,10 @@ FLAG_BITS = {'mean': 1, 'std': 2, 'energy': 4}
 #: edge_type -> (metric, spatial) of isb_gc_energies; only 'model' and 'spatial' are spatially normalised
 #: (reference graph_cuts.py:646)
 EDGE_MODES = {'': (0, 0), 'model': (1, 1), 'model_lT': (1, 0), 'model_l1': (2, 0), 'model_l2': (3, 0), 'spatial': (0, 1)}
+#: edge_type -> metric of isb_gc_vector_edge_weights, which compares per-label vectors (the mean colours: L1, the standardised
+#: features: L2) into weights that isb_gc_energies then takes as given (:data:`EDGE_GIVEN`)
+VECTOR_EDGE_METRICS = {'color': 2, 'features': 3}
+EDGE_GIVEN = (4, 0)
 
 #: initial capacity of a device edge table, in edges per node (per upper bound of the label count) of a 2-D label map, twice
 #: that for a volume; grown x4 whenever a table overflows.  The device then reports cap + 1 edges and writes no row past cap.
@@ -378,13 +382,13 @@ class Engine(object):
                                                list(flags).index('median'), _lib.ptr(ws), C.c_size_t(wsb), st))
         return feat
 
-    def standard_scaler(self, d_feat, d_n=None):
+    def standard_scaler(self, d_feat, d_n=None, names=('feat_scaled', 'scaler_params')):
         """sklearn StandardScaler().fit_transform of device features [N, D] bit for bit (isb_standard_scaler; the real row count
-        from the device ``d_n``): returns (scaled [N, D], mean_ | scale_ [2 D]) device tensors"""
+        from the device ``d_n``): returns (scaled [N, D], mean_ | scale_ [2 D]) device tensors, in the cached buffers ``names``"""
         torch = self.torch
         N, D = int(d_feat.shape[0]), int(d_feat.shape[1])
-        out = self.buf('feat_scaled', (N, D), torch.float64)
-        params = self.buf('scaler_params', (2 * D, ), torch.float64)
+        out = self.buf(names[0], (N, D), torch.float64)
+        params = self.buf(names[1], (2 * D, ), torch.float64)
         self._ck(self.lib.isb_standard_scaler(_lib.ptr(d_feat), N, D, int(d_feat.stride(0)), _lib.ptr(d_n), _lib.ptr(params), _lib.ptr(out),
                                               _lib.stream_ptr()))
         return out, params
@@ -477,16 +481,22 @@ class Engine(object):
                                          C.c_size_t(wsb), _lib.stream_ptr()))
         return edges, n_edges, cap
 
-    def gc_energies(self, d_proba, d_edges, E, d_n_edges, d_centres, edge_mode, edge_cost, pairwise, d_n_nodes=None):
-        """isb_gc_energies; centres [N, 3] (z, y, x) of a label volume take its 3-D spatial mode, centres [N, 2] the 2-D one"""
+    def gc_energies(self, d_proba, d_edges, E, d_n_edges, d_centres, edge_mode, edge_cost, pairwise, d_n_nodes=None, edge_w=None):
+        """isb_gc_energies; centres [N, 3] (z, y, x) of a label volume take its 3-D spatial mode, centres [N, 2] the 2-D one.
+        :data:`EDGE_GIVEN` integerises the weights ``edge_w`` [>= E] (:meth:`vector_edge_weights`), which it then scales in place."""
         torch, lib = self.torch, self.lib
+        if (tuple(edge_mode) == EDGE_GIVEN) != (edge_w is not None):
+            raise ValueError('the given-weights mode %r takes the weights as edge_w, and only it does' % (EDGE_GIVEN, ))
+        if edge_w is not None and (edge_w.dtype != torch.float64 or not edge_w.is_contiguous() or edge_w.numel() < max(int(E), 1)):
+            raise ValueError('edge_w must be a contiguous float64 tensor of at least %d weights' % max(int(E), 1))
         spatial = int(edge_mode[1])
         if spatial and d_centres is not None and d_centres.dim() == 2 and int(d_centres.shape[1]) == 3:
             spatial = 3
         N, K = int(d_proba.shape[0]), int(d_proba.shape[1])
         d_pw = self.const_device(np.ascontiguousarray(pairwise, dtype=np.float64), 'pairwise')
         unary = self.buf('unary', (N, K), torch.float64)
-        edge_w = self.buf('edge_w', (max(E, 1),), torch.float64)
+        if edge_w is None:
+            edge_w = self.buf('edge_w', (max(E, 1),), torch.float64)
         unary_i = self.buf('unary_i', (N, K), torch.int32)
         edge_wi = self.buf('edge_wi', (max(E, 1),), torch.int32)
         smooth_i = self.buf('smooth_i', (K, K), torch.int32)
@@ -497,6 +507,32 @@ class Engine(object):
                                      _lib.ptr(unary_i), _lib.ptr(edge_wi), _lib.ptr(smooth_i), _lib.ptr(ws), C.c_size_t(wsb),
                                      _lib.stream_ptr()))
         return unary, edge_w, unary_i, edge_wi, smooth_i
+
+    def unit_scaled_image(self, d_img):
+        """np.array(image, dtype=float), divided by 255 when np.max(image) > 1, of a device image: the image whose mean colours
+        compute_edge_weights compares for 'color'.  The maximum is reduced on the device (isb_image_minmax, numpy's NaN rule) and
+        never read back.  Returns an f64 cached buffer of the image's shape."""
+        torch, lib = self.torch, self.lib
+        n, code, st = C.c_longlong(int(d_img.numel())), _lib.dtype_code(d_img.dtype), _lib.stream_ptr()
+        mm = self.buf('edge_minmax', (4,), torch.float64)
+        out = self.buf('edge_img', tuple(d_img.shape), torch.float64)
+        self._ck(lib.isb_image_minmax(_lib.ptr(d_img), code, n, _lib.ptr(mm), st))
+        self._ck(lib.isb_image_unit_scale(_lib.ptr(d_img), code, n, _lib.ptr(mm), _lib.ptr(out), st))
+        return out
+
+    def vector_edge_weights(self, d_vec, d_edges, cap, d_n_edges, d_centres, metric):
+        """isb_gc_vector_edge_weights of the per-label vectors ``d_vec`` [nb, D] over the edge table (``cap`` rows, device count
+        ``d_n_edges``): returns the weights [cap] (cached buffer), which :meth:`gc_energies` takes as ``edge_w`` under
+        :data:`EDGE_GIVEN`"""
+        torch, lib = self.torch, self.lib
+        nb, D = int(d_vec.shape[0]), int(d_vec.shape[1])
+        edge_w = self.buf('edge_w_given', (max(int(cap), 1),), torch.float64)
+        wsb = lib.isb_gc_energies_workspace_bytes(nb, 1, int(cap))
+        ws = self.buf('ws_energy', (wsb,), torch.uint8)
+        self._ck(lib.isb_gc_vector_edge_weights(_lib.ptr(d_vec), nb, D, int(d_vec.stride(0)), _lib.ptr(d_edges), int(cap), _lib.ptr(d_n_edges),
+                                                _lib.ptr(d_centres), int(metric), _lib.ptr(edge_w), _lib.ptr(ws), C.c_size_t(wsb),
+                                                _lib.stream_ptr()))
+        return edge_w
 
     def alpha_expansion(self, N, K, E, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, n_iter=-1, init_labels=None,
                         d_n_nodes=None):

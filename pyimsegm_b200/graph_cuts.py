@@ -11,7 +11,7 @@ import logging
 
 import numpy as np
 
-from .engine import EDGE_MODES, get_engine
+from .engine import EDGE_GIVEN, EDGE_MODES, VECTOR_EDGE_METRICS, get_engine
 from .superpixels import (
     device_adjacency,
     make_graph_segm_connect_grid2d_conn4,
@@ -460,20 +460,63 @@ def _device_energies(eng, segments, proba, edge_type, edge_cost, pairwise):
     return d_edges, E, eng.gc_energies(d_proba, d_edges, E, None, centres, mode, float(edge_cost), pairwise)
 
 
-def device_graphcut(eng, d_seg, d_centres, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, edge_cap):
+def check_edge_type(edge_type):
+    """ValueError unless the device pipelines know ``edge_type``: '', 'spatial', 'model', 'model_lT' / '_l1' / '_l2', 'color' or
+    'features' (compute_edge_weights would weight any other name by ones)"""
+    if not (isinstance(edge_type, str) and (edge_type in EDGE_MODES or edge_type in VECTOR_EDGE_METRICS)):
+        raise ValueError('unknown gc_edge_type %r: expected one of %s' % (edge_type, sorted(set(EDGE_MODES) | set(VECTOR_EDGE_METRICS))))
+
+
+def reference_edge_type(edge_type):
+    """the edge type whose device weights are those compute_edge_weights gives ``edge_type``: itself when :func:`check_edge_type`
+    takes it, else '' -- the reference weights an unknown name, or a 'model_<metric>' of an unknown metric, by ones without the
+    spatial term"""
+    if isinstance(edge_type, str) and (edge_type in EDGE_MODES or edge_type in VECTOR_EDGE_METRICS):
+        return edge_type
+    _edge_mode(edge_type)     # logs an unknown model metric as the reference does
+    return ''
+
+
+def device_edge_vectors(eng, edge_type, d_img, d_seg, nb, d_feat, d_n):
+    """the per-label vectors [nb, D] (device) that compute_edge_weights compares for ``edge_type``, None for the types that need
+    none; nothing is read back.  'color': the mean RGB of the image as np.array(image, dtype=float), divided by 255 when its maximum
+    is above 1 (labels [H, W] of an [H, W, 3] device image); 'features': the feature table [>= nb, D] standardised by StandardScaler
+    over the ``d_n`` (device) real rows.  The device feature tables hold no NaN (every statistic kernel writes np.nan_to_num's
+    values), so they are already the table with NaN set to 0 that compute_color2d_superpixels_features returns."""
+    if edge_type == 'color':
+        if d_img.dim() != 3 or int(d_img.shape[2]) != 3:
+            raise ValueError("gc_edge_type 'color' needs an RGB image [H, W, 3], got shape %r" % (tuple(d_img.shape), ))
+        vec = eng.buf('edge_vec', (nb, 3), eng.torch.float64)
+        eng.group_stats(eng.unit_scaled_image(d_img), d_seg, nb, ('mean', ), vec, 0)
+        return vec
+    if edge_type == 'features':
+        return eng.standard_scaler(d_feat, d_n, names=('edge_feat', 'edge_feat_params'))[0]
+    return None
+
+
+def device_graphcut(eng, d_seg, d_centres, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, edge_cap, edge_vectors=None):
     """graph-cut tail of the device pipelines over the label map ``d_seg`` and its centroids ``d_centres``: adjacency,
     energies, alpha-expansion (all asynchronous).  A label volume [D, H, W] takes its 6-connected graph and its (z, y, x) centroids
     from :meth:`~.engine.Engine.graph3d` instead (pass ``d_centres`` None).  ``nb`` may be an upper bound of the label count
-    when ``d_n_nodes`` (device scalar) carries the real one.  Returns (class per label [nb] device, n_edges device int32[1]); the
-    result only holds when the table of ``edge_cap`` rows took every edge, see :func:`~.engine.edges_fit`"""
+    when ``d_n_nodes`` (device scalar) carries the real one.  'color' and 'features' weigh the edges of a label map by the vectors
+    ``edge_vectors`` [nb, D] (device, :func:`device_edge_vectors`).  Returns (class per label [nb] device, n_edges device int32[1]);
+    the result only holds when the table of ``edge_cap`` rows took every edge, see :func:`~.engine.edges_fit`"""
+    check_edge_type(gc_edge_type)
+    metric = VECTOR_EDGE_METRICS.get(gc_edge_type)
+    if metric is not None and (d_seg.dim() != 2 or edge_vectors is None):
+        raise ValueError('gc_edge_type %r compares per-superpixel vectors over a 2-D label map: pass them as edge_vectors' % gc_edge_type)
     K = int(d_proba.shape[1])
     pairwise = compute_pairwise_cost(gc_regul, (nb, K))
     if d_seg.dim() == 3:
         d_edges, d_n_edges, _, d_centres = eng.graph3d(d_seg, nb, edge_cap)
     else:
         d_edges, d_n_edges, _ = eng.adjacency(d_seg, nb, edge_cap)
-    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, edge_cap, d_n_edges, d_centres, _edge_mode(gc_edge_type), 1.0,
-                                                       pairwise, d_n_nodes=d_n_nodes)
+    mode, edge_w = _edge_mode(gc_edge_type), None
+    if metric is not None:
+        edge_w = eng.vector_edge_weights(edge_vectors, d_edges, edge_cap, d_n_edges, d_centres, metric)
+        mode = EDGE_GIVEN
+    _, _, unary_i, edge_wi, smooth_i = eng.gc_energies(d_proba, d_edges, edge_cap, d_n_edges, d_centres, mode, 1.0, pairwise,
+                                                       d_n_nodes=d_n_nodes, edge_w=edge_w)
     d_labels, _, _ = eng.alpha_expansion(nb, K, edge_cap, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, -1, d_n_nodes=d_n_nodes)
     return d_labels, d_n_edges
 

@@ -25,7 +25,7 @@ from .class_models import CompiledModel, compile_model
 from .descriptors import (FEATURES_SET_COLOR, _check_gradient_size, compute_selected_features_img2d, device_feature_table,
                           flags_are_resident, native_feature_layout)
 from .engine import edge_capacity, edges_fit, get_engine
-from .graph_cuts import class_model_spec, device_gmm_applicable, estim_class_model, segment_graph_cut_general
+from .graph_cuts import class_model_spec, device_gmm_applicable, estim_class_model, reference_edge_type, segment_graph_cut_general
 from .superpixels import _as_rgb_like, _supported_dtype, slic_params
 
 #: basic features extracted from superpixels (reference pipelines.py:35)
@@ -176,6 +176,7 @@ def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul,
     event) of :meth:`~.engine.Engine.early_soft`; ``check`` is None or (d_n_edges, edge_cap) still to be verified by the caller
     (:func:`~.engine.edges_fit`)."""
     from . import graph_cuts
+    graph_cuts.check_edge_type(gc_edge_type)
     no_cut = (not isinstance(gc_regul, (list, np.ndarray))) and gc_regul <= 0
     if not hasattr(image, 'is_cuda'):
         image = eng.to_device(_supported_dtype(_as_rgb_like(np.asarray(image))), 'image')
@@ -223,11 +224,19 @@ def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul,
     soft = eng.early_soft(res.d_seg, d_proba) if early_soft else None
 
     def second_half():
-        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res.d_seg, res.d_centres, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, cap)
+        d_vec = graph_cuts.device_edge_vectors(eng, gc_edge_type, res.d_img, res.d_seg, nb, res.d_feat, res.d_n_labels)
+        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res.d_seg, res.d_centres, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, cap,
+                                                         edge_vectors=d_vec)
         return eng.gather(res.d_seg, d_labels, None if early_soft else d_proba) + (d_n_edges, )
 
+    # 'color' and 'features' also read the image and the feature table: the captured launches hold their addresses, the image's
+    # dtype and the table's shape and row stride, so all of these are part of the key
+    vec_src = None
+    if gc_edge_type in ('color', 'features'):
+        vec_src = (res.d_img.data_ptr(), str(res.d_img.dtype), tuple(res.d_img.shape), res.d_feat.data_ptr(), tuple(res.d_feat.shape),
+                   int(res.d_feat.stride(0)))
     key2 = ('cut', id(eng), res.d_seg.data_ptr(), d_proba.data_ptr(), res.d_centres.data_ptr(), res.shape, res.nb_bound,
-            int(d_proba.shape[1]), float(gc_regul) if graphable else None, gc_edge_type, cap, not early_soft)
+            int(d_proba.shape[1]), float(gc_regul) if graphable else None, gc_edge_type, vec_src, cap, not early_soft)
     d_segm, d_soft, d_n_edges = _graph_call(eng, key2, second_half) if graphable else second_half()
     return d_segm, (soft if early_soft else d_soft), (d_n_edges, cap)
 
@@ -262,6 +271,7 @@ def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_t
         if classes is not None:
             graph_labels = classes[graph_labels]
         return graph_labels[slic], segm_soft
+    gc_edge_type = reference_edge_type(gc_edge_type)
     while True:
         d_segm, soft, check = _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, early_soft=True)
         if check is None:   # no graph cut: both gathers were done at the end of the main stream
@@ -347,6 +357,7 @@ def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIM
     else:
         model = _compiled_model(model_pipeline, dict_features) or model_pipeline.predict_proba
     classes = getattr(model_pipeline, 'classes_', None)
+    gc_edge_type = reference_edge_type(gc_edge_type)
 
     def launch(eng, image):
         d_segm, d_soft, check = _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)
@@ -608,7 +619,9 @@ def segment_resident(d_image, model, dict_features, sp_size=30, sp_regul=0.2, gc
     proba_fn(features), a fitted model (or its bound ``predict_proba``) -- evaluated on the device when
     :func:`~.class_models.compile_model` supports it -- or ('fit', nb_classes, use_scaler, max_iter) for the GPU-fitted default GMM
     (``_fit_model`` gives the tuple of the other ``estim_model`` variants and of ``pca_coef``).
-    The indices in ``segm`` are not mapped through the model's ``classes_``.
+    The indices in ``segm`` are not mapped through the model's ``classes_``.  ``gc_edge_type`` is any edge type of
+    ``graph_cuts.compute_edge_weights`` -- 'color' and 'features' weigh the edges on the device too --; an unknown name raises
+    ValueError.
     Nothing here waits for the device, so the edge count of the graph cut is not checked against its table as the host-facing
     pipelines do: after the connectivity pass every superpixel is connected, the region graph of a 2-D map is planar with at most
     3N - 6 edges, and the table holds 8 per node of an upper bound of N. """

@@ -129,6 +129,28 @@ def _combine(lib, dst_ptr, src_ptr, n, op):
     _lib.check(lib.isb_combine(C.c_void_p(dst_ptr), C.c_void_p(src_ptr), C.c_longlong(int(n)), int(op), _lib.stream_ptr()))
 
 
+def _band_extrema(lib, ptr, code, n, mm, mm_b, first):
+    """[min, max] of the ``n`` samples at device ``ptr`` into mm[0:2] (the first band of a rank) or merged into it (the others,
+    through ``mm_b``); numpy's rule: a NaN sample makes both NaN (isb_image_minmax, isb_combine)"""
+    tgt = mm if first else mm_b
+    _lib.check(lib.isb_image_minmax(C.c_void_p(ptr), code, C.c_longlong(int(n)), _lib.ptr(tgt), _lib.stream_ptr()))
+    if not first:
+        _combine(lib, mm.data_ptr(), mm_b.data_ptr(), 1, OP_MIN_F64)
+        _combine(lib, mm.data_ptr() + 8, mm_b.data_ptr() + 8, 1, OP_MAX_F64)
+
+
+def _rank_extrema(comm, mm):
+    """the extrema mm[0:2] of every rank's bands merged over the ranks"""
+    if comm.world > 1:
+        # a NaN sample makes both extrema NaN (numpy's rule, kept by isb_image_minmax and isb_combine); the collectives' min and
+        # max need not keep a NaN, so a flag carries it across the GPUs
+        has_nan = mm[0:1].isnan().to(mm.dtype)
+        comm.all_reduce(mm[0:1], 'min')
+        comm.all_reduce(mm[1:2], 'max')
+        comm.all_reduce(has_nan, 'max')
+        mm[0:2].masked_fill_(has_nan > 0, float('nan'))
+
+
 def slic_tiled(image, n_segments, compactness, sigma=1.0, max_iter=10, slic_zero=False, rescale=True, comm=None,
                bands_per_rank=1, eng=None, min_size_factor=0.5, max_size_factor=3, enforce_connectivity=True, defer_check=False,
                force_whole=False, raw_margin=0):
@@ -178,19 +200,9 @@ def slic_tiled(image, n_segments, compactness, sigma=1.0, max_iter=10, slic_zero
         res.d_raw.append(raw)
         if rescale:
             own_ptr = raw.data_ptr() + (bd.own_lo - bd.up_lo) * W * Cn * itemsize
-            tgt = mm if i == 0 else mm_b
-            _lib.check(lib.isb_image_minmax(C.c_void_p(own_ptr), code, C.c_longlong((bd.own_hi - bd.own_lo) * W * Cn), _lib.ptr(tgt), st))
-            if i > 0:
-                _combine(lib, mm.data_ptr(), mm_b.data_ptr(), 1, OP_MIN_F64)
-                _combine(lib, mm.data_ptr() + 8, mm_b.data_ptr() + 8, 1, OP_MAX_F64)
-    if rescale and comm.world > 1:
-        # a NaN sample makes both extrema NaN (numpy's rule, kept by isb_image_minmax and isb_combine); the collectives' min and
-        # max need not keep a NaN, so a flag carries it across the GPUs
-        has_nan = torch.isnan(mm[0:1]).to(torch.float64)
-        comm.all_reduce(mm[0:1], 'min')
-        comm.all_reduce(mm[1:2], 'max')
-        comm.all_reduce(has_nan, 'max')
-        mm[0:2].masked_fill_(has_nan > 0, float('nan'))
+            _band_extrema(lib, own_ptr, code, (bd.own_hi - bd.own_lo) * W * Cn, mm, mm_b, first=i == 0)
+    if rescale:
+        _rank_extrema(comm, mm)
 
     # 2) blur + rgb2lab of every raw slab, band descriptors
     descs, keep = [], []
@@ -546,6 +558,42 @@ def features_tiled(res, image_dtype, channels, layout, ncol, comm=None, eng=None
 
 
 
+def banded_edge_vectors(res, image_dtype, edge_type, comm=None, eng=None):
+    """the vectors of ``graph_cuts.device_edge_vectors`` for the banded image, the same on every rank: 'features' standardises the
+    replicated feature table ``res.d_feat``; 'color' takes the image's maximum as the bands' maxima merged over the ranks, scales the
+    owned rows of every band by it (``Engine.unit_scaled_image``'s rule) and sums their mean colours over the ranks.  None for the
+    edge types that need no vectors."""
+    from .graph_cuts import device_edge_vectors
+    eng = eng or get_engine()
+    comm = comm or default_comm()
+    if edge_type != 'color':
+        return device_edge_vectors(eng, edge_type, None, res.d_seg, int(res.nb_bound), res.d_feat, res.d_n_labels)
+    if int(res.d_raw[0].shape[-1]) != 3:
+        raise ValueError("gc_edge_type 'color' needs an RGB image [H, W, 3]")
+    torch, lib = eng.torch, eng.lib
+    W = res.shape[1]
+    code, itemsize = _lib.dtype_code(np.dtype(image_dtype)), np.dtype(image_dtype).itemsize
+    f64 = _lib.dtype_code(np.dtype(np.float64))
+    mm = eng.buf('tb_edge_minmax', (4,), torch.float64)
+    mm_b = eng.buf('tb_edge_minmax_b', (4,), torch.float64)
+    for i, b in enumerate(res.local):
+        bd = res.bands[b]
+        ptr = _raw_rows(res, i, bd.own_lo, bd.own_hi, itemsize, "gc_edge_type 'color'")
+        _band_extrema(lib, ptr, code, (bd.own_hi - bd.own_lo) * W * 3, mm, mm_b, first=i == 0)
+    _rank_extrema(comm, mm)
+
+    def scaled(i):
+        bd = res.bands[res.local[i]]
+        out = eng.buf('tb_edge_img', (bd.own_hi - bd.own_lo, W, 3), torch.float64)
+        _lib.check(lib.isb_image_unit_scale(C.c_void_p(_raw_rows(res, i, bd.own_lo, bd.own_hi, itemsize, "gc_edge_type 'color'")), code,
+                                            C.c_longlong(out.numel()), _lib.ptr(mm), _lib.ptr(out), _lib.stream_ptr()))
+        return out.data_ptr(), f64
+
+    vec = eng.buf('edge_vec', (int(res.nb_bound), 3), torch.float64)
+    _stats_banded(res, scaled, ('mean', ), vec, 0, None, comm, eng)
+    return vec
+
+
 def _admit(dict_features):
     """(layout, ncol, raw margin) of a feature dictionary the banded path takes; NotImplementedError for any other, before any
     device work"""
@@ -570,12 +618,13 @@ def _prepare_image(image, layout, sp_size, sp_regul):
     return image, n_seg, compact
 
 
-def _banded_segment(eng, shape, comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm):
+def _banded_segment(eng, shape, comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm, edge_vectors=None):
     """the tail the banded pipelines share, for an image [H, W] cut into row bands or a volume [D, H, W] cut into z-slabs:
     ``front(force_whole)`` -> (res, d_proba) runs the banded SLIC (``defer_check``), the feature table and the class probabilities;
     then the soft segmentation of the owned rows (slices), the graph cut on the replicated superpixel graph (4-connected in 2-D,
     6-connected in 3-D: :func:`~.graph_cuts.device_graphcut`), the LUT gather of the owned rows and one download.  Orphan pixels
-    beyond the halo redo the front on the whole image, an edge table that was too small redoes the cut.  Returns (segm,
+    beyond the halo redo the front on the whole image, an edge table that was too small redoes the cut.  ``edge_vectors(res)`` gives
+    the per-superpixel vectors of a 'color' / 'features' cut (:func:`banded_edge_vectors`).  Returns (segm,
     segm_soft or None, (lo, hi)) on the host, the rows (slices) [lo, hi) of this rank."""
     from . import graph_cuts
     torch = eng.torch
@@ -583,12 +632,13 @@ def _banded_segment(eng, shape, comm, bands_per_rank, front, gc_regul, gc_edge_t
     while True:
         if redo_front:
             res, d_proba = front(force_whole)
+            d_vec = edge_vectors(res) if edge_vectors is not None else None
             redo_front = False
         lo, hi = res.bands[res.local[0]].own_lo, res.bands[res.local[-1]].own_hi
         soft = eng.early_soft(res.d_seg[lo:hi], d_proba) if want_soft else None
         cap = edge_capacity(res.nb_bound, ndim=len(shape))
         d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res.d_seg, res.d_centres, res.nb_bound, d_proba, gc_regul, gc_edge_type,
-                                                         res.d_n_labels, cap)
+                                                         res.d_n_labels, cap, edge_vectors=d_vec)
         # 5) LUT gather of the owned rows
         d_full = eng.buf('segm', tuple(shape), torch.int32) if gather_segm else None
         d_segm, _ = eng.gather(res.d_seg[lo:hi], d_labels, out_i=d_full[lo:hi] if gather_segm else None)
@@ -623,6 +673,7 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
         ``segm`` is the whole [H, W] map on every rank (``segm_soft`` stays banded: it is 8*K bytes per pixel)
     """
     from . import graph_cuts
+    graph_cuts.check_edge_type(gc_edge_type)
     if sp_regul <= 0.:
         raise ValueError('slic. regularisation must be positive')
     dict_features = {'color': ['mean']} if dict_features is None else dict_features
@@ -644,7 +695,8 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
                                                 graph_cuts.RANDOM_SEED, d_n=res.d_n_labels)[0]
         return res, d_proba
 
-    return _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm)
+    return _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm,
+                           lambda res: banded_edge_vectors(res, image.dtype, gc_edge_type, comm, eng))
 
 
 def segment_color2d_slic_features_model_graphcut_tiled(image, model_pipeline, dict_features, sp_size=30, sp_regul=0.2, gc_regul=1.,
@@ -659,7 +711,9 @@ def segment_color2d_slic_features_model_graphcut_tiled(image, model_pipeline, di
     :return tuple: (segm [rows, W], segm_soft [rows, W, K] float64 or None, (row_lo, row_hi)) as
         :func:`pipe_color2d_slic_features_model_graphcut_tiled`
     """
+    from .graph_cuts import check_edge_type
     from .pipelines import _compiled_model
+    check_edge_type(gc_edge_type)
     if sp_regul <= 0.:
         raise ValueError('slic. regularisation must be positive')
     layout, ncol, margin = _admit(dict_features)
@@ -683,7 +737,8 @@ def segment_color2d_slic_features_model_graphcut_tiled(image, model_pipeline, di
         padded[:nb] = proba
         return res, eng.to_device(padded, 'proba')
 
-    segm, soft, rows = _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm)
+    segm, soft, rows = _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm,
+                                       lambda res: banded_edge_vectors(res, image.dtype, gc_edge_type, comm, eng))
     if classes is not None:
         segm = np.asarray(classes)[segm]
     return segm, soft, rows
