@@ -544,6 +544,34 @@ int isb_binary_morph_footprint(const uint8_t* in, int H, int W, const int32_t* o
                                isb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * (x') supervised training data -- the per-image step of train_classif_color2d_slic_features (imsegm/pipelines.py:293-379)
+ * ------------------------------------------------------------------------------------------------------------------ */
+
+/* one training label per superpixel: wrapper_compute_color2d_slic_features_labels (pipelines.py:272-290) over
+ * histogram_regions_labels_norm (labeling.py:245-278), without the dense [nb, max label + 1] table of isb_region_label_hist.
+ *   slic [H, W] i32 in [0, nb) (other values are not counted), annot [H, W] i32 (negative = unknown), labels out [nb] i64.
+ * With c* the largest pixel count of a known label in the superpixel, l* the smallest label with that count, u its unknown pixels and
+ * n all its pixels: labels[s] = l* when c* >= u and !((double)c* / (double)n < label_purity), else -1 -- the reference's np.argmax,
+ * which ranks its unknown bin max(annot) + 1 after every label, and its purity test.  A superpixel without pixels, or at or beyond the
+ * optional device count n_labels_dev, gets -1.  Memory and time follow H * W and nb, never the label values: (superpixel, label)
+ * pairs are counted in a hash table of 1.5 H W entries.  H * W <= 2^31.  ws: isb_train_labels_workspace_bytes(H, W, nb), 18 bytes
+ * per pixel and 16 per superpixel. */
+size_t isb_train_labels_workspace_bytes(int H, int W, int nb);
+int isb_superpixel_train_labels(const int32_t* slic, int H, int W, int nb, const int32_t* n_labels_dev, const int32_t* annot,
+                                double label_purity, int64_t* labels, void* ws, size_t ws_bytes, isb_stream_t stream);
+
+/* balance_dataset_by_(features[labels != -1], labels[labels != -1], 'unique') of one image (classification.py:1159-1216): the rows of
+ * feat [N, ld] f64 (first D columns; the real row count from the optional device n_dev) whose label [N] i64 is not -1, each value
+ * rounded as rint(x * 1000.0) / 1000.0 (np.round(x, 3), bit for bit), grouped by label ascending, sorted lexicographically within a
+ * label and without repeats (-0 equals +0 and is written as +0).  Out: rows_out [N, D] f64 (the first *n_out rows), labels_out [N]
+ * i64 (the label of each written row) and n_out (DEVICE i64).  The table must hold no NaN (the pipelines replace NaN by 0 first): a
+ * NaN in a kept row sets *n_out to -1, and nothing the call wrote is meaningful.  Nothing synchronises with the host.
+ * ws: isb_unique_rows_workspace_bytes(N, D), a rounded copy of the table and some 30 bytes per row. */
+size_t isb_unique_rows_workspace_bytes(int N, int D);
+int isb_unique_rows_rounded(const double* feat, int N, int D, int ld, const int32_t* n_dev, const int64_t* labels, double* rows_out,
+                            int64_t* labels_out, long long* n_out, void* ws, size_t ws_bytes, isb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * (xi) labeling -- imsegm/labeling.py: boundary and contour maps, the exact Euclidean distance transform, the (row, col)
  *      lists of contour_coords / compute_boundary_distances, and the final relabel gather.  Label maps are [H, W] i32.
  * ------------------------------------------------------------------------------------------------------------------ */

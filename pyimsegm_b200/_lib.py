@@ -128,6 +128,10 @@ SIGNATURES = {
     'isb_dbscan_workspace_bytes': (_sz, [_i]),
     'isb_dbscan': (_i, [_vp, _i, _d, _i, _vp, _vp, C.POINTER(_i), _vp, _sz, _vp]),
     'isb_region_label_hist': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    'isb_train_labels_workspace_bytes': (_sz, [_i, _i, _i]),
+    'isb_superpixel_train_labels': (_i, [_vp, _i, _i, _i, _vp, _vp, _d, _vp, _vp, _sz, _vp]),
+    'isb_unique_rows_workspace_bytes': (_sz, [_i, _i]),
+    'isb_unique_rows_rounded': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     'isb_gather': (_i, [_vp, _ll, _vp, _vp, _i, _vp, _vp, _vp]),
     'isb_segment_median_workspace_bytes': (_sz, [_ll, _i]),
     'isb_segment_median': (_i, [_vp, _i, _vp, _ll, _i, _i, _vp, _vp, _sz, _vp]),

@@ -534,6 +534,44 @@ class Engine(object):
                                                 _lib.stream_ptr()))
         return edge_w
 
+    # -- supervised training data ----------------------------------------------------------------------------------
+    def train_labels(self, d_seg, nb, d_annot, label_purity, d_n=None):
+        """isb_superpixel_train_labels: the training label of every superpixel of ``d_seg`` [H, W] (labels below ``nb``) from the
+        annotation ``d_annot`` [H, W] int32 (negative = unknown); returns int64 [nb] (cached buffer), -1 where no label is kept"""
+        torch, lib = self.torch, self.lib
+        H, W = int(d_seg.shape[0]), int(d_seg.shape[1])
+        labels = self.buf('train_labels', (int(nb),), torch.int64)
+        wsb = lib.isb_train_labels_workspace_bytes(H, W, int(nb))
+        ws = self.buf('ws_train_labels', (max(wsb, 1),), torch.uint8)
+        self._ck(lib.isb_superpixel_train_labels(_lib.ptr(d_seg), H, W, int(nb), _lib.ptr(d_n), _lib.ptr(d_annot), C.c_double(label_purity),
+                                                 _lib.ptr(labels), _lib.ptr(ws), C.c_size_t(wsb), _lib.stream_ptr()))
+        return labels
+
+    def nan_free_table(self, d_feat, D, d_n=None):
+        """the first ``D`` columns of ``d_feat`` [N, ld] f64 as a dense [N, D] copy with NaN -> 0 (``features[np.isnan(features)] = 0``
+        of the pipelines), rows from the optional device count ``d_n`` on left unwritten: isb_class_transform without scaler or PCA"""
+        N = int(d_feat.shape[0])
+        out = self.buf('feat_nan_free', (N, int(D)), self.torch.float64)
+        self._ck(self.lib.isb_class_transform(_lib.ptr(d_feat), N, int(d_feat.stride(0)), _lib.ptr(d_n), int(D), None, None, None, None, None,
+                                              int(D), _lib.ptr(out), None, C.c_size_t(0), _lib.stream_ptr()))
+        return out
+
+    def unique_rows(self, d_feat, d_labels, D, d_n=None):
+        """isb_unique_rows_rounded of the first ``D`` columns of ``d_feat`` [N, ld] f64 and their labels ``d_labels`` [N] int64: returns
+        (rows [N, D] f64, labels [N] int64, count int64 [1]) cached buffers, the first ``count`` rows written; a count of -1 means the
+        table held a NaN"""
+        torch, lib = self.torch, self.lib
+        N = int(d_feat.shape[0])
+        rows = self.buf('unique_rows', (N, int(D)), torch.float64)
+        labels = self.buf('unique_labels', (N,), torch.int64)
+        count = self.buf('unique_count', (1,), torch.int64)
+        wsb = lib.isb_unique_rows_workspace_bytes(N, int(D))
+        ws = self.buf('ws_unique_rows', (max(wsb, 1),), torch.uint8)
+        self._ck(lib.isb_unique_rows_rounded(_lib.ptr(d_feat), N, int(D), int(d_feat.stride(0)), _lib.ptr(d_n), _lib.ptr(d_labels),
+                                             _lib.ptr(rows), _lib.ptr(labels), _lib.ptr(count), _lib.ptr(ws), C.c_size_t(wsb),
+                                             _lib.stream_ptr()))
+        return rows, labels, count
+
     def alpha_expansion(self, N, K, E, d_n_edges, d_edges, edge_wi, unary_i, smooth_i, n_iter=-1, init_labels=None,
                         d_n_nodes=None):
         torch, lib = self.torch, self.lib

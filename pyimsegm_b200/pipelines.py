@@ -14,6 +14,13 @@ host synchronises ONCE, when the results are downloaded.  A caller-fitted mixtur
 (:mod:`.class_models`) and evaluated there too; any other model, or a self-fitted one the device GMM does not cover, costs one
 round trip: features [N, D] down, probabilities [N, K] up.
 
+The supervised training of the reference (``train_classif_color2d_slic_features``, pipelines.py:293-379) is
+:func:`train_classif_images_batch`: per annotated image, SLIC, the feature table, one training label per superpixel
+(``isb_superpixel_train_labels``) and the distinct rounded rows of each class for ``feature_balance='unique'``
+(``isb_unique_rows_rounded``) run on the device over CUDA streams, then the classifier is fitted by
+``classification.create_classif_search_train_export``.  :func:`wrapper_compute_color2d_slic_features_labels` is its one-image data
+step.  The reference's name itself still raises NotImplementedError.
+
 Gray volumes have the same resident form: :func:`segment_resident_volume` (a device volume in, device results out) and
 :func:`segment_volumes_batch` (host volumes over CUDA streams) run ``pipe_gray3d_slic_features_model_graphcut``'s stages on the device.
 """
@@ -30,9 +37,9 @@ from .superpixels import _as_rgb_like, _supported_dtype, slic_params
 
 #: basic features extracted from superpixels (reference pipelines.py:35)
 FTS_SET_SIMPLE = FEATURES_SET_COLOR
-#: default clustering for unsupervised segmentation (reference pipelines.py:39 -> classification.DEFAULT_CLUSTERING)
-#: default classifier of the supervised path (reference classification.py:54; the classifier zoo itself is out of scope)
+#: default classifier of the supervised path (reference classification.py:54)
 CLASSIF_NAME = 'RandForest'
+#: default clustering for unsupervised segmentation (reference pipelines.py:39 -> classification.DEFAULT_CLUSTERING)
 CLUSTER_METHOD = 'kMeans'
 #: images left out during cross-validation training (reference pipelines.py:41)
 CROSS_VAL_LEAVE_OUT = 2
@@ -394,41 +401,136 @@ def compute_features_batch(list_images, dict_features, sp_size=30, sp_regul=0.2,
     return _over_streams(list_images, nb_streams, max_in_flight, launch, finish)
 
 
+def train_annotation(image, annot):
+    """ the annotation as the supervised data step reads it: ``astype(int)`` as the reference casts it (floats truncate toward zero,
+    bools become 0 / 1), then int32 with every negative value as -1 (unknown).  Raises ImageDimensionError when its shape is not the
+    image's [H, W], ValueError for a label above 2^31 - 1, and the reference's ValueError when every value is below -1 (its unknown
+    label ``max(annot) + 1`` is then itself negative)
+
+    :return ndarray: int32 [H, W]
+    """
+    from .utilities import ImageDimensionError
+    annot = np.asarray(annot).astype(int)
+    if np.shape(image)[:2] != annot.shape[:2] or annot.ndim != 2:
+        raise ImageDimensionError('image %r and annot %r should match' % (np.shape(image), annot.shape))
+    if annot.size and int(annot.max()) > np.iinfo(np.int32).max:
+        raise ValueError('annotation label %d is above 2^31 - 1' % int(annot.max()))
+    if annot.size and int(annot.max()) < -1:
+        raise ValueError('only positive labels are allowed')
+    return np.maximum(annot, -1).astype(np.int32)
+
+
+def _train_data(list_images, list_annots, dict_features, sp_size, sp_regul, label_purity, unique, nb_streams, max_in_flight):
+    """ the per-image data step of the supervised training on annotations that :func:`train_annotation` has checked: per image
+    (slic int64 [H, W], features [N, D] with NaN -> 0, labels int64 [N], balanced) where ``balanced`` is the image's
+    ``balance_dataset_by_(features[labels != -1], labels[labels != -1], 'unique')`` as (rows, labels) when ``unique`` and the image
+    took the resident path, else None.  Colour images with a dictionary of the resident feature table alternate over
+    ``nb_streams`` CUDA streams as in :func:`compute_features_batch` (SLIC, features, labels and unique rows on the device, one
+    download); other images compute their superpixels and features through :func:`compute_color2d_superpixels_features` and
+    their labels on the device. """
+    D = native_feature_layout(dict_features)[1] if flags_are_resident(dict_features) else 0
+    if D == 0 or any(np.ndim(im) != 3 for im in list_images):
+        eng = get_engine()
+        out = []
+        for image, annot in zip(list_images, list_annots):
+            slic, features = compute_color2d_superpixels_features(image, dict_features, sp_size=sp_size, sp_regul=sp_regul)
+            n = int(slic.max()) + 1
+            d_seg = eng.to_device(slic.astype(np.int32), 'train_slic')
+            labels = eng.to_host(eng.train_labels(d_seg, n, eng.to_device(annot, 'train_annot'), label_purity)).copy()
+            out.append((slic, features, labels, None))
+        return out
+
+    def launch(eng, idx):        # _over_streams walks the image indices: the annotation goes with its image
+        res = _device_slic_features(eng, np.asarray(list_images[int(idx)]), dict_features, sp_size, sp_regul)
+        d_labels = eng.train_labels(res.d_seg, res.nb_bound, eng.to_device(list_annots[int(idx)], 'train_annot'), label_purity,
+                                    d_n=res.d_n_labels)
+        d_x = eng.nan_free_table(res.d_feat, D, res.d_n_labels)
+        outs = (res.d_n_labels, res.d_seg, d_x, d_labels)
+        if unique:
+            outs += eng.unique_rows(d_x, d_labels, D, d_n=res.d_n_labels)
+        return eng.download(outs) + (None, )
+
+    def finish(idx, hosts, _):
+        n = int(hosts[0][0])
+        balanced = None
+        if unique:
+            m = int(hosts[6][0])
+            if m < 0:
+                raise ValueError('the feature table of image %d holds NaN' % idx)
+            balanced = (hosts[4].numpy()[:m].copy(), hosts[5].numpy()[:m].copy())
+        return hosts[1].numpy().astype(np.int64), hosts[2].numpy()[:n].copy(), hosts[3].numpy()[:n].copy(), balanced
+
+    return _over_streams(range(len(list_images)), nb_streams, max_in_flight, launch, finish)
+
+
 def wrapper_compute_color2d_slic_features_labels(img_annot, sp_size, sp_regul, dict_features, label_purity):
     """ superpixels, their features and one training label per superpixel from an annotated image -- the data step of the
     supervised path (reference pipelines.py:272-290): a superpixel takes the annotation label that covers most of it, or -1
-    when that share is below ``label_purity`` (or the winner is the negative / unknown label)
+    when that share is below ``label_purity`` (or the winner is the negative / unknown label).  A one-image call of the data step
+    of :func:`train_classif_images_batch`; the labels come from ``isb_superpixel_train_labels``.
 
     :param tuple(ndarray,ndarray) img_annot: image and its annotation (negative values = unknown)
     :return tuple(ndarray,ndarray,ndarray): slic [H, W], features [N, D], labels [N]
     """
-    from .labeling import histogram_regions_labels_norm
-    from .utilities import ImageDimensionError
     img, annot = img_annot
-    annot = np.asarray(annot).astype(int)
-    if np.shape(img)[:2] != annot.shape[:2]:
-        raise ImageDimensionError('image %r and annot %r should match' % (np.shape(img), annot.shape))
-    slic, features = compute_color2d_superpixels_features(img, dict_features, sp_size=sp_size, sp_regul=sp_regul)
-    neg_label = int(np.max(annot)) + 1 if np.any(annot < 0) else None
-    if neg_label is not None:
-        annot = np.where(annot < 0, neg_label, annot)
-    label_hist = histogram_regions_labels_norm(slic, annot)       # joint histogram on the device (isb_region_label_hist)
-    labels = np.argmax(label_hist, axis=1)
-    purity = np.max(label_hist, axis=1)
-    if neg_label is not None:
-        labels[labels == neg_label] = -1
-    labels[purity < label_purity] = -1
-    return slic, features, labels
+    annot = train_annotation(img, annot)
+    return _train_data([img], [annot], dict_features, sp_size, sp_regul, label_purity, False, 1, 1)[0][:3]
+
+
+def train_classif_images_batch(list_images, list_annots, dict_features, sp_size=30, sp_regul=0.2, clf_name=CLASSIF_NAME, label_purity=0.9,
+                               feature_balance='unique', pca_coef=None, nb_classif_search=1, nb_hold_out=CROSS_VAL_LEAVE_OUT, nb_workers=1,
+                               nb_streams=3, max_in_flight=6):
+    """ train a superpixel classifier on annotated images: the reference's ``train_classif_color2d_slic_features``
+    (pipelines.py:293-379) with the per-image data step on the GPU.  Consecutive images alternate over ``nb_streams`` CUDA streams
+    with their own buffers; for each the device runs SLIC, the feature table, the training label of every superpixel
+    (``isb_superpixel_train_labels``) and, for ``feature_balance='unique'``, the image's distinct rounded rows per class
+    (``isb_unique_rows_rounded``), and the host downloads them once.  Then as the reference: 'random', 'kmeans' and unknown names
+    balance every image with ``balance_dataset_by_`` in image order (so the global RNGs are drawn from in the reference's order),
+    None keeps every labelled row; an image without a labelled superpixel raises the reference's ValueError unless
+    ``feature_balance`` is None; the images' rows are concatenated and ``create_classif_search_train_export`` fits the classifier,
+    cross-validated over the images by ``CrossValidateGroups`` when there are more than ``5 * nb_hold_out`` of them.
+    Dictionaries outside the resident feature table and gray images compute their superpixels and features through
+    :func:`compute_color2d_superpixels_features` and are balanced on the host.
+
+    :return tuple: (classif, list_slic int64 [H, W], list_features f64 [N, D], list_labels int64 [N])
+    """
+    from .classification import CrossValidateGroups, _rows_array, balance_dataset_by_, create_classif_search_train_export
+    logging.info('TRAIN Superpixels-Features-Classifier')
+    if len(list_images) != len(list_annots):
+        raise ValueError('size of images (%i) and annotations (%i) should match' % (len(list_images), len(list_annots)))
+    annots = [train_annotation(img, annot) for img, annot in zip(list_images, list_annots)]
+    if sp_regul <= 0.:
+        raise ValueError('slic. regularisation must be positive')
+    unique = feature_balance is not None and feature_balance.lower() == 'unique'
+    data = _train_data(list_images, annots, dict_features, sp_size, sp_regul, label_purity, unique, nb_streams, max_in_flight)
+    list_slic, list_features, list_labels = [d[0] for d in data], [d[1] for d in data], [d[2] for d in data]
+    blocks, labels_all, sizes = [], [], []
+    for _, features, labels, balanced in data:
+        keep = labels != -1
+        if feature_balance is None:
+            features, labels = features[keep], labels[keep]
+        elif balanced is not None and keep.any():
+            features, labels = balanced
+        else:
+            features, labels = balance_dataset_by_(features[keep], labels[keep], balance_type=feature_balance)
+        blocks.append(features)
+        labels_all += np.asarray(labels).tolist()
+        sizes.append(len(labels))
+    features = np.nan_to_num(_rows_array(blocks))
+    labels = np.array(labels_all, dtype=int)
+    cv = CrossValidateGroups(sizes, nb_hold_out=nb_hold_out) if len(sizes) > nb_hold_out * 5 else 10
+    classif, _ = create_classif_search_train_export(clf_name, features, labels, pca_coef=pca_coef, cross_val=cv,
+                                                    nb_search_iter=nb_classif_search, nb_workers=nb_workers)
+    return classif, list_slic, list_features, list_labels
 
 
 def train_classif_color2d_slic_features(list_images, list_annots, dict_features, sp_size=30, sp_regul=0.2, clf_name=CLASSIF_NAME,
                                         label_purity=0.9, feature_balance='unique', pca_coef=None, nb_classif_search=1,
                                         nb_hold_out=CROSS_VAL_LEAVE_OUT, nb_workers=1):
-    """ the supervised training wrapper of the reference (pipelines.py:293-379).  Its data step is available here
-    (:func:`wrapper_compute_color2d_slic_features_labels`); the classifier zoo, hyper-parameter search and dataset balancing it
-    hands the data to (``imsegm/classification.py``) are outside the accelerated hot path (SURVEY.md section 2, row 8) """
-    raise NotImplementedError('supervised classifier training (imsegm.classification) is outside the GPU hot path; '
-                              'use wrapper_compute_color2d_slic_features_labels for the features and labels')
+    """ the supervised training wrapper of the reference (pipelines.py:293-379).  Not provided under this name: the same training,
+    with the per-image data step on the GPU, is :func:`train_classif_images_batch` """
+    raise NotImplementedError('use pipelines.train_classif_images_batch, which trains the classifier as the reference\'s '
+                              'train_classif_color2d_slic_features does, with the data step on the GPU')
 
 
 def pipe_gray3d_slic_features_model_graphcut(image, nb_classes, dict_features, spacing=(12, 1, 1), sp_size=15, sp_regul=0.2,
