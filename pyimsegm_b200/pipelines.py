@@ -49,8 +49,9 @@ NB_WORKERS = 1
 
 
 class DeviceSuperpixels(object):
-    """device-resident result of SLIC + descriptors for one image"""
-    __slots__ = ('d_img', 'd_seg', 'd_n_labels', 'nb_bound', 'd_feat', 'd_centres', 'shape', 'd_params', 'd_n_edges', 'edge_cap')
+    """device-resident result of SLIC + descriptors for one image or volume: ``d_feat`` is the table the class model reads,
+    ``d_centres`` None for a volume (its 6-connected graph takes the centroids from the label volume)"""
+    __slots__ = ('d_img', 'd_seg', 'd_n_labels', 'nb_bound', 'd_feat', 'd_centres', 'shape')
 
 
 def _device_slic_features(eng, image, dict_features, sp_size, sp_regul):
@@ -142,23 +143,33 @@ def _features_key(dict_features):
     return tuple(sorted((k, tuple(v)) for k, v in dict_features.items()))
 
 
-def _compiled_model(model, dict_features):
-    """the device form of a caller-fitted model for the native path (its feature count has to match the native feature layout), or
-    None: then its predict_proba runs on the host"""
+def _resident_width(dict_features):
+    """the column count of the resident feature table of ``dict_features``, or None when the dictionary is not resident"""
+    return native_feature_layout(dict_features)[1] if flags_are_resident(dict_features) else None
+
+
+def _device_model(model, n_features):
+    """``model`` in the form :func:`_device_proba` runs: a resident fit tuple (:func:`_fit_model`) and a
+    :class:`~.class_models.CompiledModel` stay as they are; a fitted model (or its bound ``predict_proba``) is compiled to device
+    tables when :func:`~.class_models.compile_model` takes it and its feature count is ``n_features`` (None: the table is not
+    resident, never compile); anything else is the host callable proba_fn(features) -- ``model`` itself when it is callable, else
+    its ``predict_proba``"""
     from . import graph_cuts
-    if not graph_cuts.USE_DEVICE_PREDICT or not flags_are_resident(dict_features):
-        return None
-    cm = compile_model(model)
-    if cm is None or cm.n_features_in != native_feature_layout(dict_features)[1]:
-        return None
-    return cm
+    if isinstance(model, (tuple, CompiledModel)):
+        return model
+    if graph_cuts.USE_DEVICE_PREDICT and n_features is not None:
+        fitted = model.__self__ if getattr(model, '__name__', None) == 'predict_proba' and hasattr(model, '__self__') else model
+        cm = compile_model(fitted)
+        if cm is not None and cm.n_features_in == n_features:
+            return cm
+    return model if callable(model) else model.predict_proba
 
 
-def _fit_model(nb_classes, use_scaler, estim_model='GMM', pca_coef=None):
-    """the resident model tuple of a device-fitted class model: ('fit', nb_classes, use_scaler, max_iter) for the default 'GMM',
-    ('fit', nb_classes, use_scaler, max_iter, kind, n_init, pca_coef) for any other variant (graph_cuts.class_model_spec).  It is
-    part of the CUDA-graph key, so a configuration never replays the graph of another."""
-    kind, n_init, max_iter = class_model_spec(estim_model, nb_classes)
+def _fit_model(nb_classes, use_scaler, estim_model='GMM', pca_coef=None, max_iter=99):
+    """the resident model tuple of a device-fitted class model: ('fit', nb_classes, use_scaler, 99) for the default 'GMM' with
+    ``max_iter`` 99, ('fit', nb_classes, use_scaler, max_iter, kind, n_init, pca_coef) for any other variant
+    (graph_cuts.class_model_spec).  It is part of the CUDA-graph key, so a configuration never replays the graph of another."""
+    kind, n_init, max_iter = class_model_spec(estim_model, nb_classes, max_iter)
     if kind == 'GMM' and n_init == max(1, int(np.sqrt(max_iter))) and max_iter == 99 and pca_coef is None:
         return ('fit', nb_classes, use_scaler, max_iter)
     return ('fit', nb_classes, use_scaler, max_iter, kind, n_init, pca_coef)
@@ -171,81 +182,96 @@ def _fit_spec(model):
     return nb_classes, use_scaler, max_iter, kind, n_init, pca_coef
 
 
-def _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, early_soft=False):
-    """the whole hot path on the device.  ``model`` is either ('fit', nb_classes, use_scaler, max_iter[, kind, n_init, pca_coef])
-    (:func:`_fit_model`) -> the class model is fitted on the GPU and NOTHING syncs with the host until the results are ready (a
-    float pca_coef reads its component count back, and D > 16 features read one flag per EM iteration); or a
-    :class:`~.class_models.CompiledModel` -> a caller-fitted model evaluated on the device, again without a sync; or a callable
-    proba_fn(features) -> one round trip (features down, probabilities up) as in the reference.
-    With a device-fitted or compiled model and colour features the two halves -- image -> class probabilities, probabilities -> cut
-    and LUT gathers -- are CUDA-graph replays (:func:`_graph_call`); the image then has to sit in one of the engine's cached buffers.
+def _device_proba(eng, model, d_feat, d_n, nb):
+    """class probabilities [nb, K] (device) of the first ``d_n`` (device count) rows of the feature table ``d_feat`` [nb, D] under
+    a model of :func:`_device_model`: a fit tuple is fitted on the GPU and a CompiledModel evaluated there, neither syncs with the
+    host (a float pca_coef reads its component count back, and D > 16 features read one flag per EM iteration); a host callable
+    costs one round trip -- the rows down with NaN set to 0, its probabilities up, padded with zero rows to the label bound ``nb``
+    as a device model leaves them"""
+    from . import graph_cuts
+    if isinstance(model, CompiledModel):
+        return eng.class_model_predict(d_feat, model, d_n=d_n)
+    if isinstance(model, tuple):
+        nb_classes, use_scaler, max_iter, kind, n_init, pca_coef = _fit_spec(model)
+        return graph_cuts.device_fit_predict(eng, d_feat, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef, d_n=d_n)[0]
+    n = int(eng.to_host(d_n)[0])
+    features = eng.to_host(d_feat[:n]).copy()
+    features[np.isnan(features)] = 0
+    proba = np.asarray(model(features), dtype=np.float64)
+    logging.debug('list of probabilities: %r', proba.shape)
+    padded = np.zeros((int(nb), proba.shape[1]))
+    padded[:n] = proba
+    return eng.to_device(padded, 'proba')
+
+
+def _run_resident(eng, front, model, gc_regul, gc_edge_type, graph_key=None, early_soft=False):
+    """the hot path on the device after the caller's argument checks: ``front()`` -> :class:`DeviceSuperpixels`, the class
+    probabilities of ``model`` (:func:`_device_proba`), then the argmin of the probabilities when ``gc_regul`` <= 0 (read on the
+    host) or the graph cut over the superpixel graph (4-connected in 2-D, 6-connected in 3-D) and the LUT gathers.  With a fit
+    tuple or a CompiledModel nothing syncs with the host until the results are ready.
+    With ``graph_key`` (the caller's key of the front and the model) and a cut, the two halves -- front + probabilities,
+    probabilities -> cut and LUT gathers -- are CUDA-graph replays (:func:`_graph_call`).
     Returns (d_segm, soft, check): ``soft`` is the device segm_soft, or with ``early_soft`` and a graph cut the (pinned host tensor,
     event) of :meth:`~.engine.Engine.early_soft`; ``check`` is None or (d_n_edges, edge_cap) still to be verified by the caller
     (:func:`~.engine.edges_fit`)."""
     from . import graph_cuts
-    graph_cuts.check_edge_type(gc_edge_type)
     no_cut = (not isinstance(gc_regul, (list, np.ndarray))) and gc_regul <= 0
-    if not hasattr(image, 'is_cuda'):
-        image = eng.to_device(_supported_dtype(_as_rgb_like(np.asarray(image))), 'image')
-    on_device = isinstance(model, (tuple, CompiledModel))
-    graphable = (on_device and USE_CUDA_GRAPHS and not no_cut and all(k.startswith('color') for k in dict_features)
-                 and flags_are_resident(dict_features))
-    if isinstance(model, CompiledModel):
-        model_key = ('compiled', model.digest)
+    graphed = graph_key is not None and not no_cut
 
-        def predict(res):
-            return eng.class_model_predict(res.d_feat, model, d_n=res.d_n_labels)
-    elif on_device:
-        nb_classes, use_scaler, max_iter, kind, n_init, pca_coef = _fit_spec(model)
-        model_key = model
-        graphable = (graphable and pca_coef is None
-                     and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES)
+    def first_half():
+        res = front()
+        return res, _device_proba(eng, model, res.d_feat, res.d_n_labels, res.nb_bound)
 
-        def predict(res):
-            return graph_cuts.device_fit_predict(eng, res.d_feat, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef,
-                                                 d_n=res.d_n_labels)[0]
-
-    proba = None
-    if on_device:
-        def first_half():
-            res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
-            return res, predict(res)
-
-        key1 = ('probabilities', id(eng), image.data_ptr(), tuple(image.shape), str(image.dtype), model_key, _features_key(dict_features),
-                sp_size, sp_regul)
-        res, d_proba = _graph_call(eng, key1, first_half) if graphable else first_half()
-        nb, d_n_nodes = res.nb_bound, res.d_n_labels
-    else:
-        res = _device_slic_features(eng, image, dict_features, sp_size, sp_regul)
-        nb, d_n_nodes = int(eng.to_host(res.d_n_labels)[0]), None
-        features = eng.to_host(res.d_feat[:nb]).copy()
-        features[np.isnan(features)] = 0
-        proba = np.ascontiguousarray(model(features), dtype=np.float64)
-        logging.debug('list of probabilities: %r', proba.shape)
-        d_proba = eng.to_device(proba, 'proba')
+    res, d_proba = _graph_call(eng, graph_key, first_half) if graphed else first_half()
+    nb = res.nb_bound
     if no_cut:
-        if proba is None:
-            proba = eng.to_host(d_proba[:int(eng.to_host(d_n_nodes)[0])])
+        proba = eng.to_host(d_proba[:int(eng.to_host(res.d_n_labels)[0])])
         return eng.gather(res.d_seg, _argmin_labels_device(eng, proba), d_proba) + (None, )
-    cap = edge_capacity(nb)
+    cap = edge_capacity(nb, ndim=len(res.shape))
     soft = eng.early_soft(res.d_seg, d_proba) if early_soft else None
 
     def second_half():
         d_vec = graph_cuts.device_edge_vectors(eng, gc_edge_type, res.d_img, res.d_seg, nb, res.d_feat, res.d_n_labels)
-        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res.d_seg, res.d_centres, nb, d_proba, gc_regul, gc_edge_type, d_n_nodes, cap,
-                                                         edge_vectors=d_vec)
+        d_labels, d_n_edges = graph_cuts.device_graphcut(eng, res.d_seg, res.d_centres, nb, d_proba, gc_regul, gc_edge_type, res.d_n_labels,
+                                                         cap, edge_vectors=d_vec)
         return eng.gather(res.d_seg, d_labels, None if early_soft else d_proba) + (d_n_edges, )
 
-    # 'color' and 'features' also read the image and the feature table: the captured launches hold their addresses, the image's
-    # dtype and the table's shape and row stride, so all of these are part of the key
-    vec_src = None
-    if gc_edge_type in ('color', 'features'):
-        vec_src = (res.d_img.data_ptr(), str(res.d_img.dtype), tuple(res.d_img.shape), res.d_feat.data_ptr(), tuple(res.d_feat.shape),
-                   int(res.d_feat.stride(0)))
-    key2 = ('cut', id(eng), res.d_seg.data_ptr(), d_proba.data_ptr(), res.d_centres.data_ptr(), res.shape, res.nb_bound,
-            int(d_proba.shape[1]), float(gc_regul) if graphable else None, gc_edge_type, vec_src, cap, not early_soft)
-    d_segm, d_soft, d_n_edges = _graph_call(eng, key2, second_half) if graphable else second_half()
+    if graphed:
+        # 'color' and 'features' also read the image and the feature table: the captured launches hold their addresses, the
+        # image's dtype and the table's shape and row stride, so all of these are part of the key
+        vec_src = None
+        if gc_edge_type in ('color', 'features'):
+            vec_src = (res.d_img.data_ptr(), str(res.d_img.dtype), tuple(res.d_img.shape), res.d_feat.data_ptr(), tuple(res.d_feat.shape),
+                       int(res.d_feat.stride(0)))
+        key2 = ('cut', id(eng), res.d_seg.data_ptr(), d_proba.data_ptr(), res.d_centres.data_ptr(), res.shape, res.nb_bound,
+                int(d_proba.shape[1]), float(gc_regul), gc_edge_type, vec_src, cap, not early_soft)
+        d_segm, d_soft, d_n_edges = _graph_call(eng, key2, second_half)
+    else:
+        d_segm, d_soft, d_n_edges = second_half()
     return d_segm, (soft if early_soft else d_soft), (d_n_edges, cap)
+
+
+def _run_resident_image(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, early_soft=False):
+    """:func:`_run_resident` for one colour image (host, or a device tensor that is used where it is), with SLIC and the feature
+    table of :func:`_device_slic_features` as the front.  With a fit tuple or a CompiledModel and colour features the path is a
+    CUDA-graph replay; the image then has to sit in one of the engine's cached buffers."""
+    from . import graph_cuts
+    graph_cuts.check_edge_type(gc_edge_type)
+    if not hasattr(image, 'is_cuda'):
+        image = eng.to_device(_supported_dtype(_as_rgb_like(np.asarray(image))), 'image')
+    graphable = USE_CUDA_GRAPHS and all(k.startswith('color') for k in dict_features) and flags_are_resident(dict_features)
+    model_key = None
+    if graphable and isinstance(model, CompiledModel):
+        model_key = ('compiled', model.digest)
+    elif (graphable and isinstance(model, tuple) and _fit_spec(model)[5] is None
+          and native_feature_layout(dict_features)[1] <= graph_cuts.DEVICE_GMM_SINGLE_KERNEL_MAX_FEATURES):
+        model_key = model
+    key1 = None
+    if model_key is not None:
+        key1 = ('probabilities', id(eng), image.data_ptr(), tuple(image.shape), str(image.dtype), model_key, _features_key(dict_features),
+                sp_size, sp_regul)
+    return _run_resident(eng, lambda: _device_slic_features(eng, image, dict_features, sp_size, sp_regul), model, gc_regul, gc_edge_type,
+                         key1, early_soft)
 
 
 def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, debug_visual, classes=None):
@@ -280,7 +306,8 @@ def _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_t
         return graph_labels[slic], segm_soft
     gc_edge_type = reference_edge_type(gc_edge_type)
     while True:
-        d_segm, soft, check = _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, early_soft=True)
+        d_segm, soft, check = _run_resident_image(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type,
+                                                  early_soft=True)
         if check is None:   # no graph cut: both gathers were done at the end of the main stream
             (segm, soft), done = eng.download((d_segm, soft))
             done.synchronize()
@@ -337,6 +364,24 @@ def _over_streams(list_images, nb_streams, max_in_flight, launch, finish):
     return results
 
 
+def _resident_batch(items, nb_streams, max_in_flight, run, redo, classes):
+    """``run(eng, item)`` -> :func:`_run_resident`'s (d_segm, d_soft, check) for every item of a batch over :func:`_over_streams`,
+    each item's results downloaded with its edge count; an item whose edge table overflowed is redone by ``redo(index)`` -> host
+    (segm, segm_soft).  Returns (segm mapped through ``classes`` unless it is None, segm_soft) per item, in input order"""
+    def launch(eng, item):
+        d_segm, d_soft, check = run(eng, item)
+        return eng.download((d_segm, d_soft) + ((check[0], ) if check is not None else ())) + (check, )
+
+    def finish(idx, hosts, check):
+        if check is not None and not edges_fit(hosts[2][0], check[1]):
+            segm, soft = redo(idx)
+        else:
+            segm, soft = hosts[0].numpy(), hosts[1].numpy()
+        return (segm if classes is None else np.asarray(classes)[segm]), soft
+
+    return _over_streams(items, nb_streams, max_in_flight, launch, finish)
+
+
 def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIMPLE, sp_size=30, sp_regul=0.2, use_scaler=True,
                          gc_regul=1., gc_edge_type='model', model_pipeline=None, nb_streams=3, max_in_flight=6, estim_model='GMM',
                          pca_coef=None):
@@ -362,22 +407,16 @@ def segment_images_batch(list_images, nb_classes=None, dict_features=FTS_SET_SIM
     if model_pipeline is None:
         model = _fit_model(nb_classes, use_scaler, estim_model, pca_coef)
     else:
-        model = _compiled_model(model_pipeline, dict_features) or model_pipeline.predict_proba
-    classes = getattr(model_pipeline, 'classes_', None)
+        model = _device_model(model_pipeline.predict_proba, nb_fts)
     gc_edge_type = reference_edge_type(gc_edge_type)
 
-    def launch(eng, image):
-        d_segm, d_soft, check = _run_resident(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)
-        return eng.download((d_segm, d_soft) + ((check[0], ) if check is not None else ())) + (check, )
+    def run(eng, image):
+        return _run_resident_image(eng, image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)
 
-    def finish(idx, hosts, check):
-        if check is not None and not edges_fit(hosts[2][0], check[1]):
-            # the edge table overflowed: redo this image through the single-image path
-            return _segment(list_images[idx], model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, None, classes=classes)
-        segm = hosts[0].numpy()
-        return (segm if classes is None else np.asarray(classes)[segm]), hosts[1].numpy()
+    def redo(idx):      # through the single-image path
+        return _segment(list_images[idx], model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, None)
 
-    return _over_streams(list_images, nb_streams, max_in_flight, launch, finish)
+    return _resident_batch(list_images, nb_streams, max_in_flight, run, redo, getattr(model_pipeline, 'classes_', None))
 
 
 def compute_features_batch(list_images, dict_features, sp_size=30, sp_regul=0.2, nb_streams=3, max_in_flight=6):
@@ -571,33 +610,10 @@ def _volume_flags(dict_features):
     return [f for f in NAMES_FEATURE_FLAGS if f in flags]
 
 
-def _compiled_volume_model(model, n_features):
-    """the device form of a caller-fitted model for a volume feature table of ``n_features`` columns, or None (host predict_proba)"""
-    from . import graph_cuts
-    if not graph_cuts.USE_DEVICE_PREDICT:
-        return None
-    cm = compile_model(model)
-    return cm if cm is not None and cm.n_features_in == n_features else None
-
-
-def _volume_model(model, n_features):
-    """``model`` as _run_resident_volume takes it: a resident fit tuple and a CompiledModel stay as they are, a fitted model (or its
-    bound ``predict_proba``) is compiled when class_models supports it, anything else is called as proba_fn(features)"""
-    if isinstance(model, (tuple, CompiledModel)):
-        return model
-    fitted = model.__self__ if getattr(model, '__name__', None) == 'predict_proba' and hasattr(model, '__self__') else model
-    return _compiled_volume_model(fitted, n_features) or (model if callable(model) else model.predict_proba)
-
-
-def _run_resident_volume(eng, d_vol, model, dict_features, spacing, sp_size, sp_regul, gc_regul, gc_edge_type='model'):
-    """pipe_gray3d_slic_features_model_graphcut's hot path on the device: 3-D SLIC, the gray statistics into a device table,
-    norm_features (StandardScaler, bit for bit), the class model, the 6-connected supervoxel graph, its energies with the (z, y, x)
-    centroids, alpha-expansion and the two gathers.  ``model``: ('fit', nb_classes, use_scaler, max_iter[, kind, n_init, pca_coef])
-    (:func:`_fit_model`) or a :class:`~.class_models.CompiledModel` -> nothing syncs with the host; a callable proba_fn(features) ->
-    one round trip (the standardised features down, the probabilities up).  ``d_vol``: a gray volume [D, H, W] on the device or on
-    the host (uploaded).  Returns (d_segm int32 [D, H, W], d_soft f64 [D, H, W, K], check): ``check`` is None or (d_n_edges, edge_cap)
-    still to be verified by the caller (:func:`~.engine.edges_fit`)."""
-    from . import graph_cuts
+def _device_slic3d_features(eng, d_vol, dict_features, spacing, sp_size, sp_regul):
+    """pipe_gray3d_slic_features_model_graphcut's front on the device: 3-D SLIC, the gray statistics into a device table and
+    norm_features (StandardScaler, bit for bit), whose standardised table is ``d_feat``.  ``d_vol``: a gray volume [D, H, W] on the
+    device or on the host (uploaded)."""
     from .superpixels import slic3d_params
     flags = _volume_flags(dict_features)
     if flags is None:
@@ -613,26 +629,12 @@ def _run_resident_volume(eng, d_vol, model, dict_features, spacing, sp_size, sp_
     n_seg, compact = slic3d_params(shape, sp_size, sp_regul, spacing)
     if n_seg < 1 or compact < 1:
         raise ValueError('superpixel size %r / compactness do not fit the volume %r' % (sp_size, shape))
-    d_seg, d_n = eng.slic3d(d_vol, n_seg, compact, spacing, sigma=1.0)
-    nb = eng.slic_label_bound(int(np.prod(shape)), 1, n_seg)
-    d_feat = eng.gray_table(d_vol, d_seg, nb, flags)
-    d_x, _ = eng.standard_scaler(d_feat, d_n)
-    if isinstance(model, CompiledModel):
-        d_proba = eng.class_model_predict(d_x, model, d_n=d_n)
-    elif isinstance(model, tuple):
-        nb_classes, use_scaler, max_iter, kind, n_init, pca_coef = _fit_spec(model)
-        d_proba = graph_cuts.device_fit_predict(eng, d_x, nb_classes, use_scaler, kind, n_init, max_iter, pca_coef, d_n=d_n)[0]
-    else:
-        n = int(eng.to_host(d_n)[0])
-        proba = np.ascontiguousarray(model(eng.to_host(d_x[:n]).copy()), dtype=np.float64)
-        d_proba = eng.to_device(np.concatenate([proba, np.zeros((nb - n, proba.shape[1]))]), 'proba')
-    if (not isinstance(gc_regul, (list, np.ndarray))) and gc_regul <= 0:
-        proba = eng.to_host(d_proba[:int(eng.to_host(d_n)[0])])
-        return eng.gather(d_seg, _argmin_labels_device(eng, proba), d_proba) + (None, )
-    cap = edge_capacity(nb, ndim=3)
-    d_labels, d_n_edges = graph_cuts.device_graphcut(eng, d_seg, None, nb, d_proba, gc_regul, gc_edge_type, d_n, cap)
-    d_segm, d_soft = eng.gather(d_seg, d_labels, d_proba)
-    return d_segm, d_soft, (d_n_edges, cap)
+    res = DeviceSuperpixels()
+    res.shape, res.d_img, res.d_centres = shape, d_vol, None
+    res.d_seg, res.d_n_labels = eng.slic3d(d_vol, n_seg, compact, spacing, sigma=1.0)
+    res.nb_bound = eng.slic_label_bound(int(np.prod(shape)), 1, n_seg)
+    res.d_feat = eng.standard_scaler(eng.gray_table(d_vol, res.d_seg, res.nb_bound, flags), res.d_n_labels)[0]
+    return res
 
 
 def segment_resident_volume(d_vol, model, dict_features, spacing=(12, 1, 1), sp_size=15, sp_regul=0.2, gc_regul=0.1):
@@ -646,9 +648,10 @@ def segment_resident_volume(d_vol, model, dict_features, spacing=(12, 1, 1), sp_
     enqueued and redoes the volume with a larger table when it overflowed; nothing else synchronises with the host. """
     eng = get_engine()
     flags = _volume_flags(dict_features)
-    model = _volume_model(model, len(flags) if flags else 0)
+    model = _device_model(model, len(flags) if flags else None)
     while True:
-        d_segm, d_soft, check = _run_resident_volume(eng, d_vol, model, dict_features, spacing, sp_size, sp_regul, gc_regul)
+        d_segm, d_soft, check = _run_resident(eng, lambda: _device_slic3d_features(eng, d_vol, dict_features, spacing, sp_size, sp_regul),
+                                              model, gc_regul, 'model')
         if check is None or edges_fit(eng.to_host(check[0])[0], check[1]):
             return d_segm, d_soft
 
@@ -688,31 +691,25 @@ def segment_volumes_batch(list_volumes, nb_classes=None, model_pipeline=None, di
             return [_segment_volume_stages(v, proba_fn, dict_features, spacing, sp_size, sp_regul, gc_regul) for v in list_volumes]
         model = _fit_model(nb_classes, use_scaler)
     else:
-        model = _volume_model(model_pipeline, len(flags)) if flags is not None else model_pipeline.predict_proba
+        model = _device_model(model_pipeline, len(flags)) if flags is not None else model_pipeline.predict_proba
     classes = getattr(model_pipeline, 'classes_', None)
-
-    def relabel(segm):
-        return segm if classes is None else np.asarray(classes)[segm]
-
     if flags is None:
-        return [(relabel(segm), soft) for segm, soft in
-                (_segment_volume_stages(v, model, dict_features, spacing, sp_size, sp_regul, gc_regul) for v in list_volumes)]
+        out = [_segment_volume_stages(v, model, dict_features, spacing, sp_size, sp_regul, gc_regul) for v in list_volumes]
+        return [(segm if classes is None else np.asarray(classes)[segm], soft) for segm, soft in out]
 
-    def launch(eng, volume):
-        d_segm, d_soft, check = _run_resident_volume(eng, volume, model, dict_features, spacing, sp_size, sp_regul, gc_regul)
-        return eng.download((d_segm, d_soft) + ((check[0], ) if check is not None else ())) + (check, )
+    def run(eng, volume):
+        return _run_resident(eng, lambda: _device_slic3d_features(eng, volume, dict_features, spacing, sp_size, sp_regul), model, gc_regul,
+                             'model')
 
-    def finish(idx, hosts, check):
-        if check is not None and not edges_fit(hosts[2][0], check[1]):
-            # the edge table overflowed: redo this volume on the caller's stream with the grown table
-            d_segm, d_soft = segment_resident_volume(get_engine().to_device(_supported_dtype(np.asarray(list_volumes[idx])), 'volume'),
-                                                     model, dict_features, spacing, sp_size, sp_regul, gc_regul)
-            (segm, soft), done = get_engine().download((d_segm, d_soft))
-            done.synchronize()
-            return relabel(segm.numpy()), soft.numpy()
-        return relabel(hosts[0].numpy()), hosts[1].numpy()
+    def redo(idx):      # on the caller's stream with the grown table
+        eng = get_engine()
+        d_segm, d_soft = segment_resident_volume(eng.to_device(_supported_dtype(np.asarray(list_volumes[idx])), 'volume'), model,
+                                                 dict_features, spacing, sp_size, sp_regul, gc_regul)
+        (segm, soft), done = eng.download((d_segm, d_soft))
+        done.synchronize()
+        return segm.numpy(), soft.numpy()
 
-    return _over_streams(list_volumes, nb_streams, max_in_flight, launch, finish)
+    return _resident_batch(list_volumes, nb_streams, max_in_flight, run, redo, classes)
 
 
 def segment_resident(d_image, model, dict_features, sp_size=30, sp_regul=0.2, gc_regul=1., gc_edge_type='model'):
@@ -727,10 +724,8 @@ def segment_resident(d_image, model, dict_features, sp_size=30, sp_regul=0.2, gc
     Nothing here waits for the device, so the edge count of the graph cut is not checked against its table as the host-facing
     pipelines do: after the connectivity pass every superpixel is connected, the region graph of a 2-D map is planar with at most
     3N - 6 edges, and the table holds 8 per node of an upper bound of N. """
-    if not isinstance(model, (tuple, CompiledModel)):
-        fitted = model.__self__ if getattr(model, '__name__', None) == 'predict_proba' and hasattr(model, '__self__') else model
-        model = _compiled_model(fitted, dict_features) or (model if callable(model) else model.predict_proba)
-    return _run_resident(get_engine(), d_image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)[:2]
+    model = _device_model(model, _resident_width(dict_features))
+    return _run_resident_image(get_engine(), d_image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type)[:2]
 
 
 def pipe_color2d_slic_features_model_graphcut(image, nb_classes, dict_features, sp_size=30, sp_regul=0.2, pca_coef=None,
@@ -777,5 +772,5 @@ def segment_color2d_slic_features_model_graphcut(image, model_pipeline, dict_fea
     classes = getattr(model_pipeline, 'classes_', None)
     model = model_pipeline.predict_proba
     if debug_visual is None and np.ndim(image) == 3 and gc_edge_type not in ('color', 'features'):
-        model = _compiled_model(model_pipeline, dict_features) or model
+        model = _device_model(model, _resident_width(dict_features))
     return _segment(image, model, dict_features, sp_size, sp_regul, gc_regul, gc_edge_type, debug_visual, classes=classes)

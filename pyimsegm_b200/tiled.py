@@ -661,6 +661,25 @@ def _banded_segment(eng, shape, comm, bands_per_rank, front, gc_regul, gc_edge_t
     return h_segm.numpy(), (soft[0].numpy() if want_soft else None), (lo, hi)
 
 
+def _segment_banded_image(image, n_seg, compact, layout, ncol, margin, model, gc_regul, gc_edge_type, comm, bands_per_rank, want_soft,
+                          gather_segm):
+    """the banded image pipeline after the argument checks (:func:`_admit`, :func:`_prepare_image`): banded SLIC, the feature table
+    of ``layout``, the class probabilities of ``model`` (a model of :func:`~.pipelines._device_proba`, on the replicated table of
+    every rank) and the tail of :func:`_banded_segment`"""
+    from .pipelines import _device_proba
+    eng = get_engine()
+    comm = comm or default_comm()
+
+    def front(force_whole):
+        res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
+                         force_whole=force_whole, raw_margin=margin)
+        features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
+        return res, _device_proba(eng, model, res.d_feat, res.d_n_labels, res.nb_bound)
+
+    return _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm,
+                           lambda res: banded_edge_vectors(res, image.dtype, gc_edge_type, comm, eng))
+
+
 def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_features=None, sp_size=30, sp_regul=0.2, use_scaler=True,
                                                     gc_regul=1., gc_edge_type='model', max_iter=99, comm=None, bands_per_rank=1,
                                                     want_soft=True, gather_segm=False, estim_model='GMM', pca_coef=None):
@@ -673,6 +692,7 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
         ``segm`` is the whole [H, W] map on every rank (``segm_soft`` stays banded: it is 8*K bytes per pixel)
     """
     from . import graph_cuts
+    from .pipelines import _fit_model
     graph_cuts.check_edge_type(gc_edge_type)
     if sp_regul <= 0.:
         raise ValueError('slic. regularisation must be positive')
@@ -682,21 +702,10 @@ def pipe_color2d_slic_features_model_graphcut_tiled(image, nb_classes, dict_feat
         raise NotImplementedError('the banded path fits the class model on the GPU, which does not take estim_model=%r, pca_coef=%r with '
                                   '%d features and %d classes' % (estim_model, pca_coef, ncol, nb_classes))
     # the default 'GMM' gives (GMM, sqrt(max_iter) restarts, max_iter): the mixture fit the banded path has always made
-    kind, n_init, n_iter = graph_cuts.class_model_spec(estim_model, nb_classes, max_iter)
+    model = _fit_model(int(nb_classes), use_scaler, estim_model, pca_coef, max_iter)
     image, n_seg, compact = _prepare_image(image, layout, sp_size, sp_regul)
-    eng = get_engine()
-    comm = comm or default_comm()
-
-    def front(force_whole):
-        res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
-                         force_whole=force_whole, raw_margin=margin)
-        features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
-        d_proba = graph_cuts.device_fit_predict(eng, res.d_feat, int(nb_classes), use_scaler, kind, n_init, n_iter, pca_coef,
-                                                graph_cuts.RANDOM_SEED, d_n=res.d_n_labels)[0]
-        return res, d_proba
-
-    return _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm,
-                           lambda res: banded_edge_vectors(res, image.dtype, gc_edge_type, comm, eng))
+    return _segment_banded_image(image, n_seg, compact, layout, ncol, margin, model, gc_regul, gc_edge_type, comm, bands_per_rank, want_soft,
+                                 gather_segm)
 
 
 def segment_color2d_slic_features_model_graphcut_tiled(image, model_pipeline, dict_features, sp_size=30, sp_regul=0.2, gc_regul=1.,
@@ -712,33 +721,16 @@ def segment_color2d_slic_features_model_graphcut_tiled(image, model_pipeline, di
         :func:`pipe_color2d_slic_features_model_graphcut_tiled`
     """
     from .graph_cuts import check_edge_type
-    from .pipelines import _compiled_model
+    from .pipelines import _device_model
     check_edge_type(gc_edge_type)
     if sp_regul <= 0.:
         raise ValueError('slic. regularisation must be positive')
     layout, ncol, margin = _admit(dict_features)
     image, n_seg, compact = _prepare_image(image, layout, sp_size, sp_regul)
+    model = _device_model(model_pipeline.predict_proba, ncol)
+    segm, soft, rows = _segment_banded_image(image, n_seg, compact, layout, ncol, margin, model, gc_regul, gc_edge_type, comm, bands_per_rank,
+                                             want_soft, gather_segm)
     classes = getattr(model_pipeline, 'classes_', None)
-    eng = get_engine()
-    comm = comm or default_comm()
-    compiled = _compiled_model(model_pipeline, dict_features)
-
-    def front(force_whole):
-        res = slic_tiled(image, n_seg, compact, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
-                         force_whole=force_whole, raw_margin=margin)
-        features_tiled(res, image.dtype, int(image.shape[2]), layout, ncol, comm=comm, eng=eng)
-        if compiled is not None:
-            return res, eng.class_model_predict(res.d_feat, compiled, d_n=res.d_n_labels)
-        nb = int(eng.to_host(res.d_n_labels)[0])
-        features = eng.to_host(res.d_feat[:nb, :ncol]).copy()
-        features[np.isnan(features)] = 0
-        proba = np.asarray(model_pipeline.predict_proba(features), dtype=np.float64)
-        padded = np.zeros((int(res.nb_bound), proba.shape[1]))      # the rows of the label bound, as a device model gives
-        padded[:nb] = proba
-        return res, eng.to_device(padded, 'proba')
-
-    segm, soft, rows = _banded_segment(eng, image.shape[:2], comm, bands_per_rank, front, gc_regul, gc_edge_type, want_soft, gather_segm,
-                                       lambda res: banded_edge_vectors(res, image.dtype, gc_edge_type, comm, eng))
     if classes is not None:
         segm = np.asarray(classes)[segm]
     return segm, soft, rows
@@ -920,12 +912,20 @@ def _prepare_volume(volume, sp_size, sp_regul, spacing, n_slabs):
     return _supported_dtype(volume), n_seg, compact
 
 
-def _volume_front(eng, volume, n_seg, compact, spacing, flags, comm, bands_per_rank, force_whole):
-    """slab SLIC, the statistics table and norm_features (the device StandardScaler): (res, standardised features [nb, len(flags)])"""
-    res = slic3d_tiled(volume, n_seg, compact, spacing, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
-                       force_whole=force_whole)
-    feat = gray_stats_tiled(res, volume.dtype, flags, comm=comm, eng=eng)
-    return res, eng.standard_scaler(feat, res.d_n_labels)[0]
+def _segment_banded_volume(volume, n_seg, compact, spacing, flags, model, gc_regul, comm, bands_per_rank, want_soft, gather_segm):
+    """the slab volume pipeline after the argument checks (:func:`_admit_volume`, :func:`_prepare_volume`): slab SLIC, the statistics
+    table and norm_features (the device StandardScaler), the class probabilities of ``model`` (a model of
+    :func:`~.pipelines._device_proba`, on the replicated standardised table of every rank) and the tail of :func:`_banded_segment`"""
+    from .pipelines import _device_proba
+    eng = get_engine()
+
+    def front(force_whole):
+        res = slic3d_tiled(volume, n_seg, compact, spacing, sigma=1.0, comm=comm, bands_per_rank=bands_per_rank, eng=eng, defer_check=True,
+                           force_whole=force_whole)
+        d_x = eng.standard_scaler(gray_stats_tiled(res, volume.dtype, flags, comm=comm, eng=eng), res.d_n_labels)[0]
+        return res, _device_proba(eng, model, d_x, res.d_n_labels, res.nb_bound)
+
+    return _banded_segment(eng, volume.shape, comm, bands_per_rank, front, gc_regul, 'model', want_soft, gather_segm)
 
 
 def pipe_gray3d_slic_features_model_graphcut_tiled(volume, nb_classes, dict_features, spacing=(12, 1, 1), sp_size=15, sp_regul=0.2,
@@ -940,19 +940,14 @@ def pipe_gray3d_slic_features_model_graphcut_tiled(volume, nb_classes, dict_feat
         ``segm`` is the whole [D, H, W] volume on every rank (``segm_soft`` stays sliced: it is 8*K bytes per voxel)
     """
     from . import graph_cuts
+    from .pipelines import _fit_model
     flags = _admit_volume(dict_features)
     if not graph_cuts.device_gmm_applicable(len(flags), nb_classes):
         raise NotImplementedError('the slab path fits the class model on the GPU, which does not take %d classes' % nb_classes)
-    kind, n_init, n_iter = graph_cuts.class_model_spec('GMM', nb_classes, max_iter)
+    model = _fit_model(int(nb_classes), use_scaler, 'GMM', None, max_iter)
     comm = comm or default_comm()
     volume, n_seg, compact = _prepare_volume(volume, sp_size, sp_regul, spacing, comm.world * int(bands_per_rank))
-    eng = get_engine()
-
-    def front(force_whole):
-        res, d_x = _volume_front(eng, volume, n_seg, compact, spacing, flags, comm, bands_per_rank, force_whole)
-        return res, graph_cuts.device_fit_predict(eng, d_x, int(nb_classes), use_scaler, kind, n_init, n_iter, None, d_n=res.d_n_labels)[0]
-
-    return _banded_segment(eng, volume.shape, comm, bands_per_rank, front, gc_regul, 'model', want_soft, gather_segm)
+    return _segment_banded_volume(volume, n_seg, compact, spacing, flags, model, gc_regul, comm, bands_per_rank, want_soft, gather_segm)
 
 
 def segment_gray3d_slic_features_model_graphcut_tiled(volume, model_pipeline, dict_features, spacing=(12, 1, 1), sp_size=15, sp_regul=0.2,
@@ -965,25 +960,14 @@ def segment_gray3d_slic_features_model_graphcut_tiled(volume, model_pipeline, di
     :return tuple: (segm [slices, H, W], segm_soft [slices, H, W, K] float64 or None, (z_lo, z_hi)) as
         :func:`pipe_gray3d_slic_features_model_graphcut_tiled`
     """
-    from .pipelines import _compiled_volume_model
+    from .pipelines import _device_model
     flags = _admit_volume(dict_features)
     comm = comm or default_comm()
     volume, n_seg, compact = _prepare_volume(volume, sp_size, sp_regul, spacing, comm.world * int(bands_per_rank))
+    model = _device_model(model_pipeline.predict_proba, len(flags))
+    segm, soft, rows = _segment_banded_volume(volume, n_seg, compact, spacing, flags, model, gc_regul, comm, bands_per_rank, want_soft,
+                                              gather_segm)
     classes = getattr(model_pipeline, 'classes_', None)
-    eng = get_engine()
-    compiled = _compiled_volume_model(model_pipeline, len(flags))
-
-    def front(force_whole):
-        res, d_x = _volume_front(eng, volume, n_seg, compact, spacing, flags, comm, bands_per_rank, force_whole)
-        if compiled is not None:
-            return res, eng.class_model_predict(d_x, compiled, d_n=res.d_n_labels)
-        nb = int(eng.to_host(res.d_n_labels)[0])
-        proba = np.asarray(model_pipeline.predict_proba(eng.to_host(d_x[:nb]).copy()), dtype=np.float64)
-        padded = np.zeros((int(res.nb_bound), proba.shape[1]))      # the rows of the label bound, as a device model gives
-        padded[:nb] = proba
-        return res, eng.to_device(padded, 'proba')
-
-    segm, soft, rows = _banded_segment(eng, volume.shape, comm, bands_per_rank, front, gc_regul, 'model', want_soft, gather_segm)
     if classes is not None:
         segm = np.asarray(classes)[segm]
     return segm, soft, rows
