@@ -187,7 +187,8 @@ int isb_enforce_connectivity3d(const int32_t* labels, int D, int H, int W, int m
 
 /* computeColorImage2dMean :81, ...Energy :101, ...Variance :122 and normColorFeatures :59 in one launch family,
  * plus the centroids of imsegm/superpixels.py:205-224.  Pixels are converted to f32 (descriptors.py:233),
- * accumulated in f64.
+ * accumulated in f64: per-column runs, summed across the lanes of a warp, then the correctly rounded sum of those partials
+ * per label, so a rerun on the same input gives the same bits.  At most 2^31 pixels per call.
  *   img     : [H,W,3] interleaved, dtype = isb_dtype (NaN -> 0 as descriptors.py:824)
  *   seg     : [H,W] i32 in [0, nb)
  *   flags   : bit0 mean, bit1 std, bit2 energy  -> feature columns in that order, 3 channels each
@@ -199,8 +200,10 @@ int isb_segment_stats_2d(const void* img, int dtype, const int32_t* seg, int H, 
 
 /* The same statistics with caller-owned accumulators, so that row bands of one image can be merged by a collective between
  * the calls: acc [nb,6] f64 (sum c0..c2, sum of squares c0..c2), iacc [nb,3] i64 (count, sum row, sum col), var [nb,3] f64
- * (squared deviations from the f32 mean).  accumulate / deviation ADD into acc+iacc / var (the caller zeroes them);
- * rows are global rows [y_off, y_off + H) of the image for the row sums. */
+ * (squared deviations from the f32 mean).  accumulate / deviation ADD into acc+iacc / var (the caller zeroes them), one f64
+ * add per entry of the band's rounded sums, so a rerun with the same bands gives the same bits (other bands, other bits);
+ * rows are global rows [y_off, y_off + H) of the image for the row sums.  The band's exact sums (484 B per label for accumulate,
+ * 244 B for deviation) are allocated and freed on `stream` within the call (cudaMallocAsync / cudaFreeAsync). */
 int isb_segment_stats_accumulate(const void* img, int dtype, const int32_t* seg, int H, int W, int y_off, int nb, double* acc,
                                  int64_t* iacc, isb_stream_t stream);
 int isb_segment_stats_deviation(const void* img, int dtype, const int32_t* seg, int H, int W, int nb, const double* acc,
@@ -208,14 +211,16 @@ int isb_segment_stats_deviation(const void* img, int dtype, const int32_t* seg, 
 int isb_segment_stats_finish(int nb, int flags, const double* acc, const double* var, const int64_t* iacc, double* feat, int ld,
                              int col0, double* centres, int32_t* counts, isb_stream_t stream);
 
-/* computeGrayImage3dMean :144 / Energy :169 / Variance :194 of features_cython.pyx: one channel, any rank (n voxels).
+/* computeGrayImage3dMean :144 / Energy :169 / Variance :194 of features_cython.pyx: one channel, any rank (n <= 2^31 voxels).
+ * Runs of 16 voxels, then the correctly rounded sum of their partials per label: a rerun gives the same bits.
  *   flags bit0 mean, bit1 std, bit2 energy -> columns col0.. of feat [nb, ld] in that order */
 size_t isb_gray_stats_workspace_bytes(int nb);
 int isb_gray_stats(const void* img, int dtype, const int32_t* seg, long long n, int nb, int flags, double* feat, int ld, int col0,
                    void* ws, size_t ws_bytes, isb_stream_t stream);
 /* The same statistics with caller-owned accumulators, so that z-slabs of one volume can be merged by a collective between the
  * calls (isb_gray_stats runs exactly these three steps): acc [nb,2] f64 (sum, sum of squares), cnt [nb] i64, var [nb] f64
- * (squared deviations from the f32 mean).  accumulate / deviation ADD into acc+cnt / var (the caller zeroes them). */
+ * (squared deviations from the f32 mean).  accumulate / deviation ADD into acc+cnt / var (the caller zeroes them), one f64 add
+ * per entry of the slab's rounded sums; the slab's exact sums are allocated and freed on `stream` within the call, as above. */
 int isb_gray_stats_accumulate(const void* img, int dtype, const int32_t* seg, long long n, int nb, double* acc, int64_t* cnt,
                               isb_stream_t stream);
 int isb_gray_stats_deviation(const void* img, int dtype, const int32_t* seg, long long n, int nb, const double* acc, const int64_t* cnt,

@@ -4,7 +4,7 @@
 //   computeRayFeaturesBinary2d :239                                  (distance to the first boundary along rays, f32 marching)
 // They sit beside the hot path (3-D gray pipeline, RG2SP / centre detection: SURVEY.md section 8f) and are provided so that
 // the whole native surface of the reference has a device entry point.
-#include "common.cuh"
+#include "exact_sum.cuh"
 
 namespace {
 
@@ -12,9 +12,11 @@ constexpr int GSTRIP = 16;
 
 __device__ __forceinline__ float clean(float v) { return isnan(v) ? 0.0f : v; }
 
-// pass 0: sum, sum of squares (f32 product) -> acc [nb][2], count -> cnt.  pass 1: sum (v - mean_f32)^2 -> acc [nb] (the variance sums).
+// pass 0: sum, sum of squares (f32 product) -> exact sums x [nb][2][XS_DIGITS], count -> cnt.  pass 1: sum (v - mean_f32)^2 -> x [nb][1][..]
+// (the variance sums).  Every run a thread ends flushes its partials into the label's exact sums (exact_sum.cuh), so the totals do
+// not depend on the order of the flushes.
 __global__ void __launch_bounds__(256) k_gray_stats(const void* __restrict__ img, int dtype, const int* __restrict__ seg, long long n, int pass,
-                                                    double* acc, long long* cnt, const float* meanf)
+                                                    long long* x, unsigned* xflag, long long* cnt, const float* meanf)
 {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long beg = t * GSTRIP, end = min(beg + GSTRIP, n);
@@ -27,8 +29,11 @@ __global__ void __launch_bounds__(256) k_gray_stats(const void* __restrict__ img
         const int l = i < end ? seg[i] : -1;
         if (l != cur) {
             if (cur >= 0) {
-                if (pass == 0) { atomicAdd(&acc[2 * (size_t)cur], s); atomicAdd(&acc[2 * (size_t)cur + 1], e); atomicAdd((unsigned long long*)&cnt[cur], (unsigned long long)c); }
-                else atomicAdd(&acc[cur], s);
+                if (pass == 0) {
+                    long long* xa = x + 2 * XS_DIGITS * (size_t)cur;
+                    xs_add(xa, xflag + cur, 0, s); xs_add(xa + XS_DIGITS, xflag + cur, 1, e);
+                    atomicAdd((unsigned long long*)&cnt[cur], (unsigned long long)c);
+                } else xs_add(x + XS_DIGITS * (size_t)cur, xflag + cur, 0, s);
             }
             cur = l; s = 0; e = 0; c = 0;
             if (pass == 1 && l >= 0) m = meanf[l];
@@ -149,21 +154,60 @@ struct GrayWs {
     long long* cnt;   // [nb]
     float* meanf;     // [nb]
     double* var;      // [nb]
+    long long* xacc;  // [nb][2][XS_DIGITS]  exact sums of pass 0, rounded into acc
+    unsigned* xflag0; // [nb]
+    long long* xvar;  // [nb][XS_DIGITS]     exact sums of pass 1, rounded into var
+    unsigned* xflag1; // [nb]
 };
 
-static size_t carve_gray(GrayWs& w, void* ws, size_t bytes, int nb)
+// dense tables first, then the exact sums of pass 0 (from *x0) and of pass 1 (from *x1), each a contiguous range that its pass zeroes
+static size_t carve_gray(GrayWs& w, void* ws, size_t bytes, int nb, size_t* x0 = nullptr, size_t* x1 = nullptr)
 {
     WsCarver c(ws, bytes);
     w.acc = c.take<double>(2 * (size_t)nb);
     w.cnt = c.take<long long>(nb);
     w.meanf = c.take<float>(nb);
     w.var = c.take<double>(nb);
-    return isb_align(c.off);
+    const size_t o0 = isb_align(c.off);
+    const size_t o1 = o0 + xs_carve((char*)ws + o0, nb, 2, &w.xacc, &w.xflag0);
+    const size_t end = o1 + xs_carve((char*)ws + o1, nb, 1, &w.xvar, &w.xflag1);
+    if (x0) *x0 = o0;
+    if (x1) *x1 = o1;
+    return end;
 }
 
 static unsigned gray_blocks(long long n) { return (unsigned)(((n + GSTRIP - 1) / GSTRIP + 255) / 256); }
 
+// pass 0 into the exact sums (xbytes from x, zeroed here: digits xacc, flags xflag), rounded and added into acc; counts into cnt
+static int gray_pass0(const void* img, int dtype, const int32_t* seg, long long n, int nb, double* acc, int64_t* cnt, long long* xacc,
+                      unsigned* xflag, void* x, size_t xbytes, cudaStream_t st)
+{
+    ISB_CUDA_CHECK(cudaMemsetAsync(x, 0, xbytes, st));
+    k_gray_stats<<<gray_blocks(n), 256, 0, st>>>(img, dtype, seg, n, 0, xacc, xflag, (long long*)cnt, nullptr);
+    ISB_LAUNCH_CHECK();
+    k_exact_fold<<<(unsigned)((2 * (long long)nb + 255) / 256), 256, 0, st>>>(nb, 2, xacc, xflag, acc);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+// the f32 means into meanf, pass 1 into the exact sums (as pass 0), rounded and added into var
+static int gray_pass1(const void* img, int dtype, const int32_t* seg, long long n, int nb, const double* acc, const int64_t* cnt,
+                      float* meanf, double* var, long long* xvar, unsigned* xflag, void* x, size_t xbytes, cudaStream_t st)
+{
+    ISB_CUDA_CHECK(cudaMemsetAsync(x, 0, xbytes, st));
+    k_gray_means<<<(nb + 255) / 256, 256, 0, st>>>(nb, acc, (const long long*)cnt, meanf);
+    ISB_LAUNCH_CHECK();
+    k_gray_stats<<<gray_blocks(n), 256, 0, st>>>(img, dtype, seg, n, 1, xvar, xflag, nullptr, meanf);
+    ISB_LAUNCH_CHECK();
+    k_exact_fold<<<(unsigned)((nb + 255) / 256), 256, 0, st>>>(nb, 1, xvar, xflag, var);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
 } // namespace
+
+// a label's exact sums take one partial per flushed run, at most one per voxel: 2^31 of them fit (exact_sum.cuh)
+#define ISB_REQUIRE_FLUSHES(n) ISB_REQUIRE((n) <= (1ll << 31), "more than 2^31 voxels in one call")
 
 extern "C" size_t isb_gray_stats_workspace_bytes(int nb)
 {
@@ -171,14 +215,21 @@ extern "C" size_t isb_gray_stats_workspace_bytes(int nb)
     return carve_gray(w, nullptr, 0, nb);
 }
 
+// the slab's exact sums live in memory allocated on the caller's stream for the call
 extern "C" int isb_gray_stats_accumulate(const void* img, int dtype, const int32_t* seg, long long n, int nb, double* acc, int64_t* cnt,
                                          isb_stream_t stream)
 {
     ISB_REQUIRE(img && seg && acc && cnt, "null pointer");
     ISB_REQUIRE(n > 0 && nb > 0 && dtype >= ISB_U8 && dtype <= ISB_F64, "bad arguments");
-    k_gray_stats<<<gray_blocks(n), 256, 0, (cudaStream_t)stream>>>(img, dtype, seg, n, 0, acc, (long long*)cnt, nullptr);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
+    ISB_REQUIRE_FLUSHES(n);
+    cudaStream_t st = (cudaStream_t)stream;
+    long long* xacc;
+    unsigned* xflag;
+    const size_t xb = xs_carve(nullptr, nb, 2, &xacc, &xflag);
+    StreamScratch x(st);
+    ISB_CUDA_CHECK(cudaMallocAsync(&x.p, xb, st));
+    xs_carve(x.p, nb, 2, &xacc, &xflag);
+    return gray_pass0(img, dtype, seg, n, nb, acc, cnt, xacc, xflag, x.p, xb, st);
 }
 
 extern "C" int isb_gray_stats_deviation(const void* img, int dtype, const int32_t* seg, long long n, int nb, const double* acc,
@@ -186,12 +237,15 @@ extern "C" int isb_gray_stats_deviation(const void* img, int dtype, const int32_
 {
     ISB_REQUIRE(img && seg && acc && cnt && meanf_scratch && var, "null pointer");
     ISB_REQUIRE(n > 0 && nb > 0 && dtype >= ISB_U8 && dtype <= ISB_F64, "bad arguments");
+    ISB_REQUIRE_FLUSHES(n);
     cudaStream_t st = (cudaStream_t)stream;
-    k_gray_means<<<(nb + 255) / 256, 256, 0, st>>>(nb, acc, (const long long*)cnt, meanf_scratch);
-    ISB_LAUNCH_CHECK();
-    k_gray_stats<<<gray_blocks(n), 256, 0, st>>>(img, dtype, seg, n, 1, var, nullptr, meanf_scratch);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
+    long long* xvar;
+    unsigned* xflag;
+    const size_t xb = xs_carve(nullptr, nb, 1, &xvar, &xflag);
+    StreamScratch x(st);
+    ISB_CUDA_CHECK(cudaMallocAsync(&x.p, xb, st));
+    xs_carve(x.p, nb, 1, &xvar, &xflag);
+    return gray_pass1(img, dtype, seg, n, nb, acc, cnt, meanf_scratch, var, xvar, xflag, x.p, xb, st);
 }
 
 extern "C" int isb_gray_stats_finish(int nb, int flags, const double* acc, const double* var, const int64_t* cnt, double* feat, int ld,
@@ -209,14 +263,17 @@ extern "C" int isb_gray_stats(const void* img, int dtype, const int32_t* seg, lo
 {
     ISB_REQUIRE(img && seg && feat && ws, "null pointer");
     ISB_REQUIRE(n > 0 && nb > 0 && dtype >= ISB_U8 && dtype <= ISB_F64, "bad arguments");
+    ISB_REQUIRE_FLUSHES(n);
     GrayWs w;
-    const size_t need = carve_gray(w, ws, ws_bytes, nb);
+    size_t x0, x1;
+    const size_t need = carve_gray(w, ws, ws_bytes, nb, &x0, &x1);
     ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    ISB_CUDA_CHECK(cudaMemsetAsync(ws, 0, need, st));
-    if (int rc = isb_gray_stats_accumulate(img, dtype, seg, n, nb, w.acc, (int64_t*)w.cnt, stream)) return rc;
+    ISB_CUDA_CHECK(cudaMemsetAsync(ws, 0, x0, st));
+    if (int rc = gray_pass0(img, dtype, seg, n, nb, w.acc, (int64_t*)w.cnt, w.xacc, w.xflag0, (char*)ws + x0, x1 - x0, st)) return rc;
     if (flags & 2)
-        if (int rc = isb_gray_stats_deviation(img, dtype, seg, n, nb, w.acc, (const int64_t*)w.cnt, w.meanf, w.var, stream)) return rc;
+        if (int rc = gray_pass1(img, dtype, seg, n, nb, w.acc, (const int64_t*)w.cnt, w.meanf, w.var, w.xvar, w.xflag1, (char*)ws + x1,
+                                need - x1, st)) return rc;
     return isb_gray_stats_finish(nb, flags, w.acc, w.var, (const int64_t*)w.cnt, feat, ld, col0, stream);
 }
 

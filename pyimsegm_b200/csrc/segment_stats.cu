@@ -10,9 +10,11 @@
 //
 // Mapping: a thread owns one image column inside a strip of SROWS rows, so warp loads are coalesced along x and
 // label runs along y (~ one superpixel height) are accumulated in registers; the runs that end in the same row on neighbouring
-// lanes with the same label are summed across the warp, and one lane flushes them with one set of atomics.
+// lanes with the same label are summed across the warp, and one lane flushes them.  The f64 sums of the flushes are added exactly
+// (exact_sum.cuh) and rounded once per label, so a launch gives the same bits whatever order the warps flush in; the integer sums
+// (count, rows, columns) keep plain integer atomics.
 // Algorithmic HBM bytes: pass 1 = image bytes + 4 B/px labels, pass 2 the same.
-#include "common.cuh"
+#include "exact_sum.cuh"
 
 namespace {
 
@@ -23,6 +25,10 @@ struct StatWs {
     double* var;      // [nb][3]
     long long* iacc;  // [nb][3]  count, sum row, sum col
     float* meanf;     // [nb][3]
+    long long* xacc;  // [nb][6][XS_DIGITS]  exact sums of pass 1, rounded into acc
+    unsigned* xflag1; // [nb]
+    long long* xvar;  // [nb][3][XS_DIGITS]  exact sums of pass 2, rounded into var
+    unsigned* xflag2; // [nb]
 };
 
 __device__ __forceinline__ float clean(float v) { return isnan(v) ? 0.0f : v; } // np.nan_to_num (descriptors.py:824)
@@ -89,9 +95,10 @@ __global__ void __launch_bounds__(256) k_stats_pass1(const void* __restrict__ im
             const int tc = seg_sum(cnt, end);
             const long long ty = seg_sum(sy, end), tx = seg_sum((long long)cnt * x, end);
             if (head) {
-                double* a = ws.acc + 6 * (size_t)cur;
-                atomicAdd(a, t0); atomicAdd(a + 1, t1); atomicAdd(a + 2, t2);
-                atomicAdd(a + 3, u0); atomicAdd(a + 4, u1); atomicAdd(a + 5, u2);
+                long long* xa = ws.xacc + 6 * XS_DIGITS * (size_t)cur;
+                unsigned* fl = ws.xflag1 + cur;
+                xs_add(xa, fl, 0, t0); xs_add(xa + XS_DIGITS, fl, 1, t1); xs_add(xa + 2 * XS_DIGITS, fl, 2, t2);
+                xs_add(xa + 3 * XS_DIGITS, fl, 3, u0); xs_add(xa + 4 * XS_DIGITS, fl, 4, u1); xs_add(xa + 5 * XS_DIGITS, fl, 5, u2);
                 unsigned long long* ia = (unsigned long long*)(ws.iacc + 3 * (size_t)cur);
                 atomicAdd(ia, (unsigned long long)tc);
                 atomicAdd(ia + 1, (unsigned long long)ty);
@@ -154,8 +161,9 @@ __global__ void __launch_bounds__(256) k_stats_pass2(const void* __restrict__ im
             const int end = run_segment_end(flush, cur, &head);
             const double t0 = seg_sum(a0, end), t1 = seg_sum(a1, end), t2 = seg_sum(a2, end);
             if (head) {
-                double* a = ws.var + 3 * (size_t)cur;
-                atomicAdd(a, t0); atomicAdd(a + 1, t1); atomicAdd(a + 2, t2);
+                long long* xv = ws.xvar + 3 * XS_DIGITS * (size_t)cur;
+                unsigned* fl = ws.xflag2 + cur;
+                xs_add(xv, fl, 0, t0); xs_add(xv + XS_DIGITS, fl, 1, t1); xs_add(xv + 2 * XS_DIGITS, fl, 2, t2);
             }
         }
         if (l != cur) {
@@ -197,17 +205,54 @@ __global__ void k_stats_finalize(int nb, int flags, StatWs ws, double* feat, int
     if (counts) counts[k] = (int)c;
 }
 
-static size_t carve(StatWs& w, void* ws, size_t bytes, int nb)
+// dense tables first, then the exact sums of pass 1 (from *x1) and of pass 2 (from *x2), each a contiguous range that its pass zeroes
+static size_t carve(StatWs& w, void* ws, size_t bytes, int nb, size_t* x1 = nullptr, size_t* x2 = nullptr)
 {
     WsCarver c(ws, bytes);
     w.acc = c.take<double>(6 * (size_t)nb);
     w.var = c.take<double>(3 * (size_t)nb);
     w.iacc = c.take<long long>(3 * (size_t)nb);
     w.meanf = c.take<float>(3 * (size_t)nb);
-    return isb_align(c.off);
+    const size_t o1 = isb_align(c.off);
+    const size_t o2 = o1 + xs_carve((char*)ws + o1, nb, 6, &w.xacc, &w.xflag1);
+    const size_t end = o2 + xs_carve((char*)ws + o2, nb, 3, &w.xvar, &w.xflag2);
+    if (x1) *x1 = o1;
+    if (x2) *x2 = o2;
+    return end;
+}
+
+// pass 1 into the exact sums w.xacc / w.xflag1 (the xbytes from x, zeroed here), rounded and added into w.acc; the integer sums
+// go straight into w.iacc
+static int stats_pass1(const void* img, int dtype, const int32_t* seg, int H, int W, int y_off, int nb, const StatWs& w, void* x,
+                       size_t xbytes, cudaStream_t st)
+{
+    ISB_CUDA_CHECK(cudaMemsetAsync(x, 0, xbytes, st));
+    k_stats_pass1<<<dim3((W + 255) / 256, (H + SROWS - 1) / SROWS), 256, 0, st>>>(img, dtype, seg, H, W, y_off, w);
+    ISB_LAUNCH_CHECK();
+    k_exact_fold<<<(unsigned)((6 * (long long)nb + 255) / 256), 256, 0, st>>>(nb, 6, w.xacc, w.xflag1, w.acc);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
+}
+
+// the f32 means from w.acc / w.iacc into w.meanf, pass 2 into the exact sums w.xvar / w.xflag2 (the xbytes from x, zeroed here),
+// rounded and added into w.var
+static int stats_pass2(const void* img, int dtype, const int32_t* seg, int H, int W, int nb, const StatWs& w, void* x, size_t xbytes,
+                       cudaStream_t st)
+{
+    ISB_CUDA_CHECK(cudaMemsetAsync(x, 0, xbytes, st));
+    k_stats_means<<<(nb + 255) / 256, 256, 0, st>>>(nb, w);
+    ISB_LAUNCH_CHECK();
+    k_stats_pass2<<<dim3((W + 255) / 256, (H + SROWS - 1) / SROWS), 256, 0, st>>>(img, dtype, seg, H, W, w);
+    ISB_LAUNCH_CHECK();
+    k_exact_fold<<<(unsigned)((3 * (long long)nb + 255) / 256), 256, 0, st>>>(nb, 3, w.xvar, w.xflag2, w.var);
+    ISB_LAUNCH_CHECK();
+    return ISB_OK;
 }
 
 } // namespace
+
+// a label's exact sums take one partial per flush, at most one per pixel: 2^31 of them fit (exact_sum.cuh)
+#define ISB_REQUIRE_FLUSHES(npx) ISB_REQUIRE((npx) <= (1ll << 31), "more than 2^31 pixels in one call")
 
 extern "C" size_t isb_segment_stats_workspace_bytes(int nb)
 {
@@ -221,43 +266,42 @@ extern "C" int isb_segment_stats_2d(const void* img, int dtype, const int32_t* s
 {
     ISB_REQUIRE(seg && ws && (img || (flags & 7) == 0), "null pointer");
     ISB_REQUIRE(H > 0 && W > 0 && nb > 0, "bad sizes");
+    ISB_REQUIRE_FLUSHES((long long)H * W);
     ISB_REQUIRE(dtype >= ISB_U8 && dtype <= ISB_F64, "bad dtype");
     StatWs w;
-    size_t need = carve(w, ws, ws_bytes, nb);
+    size_t x1, x2;
+    const size_t need = carve(w, ws, ws_bytes, nb, &x1, &x2);
     ISB_REQUIRE(need <= ws_bytes, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope prof(ISB_PROF_STATS, st);
-    ISB_CUDA_CHECK(cudaMemsetAsync(ws, 0, need, st));
-    dim3 grid((W + 255) / 256, (H + SROWS - 1) / SROWS);
-    k_stats_pass1<<<grid, 256, 0, st>>>(img, dtype, seg, H, W, 0, w);
-    ISB_LAUNCH_CHECK();
-    if (flags & 2) {
-        k_stats_means<<<(nb + 255) / 256, 256, 0, st>>>(nb, w);
-        ISB_LAUNCH_CHECK();
-        k_stats_pass2<<<grid, 256, 0, st>>>(img, dtype, seg, H, W, w);
-        ISB_LAUNCH_CHECK();
-    }
+    ISB_CUDA_CHECK(cudaMemsetAsync(ws, 0, x1, st));
+    if (int rc = stats_pass1(img, dtype, seg, H, W, 0, nb, w, (char*)ws + x1, x2 - x1, st)) return rc;
+    if (flags & 2)
+        if (int rc = stats_pass2(img, dtype, seg, H, W, nb, w, (char*)ws + x2, need - x2, st)) return rc;
     k_stats_finalize<<<(nb + 255) / 256, 256, 0, st>>>(nb, flags, w, feat, ld, col0, centres, counts);
     ISB_LAUNCH_CHECK();
     return ISB_OK;
 }
 
 // ---- caller-owned accumulators (row bands of one image merged by a collective between the calls) -------------------------
+// The band's exact sums live in memory allocated on the caller's stream for the call.
 
 extern "C" int isb_segment_stats_accumulate(const void* img, int dtype, const int32_t* seg, int H, int W, int y_off, int nb, double* acc,
                                             int64_t* iacc, isb_stream_t stream)
 {
     ISB_REQUIRE(seg && acc && iacc, "null pointer");
     ISB_REQUIRE(H > 0 && W > 0 && nb > 0 && y_off >= 0, "bad sizes");
+    ISB_REQUIRE_FLUSHES((long long)H * W);
     ISB_REQUIRE(dtype >= ISB_U8 && dtype <= ISB_F64, "bad dtype");
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope prof(ISB_PROF_STATS, st);
     StatWs w;
-    w.acc = acc; w.iacc = (long long*)iacc; w.var = nullptr; w.meanf = nullptr;
-    dim3 grid((W + 255) / 256, (H + SROWS - 1) / SROWS);
-    k_stats_pass1<<<grid, 256, 0, st>>>(img, dtype, seg, H, W, y_off, w);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
+    w.acc = acc; w.iacc = (long long*)iacc; w.var = nullptr; w.meanf = nullptr; w.xvar = nullptr; w.xflag2 = nullptr;
+    const size_t xb = xs_carve(nullptr, nb, 6, &w.xacc, &w.xflag1);
+    StreamScratch x(st);
+    ISB_CUDA_CHECK(cudaMallocAsync(&x.p, xb, st));
+    xs_carve(x.p, nb, 6, &w.xacc, &w.xflag1);
+    return stats_pass1(img, dtype, seg, H, W, y_off, nb, w, x.p, xb, st);
 }
 
 extern "C" int isb_segment_stats_deviation(const void* img, int dtype, const int32_t* seg, int H, int W, int nb, const double* acc,
@@ -265,17 +309,17 @@ extern "C" int isb_segment_stats_deviation(const void* img, int dtype, const int
 {
     ISB_REQUIRE(img && seg && acc && iacc && meanf_scratch && var, "null pointer");
     ISB_REQUIRE(H > 0 && W > 0 && nb > 0, "bad sizes");
+    ISB_REQUIRE_FLUSHES((long long)H * W);
     ISB_REQUIRE(dtype >= ISB_U8 && dtype <= ISB_F64, "bad dtype");
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope prof(ISB_PROF_STATS, st);
     StatWs w;
-    w.acc = (double*)acc; w.iacc = (long long*)iacc; w.var = var; w.meanf = meanf_scratch;
-    k_stats_means<<<(nb + 255) / 256, 256, 0, st>>>(nb, w);
-    ISB_LAUNCH_CHECK();
-    dim3 grid((W + 255) / 256, (H + SROWS - 1) / SROWS);
-    k_stats_pass2<<<grid, 256, 0, st>>>(img, dtype, seg, H, W, w);
-    ISB_LAUNCH_CHECK();
-    return ISB_OK;
+    w.acc = (double*)acc; w.iacc = (long long*)iacc; w.var = var; w.meanf = meanf_scratch; w.xacc = nullptr; w.xflag1 = nullptr;
+    const size_t xb = xs_carve(nullptr, nb, 3, &w.xvar, &w.xflag2);
+    StreamScratch x(st);
+    ISB_CUDA_CHECK(cudaMallocAsync(&x.p, xb, st));
+    xs_carve(x.p, nb, 3, &w.xvar, &w.xflag2);
+    return stats_pass2(img, dtype, seg, H, W, nb, w, x.p, xb, st);
 }
 
 extern "C" int isb_segment_stats_finish(int nb, int flags, const double* acc, const double* var, const int64_t* iacc, double* feat, int ld,

@@ -1,7 +1,7 @@
 """
 The banded path (pyimsegm_b200/tiled.py) with the colour-space groups, meanGrad, every device-fitted class model and a caller-fitted
-model, against the single-image drivers.  Statistics are compared on the same label map (``res.d_seg``); both sides sum with f64
-atomics, so a column may differ in its last bits.  On one GPU the bands live side by side in one process; the real multi-GPU run
+model, against the single-image drivers.  Statistics are compared on the same label map (``res.d_seg``); the bands add their own rounded sums, the single image rounds
+its whole sums once, so a column may differ in its last bits and keeps a bound.  On one GPU the bands live side by side in one process; the real multi-GPU run
 is tests/run_tiled_features_ranks.py under torchrun (spawned by test_two_ranks_nccl_features on a host with two GPUs).
 """
 import os
